@@ -49,6 +49,7 @@ UNIT = "recomputes/s"
 K_PEERS = 5
 B_ALG_APPLY = 76                      # SURVEY 8(d): bytes per applied AppendResponse
 N_ARENAS = 4                          # rotated so consecutive steps never share L2 contents
+DUMP_MAX_GROUPS = 2_000_000           # --dump-outputs: 20 B per group, at most 40 MB over all ranks
 
 # BASELINE.json configs: groups per GPU, peer slots in the voter union, joint?, seed
 WORKLOADS = {
@@ -77,7 +78,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 class ClockSampler:
@@ -183,7 +184,7 @@ def cpu_leg(n_groups, seed, rounds_wanted, threads, budget_s=20.0, joint=False):
 
 def run_reference(args, rank, world):
     """--impl reference: the reference's CPU implementation of the path.  raft-rs is Rust and
-    this image has no rustc/cargo, so the arm runs the pinned C port (oracle/) with every host
+    the project does not assume a Rust toolchain, so the arm runs the pinned C port (oracle/) with every host
     thread, on the same config / metric as the GPU arm: it consumes the same 24-byte records the
     GPU arm's `e2e` starts from."""
     if rank != 0:
@@ -237,8 +238,15 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sublegs", action="store_true", help="skip recompute_only / scatter / secondary e2e legs")
     ap.add_argument("--profile", action="store_true",
-                    help="device-resident loop only (for ncu): no clock warm loop, no e2e, no CPU leg")
+                    help="device-resident loop only (for a profiler): no clock warm loop, no e2e, no CPU leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="after the timed steps, write what the last timed step returned (advanced flag and commit "
+                         "index of every group) as DIR/<name>.npy (DIR/<name>_rank<r>.npy per rank under torchrun); "
+                         "beyond 2M groups over all ranks, a fixed seeded sample of each rank's groups and their "
+                         "indexes (group.npy)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs records the GPU path's outputs; the reference arm runs another stream")
     args.warmup = max(args.warmup, 3)
 
     rank = int(os.environ.get("RANK", "0"))
@@ -326,9 +334,9 @@ def main():
 
     def timed(fn, first, count, per_launch=True):
         """count back-to-back steps under CUDA events on the launching stream -> (ms total, ms in kernels).
-        per_launch: an event pair around every launch (the fused kernel: 70 us, the pair costs nothing
-        visible); without it the launches are captured into ONE CUDA graph and replayed, so that short
-        kernels (the 14 us recompute pass) run back to back instead of at the pace Python issues them."""
+        per_launch: an event pair around every launch; without it the launches are captured into ONE CUDA
+        graph and replayed, so that short kernels (the recompute pass) run back to back instead of at the
+        pace Python issues them."""
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         graph = None
         if not per_launch:
@@ -380,6 +388,19 @@ def main():
         # average duration is the timed region / K (no per-launch event pairs, no Python launch pacing in between)
         ms_total, ms_kernel = timed(step_fused, W, K, per_launch=False)
         n_records = sum(round_len[a][r][1] for a, r in schedule[W:W + K])
+        if args.dump_outputs:
+            # the last timed step's outputs, read back before the other legs reuse the buffers
+            a_last = schedule[W + K - 1][0]
+            bm, com = np.empty((n + 31) // 32, dtype=np.uint32), np.empty(n, dtype=np.uint64)
+            arenas[a_last].d2h(bm, d_outs[a_last][0])
+            arenas[a_last].d2h(com, d_outs[a_last][1])
+            dump = {"advanced": np.unpackbits(bm.view(np.uint8), bitorder="little")[:n].astype(np.float32),
+                    "commit_index": com.astype(np.float64)}    # indexes stay below 2^53: exact in float64
+            per_rank = DUMP_MAX_GROUPS // world
+            if n > per_rank:   # a fixed, seeded sample of each rank's groups keeps all ranks' files under 64 MB
+                g = np.sort(np.random.default_rng(0x5EED).choice(n, per_rank, replace=False))
+                dump = {k: v[g] for k, v in dump.items()}
+                dump["group"] = g.astype(np.float64)
         sc = ro = None
         if sublegs:
             # scatter: the same streams continue through the general path (no group order needed)
@@ -417,9 +438,8 @@ def main():
     if ranks_per_node > 1:
         os.environ.setdefault("RAFTGPU_CPU_SHARE", f"{same_node.index(local_rank)}/{ranks_per_node}")
     # three quarters of the rank's share of the GPU-local logical CPUs: every physical core plus half of the SMT
-    # siblings (measured at N = 1: 32 threads 0.91e9/s, 48 threads 1.06e9/s, 56 threads stall -- the caller's and the
-    # submitter's threads need CPUs too)
-    e2e_threads = args.e2e_threads or max(4, min(48, (3 * (len(local_cpus) or 64)) // (4 * ranks_per_node)))
+    # siblings (the caller's and the submitter's threads need CPUs too)
+    e2e_threads = args.e2e_threads or max(4, min(48, (3 * (len(local_cpus) or len(all_cpus))) // (4 * ranks_per_node)))
     os.environ.setdefault("RAFTGPU_HOST_THREADS", str(e2e_threads))
     e2e_steps = 0 if args.profile else (args.e2e_steps or K)
     chunk = max(2, args.e2e_chunk or min(32, e2e_steps))    # `e2e`: one pinned record buffer per step of a chunk
@@ -494,7 +514,7 @@ def main():
         # (RAFTGPU_STEP_ASYNC: the call returns once the staging threads have the batch; the records stay untouched
         # in their pinned buffer until the step's raftgpu_step_wait, which is what this loop does anyway)
         # With a small CPU share (several GPUs per socket) packing is the bottleneck: the records then cross PCIe as
-        # they are (RAFTGPU_STEP_RAW: 3.7x the bytes, no host work at all).  Crossover ~12 staging threads (DESIGN 5).
+        # they are (RAFTGPU_STEP_RAW: 3.7x the bytes, no host work at all).
         # Default: HYBRID -- the library packs the head of the batch while the DMA engine ships the tail as it is,
         # split so that the staging threads and PCIe finish together (include/raftgpu.h RAFTGPU_STEP_HYBRID).
         e2e_mode = os.environ.get("BENCH_E2E_MODE") or "hybrid"
@@ -538,26 +558,14 @@ def main():
     value = world * n * K / (maxes["ms_total"] * 1e-3)
 
     if rank == 0:
-        try:
-            with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-                traffic = json.load(f)
-        except Exception:
-            traffic = {}
         alg_bytes = n_records * B_ALG_APPLY + n * K * b_alg_recompute
         gbs = alg_bytes / (ms_kernel * 1e-3) / 1e9
-        tkey = "step_tile_kernel" + ("" if args.workload in ("cfg3", "cfg5", "cfg2") else "_" + args.workload)
-        tr = traffic.get(tkey)
-        if tr and n != 1_000_000:
-            tr = int(tr * n / 1_000_000)   # the captures are of 1M-group launches; the kernel's traffic is linear in the groups
         dom = {"kernel": "step_tile_kernel", "avg_us": 1e3 * ms_kernel / K, "share": ms_kernel / ms_total,
-               "alg_bytes_per_launch": alg_bytes / K, "achieved": gbs, "frac": gbs / peak_gbs, "traffic": tr}
-        if tr:   # the honest bandwidth fraction: DRAM bytes the kernel really moves (ncu) / its duration
-            dom["dram_gbs"] = tr / (dom["avg_us"] * 1e-6) / 1e9
-            dom["dram_frac"] = dom["dram_gbs"] / peak_gbs
+               "alg_bytes_per_launch": alg_bytes / K, "achieved": gbs, "frac": gbs / peak_gbs}
         cfg = config_of(args)    # identical to the reference arm's
         details = {"records_per_step": n_records / K, "record_format": "16 B packed (raftgpu_pack_records), group order",
                    "device_path": "fused tile kernel (raftgpu_step_sorted_device, group-ordered batch + tile index)",
-                   "outputs": "advanced bitmap + new commit index per advanced group written to HBM inside the timed launches",
+                   "outputs": "advanced bitmap + every group's commit index written to HBM inside the timed launches",
                    "prepared_outside": "packed records and the tile index (4 B per 256 groups) are device resident before the timed "
                                        "region; the `scatter` object is the same step for any arrival order with no index"}
         line = {
@@ -565,12 +573,10 @@ def main():
             "ms_per_step": maxes["ms_total"] / K, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "u64", "data": "synthetic", "config": cfg, "details": details,
             "roofline": {"bound": "hbm", "kernel": dom["kernel"], "achieved": dom["achieved"],
-                         "peak": peak_gbs, "unit": "GB/s", "frac": dom["frac"], "traffic": dom["traffic"],
-                         "dram_frac": dom.get("dram_frac"), "peak_source": peak_src,
+                         "peak": peak_gbs, "unit": "GB/s", "frac": dom["frac"], "peak_source": peak_src,
                          "note": "achieved = SURVEY 8(d) algorithmic bytes (76 B per record + 8K+34 B per group) / the kernel's "
-                                 "average duration (CUDA events); dram_frac = ncu DRAM bytes per launch (profiles/traffic.json) / "
-                                 "the same duration: the fused kernel reads `matched` once, so it moves fewer bytes than the "
-                                 "two-pass algorithmic count"},
+                                 "average duration (CUDA events): the fused kernel reads `matched` once, so it moves fewer "
+                                 "bytes than the two-pass algorithmic count"},
             "kernels": [dom],
             "gpu_launches": K,
             "clocks": clocks,
@@ -584,11 +590,10 @@ def main():
                 "api": "raftgpu_apply_device_packed + raftgpu_recompute: the general path, any arrival order (one record per "
                        "cell per call), no tile index"}
             ro_gbs = world * n * K * b_alg_recompute / (maxes["ro_ms"] * 1e-3) / 1e9
-            rkey = "recompute_kernel" + ("" if args.workload in ("cfg3", "cfg5", "cfg2") else "_" + args.workload)
             line["recompute_only"] = {
                 "value": world * n * K / (maxes["ro_ms"] * 1e-3), "unit": UNIT, "us_per_pass": 1e3 * maxes["ro_ms"] / K,
                 "bytes_per_recompute": b_alg_recompute, "achieved_gbs_per_gpu": ro_gbs / world,
-                "frac": ro_gbs / world / peak_gbs, "traffic": (int(traffic[rkey] * n / 1_000_000) if traffic.get(rkey) else None),
+                "frac": ro_gbs / world / peak_gbs,
                 "api": "raftgpu_recompute: Raft::maybe_commit for every group, nothing applied (BASELINE.md 3: rate x (8K+34) B)"}
         apis = {
             "e2e": "raftgpu_step_begin_records(READ_COMMITTED | ASYNC | HYBRID) + raftgpu_step_wait (`mode`: hybrid; packed = "
@@ -612,7 +617,7 @@ def main():
                           "api": apis[name]}
         if "e2e" in line:
             line["e2e"].update({"caller_record_bytes_per_step": 24.0 * n_records / K, "host_threads": e2e_threads, "mode": e2e_mode,
-                                "host_cpus_bound": len(local_cpus) or None})
+                                "host_cpus_bound": len(local_cpus) or None, "host_cpus": len(all_cpus)})
         if world == 1 and not args.no_cpu_baseline and not args.profile:
             os.sched_setaffinity(0, all_cpus)   # the CPU baseline gets every host core
             threads = len(all_cpus)
@@ -622,6 +627,10 @@ def main():
                 "sample": f"{done} rounds of the same {args.workload} stream (apply + recompute), {threads} "
                           "pthreads, oracle/raft_oracle.c tuned path (ro_bench_step_fast, == the literal port)"}
         print(json.dumps(line), flush=True)
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + (f"_rank{rank}" if world > 1 else "") + ".npy"), arr)
     for a in arenas:
         a.close()
     ea.close()

@@ -1,5 +1,5 @@
 /*
- * raftgpu.h -- C-ABI boundary of the B200 batched multi-raft commit-index engine.
+ * raftgpu.h -- C-ABI boundary of the H100 batched multi-raft commit-index engine.
  *
  * raft-rs (pingcap/raft-rs, crate `raft` 0.6.0 @ 7c21f8d) has no FFI/plugin
  * interface for this path: the boundary is the Rust method surface of
@@ -543,7 +543,7 @@ int32_t raftgpu_step_slot_results(raftgpu_arena *arena, const uint8_t **results,
 /* raftgpu_step_begin_records only: ship the 24-byte records AS THEY ARE (one H2D straight from the caller's buffer,
  * which should be pinned: raftgpu_host_alloc) and apply them with the scatter kernel -- no host packing at all.
  * 3.7x the PCIe bytes of the compact stream, zero CPU: the better choice when the caller's CPU share is small
- * (several GPUs per socket: packing is CPU-bound, ~7 ns per record per staging thread, DESIGN.md 5/7).  Contract of
+ * (several GPUs per socket: packing is CPU-bound, DESIGN.md 4/7).  Contract of
  * the zero-copy paths: at most ONE record per (group, peer) cell, verified on the GPU (a duplicate is not applied,
  * counted in n_duplicates, raftgpu_step_wait returns RAFTGPU_ERR_INVALID); `records` stays untouched until the
  * step's raftgpu_step_wait returns. */

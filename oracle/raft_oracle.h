@@ -12,7 +12,7 @@
  * reference's own golden vectors (tests/golden/quorum/ .txt files, copied from
  * src/quorum/testdata/) and against the table tests listed next to each
  * function (tests/test_oracle_*.py).  The reference itself is Rust and cannot
- * be built in this image (no rustc/cargo), so there is no oracle/_ref.
+ * be built without a Rust toolchain, which the project does not assume, so there is no oracle/_ref.
  *
  * Every function cites the reference file:line it restates (paths relative to
  * the reference checkout).

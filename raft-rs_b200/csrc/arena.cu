@@ -123,7 +123,7 @@ struct RecJob {
 struct HostPool {
     // One sleeper slot per worker: a worker that has spun long enough sleeps on ITS OWN condition variable.
     // (One shared condition variable makes the wake-up a convoy: the woken threads queue on the one mutex and
-    // come back one after the other, each paying its core's idle-state exit -- measured 6-8 ms for 32 workers.)
+    // come back one after the other, each paying its core's idle-state exit.)
     struct alignas(128) Sleeper {
         std::mutex mu;
         std::condition_variable cv;
@@ -185,8 +185,8 @@ struct HostPool {
             while (generation.load(std::memory_order_acquire) == seen && !stop.load(std::memory_order_relaxed)) {
                 cpu_relax();
                 // a spinning worker owns its CPU as far as the scheduler can tell: give way to whatever else is
-                // runnable there (measured: the caller's thread, time-sliced against a spinning worker, lost ~0.4 ms
-                // per call)
+                // runnable there (the caller's thread, time-sliced against a spinning worker, loses time on
+                // every call)
                 if ((++spins & 127u) == 0) sched_yield();
                 if ((spins & 255u) == 0 &&
                     std::chrono::steady_clock::now() - t_idle > std::chrono::microseconds(spin_us)) {
@@ -284,8 +284,7 @@ namespace {
 thread_local std::string g_create_error;
 
 // Pinned staging must live on the NUMA node the GPU's PCIe root hangs off: DMA reads of
-// remote-socket memory cross the inter-socket link and lose about half of the H2D bandwidth
-// (measured on the 2-socket B200 hosts: 27 GB/s remote vs ~55 GB/s local).  cudaHostAlloc
+// remote-socket memory cross the inter-socket link and lose H2D bandwidth.  cudaHostAlloc
 // places pages by first touch, so the allocating thread is moved onto the GPU-local CPUs
 // (sysfs local_cpulist of the device) for the duration of the allocations.
 struct LocalCpuGuard {

@@ -31,8 +31,8 @@ __device__ __forceinline__ void reset_state(const Columns &c, size_t cell, Cell 
 //                        committed_index) of element k+1,
 //   and computes / stores element k,
 // so every load has a whole iteration to land.  (An extra L2-prefetch stage, kPrefetch, was
-// measured and does not help: at ~12 MB in flight the kernel is limited by the DRAM
-// efficiency of sector-granular scattered accesses, not by latency -- profiles/.)
+// measured and does not help: with this many loads in flight the kernel is limited by the DRAM
+// efficiency of sector-granular scattered accesses, not by latency.)
 // Algorithmic bytes per record: 24 (record) + RMW of matched, next_idx,
 // committed_index (48) + flag byte and meta (~4) = 76.
 struct RecRegs {

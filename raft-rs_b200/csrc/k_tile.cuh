@@ -4,7 +4,7 @@
 // ---------------------------------------------------------------------------
 // step_tile_kernel: apply + recompute FUSED, for batches whose records are in group order.
 //
-// The scatter apply kernel above moves ~12 MB in flight but tops out near 3.7 TB/s: its cell
+// The scatter apply kernel above keeps many loads in flight but stays far below the HBM peak: its cell
 // accesses are sector-granular (8 useful bytes per 32-byte sector request, several rows per
 // record), which HBM serves at roughly half the efficiency of dense bursts.  When the batch is
 // ordered by group, a tile of kFTile consecutive groups owns a CONTIGUOUS record range, so the
@@ -231,8 +231,8 @@ __global__ void __launch_bounds__(kCT *kNG + 64, 1) step_tile_kernel(Columns c, 
             const PackedRec *s_recs = reinterpret_cast<const PackedRec *>(sb + o_recs);
             const ulonglong2 *g_recs = reinterpret_cast<const ulonglong2 *>(a.recs + rbeg);
             // direct records: this thread's first record is requested BEFORE the wait for the stage (its address does
-            // not depend on it); the loop then fetches one record ahead.  (Two ahead measured 11 % SLOWER -- 83.5 vs
-            // 75.0 us, scripts/micro_tile.py: the kernel sits at its 72-register ceiling and the consumers are bound by
+            // not depend on it); the loop then fetches one record ahead.  (Two ahead was slower
+            // with scripts/micro_tile.py: the kernel sits near its register ceiling and the consumers are bound by
             // issue latency, not by the record reads.)
             ulonglong2 q_next = make_ulonglong2(kPkExt, 0ull);
             if (staged == 0 && tid < cnt) q_next = g_recs[tid];

@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a device code of the batched commit-index engine.
+// kernels.cuh -- sm_90a device code of the batched commit-index engine.
 //
 // Every kernel here is HBM-bound u64 index arithmetic over the SoA arena
 // (DESIGN.md); there is no floating point and no tensor-core work on this path.

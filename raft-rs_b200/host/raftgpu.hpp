@@ -1,6 +1,6 @@
 // raftgpu.hpp -- C++17 mirror of the raft-rs tracker / quorum surface over the C-ABI.
 //
-// The reference is a Rust crate and this image has no Rust toolchain, so the host side above
+// The reference is a Rust crate and the project builds without a Rust toolchain, so the host side above
 // include/raftgpu.h is written in C++: same type and method names, argument meaning and error
 // behaviour as the crate (file:line of each counterpart is given), every piece of arithmetic
 // forwarded to libraftgpu.so -- there is no CPU implementation of the path in here.  The Rust

@@ -5,7 +5,7 @@ The reference serializes messages with rust-protobuf 2 / prost 0.7 (proto/Cargo.
 vendored nor buildable here, and holds no wire-format goldens for this path.  The vectors are therefore
 produced by an INDEPENDENT implementation of the same published format: Google's python-protobuf,
 from a descriptor that restates `message Message` / `Entry` / `Snapshot` of
-/root/reference/proto/proto/eraftpb.proto:23-92 field for field (numbers and types).  "Parity unpinned by
+the reference's proto/proto/eraftpb.proto:23-92 field for field (numbers and types).  "Parity unpinned by
 the reference" (DESIGN.md 6): what is pinned is proto3 wire compatibility.
 
     python scripts/gen_wire_golden.py            # rewrites tests/golden/wire/messages.json

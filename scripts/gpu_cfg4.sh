@@ -1,6 +1,6 @@
 #!/bin/bash
 # cfg4 (1M x 7 joint) measurements: fused, scatter, with CPU arm
-OUT=gpurun_out/cfg4; mkdir -p $OUT
+OUT=runs/cfg4; mkdir -p $OUT
 timeout 600 python bench.py --workload cfg4 --steps 60 --warmup 6 --e2e-steps 8 > $OUT/fused.json 2> $OUT/fused.err
 timeout 600 python bench.py --workload cfg4 --steps 60 --warmup 6 --e2e-steps 8 --no-cpu-baseline --scatter > $OUT/scatter.json 2> $OUT/scatter.err
 python - <<PY

@@ -1,6 +1,6 @@
 #!/bin/bash
 # cfg5-sized run: 10M groups x 5 peers over 8 GPUs (1.25M per GPU), as the driver launches bench.py
-N=${1:-8}; OUT=gpurun_out/multi; mkdir -p $OUT
+N=${1:-8}; OUT=runs/multi; mkdir -p $OUT
 python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1 --master-port 29541 \
   bench.py --gpus $N --steps 40 --warmup 4 --e2e-steps 8 --groups 1250000 > $OUT/bench_cfg5_n$N.json 2> $OUT/bench_cfg5_n$N.err
 echo "rc=$?"

@@ -2,7 +2,7 @@
 # Round-2 final evidence call: ncu launch list + --set full captures (fused tile kernel cfg3 / cfg4, recompute, wire,
 # the compact tile kernel the e2e step runs), SASS mnemonic summary, then the bench lines (driver flags) for cfg3 /
 # cfg4 / cfg5-per-GPU and the reference arm.  usage: scripts/gpu_final_r2.sh <tag>
-TAG=${1:-r02c}; OUT=gpurun_out/$TAG; mkdir -p $OUT
+TAG=${1:-r02c}; OUT=runs/$TAG; mkdir -p $OUT
 timeout 1500 python -m pytest tests -q -m gpu 2>&1 | grep -v "^    " | tail -6 > $OUT/pytest_gpu.txt; cat $OUT/pytest_gpu.txt
 PROF="python bench.py --profile --steps 8 --warmup 3"
 timeout 300 ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file $OUT/launches.csv $PROF > $OUT/ncu_launches.log 2>&1

@@ -1,6 +1,6 @@
 #!/bin/bash
 # hybrid staging: smoke, then the e2e leg in its modes at several staging-thread counts (strict timeouts)
-OUT=gpurun_out/${1:-hyb}; mkdir -p $OUT
+OUT=runs/${1:-hyb}; mkdir -p $OUT
 timeout 200 python __graft_entry__.py smoke 2>&1 | tail -2
 for T in ${2:-48 12}; do
   for M in ${3:-hybrid packed raw}; do

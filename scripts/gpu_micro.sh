@@ -1,5 +1,5 @@
 #!/bin/bash
-OUT=gpurun_out/micro; mkdir -p $OUT
+OUT=runs/micro; mkdir -p $OUT
 {
 python scripts/micro_recompute.py
 RAFTGPU_FORCE_GENERAL=1 python scripts/micro_recompute.py

@@ -1,6 +1,6 @@
 #!/bin/bash
 # multi-GPU bench under torchrun, as the driver launches it (strict timeouts)
-N=${1:-2}; OUT=gpurun_out/multi; mkdir -p $OUT
+N=${1:-2}; OUT=runs/multi; mkdir -p $OUT
 nvidia-smi --query-gpu=index,name --format=csv,noheader | head -8
 timeout ${2:-240} python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1 --master-port 29533 \
   bench.py --gpus $N --steps 20 --warmup 5 --no-sublegs --no-cpu-baseline > $OUT/bench_n$N.json 2> $OUT/bench_n$N.err

@@ -1,7 +1,7 @@
 #!/bin/bash
 # quick GPU iteration: selected parity tests, then the device-resident bench with phase timing
 # usage: gpu_quick.sh [pytest -k expression]
-OUT=gpurun_out/quick; mkdir -p $OUT
+OUT=runs/quick; mkdir -p $OUT
 timeout 1500 python -m pytest tests -m gpu -x -q -k "${1:-fused or every_ingest or golden}" > $OUT/pytest.txt 2>&1; tail -n 4 $OUT/pytest.txt
 RAFTGPU_TILE_DEBUG=1 timeout 600 python bench.py --steps 60 --warmup 6 --no-cpu-baseline --e2e-steps 4 > $OUT/bench.json 2> $OUT/bench.err
 grep "tile debug" $OUT/bench.err

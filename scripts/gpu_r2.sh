@@ -1,7 +1,7 @@
 #!/bin/bash
 # Round-2 GPU call: parity tests, the host packer's thread scaling on the box's CPUs, the bench line.
 # usage: scripts/gpu_r2.sh <tag> [steps]
-TAG=${1:-r2}; STEPS=${2:-20}; OUT=gpurun_out/$TAG; mkdir -p $OUT
+TAG=${1:-r2}; STEPS=${2:-20}; OUT=runs/$TAG; mkdir -p $OUT
 lscpu | grep -E "Model name|^CPU\(s\)|Thread|Socket|NUMA" > $OUT/env.txt
 timeout 900 python -m pytest tests -m gpu -x -q > $OUT/pytest_gpu.txt 2>&1; echo "pytest rc=$?" >> $OUT/pytest_gpu.txt
 tail -n 3 $OUT/pytest_gpu.txt

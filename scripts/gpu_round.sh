@@ -1,7 +1,7 @@
 #!/bin/bash
 # One GPU round: parity tests, smoke, bench (fused default + scatter), ncu launch lists + full captures.
 # usage: scripts/gpu_round.sh <tag> [skip_tests]
-TAG=${1:-r}; OUT=gpurun_out/$TAG; mkdir -p $OUT
+TAG=${1:-r}; OUT=runs/$TAG; mkdir -p $OUT
 if [ -z "$2" ]; then
   timeout 300 python __graft_entry__.py smoke > $OUT/smoke.txt 2>&1; echo "smoke rc=$?" >> $OUT/smoke.txt
   timeout 1800 python -m pytest tests -m gpu -x -q > $OUT/pytest_gpu.txt 2>&1; echo "pytest rc=$?" >> $OUT/pytest_gpu.txt

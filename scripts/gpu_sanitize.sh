@@ -1,6 +1,6 @@
 #!/bin/bash
 # compute-sanitizer over the small parity tests of the new kernels, then the whole GPU suite
-OUT=gpurun_out/sanitize; mkdir -p $OUT
+OUT=runs/sanitize; mkdir -p $OUT
 K='corner_cases or send_list or (compact_stream_submission and 40000) or (step_begin_records and (900 or 30000)) or golden or every_ingest_path or fused_tile_step_learners'
 timeout 1500 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_parity.py -m gpu -x -q -k "$K" > $OUT/memcheck.txt 2>&1; echo "memcheck rc=$?" | tee -a $OUT/memcheck.txt
 grep -E "ERROR SUMMARY|passed|failed|Invalid|out of bounds" $OUT/memcheck.txt | tail -6

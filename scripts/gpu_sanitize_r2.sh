@@ -1,7 +1,7 @@
 #!/bin/bash
 # Round-2 sanitizer call: compute-sanitizer (memcheck + racecheck) on the new / changed kernels, and the whole
 # -m gpu suite's host side under an ASan + UBSan build of the library.  usage: scripts/gpu_sanitize_r2.sh <tag>
-TAG=${1:-r02s}; OUT=gpurun_out/$TAG; mkdir -p $OUT
+TAG=${1:-r02s}; OUT=runs/$TAG; mkdir -p $OUT
 K="wire or heartbeat or update_state or every_ingest or raw_record or async_record"
 timeout 900 compute-sanitizer --tool memcheck --error-exitcode 7 python -m pytest tests -m gpu -x -q -k "$K" > $OUT/memcheck.txt 2>&1; echo "memcheck rc=$?" >> $OUT/memcheck.txt
 timeout 900 compute-sanitizer --tool racecheck --error-exitcode 7 python -m pytest tests/test_gpu_wire.py tests/test_gpu_parity.py -m gpu -x -q -k "wire_golden or golden_messages or every_ingest or heartbeat" > $OUT/racecheck.txt 2>&1; echo "racecheck rc=$?" >> $OUT/racecheck.txt

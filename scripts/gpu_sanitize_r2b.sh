@@ -2,7 +2,7 @@
 # Round-2 second sanitizer call (code added after the first): compute-sanitizer racecheck + memcheck on the fused kernels'
 # new stage hand-over (wait_stage) at small sizes, and the host side of the wide-group / hybrid / fallback code under
 # ASan + UBSan.  usage: scripts/gpu_sanitize_r2b.sh <tag>
-TAG=${1:-r02s2}; OUT=gpurun_out/$TAG; mkdir -p $OUT
+TAG=${1:-r02s2}; OUT=runs/$TAG; mkdir -p $OUT
 K="fused_compact_step_corner or fused_tile_step_learners or fused_kernels_in_their_other or golden_vectors_through_a_wide or wide_control"
 timeout 400 compute-sanitizer --tool racecheck --error-exitcode 7 python -m pytest tests -m gpu -x -q -k "$K" > $OUT/racecheck.txt 2>&1; echo "racecheck rc=$?" >> $OUT/racecheck.txt
 timeout 400 compute-sanitizer --tool memcheck --error-exitcode 7 python -m pytest tests -m gpu -x -q -k "$K or steps_over_mixed" > $OUT/memcheck.txt 2>&1; echo "memcheck rc=$?" >> $OUT/memcheck.txt

@@ -1,10 +1,10 @@
-"""Summarise ncu captures (gpurun_out/<tag>/) into a committed profiles/<name>.md."""
+"""Summarise ncu captures (runs/<tag>/) into a markdown file <name>.md."""
 import csv, json, subprocess, sys, os, collections
 
 tag, out = sys.argv[1], sys.argv[2]
-d = f"gpurun_out/{tag}"
+d = f"runs/{tag}"
 L = []
-L.append(f"# ncu summary `{tag}` (B200, sm_100a)\n")
+L.append(f"# ncu summary `{tag}` (H100, sm_90a)\n")
 L.append("Source: `scripts/gpu_final_r2.sh` (round 1: `scripts/gpu_round.sh`) -> `ncu --set full --clock-control none --import-source on` on "
          "`python bench.py --profile --steps 8 --warmup 3` (1M groups x 5 peers, 4 arenas rotated), and the "
          "`--metrics gpu__time_duration.sum` launch list of the same command.  ncu serialises kernels and "

@@ -3,7 +3,7 @@
 Bit-exact (integer / index work): golden vectors replayed THROUGH the GPU, the
 reference's table tests, full element-wise comparison of every column on the
 synthetic streams (BASELINE configs 2-4), and size-independent properties at the
-full sizes.  Run with ``-m gpu`` on a B200.
+full sizes.  Run with ``-m gpu`` on an H100.
 """
 import ctypes as C
 import os
