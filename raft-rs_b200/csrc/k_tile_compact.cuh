@@ -3,7 +3,7 @@
 
 // step_tile_compact_kernel: the fused step for a TILEABLE compact stream (groups ascending, every
 // run headed -- raftgpu_compact_hdr.flags & RAFTGPU_COMPACT_TILEABLE).  Same producer / store
-// warps and stage ring as step_tile_kernel; the consumers work per GROUP instead of per record:
+// warps and stage ring (TileRing, k_tile.cuh) as step_tile_kernel; the consumers work per GROUP instead of per record:
 //   0. a unit-parallel pre-pass finds, for every group of the tile, the first unit of its first
 //      run (shared-memory atomicMin on the run headers),
 //   1. thread gl then walks the runs of group g0+gl SEQUENTIALLY -- header decoded once, each
@@ -15,314 +15,54 @@
 // header/cell address arithmetic, no three-way divergence on the record kind) and a third of the
 // record bytes.  tile_off[t] = unit position of the first run header of tile t.
 struct CTileArgs {
+    TileRingArgs r;
     CompactSrc src;
-    const uint32_t *tile_off;  // [n_tiles + 1], unit positions
     const uint2 *tile_gb;      // [n_tiles]: g_base of the unit block tile t starts in, and of the next block
-    uint32_t n_groups;
-    uint32_t hint;
-    int n_stages;
-    uint32_t unit_cap;         // units staged in shared memory per tile (multiple of 4); the rest is read from HBM
-    uint8_t *results;          // nullable, one byte per unit
-    uint32_t *adv_bitmap;      // nullable
-    uint64_t *commit_out;      // nullable
-    uint32_t *step_advanced;   // nullable
-    unsigned long long *counters;
-    unsigned long long *dbg;   // nullable
     uint32_t *dup_count;       // nullable (!kOrdered): bumped for a second record on one cell, which is not applied
 };
-
-__host__ __device__ constexpr uint32_t ctile_stage_bytes(uint32_t H, uint32_t unit_cap) {
-    return 3u * H * kFRow64 + 3u * kFRow64 + kFTile * 4u + H * kFRow8 + unit_cap * 4u;
-}
-// dynamic shared memory: the stages, then one u32 run index per group per consumer group
-__host__ __device__ constexpr uint32_t ctile_smem_bytes(uint32_t H, uint32_t unit_cap, int stages, int n_groups_c) {
-    return static_cast<uint32_t>(stages) * ctile_stage_bytes(H, unit_cap) + static_cast<uint32_t>(n_groups_c) * kFTile * 4u;
-}
-
-struct TileRows {
-    uint64_t *matched, *next, *pc, *committed, *ts, *li;
-    uint32_t *meta;
-    uint8_t *flags;
-};
-
-// A record that is not on the fast path (Snapshot state, a REJECT / hostile value from the side
-// table, a peer slot outside the hint): the literal apply_one against the shared-memory cell, or
-// against HBM for a slot the tile does not stage.
-__device__ __forceinline__ uint32_t tile_general_apply(const Columns &c, const RecRegs &rec, uint64_t ext_hint,
-                                                    uint64_t ext_snapshot, uint32_t gl, uint32_t hint,
-                                                    const TileRows &t, uint32_t *local) {
-    constexpr uint32_t R64 = kFRow64 / 8;
-    const uint32_t slot = static_cast<uint32_t>(rec.w0 >> 32) & 0xffu;
-    if (slot < kSlots && ((hint >> slot) & 1u)) {
-        const uint32_t r = __popc(hint & ((1u << slot) - 1u));
-        CellRegs cd;
-        cd.meta = t.meta[gl];
-        cd.matched = t.matched[r * R64 + gl];
-        cd.next_idx = t.next[r * R64 + gl];
-        cd.flags = t.flags[r * kFRow8 + gl];
-        cd.peer_committed = t.pc[r * R64 + gl];
-        const CellPtrs sp{&t.matched[r * R64 + gl], &t.next[r * R64 + gl], &t.pc[r * R64 + gl], &t.li[gl],
-                          &t.flags[r * kFRow8 + gl]};
-        return apply_one<2>(c, nullptr, ext_hint, ext_snapshot, rec, cd, sp, local);
-    }
-    CellRegs cd = load_cell(c, rec);
-    cd.meta = t.meta[gl];
-    CellPtrs gp = global_cell_ptrs(c, rec);
-    gp.last_index = &t.li[gl];
-    return apply_one<2>(c, nullptr, ext_hint, ext_snapshot, rec, cd, gp, local);
-}
-
-// The common records -- accept, leader-local, rejection without a snapshot request -- for a peer
-// in Replicate or Probe state whose cell is staged in shared memory: statement for statement the
-// branches of apply_one (raft.rs:1674-1677, 1709-1730, 974-991, 1010-1014; progress.rs:95-114,
-// 138-157, 168-206).  Returns false (nothing touched) when the record needs the general path.
-template <bool kSimple5>
-__device__ __forceinline__ bool tile_fast_apply(const Columns &c, const TileRows &t, uint32_t gl, uint32_t g, uint32_t slot,
-                                                uint64_t index, uint64_t commit, bool is_local, bool is_reject,
-                                                uint64_t ext_hint, uint32_t hint, uint32_t present_mask, uint32_t *local,
-                                                uint32_t &res) {
-    constexpr uint32_t R64 = kFRow64 / 8;
-    if (!((hint >> slot) & 1u)) return false;
-    const uint32_t r = kSimple5 ? slot : static_cast<uint32_t>(__popc(hint & ((1u << slot) - 1u)));
-    const uint32_t ci = r * R64 + gl;
-    const uint32_t f0 = t.flags[r * kFRow8 + gl];
-    const uint32_t state = f0 & RAFTGPU_PF_STATE_MASK;
-    if (!((present_mask >> slot) & 1u) || state == RAFTGPU_STATE_SNAPSHOT) return false;
-    uint64_t m = t.matched[ci], nx = t.next[ci];
-    const uint64_t m0 = m, nx0 = nx;
-    uint32_t f = f0;
-    local[0]++;
-    if (is_local) {
-        if (commit != 0) t.li[gl] = commit;
-    } else {
-        f |= RAFTGPU_PF_RECENT_ACTIVE;
-        if (commit > t.pc[ci]) t.pc[ci] = commit;
-    }
-    if (is_reject) {  // maybe_decr_to without a snapshot request
-        local[2]++;
-        bool ok;
-        if (state == RAFTGPU_STATE_REPLICATE) {
-            ok = index > m;                              // progress.rs:173-177 stale otherwise
-            if (ok) nx = m + 1;                          // :178-179
-        } else if (nx == 0 || nx - 1 != index) {
-            ok = false;                                  // :188-192 stale
-        } else {
-            nx = umin64(index, ext_hint + 1);            // :195-199
-            if (nx < 1) nx = 1;
-            f &= ~RAFTGPU_PF_PAUSED;                     // :204
-            ok = true;
-        }
-        if (ok) {
-            local[3]++;
-            res = RAFTGPU_RES_OK | RAFTGPU_RES_SEND;
-            if (state == RAFTGPU_STATE_REPLICATE) {      // raft.rs:1716-1718 become_probe
-                f = (f & ~(RAFTGPU_PF_PAUSED | RAFTGPU_PF_INS_FULL | RAFTGPU_PF_STATE_MASK)) | RAFTGPU_STATE_PROBE;
-                c.pending_snapshot[static_cast<size_t>(slot) * c.cap + g] = 0;
-                nx = m + 1;
-            }
-        }
-    } else {
-        const bool old_paused = !is_local && (state == RAFTGPU_STATE_PROBE ? (f & RAFTGPU_PF_PAUSED) != 0
-                                                                           : (f & RAFTGPU_PF_INS_FULL) != 0);
-        const bool need = m < index;
-        if (need) {
-            m = index;
-            f &= ~RAFTGPU_PF_PAUSED;
-            local[1]++;
-            res = RAFTGPU_RES_OK | (old_paused ? RAFTGPU_RES_OLD_PAUSED : 0u);
-        }
-        if (nx < index + 1) nx = index + 1;
-        if (need && !is_local && state == RAFTGPU_STATE_PROBE) {
-            f = (f & ~(RAFTGPU_PF_PAUSED | RAFTGPU_PF_INS_FULL | RAFTGPU_PF_STATE_MASK)) | RAFTGPU_STATE_REPLICATE;
-            c.pending_snapshot[static_cast<size_t>(slot) * c.cap + g] = 0;
-            nx = m + 1;
-        }
-    }
-    if (m != m0) t.matched[ci] = m;
-    if (nx != nx0) t.next[ci] = nx;
-    if (f != f0) t.flags[r * kFRow8 + gl] = static_cast<uint8_t>(f);
-    return true;
-}
 
 // kOrdered: per-group walk (records of a cell apply in stream order; any number per cell).
 // !kOrdered: one thread per unit (faster; at most one record per (group, peer) cell per batch --
 // checked on the fly in a shared-memory bitmap when a.dup_count is given).
-template <bool kSimple5, int kNG, bool kOrdered>
-__global__ void __launch_bounds__(kFTile *kNG + 64, 1) step_tile_compact_kernel(Columns c, CTileArgs a) {
-    constexpr int kCT = kFTile;
+template <bool kSimple5, bool kOrdered>
+__global__ void __launch_bounds__(kFThreads, 1) step_tile_compact_kernel(Columns c, CTileArgs a) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ __align__(8) uint64_t full_bar[kFMaxStages];
-    __shared__ __align__(8) uint64_t done_bar[kFMaxStages];
-    __shared__ __align__(8) uint64_t empty_bar[kFMaxStages];
+    __shared__ __align__(8) TileBarriers bars;
 
-    const uint32_t hint = kSimple5 ? 0x1fu : (a.hint & 0xffu);
-    const uint32_t H = kSimple5 ? 5u : static_cast<uint32_t>(__popc(hint));
-    const uint32_t o_matched = 0, o_next = H * kFRow64, o_pc = 2u * H * kFRow64, o_committed = 3u * H * kFRow64,
-                   o_ts = o_committed + kFRow64, o_li = o_ts + kFRow64, o_meta = o_li + kFRow64,
-                   o_flags = o_meta + kFTile * 4u, o_units = o_flags + H * kFRow8,
-                   stage_bytes = ctile_stage_bytes(H, a.unit_cap);
-    const uint32_t n_tiles = (a.n_groups + kFTile - 1) / kFTile;
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t *s_run_all = reinterpret_cast<uint32_t *>(smem + static_cast<size_t>(a.n_stages) * stage_bytes);
+    const TileRing<kSimple5, kCUnitCap> ring(a.r, &bars, smem);
+    const uint32_t warp = threadIdx.x >> 5;
+    const uint32_t hint = ring.hint;
+    uint32_t *s_run_all = reinterpret_cast<uint32_t *>(ring.extra());
+    if (threadIdx.x < kFGroups * kFTile) s_run_all[threadIdx.x] = kOrdered ? 0xffffffffu : 0u;
+    ring.init_barriers();
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < a.n_stages; s++) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&done_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (threadIdx.x < kNG * kCT) s_run_all[threadIdx.x] = kOrdered ? 0xffffffffu : 0u;
-    __syncthreads();
-
-    uint32_t local[7] = {0, 0, 0, 0, 0, 0, 0};  // records, updates, rejects, decrements, no_progress | recomputes, advanced
-    if (warp == kNG * kCT / 32 + 1) {
-        // ===================== store warp =====================
-        const uint32_t n_out = 4u * H + 2u + (a.commit_out ? 1u : 0u);
-        uint32_t it = 0;
-        for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, it++) {
-            const int st = it % a.n_stages;
-            const uint32_t ph = (it / a.n_stages) & 1u;
-            const uint32_t g0 = tile * kFTile;
-            const uint32_t ng = a.n_groups - g0 < kFTile ? a.n_groups - g0 : kFTile;
-            const uint32_t ng16 = (ng + 15u) & ~15u;
-            uint8_t *sb = smem + static_cast<size_t>(st) * stage_bytes;
-            mbar_wait(&done_bar[st], ph);
-            for (uint32_t j = lane; j < n_out; j += 32) {
-                if (j < 4u * H) {
-                    const uint32_t col = j / H, r = j % H;
-                    uint32_t slot = 0, seen = 0;
-                    for (uint32_t s2 = 0; s2 < kSlots; s2++)
-                        if ((hint >> s2) & 1u) {
-                            if (seen == r) slot = s2;
-                            seen++;
-                        }
-                    const size_t cell = static_cast<size_t>(slot) * c.cap + g0;
-                    if (col == 0) tma_store_1d(c.matched + cell, sb + o_matched + r * kFRow64, ng16 * 8u);
-                    if (col == 1) tma_store_1d(c.next_idx + cell, sb + o_next + r * kFRow64, ng16 * 8u);
-                    if (col == 2) tma_store_1d(c.peer_committed + cell, sb + o_pc + r * kFRow64, ng16 * 8u);
-                    if (col == 3) tma_store_1d(c.pflags + cell, sb + o_flags + r * kFRow8, ng16);
-                } else if (j == 4u * H) {
-                    tma_store_1d(c.committed + g0, sb + o_committed, ng16 * 8u);
-                } else if (j == 4u * H + 1u) {
-                    tma_store_1d(c.last_index + g0, sb + o_li, ng16 * 8u);
-                } else {  // the step's commit-index output: the tile's `committed` row, one dense copy (not 8-byte scatters)
-                    tma_store_1d(a.commit_out + g0, sb + o_committed, ng16 * 8u);
-                }
-            }
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[st]);
-        }
-        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    } else if (warp == kNG * kCT / 32) {
-        // ===================== load warp =====================
-        const uint32_t n_copies = 4u * H + 5u;
-        uint32_t it = 0;
-        uint32_t nx_u0 = blockIdx.x < n_tiles ? a.tile_off[blockIdx.x] : 0u, nx_u1 = blockIdx.x < n_tiles ? a.tile_off[blockIdx.x + 1] : 0u;
-        for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, it++) {
-            const int st = it % a.n_stages;
-            const uint32_t ph = (it / a.n_stages) & 1u;
-            const uint32_t g0 = tile * kFTile;
-            const uint32_t ng = a.n_groups - g0 < kFTile ? a.n_groups - g0 : kFTile;
-            const uint32_t ng16 = (ng + 15u) & ~15u;
-            // the tile's units, from the 16-byte boundary below its first one
-            const uint32_t u0 = nx_u0, u1 = nx_u1;
-            if (tile + gridDim.x < n_tiles) {  // next tile's index: fetched while this one is being issued
-                nx_u0 = a.tile_off[tile + gridDim.x];
-                nx_u1 = a.tile_off[tile + gridDim.x + 1];
-            }
-            const uint32_t ua = u0 & ~3u;
-            const uint32_t cnt4 = (u1 - ua + 3u) & ~3u;
-            const uint32_t staged = u1 > u0 ? (cnt4 < a.unit_cap ? cnt4 : a.unit_cap) : 0u;
-            if (lane == 0) {
-                mbar_wait(&empty_bar[st], ph ^ 1u);
-                mbar_expect_tx(&full_bar[st], 3u * H * ng16 * 8u + H * ng16 + 3u * ng16 * 8u + ng16 * 4u + staged * 4u);
-            }
-            __syncwarp();
-            uint8_t *sb = smem + static_cast<size_t>(st) * stage_bytes;
-            for (uint32_t j = lane; j < n_copies; j += 32) {
-                if (j < 4u * H) {
-                    const uint32_t col = j / H, r = j % H;
-                    uint32_t slot = 0, seen = 0;
-                    for (uint32_t s2 = 0; s2 < kSlots; s2++)
-                        if ((hint >> s2) & 1u) {
-                            if (seen == r) slot = s2;
-                            seen++;
-                        }
-                    const size_t cell = static_cast<size_t>(slot) * c.cap + g0;
-                    if (col == 0) tma_load_1d(sb + o_matched + r * kFRow64, c.matched + cell, ng16 * 8u, &full_bar[st]);
-                    if (col == 1) tma_load_1d(sb + o_next + r * kFRow64, c.next_idx + cell, ng16 * 8u, &full_bar[st]);
-                    if (col == 2) tma_load_1d(sb + o_pc + r * kFRow64, c.peer_committed + cell, ng16 * 8u, &full_bar[st]);
-                    if (col == 3) tma_load_1d(sb + o_flags + r * kFRow8, c.pflags + cell, ng16, &full_bar[st]);
-                } else if (j == 4u * H) {
-                    tma_load_1d(sb + o_committed, c.committed + g0, ng16 * 8u, &full_bar[st]);
-                } else if (j == 4u * H + 1) {
-                    tma_load_1d(sb + o_ts, c.term_start + g0, ng16 * 8u, &full_bar[st]);
-                } else if (j == 4u * H + 2) {
-                    tma_load_1d(sb + o_li, c.last_index + g0, ng16 * 8u, &full_bar[st]);
-                } else if (j == 4u * H + 3) {
-                    tma_load_1d(sb + o_meta, c.meta + g0, ng16 * 4u, &full_bar[st]);
-                } else if (staged) {
-                    tma_load_1d(sb + o_units, a.src.units + ua, staged * 4u, &full_bar[st]);
-                }
-            }
-        }
+    uint32_t local[7] = {0, 0, 0, 0, 0, 0, 0};
+    if (warp == kFGroups * kFTile / 32 + 1) {
+        ring.store_warp(c);
+    } else if (warp == kFGroups * kFTile / 32) {
+        ring.load_warp(c, a.src.units);
     } else {
         // ===================== consumers: thread gl of group cg owns group g0 + gl of its tiles =====================
-        const uint32_t cg = warp / (kCT / 32);
-        const uint32_t tid = threadIdx.x - cg * kCT;
+        const uint32_t cg = warp / (kFTile / 32);
+        const uint32_t tid = threadIdx.x % kFTile;
         const int bar_id = 1 + static_cast<int>(cg);
-        constexpr uint32_t R64 = kFRow64 / 8;
         uint32_t *s_run = s_run_all + cg * kFTile;
-        uint32_t it = 0;
-        // tile index and g_base words of this consumer group's NEXT tile are fetched during the current
-        // one (tile_gb[t] = the g_base words of the two unit blocks tile t starts in)
-        const uint32_t first_tile = blockIdx.x + cg * gridDim.x, tile_step = kNG * gridDim.x;
-        uint32_t nx_u0 = 0, nx_u1 = 0;
-        uint2 nx_gb = make_uint2(0u, 0u);
-        if (first_tile < n_tiles) {
-            nx_u0 = a.tile_off[first_tile];
-            nx_u1 = a.tile_off[first_tile + 1];
-            nx_gb = a.tile_gb[first_tile];
-        }
-        it = cg;
-        for (uint32_t tile = first_tile; tile < n_tiles; tile += tile_step, it += kNG) {
-
-            const int st = it % a.n_stages;
-            const uint32_t ph = (it / a.n_stages) & 1u;
-            const uint32_t g0 = tile * kFTile;
-            const uint32_t ng = a.n_groups - g0 < kFTile ? a.n_groups - g0 : kFTile;
-            const uint32_t u0 = nx_u0, u1 = nx_u1;
+        TileCursor t = ring.first(cg);
+        // the g_base words of this consumer group's NEXT tile are fetched during the current one
+        // (tile_gb[t] = the g_base words of the two unit blocks tile t starts in)
+        uint2 nx_gb = t.tile < ring.n_tiles ? a.tile_gb[t.tile] : make_uint2(0u, 0u);
+        for (; t.tile < ring.n_tiles; ring.next(t)) {
+            const uint32_t g0 = t.tile * kFTile;
+            const uint32_t ng = ring.groups_of(g0);
             const uint32_t gb0 = nx_gb.x, gb1 = nx_gb.y;
-            if (tile + tile_step < n_tiles) {
-                nx_u0 = a.tile_off[tile + tile_step];
-                nx_u1 = a.tile_off[tile + tile_step + 1];
-                nx_gb = a.tile_gb[tile + tile_step];
-            }
-            const uint32_t ua = u0 & ~3u;
-            const uint32_t lead = u0 - ua, cnt = u1 - ua;  // local unit positions [lead, cnt)
-            const uint32_t cnt4 = (cnt + 3u) & ~3u;
-            const uint32_t staged = u1 > u0 ? (cnt4 < a.unit_cap ? cnt4 : a.unit_cap) : 0u;
-            uint8_t *sb = smem + static_cast<size_t>(st) * stage_bytes;
-            TileRows t;
-            t.matched = reinterpret_cast<uint64_t *>(sb + o_matched);
-            t.next = reinterpret_cast<uint64_t *>(sb + o_next);
-            t.pc = reinterpret_cast<uint64_t *>(sb + o_pc);
-            t.committed = reinterpret_cast<uint64_t *>(sb + o_committed);
-            t.ts = reinterpret_cast<uint64_t *>(sb + o_ts);
-            t.li = reinterpret_cast<uint64_t *>(sb + o_li);
-            t.meta = reinterpret_cast<uint32_t *>(sb + o_meta);
-            t.flags = sb + o_flags;
-            const uint32_t *s_units = reinterpret_cast<const uint32_t *>(sb + o_units);
+            if (t.tile + ring.tile_step() < ring.n_tiles) nx_gb = a.tile_gb[t.tile + ring.tile_step()];
+            const uint32_t ua = t.u0 & ~3u;
+            const uint32_t lead = t.u0 - ua, cnt = t.u1 - ua;  // local unit positions [lead, cnt)
+            const uint32_t staged = ring.staged_units(t.u0, t.u1);
             const uint32_t *g_units = a.src.units + ua;
             const uint32_t blk0 = ua / RAFTGPU_COMPACT_BLOCK;
-            long long t0 = 0, t1 = 0, t2 = 0, t3 = 0, t4 = 0;
-            if (a.dbg && tid == 0) t0 = clock64();
-            wait_stage(&full_bar[st], &done_bar[st], ph);  // (k_tile.cuh: exact although this group skips phases)
-            if (a.dbg && tid == 0) t1 = clock64();
+            const TileRows s = ring.wait(t);
+            const uint32_t *s_units = s.units;
 
             // ---- 0: first run header of every group of the tile.  The g_base words of the (at most
             // two, unless the tile is crowded) unit blocks the tile spans were fetched before the wait.
@@ -335,7 +75,7 @@ __global__ void __launch_bounds__(kFTile *kNG + 64, 1) step_tile_compact_kernel(
             const bool active = gl < ng;
             const uint32_t g = g0 + gl;
             if constexpr (kOrdered) {
-                for (uint32_t p = lead + tid; p < cnt; p += kCT) {
+                for (uint32_t p = lead + tid; p < cnt; p += kFTile) {
                     const uint32_t u = p < staged ? s_units[p] : g_units[p];
                     const uint32_t kind = u & 3u;
                     if (kind == kCuEsc) {  // a side-table record: start pulling it towards L1 for the walk below
@@ -352,16 +92,13 @@ __global__ void __launch_bounds__(kFTile *kNG + 64, 1) step_tile_compact_kernel(
                     const uint32_t gt = group_of(p, hb) - g0;
                     if (gt < ng) atomicMin(&s_run[gt], p);
                 }
-                named_bar_sync(bar_id, kCT);
-                if (a.dbg && tid == 0) t2 = clock64();
+                named_bar_sync(bar_id, kFTile);
 
                 // ---- 1: the runs of group g, record by record (raft.rs:1663-1743)
                 uint32_t p = s_run[gl];
                 s_run[gl] = 0xffffffffu;  // ready for this consumer group's next tile
                 if (active && p != 0xffffffffu) {
-                    const uint32_t meta = t.meta[gl];
-                    const uint32_t present_mask = kSimple5 ? 0x1fu
-                                                           : (RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta));
+                    const uint32_t present_mask = kSimple5 ? 0x1fu : present_of(s.meta[gl]);
                     uint64_t base = 0;
                     while (p < cnt) {
                         const uint32_t u = p < staged ? s_units[p] : g_units[p];
@@ -395,7 +132,7 @@ __global__ void __launch_bounds__(kFTile *kNG + 64, 1) step_tile_compact_kernel(
                                     step = 2;
                                 }
                             }
-                            const bool fast = tile_fast_apply<kSimple5>(c, t, gl, g, slot, index, commit, is_local, is_reject, ext_hint,
+                            const bool fast = tile_fast_apply<kSimple5>(c, s, gl, g, slot, index, commit, is_local, is_reject, ext_hint,
                                                                         hint, present_mask, local, res);
                             if (!fast) {
                                 general = true;
@@ -425,15 +162,15 @@ __global__ void __launch_bounds__(kFTile *kNG + 64, 1) step_tile_compact_kernel(
                                 }
                             }
                         }
-                        if (general) res = tile_general_apply(c, rec, ext_hint, ext_snapshot, gl, hint, t, local);
-                        if (a.results) a.results[ua + p] = static_cast<uint8_t>(res);
+                        if (general) res = tile_general_apply(c, rec, ext_hint, ext_snapshot, gl, hint, s, local);
+                        if (a.r.results) a.r.results[ua + p] = static_cast<uint8_t>(res);
                         p += step;
                     }
                 }
             } else {
                 // ---- 1': one thread per unit; a record finds its run header `back` units behind it
                 uint32_t *s_touch = s_run;  // 2048 bits: (group, peer slot) cells seen in this tile
-                for (uint32_t k = lead + tid; k < cnt; k += kCT) {
+                for (uint32_t k = lead + tid; k < cnt; k += kFTile) {
                     const uint32_t u = k < staged ? s_units[k] : g_units[k];
                     const uint32_t kind = u & 3u;
                     if (kind == kCuHdrA || kind == kCuHdrB) continue;
@@ -487,79 +224,25 @@ __global__ void __launch_bounds__(kFTile *kNG + 64, 1) step_tile_compact_kernel(
                             if (dup) atomicAdd(a.dup_count, 1u);
                         }
                         if (!dup) {
-                            const uint32_t present_mask =
-                                kSimple5 ? 0x1fu
-                                         : (RAFTGPU_META_IN(t.meta[gt]) | RAFTGPU_META_OUT(t.meta[gt]) | RAFTGPU_META_LEARN(t.meta[gt]));
-                            general = !(fast_ok && tile_fast_apply<kSimple5>(c, t, gt, g0 + gt, slot, rec.index, rec.commit, is_local,
+                            const uint32_t present_mask = kSimple5 ? 0x1fu : present_of(s.meta[gt]);
+                            general = !(fast_ok && tile_fast_apply<kSimple5>(c, s, gt, g0 + gt, slot, rec.index, rec.commit, is_local,
                                                                              is_reject, ext_hint, hint, present_mask, local, res));
-                            if (general) res = tile_general_apply(c, rec, ext_hint, ext_snapshot, gt, hint, t, local);
+                            if (general) res = tile_general_apply(c, rec, ext_hint, ext_snapshot, gt, hint, s, local);
                         }
                     }
-                    if (a.results) a.results[ua + k] = static_cast<uint8_t>(res);
+                    if (a.r.results) a.r.results[ua + k] = static_cast<uint8_t>(res);
                 }
-                named_bar_sync(bar_id, kCT);
+                named_bar_sync(bar_id, kFTile);
                 if (a.dup_count && tid < kFTile / 4) s_touch[tid] = 0;  // clean for this consumer group's next tile
-                if (a.dbg && tid == 0) t2 = clock64();
             }
             __syncwarp();
-            if (a.dbg && tid == 0) t3 = clock64();
 
-            // ---- 2: Raft::maybe_commit for this thread's group (raft.rs:893-904)
-            {
-                bool advanced = false;
-                if (active) {
-                    const uint32_t meta = t.meta[gl];
-                    uint64_t v[kSlots];
-                    uint32_t r = 0;
-#pragma unroll
-                    for (int s2 = 0; s2 < kSlots; s2++) {
-                        v[s2] = 0;
-                        if ((hint >> s2) & 1u) {
-                            v[s2] = t.matched[r * R64 + gl];
-                            r++;
-                        }
-                    }
-                    uint64_t mci;
-                    bool use_gc;
-                    eval_mci<kSimple5>(c, g, meta, v, hint, mci, use_gc);
-                    advanced = mci > t.committed[gl] && mci >= t.ts[gl] && mci <= t.li[gl];  // raft_log.rs:488
-                    if (advanced) {
-                        t.committed[gl] = mci;  // (the store warp copies the row to commit_out too)
-                        if (meta & RAFTGPU_META_HAS_SELF) {  // raft.rs:896-900
-                            const uint32_t self = RAFTGPU_META_SELF(meta);
-                            uint64_t *pc = ((hint >> self) & 1u)
-                                               ? &t.pc[__popc(hint & ((1u << self) - 1u)) * R64 + gl]
-                                               : &c.peer_committed[static_cast<size_t>(self) * c.cap + g];
-                            if (mci > *pc) *pc = mci;
-                        }
-                    }
-                }
-                uint32_t lc[2] = {0, 0};
-                publish_tile(a.adv_bitmap, static_cast<uint64_t>(g0) + gl, lane, active, advanced, lc);
-                local[5] += lc[0];
-                local[6] += lc[1];
-            }
-
-            // ---- 3: hand the stage to the store warp
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            named_bar_sync(bar_id, kCT);
-            if (tid == 0) mbar_arrive(&done_bar[st]);
-            if (a.dbg && tid == 0) {
-                t4 = clock64();
-                atomicAdd(&a.dbg[0], static_cast<unsigned long long>(t1 - t0));  // waiting for the TMA loads
-                atomicAdd(&a.dbg[1], static_cast<unsigned long long>(t2 - t1));  // 0: run index
-                atomicAdd(&a.dbg[2], static_cast<unsigned long long>(t3 - t2));  // 1: records
-                atomicAdd(&a.dbg[3], static_cast<unsigned long long>(t4 - t3));  // 2 + 3: recompute, fence, barrier
-                atomicAdd(&a.dbg[4], 1ull);
-            }
+            // ---- 2: Raft::maybe_commit for this thread's group: its cells were written by this very thread (ordered)
+            // or are final after the barrier above; then the stage goes to the store warp
+            ring.finish(c, t, s, local);
         }
     }
-    const int which[7] = {kCntRecords, kCntUpdates, kCntRejects, kCntDecrements, kCntNoProgress, kCntRecomputes, kCntAdvanced};
-    block_flush_counts<7>(local, which, a.counters, nullptr);
-    if (a.step_advanced) {
-        const uint32_t w = __reduce_add_sync(0xffffffffu, local[6]);
-        if (lane == 0 && w) atomicAdd(a.step_advanced, w);
-    }
+    ring.flush(local);
 }
 
 // Tile index of a tileable compact stream, on the device (the zero-copy step has no host pass
