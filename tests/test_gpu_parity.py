@@ -12,7 +12,7 @@ import random
 import numpy as np
 import pytest
 
-from helpers import B, O, assert_columns_equal, bitmap_to_bool, checksum
+from helpers import B, O, assert_columns_equal, bitmap_to_bool, checksum, compact_bufs, compact_round, fused_round
 from oracle import datadriven as dd
 
 pytestmark = pytest.mark.gpu
@@ -606,31 +606,6 @@ def test_compact_stream_submission_vs_oracle(n, joint, shuffle):
     arena.close()
 
 
-def _fused_round(arena, n, recs, ref, pk, d_bufs):
-    """One fused step (raftgpu_step_sorted_device) on `recs` (group order) checked against the oracle."""
-    k = arena.pack_records(recs, pk)
-    off = B.tile_index(pk, k, n)
-    d_pk, d_off, d_res, d_bm, d_com = d_bufs
-    arena.h2d(d_pk, pk[:k])
-    arena.h2d(d_off, off)
-    arena.h2d(d_bm, np.zeros(arena.cap // 32, dtype=np.uint32))   # bits past n_groups are left untouched
-    arena.step_sorted_device(d_pk, k, d_off, d_results=d_res, d_adv=d_bm, d_commit=d_com)
-    res = np.zeros(k, dtype=np.uint8)
-    bm = np.zeros(arena.cap // 32, dtype=np.uint32)
-    arena.d2h(res, d_res)
-    arena.d2h(bm, d_bm)
-    want_res = O.arena_apply(ref, recs, mode=0)
-    want_adv, want_bm, _, _ = O.arena_recompute(ref)
-    main_pk = (pk[:k, 0] & np.uint64(1 << 37)) == 0           # packed records that are not EXT payloads
-    main_orig = (recs["flags"] & B.REC_EXT) == 0
-    assert np.array_equal(res[main_pk], want_res[main_orig]), "per-record results differ"
-    assert not res[~main_pk].any()
-    words = (n + 31) // 32
-    assert np.array_equal(bm[:words], want_bm[:words])
-    assert_columns_equal(arena.read_columns(n), ref, n, "fused step")
-    return want_adv
-
-
 @pytest.mark.parametrize("n,joint", [(100_003, False), (70_001, True), (1_000_000, False)])
 def test_fused_tile_step_vs_oracle(n, joint):
     """raftgpu_step_sorted_device: the fused apply + recompute kernel on group-ordered batches,
@@ -645,7 +620,7 @@ def test_fused_tile_step_vs_oracle(n, joint):
               arena.device_alloc(9 * n + 64), arena.device_alloc(arena.cap // 8), arena.device_alloc(8 * arena.cap))
     total = 0
     for _ in range(3 if n >= 1_000_000 else 6):
-        total += _fused_round(arena, n, synth.next_round().copy(), ref, pk, d_bufs)
+        total += fused_round(arena, n, synth.next_round().copy(), ref, pk, d_bufs)[0]
     assert total > n // 2
     cnt = arena.counters()
     assert cnt["recomputes"] % n == 0 and cnt["advanced"] == total
@@ -692,7 +667,7 @@ def test_fused_tile_step_learners_group_commit_and_crowded_tiles():
             recs = np.concatenate([recs, np.array(crowd, dtype=B.APPEND_RESP_DTYPE)])
         order = np.argsort(recs["group"], kind="stable")   # group order, arrival order kept inside a group
         recs = np.ascontiguousarray(recs[order])
-        adv = _fused_round(arena, n, recs, ref, pk, d_bufs)
+        fused_round(arena, n, recs, ref, pk, d_bufs)
     # a record filed under the wrong tile is not applied
     bad = np.zeros(2, dtype=B.APPEND_RESP_DTYPE)
     bad[0] = (10, 1, 0, 0, int(ref.matched[1, 10]) + 1, int(ref.matched[1, 10]))
@@ -777,49 +752,6 @@ def test_step_begin_records_vs_oracle(n, joint, mode):
     arena.close()
 
 
-def _compact_round(arena, n, recs, ref, blob, d_bufs, ordered=False):
-    """One fused compact step (raftgpu_step_compact_device) on `recs` (group order) vs the oracle."""
-    nb, units = B.pack_compact(recs, blob, want_units=True)
-    hdr = blob[:64].view(B.COMPACT_HDR_DTYPE)[0]
-    assert hdr["flags"] & B.COMPACT_TILEABLE
-    d_blob, d_off, d_res, d_bm, d_com, d_bad = d_bufs
-    nu = int(hdr["n_units"])
-    arena.h2d(d_blob, blob[:nb])
-    arena.h2d(d_bm, np.zeros(arena.cap // 32, dtype=np.uint32))
-    arena.h2d(d_res, np.zeros(max(nu, 1), dtype=np.uint8))
-    arena.h2d(d_bad, np.zeros(1, dtype=np.uint32))
-    arena.compact_tile_index_device(d_blob, blob, d_off, d_bad)
-    arena.step_compact_device(d_blob, blob, d_off, d_results=d_res, d_adv=d_bm, d_commit=d_com, d_dup=d_bad,
-                              ordered=ordered)
-    res = np.zeros(max(nu, 1), dtype=np.uint8)
-    bm = np.zeros(arena.cap // 32, dtype=np.uint32)
-    bad = np.zeros(1, dtype=np.uint32)
-    arena.d2h(res, d_res)
-    arena.d2h(bm, d_bm)
-    arena.d2h(bad, d_bad)
-    assert bad[0] == 0
-    want_res = O.arena_apply(ref, recs, mode=0)
-    want_adv, want_bm, _, _ = O.arena_recompute(ref)
-    main = (recs["flags"] & B.REC_EXT) == 0
-    assert np.array_equal(res[units[main]], want_res[main]), "per-record results differ"
-    other = np.ones(len(res), dtype=bool)
-    other[units[main]] = False
-    assert not res[other].any()
-    words = (n + 31) // 32
-    assert np.array_equal(bm[:words], want_bm[:words])
-    assert_columns_equal(arena.read_columns(n), ref, n, "fused compact step")
-    return want_adv
-
-
-def _compact_bufs(arena, n, per_group):
-    cap_b = B.compact_bound(per_group * n + 64)
-    blob = np.zeros(cap_b, dtype=np.uint8)
-    d = (arena.device_alloc(cap_b), arena.device_alloc(4 * (3 * (arena.cap // B.tile_groups() + 2) + 2)),
-         arena.device_alloc(3 * per_group * n + 64), arena.device_alloc(arena.cap // 8),
-         arena.device_alloc(8 * arena.cap), arena.device_alloc(4))
-    return blob, d
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("n,joint,ordered", [(100_003, False, False), (100_003, False, True), (70_001, True, False),
                                              (70_001, True, True), (1_000_000, False, False)])
@@ -832,10 +764,10 @@ def test_fused_compact_step_vs_oracle(n, joint, ordered):
     arena.group_alloc_range(n)
     arena.load_columns(synth.initial)
     ref = O.copy_columns(synth.initial)
-    blob, d_bufs = _compact_bufs(arena, n, 9)
+    blob, d_bufs = compact_bufs(arena, n, 9)
     total = 0
     for _ in range(3 if n >= 1_000_000 else 6):
-        total += _compact_round(arena, n, synth.next_round().copy(), ref, blob, d_bufs, ordered=ordered)
+        total += compact_round(arena, n, synth.next_round().copy(), ref, blob, d_bufs, ordered=ordered)[0]
     assert total > n // 2
     cnt = arena.counters()
     assert cnt["recomputes"] % n == 0 and cnt["advanced"] == total
@@ -865,7 +797,7 @@ def test_fused_compact_step_corner_cases():
     arena.group_alloc_range(n)
     arena.load_columns(cols)
     ref = O.copy_columns(cols)
-    blob, d_bufs = _compact_bufs(arena, n, 40)
+    blob, d_bufs = compact_bufs(arena, n, 40)
     tg = B.tile_groups()
     for rnd in range(4):
         base = synth.next_round().copy()
@@ -889,13 +821,13 @@ def test_fused_compact_step_corner_cases():
             recs = recs[(recs["group"] % 700) < 3]
         # group order; inside a group arrival order, with each EXT right behind its REJECT
         order = np.argsort(recs["group"], kind="stable")
-        _compact_round(arena, n, np.ascontiguousarray(recs[order]), ref, blob, d_bufs)
+        compact_round(arena, n, np.ascontiguousarray(recs[order]), ref, blob, d_bufs)
         if rnd == 1:   # the crowded tile spans more units than a stage holds (1536): the kernel read the rest from HBM
             off = np.zeros((n + tg - 1) // tg + 1, dtype=np.uint32)
             arena.d2h(off, d_bufs[1])
             assert (off[1:].astype(np.int64) - (off[:-1] & ~np.uint32(3))).max() > 1536
     # empty stream
-    _compact_round(arena, n, np.zeros(0, dtype=B.APPEND_RESP_DTYPE), ref, blob, d_bufs)
+    compact_round(arena, n, np.zeros(0, dtype=B.APPEND_RESP_DTYPE), ref, blob, d_bufs)
     # a stream that claims ONE_WAVE but holds two records for one cell: the per-unit kernel applies
     # the first it sees, refuses the other and counts it
     dup = np.zeros(2, dtype=B.APPEND_RESP_DTYPE)
@@ -1003,7 +935,7 @@ def test_every_ingest_path_agrees_with_the_oracle_on_random_states(seed):
     pk = np.zeros((40 * n, 2), dtype=np.uint64)
     f16 = arenas["fused16"]
     d16 = (f16.device_alloc(pk.nbytes), f16.device_alloc(4 * (n // B.tile_groups() + 2)))
-    blob, dc = _compact_bufs(arenas["fusedc"], n, 40)
+    blob, dc = compact_bufs(arenas["fusedc"], n, 40)
     for rnd in range(5):
         per_cell = 3 if rnd >= 3 else 1          # the last rounds: several records per (group, peer)
         recs = _random_batch(ref, n, rng, per_cell)
