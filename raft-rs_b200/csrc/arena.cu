@@ -18,6 +18,7 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -81,8 +82,6 @@ struct StagingSet {
     uint8_t *d_wire = nullptr;   // also the device copy of a RAFTGPU_STEP_RAW batch
     uint64_t d_wire_cap = 0;
     uint64_t wire_n = 0;             // frames of the wire step this set carried (0 = not a wire step)
-    uint64_t raw_n = 0;              // RAFTGPU_STEP_HYBRID: 24-byte records of this step that sit in d_wire as they are
-    uint32_t raw_min_group = 0;      // ... all of groups >= this one (the packed part ends below it)
     // sync
     cudaEvent_t ev_h2d = nullptr, ev_compute = nullptr, ev_done = nullptr;
     cudaEvent_t ev_raw0 = nullptr, ev_raw1 = nullptr;  // around the hybrid step's raw H2D copy (timing: the effective PCIe rate)
@@ -112,6 +111,8 @@ struct RecJob {
     std::chrono::steady_clock::time_point t_begin;
     std::vector<double> tr_a, tr_b;
     std::atomic<uint64_t> busy_ns{0};  // time the staging threads spent packing this job's slices (for the hybrid split)
+    uint64_t raw_n = 0;                // RAFTGPU_STEP_HYBRID: records of the batch that sit in the set's d_wire as they are
+    uint32_t raw_min_group = 0;        // ... all of groups >= this one (the packed part ends below it)
     double us_since() const { return std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t_begin).count(); }
 };
 
@@ -224,7 +225,6 @@ struct raftgpu_arena {
     uint32_t hyb_samples = 0;
     double hyb_pcie_gbs = 0.0;               // RAFTGPU_STEP_HYBRID: measured rate of the raw H2D copies (GB/s), 0 = not measured yet
     double hyb_pack_ns = 0.0;                // RAFTGPU_STEP_HYBRID: measured packing cost (ns per record and staging thread), 0 = not measured yet
-    bool rec_fallback_sorted = false;        // raftgpu_step_begin_records: the batch going to the general staging path is in group order
     uint32_t n_wide = 0;                     // wide groups (two slots each): the fused tile kernels are not used while any exist
     uint32_t n_simple5 = 0;                  // groups whose meta is the plain 5-voter configuration
     bool force_general = false;              // RAFTGPU_FORCE_GENERAL=1: never take the simple5 kernels
@@ -372,6 +372,10 @@ inline double trace_us(const raftgpu_arena *a) {
 
 inline bool group_ok(const raftgpu_arena *a, uint32_t g) { return g < a->cap && a->allocated[g]; }
 
+// PackedRec slots of a staging set's device record buffer (d_recs): wave 0 + the later waves.  Between steps the
+// buffer also stages the other forms' batches and the host calls' (host_batch_op, raftgpu_step_send_list).
+inline uint64_t rec_slots(const raftgpu_arena *a) { return static_cast<uint64_t>(a->n_chunks) * kChunk + a->overflow_records; }
+
 inline uint32_t present_mask(uint32_t meta) {
     return RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta);
 }
@@ -473,6 +477,39 @@ int32_t launch_apply(raftgpu_arena *a, cudaStream_t st, const void *d_recs, uint
     else
         apply_kernel<false><<<blocks, 256, 0, st>>>(a->cols, d_recs, n, d_results, a->d_counters);
     CKL(a);
+    return RAFTGPU_OK;
+}
+
+// The verified one-wave scatter apply of a batch no host code has looked at: a second record of a cell, or a record of
+// a group below min_group, is refused and counted in d_step_adv[1].  Src: const raftgpu_append_resp *, const PackedRec *
+// or CompactSrc (n = its units).  clear = false: the second part of a wave whose first part has marked d_touched.
+template <typename Src>
+int32_t launch_verified_apply(raftgpu_arena *a, StagingSet &s, Src src, uint64_t n, uint8_t *d_results,
+                              uint32_t min_group = 0, bool clear = true) {
+    using Rec = std::remove_cv_t<std::remove_pointer_t<Src>>;
+    if (n == 0) return RAFTGPU_OK;
+    if (clear) CK(a, cudaMemsetAsync(s.d_touched, 0, a->cap, a->s_compute));
+    const uint32_t blocks = std::min<uint32_t>(div_up(n, 256), static_cast<uint32_t>(a->grid_apply));
+    if constexpr (std::is_same_v<Src, CompactSrc>)
+        apply_compact_kernel<true><<<blocks, 256, 0, a->s_compute>>>(a->cols, src, d_results, a->d_counters, s.d_touched,
+                                                                    s.d_step_adv + 1);
+    else
+        apply_kernel<std::is_same_v<Rec, PackedRec>, true><<<blocks, 256, 0, a->s_compute>>>(
+            a->cols, src, n, d_results, a->d_counters, s.d_touched, s.d_step_adv + 1, min_group);
+    CKL(a);
+    return RAFTGPU_OK;
+}
+
+// d_wire holds at least `need` bytes (+ a quarter: a batch that grows slowly is not reallocated on every step)
+int32_t grow_wire(raftgpu_arena *a, StagingSet &s, uint64_t need) {
+    if (s.d_wire_cap >= need) return RAFTGPU_OK;
+    CK(a, cudaStreamSynchronize(a->s_compute));  // nothing may still read the old buffer
+    CK(a, cudaFree(s.d_wire));
+    s.d_wire = nullptr;
+    s.d_wire_cap = 0;
+    const int32_t rc = dev_alloc(a, &s.d_wire, need + need / 4, false);
+    if (rc != RAFTGPU_OK) return rc;
+    s.d_wire_cap = need + need / 4;
     return RAFTGPU_OK;
 }
 
@@ -633,7 +670,7 @@ int32_t create(int32_t device, uint32_t max_groups, uint32_t slots, uint32_t n_r
     TRY(pin_alloc(a, reinterpret_cast<uint8_t **>(&a->h_scratch), 256));
 
     const uint64_t wave0_total = static_cast<uint64_t>(a->n_chunks) * kChunk;
-    const uint64_t rec_total = wave0_total + a->overflow_records;
+    const uint64_t rec_total = rec_slots(a);
     LocalCpuGuard numa_guard(device);  // pinned pages on the GPU-local NUMA node
     CPU_ZERO(&a->local_cpus);
     if (numa_guard.active) {
@@ -742,6 +779,7 @@ int32_t reclaim_set(raftgpu_arena *a, StagingSet &s) {
     s.wire_n = 0;
     s.overflow_depth.clear();
     s.overflow_waves.clear();
+    s.overflow_order.clear();  // (raftgpu_step_record_results: only a step with later waves has any)
     return RAFTGPU_OK;
 }
 
@@ -760,7 +798,7 @@ int32_t host_batch_op(raftgpu_arena *a, const T *in, uint64_t n, uint8_t *result
     wait_submitter(a);
     StagingSet &s = a->sets[a->fill];
     if (s.in_flight || s.next_chunk.load() != 0) return fail(a, RAFTGPU_ERR_BUSY, "records are staged for a step: step first");
-    const uint64_t room = (static_cast<uint64_t>(a->n_chunks) * kChunk + a->overflow_records) * sizeof(PackedRec);
+    const uint64_t room = rec_slots(a) * sizeof(PackedRec);
     if (n * sizeof(T) > room || n > 4 * (room / sizeof(PackedRec))) return fail(a, RAFTGPU_ERR_FULL, "batch larger than the staging buffer");
     CK(a, cudaSetDevice(a->device));
     CK(a, cudaMemcpyAsync(s.d_recs, in, n * sizeof(T), cudaMemcpyHostToDevice, a->s_compute));
@@ -772,6 +810,116 @@ int32_t host_batch_op(raftgpu_arena *a, const T *in, uint64_t n, uint8_t *result
     CK(a, cudaStreamSynchronize(a->s_compute));
     if (out_dups) *out_dups = s.h_step_adv[1];
     return RAFTGPU_OK;
+}
+
+// ---- the step frame: every raftgpu_step_begin* form is step_admit -> the form's own function, which queues its H2D
+// copies on s_h2d and its apply kernels on s_compute and says what it queued (StepWork) -> step_finish -> step_book.
+
+// What a form queued, for the rest of the step and its raftgpu_step_result.
+struct StepWork {
+    uint64_t res_bytes = 0;    // result / status bytes to copy back from d_results
+    uint64_t wave0_slots = 0;  // result slots of wave 0 (raftgpu_step_slot_results)
+    uint64_t n_records = 0;
+    uint64_t h2d_bytes = 0;
+    uint32_t later_waves = 0;  // waves after wave 0 (a later wave needs a record of its cell in wave 0)
+    bool fused = false;        // the fused tile kernel has applied AND recomputed
+};
+
+// RAFTGPU_SYNC_DEBUG (diagnostics, read once per process): wait for every stage of a step and name it
+bool sync_debug() {
+    static const bool on = getenv("RAFTGPU_SYNC_DEBUG") != nullptr;
+    return on;
+}
+void stage_done(raftgpu_arena *a, const char *what) {
+    if (!sync_debug()) return;
+    const cudaError_t e = cudaStreamSynchronize(a->s_compute);
+    fprintf(stderr, "[raftgpu] @%.0f   stage done: %s (%s)\n", trace_us(a), what, cudaGetErrorString(e));
+}
+
+// What every form checks before it touches the fill set (*out).  `form` names a form that brings its own batch, which
+// cannot go with records enqueued for the step; nullptr: raftgpu_step_begin, which submits them.
+int32_t step_admit(raftgpu_arena *a, const char *form, StagingSet **out) {
+    wait_submitter(a);
+    if (a->n_inflight >= 2) return fail(a, RAFTGPU_ERR_BUSY, "two steps already in flight: call raftgpu_step_wait");
+    StagingSet &s = a->sets[a->fill];
+    if (s.in_flight) return RAFTGPU_ERR_BUSY;
+    if (form && (s.next_chunk.load() != 0 || !s.overflow_waves.empty()))
+        return fail(a, RAFTGPU_ERR_INVALID, std::string("records were enqueued for this step: cannot mix with ") + form);
+    CK(a, cudaSetDevice(a->device));
+    *out = &s;
+    return RAFTGPU_OK;
+}
+
+// The step's H2D copies are queued: its kernels start behind them, with d_step_adv cleared.
+int32_t compute_after_h2d(raftgpu_arena *a, StagingSet &s) {
+    CK(a, cudaEventRecord(s.ev_h2d, a->s_h2d));
+    CK(a, cudaStreamWaitEvent(a->s_compute, s.ev_h2d, 0));
+    CK(a, cudaMemsetAsync(s.d_step_adv, 0, 8, a->s_compute));
+    stage_done(a, "h2d");
+    return RAFTGPU_OK;
+}
+
+// The end of every step: recompute [0, hi) unless the fused kernel has, the D2H, the events, the set's result.  No
+// booking: the caller thread books a step (step_book), an asynchronous one before the submitter thread queues it.
+int32_t step_finish(raftgpu_arena *a, StagingSet &s, uint32_t flags, const StepWork &w) {
+    const uint32_t hi = a->hi;
+    uint64_t *d_commit = (flags & RAFTGPU_STEP_READ_COMMITTED) ? s.d_commit_out : nullptr;
+    if (!w.fused) {
+        const int32_t rc = launch_recompute(a, a->s_compute, 0, hi, a->voter_hint, s.d_adv_bitmap, d_commit, nullptr, nullptr,
+                                            s.d_step_adv);
+        if (rc != RAFTGPU_OK) return rc;
+    }
+    CK(a, cudaEventRecord(s.ev_compute, a->s_compute));
+    CK(a, cudaStreamWaitEvent(a->s_d2h, s.ev_compute, 0));
+    CK(a, cudaMemcpyAsync(s.h_step_adv, s.d_step_adv, 8, cudaMemcpyDeviceToHost, a->s_d2h));
+    if (hi)
+        CK(a, cudaMemcpyAsync(s.h_adv_bitmap, s.d_adv_bitmap, 4ull * ((hi + 31) / 32),
+                              cudaMemcpyDeviceToHost, a->s_d2h));
+    if (d_commit && hi)
+        CK(a, cudaMemcpyAsync(s.h_committed, s.d_commit_out, 8ull * hi, cudaMemcpyDeviceToHost, a->s_d2h));
+    if (w.res_bytes)
+        CK(a, cudaMemcpyAsync(s.h_results, s.d_results, w.res_bytes, cudaMemcpyDeviceToHost, a->s_d2h));
+    CK(a, cudaEventRecord(s.ev_done, a->s_d2h));
+    s.flags = flags;
+    s.wave0_slots = w.wave0_slots;
+    s.result.n_records = w.n_records;
+    s.result.h2d_bytes = w.h2d_bytes;
+    s.result.d2h_bytes = 8 + (hi ? 4ull * ((hi + 31) / 32) : 0) + ((d_commit && hi) ? 8ull * hi : 0) + w.res_bytes;
+    s.result.n_waves = (w.n_records ? 1 : 0) + w.later_waves;
+    s.result.n_groups = hi;
+    return RAFTGPU_OK;
+}
+
+// The fill set is now in flight (caller thread only): pick the next one to fill.
+int32_t step_book(raftgpu_arena *a) {
+    StagingSet &s = a->sets[a->fill];
+    s.in_flight = true;
+    a->inflight[a->n_inflight++] = a->fill;
+    // flip: a set that is neither in flight nor holding the results of the last completed step
+    // becomes the fill target (with 3 sets and <= 2 in flight there is always one)
+    int other = -1;
+    for (int k = 0; k < kNumSets; k++) {
+        if (a->sets[k].in_flight) continue;
+        if (k == a->last_done && other >= 0) continue;  // prefer keeping the last results alive
+        if (other < 0 || k != a->last_done) other = k;
+    }
+    if (other < 0) return fail(a, RAFTGPU_ERR_BUSY, "no free staging set");
+    const int32_t rc = reclaim_set(a, a->sets[other]);
+    if (rc != RAFTGPU_OK) return rc;
+    if (a->last_done == other) a->last_done = -1;  // its results are gone
+    a->fill = other;
+    return RAFTGPU_OK;
+}
+
+// One synchronous step: admission, the form's queue(StagingSet &, StepWork &), the finish, the booking.
+template <typename Queue>
+int32_t run_step(raftgpu_arena *a, const char *form, uint32_t flags, Queue &&queue) {
+    StagingSet *s = nullptr;
+    StepWork w;
+    int32_t rc = step_admit(a, form, &s);
+    if (rc == RAFTGPU_OK) rc = queue(*s, w);
+    if (rc == RAFTGPU_OK) rc = step_finish(a, *s, flags, w);
+    return rc == RAFTGPU_OK ? step_book(a) : rc;
 }
 
 }  // namespace
