@@ -550,6 +550,8 @@ void destroy(raftgpu_arena *a) {
     cudaDeviceSynchronize();
     Columns &c = a->cols;
     cudaFree(c.matched);
+    cudaFree(c.next_d);
+    cudaFree(c.pc_d);
     cudaFree(c.next_idx);
     cudaFree(c.peer_committed);
     cudaFree(c.pending_snapshot);
@@ -652,6 +654,8 @@ int32_t create(int32_t device, uint32_t max_groups, uint32_t slots, uint32_t n_r
     Columns &c = a->cols;
     c.cap = a->cap;
     TRY(dev_alloc(a, &c.matched, cells));
+    TRY(dev_alloc(a, &c.next_d, cells));  // zero offsets: next_idx = peer_committed = matched = 0
+    TRY(dev_alloc(a, &c.pc_d, cells));
     TRY(dev_alloc(a, &c.next_idx, cells));
     TRY(dev_alloc(a, &c.peer_committed, cells));
     TRY(dev_alloc(a, &c.pending_snapshot, cells));
@@ -747,6 +751,21 @@ bool column_desc(raftgpu_arena *a, int32_t col, ColumnDesc *d) {
         return true;
     default: return false;
     }
+}
+
+// next_idx and peer_committed are offsets from matched on the device (k_common.cuh), so their column IO goes through
+// the u64 escape columns: decode = materialize the values of cells [slot * cap + first, + n) there, encode = turn the
+// values there into offsets.  `column` is RAFTGPU_COL_NEXT_IDX, _PEER_COMMITTED, or _MATCHED for both.
+int32_t offset_column_io(raftgpu_arena *a, int32_t column, uint32_t slot, uint32_t first, uint32_t n, bool encode) {
+    Columns &c = a->cols;
+    const size_t cell0 = static_cast<size_t>(slot) * a->cap + first;
+    const int grid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(8ull * a->sm_count, (n + 255u) / 256u)));
+    if (column != RAFTGPU_COL_PEER_COMMITTED)
+        offset_column_kernel<<<grid, 256, 0, a->s_compute>>>(c.matched, c.next_d, c.next_idx, cell0, n, encode);
+    if (column != RAFTGPU_COL_NEXT_IDX)
+        offset_column_kernel<<<grid, 256, 0, a->s_compute>>>(c.matched, c.pc_d, c.peer_committed, cell0, n, encode);
+    CKL(a);
+    return RAFTGPU_OK;
 }
 
 // Move a duplicate-cell record (already packed) to a later wave.

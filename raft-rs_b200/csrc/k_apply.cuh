@@ -33,8 +33,8 @@ __device__ __forceinline__ void reset_state(const Columns &c, size_t cell, Cell 
 // so every load has a whole iteration to land.  (An extra L2-prefetch stage does not help: with
 // this many loads in flight the kernel is limited by the DRAM efficiency of sector-granular
 // scattered accesses, not by latency.)
-// Algorithmic bytes per record: 24 (record) + RMW of matched, next_idx,
-// committed_index (48) + flag byte and meta (~4) = 76.
+// Algorithmic bytes per record: 24 (record) + RMW of matched (16) and of the next_idx and
+// committed_index offsets (16) + flag byte and meta (~4) = 60.
 struct RecRegs {
     uint64_t w0, index, commit;
 };
@@ -44,9 +44,10 @@ struct CellRegs {
     uint64_t matched, next_idx, peer_committed;
 };
 // Where one cell's hot fields live: HBM (scatter kernel) or a shared-memory tile (fused kernel).
-// The cold columns (pending_snapshot, pending_request_snapshot) are always addressed in HBM.
+// The cold columns (pending_snapshot, pending_request_snapshot) and the offset escapes are always addressed in HBM.
 struct CellPtrs {
-    uint64_t *matched, *next_idx, *peer_committed, *last_index;
+    HotPtrs hot;
+    uint64_t *last_index;
     uint8_t *pflags;
 };
 
@@ -120,8 +121,7 @@ __device__ __forceinline__ CellPtrs global_cell_ptrs(const Columns &c, const Rec
     const uint32_t slot = static_cast<uint32_t>(r.w0 >> 32) & 0xffu;
     const bool ok = g < c.cap && slot < kSlots;
     const size_t cell = ok ? static_cast<size_t>(slot) * c.cap + g : 0;
-    return CellPtrs{c.matched + cell, c.next_idx + cell, c.peer_committed + cell, c.last_index + (ok ? g : 0),
-                    c.pflags + cell};
+    return CellPtrs{hot_ptrs(c, cell), c.last_index + (ok ? g : 0), c.pflags + cell};
 }
 
 __device__ __forceinline__ CellRegs load_cell(const Columns &c, const RecRegs &r) {
@@ -133,10 +133,11 @@ __device__ __forceinline__ CellRegs load_cell(const Columns &c, const RecRegs &r
     const size_t cell = ok ? static_cast<size_t>(slot) * c.cap + g : 0;
     CellRegs d;
     d.meta = c.meta[ok ? g : 0];
-    d.matched = c.matched[cell];
-    d.next_idx = c.next_idx[cell];
+    const HotVals h = hot_load(c, hot_ptrs(c, cell));
+    d.matched = h.matched;
+    d.next_idx = h.next_idx;
     d.flags = c.pflags[cell];
-    d.peer_committed = c.peer_committed[cell];
+    d.peer_committed = h.peer_committed;
     return d;
 }
 
@@ -168,6 +169,7 @@ __device__ __forceinline__ uint32_t apply_one(const Columns &c, const void *recs
     pr.matched = cd.matched;
     pr.next_idx = cd.next_idx;
     pr.flags = cd.flags;
+    uint64_t peer_committed = cd.peer_committed;
     const uint32_t state = pr.flags & RAFTGPU_PF_STATE_MASK;
     uint32_t res = 0;
 
@@ -185,7 +187,7 @@ __device__ __forceinline__ uint32_t apply_one(const Columns &c, const void *recs
     } else {
         pr.flags |= RAFTGPU_PF_RECENT_ACTIVE;  // raft.rs:1674
         // raft.rs:1677 pr.update_committed(m.commit), progress.rs:153-157
-        if (commit > cd.peer_committed) *ptr.peer_committed = commit;
+        if (commit > cd.peer_committed) peer_committed = commit;
 
         if (rflags & RAFTGPU_REC_REJECT) {
             local[2]++;
@@ -263,8 +265,7 @@ __device__ __forceinline__ uint32_t apply_one(const Columns &c, const void *recs
             }
         }
     }
-    if (pr.matched != cd.matched) *ptr.matched = pr.matched;
-    if (pr.next_idx != cd.next_idx) *ptr.next_idx = pr.next_idx;
+    hot_write(c, ptr.hot, HotVals{cd.matched, cd.next_idx, cd.peer_committed}, HotVals{pr.matched, pr.next_idx, peer_committed});
     if (pr.flags != cd.flags) *ptr.pflags = static_cast<uint8_t>(pr.flags);
     return res;
 }

@@ -7,6 +7,10 @@ constexpr int kSlots = RAFTGPU_SLOTS;
 struct Columns {
     uint32_t cap;
     uint64_t *matched;
+    // next_idx and peer_committed of a cell are stored as offsets from its matched (next_d, pc_d; off_* below); the
+    // u64 columns hold the exact value of the cells whose offset is kOffEscape and are not read for any other cell
+    int32_t *next_d;
+    int32_t *pc_d;
     uint64_t *next_idx;
     uint64_t *peer_committed;
     uint64_t *pending_snapshot;
@@ -47,6 +51,96 @@ __device__ __forceinline__ void prefetch_l2(const void *p) {
 
 __device__ __forceinline__ uint64_t umin64(uint64_t a, uint64_t b) { return a < b ? a : b; }
 __device__ __forceinline__ uint64_t umax64(uint64_t a, uint64_t b) { return a > b ? a : b; }
+
+// ---------------------------------------------------------------------------
+// The offset codec of next_idx and peer_committed.  In a live group both sit within the inflight window of the same
+// cell's matched, so each is stored as a signed 32-bit offset from it (next_d, pc_d): a fused step then moves 8 bytes
+// per cell for the two instead of 16.  A value the offset cannot express (a peer right after Raft::reset, whose
+// matched is 0) is stored as kOffEscape, with the exact value in the u64 column.  The format is lossless for every
+// u64 value.  Offsets are relative to matched, so every write of matched re-encodes both offsets of its cell
+// (hot_write); nothing outside this section does the arithmetic.
+constexpr int32_t kOffEscape = INT32_MIN;
+
+__device__ __forceinline__ bool off_escaped(int32_t d) { return d == kOffEscape; }
+// the value of an offset that is not kOffEscape
+__device__ __forceinline__ uint64_t off_value(int32_t d, uint64_t matched) {
+    return matched + static_cast<uint64_t>(static_cast<int64_t>(d));
+}
+__device__ __forceinline__ uint64_t off_decode(int32_t d, uint64_t matched, const uint64_t *esc) {
+    return off_escaped(d) ? *esc : off_value(d, matched);
+}
+// the offset to store for value v; a value that does not fit goes to *esc (a plain store, no read)
+__device__ __forceinline__ int32_t off_encode(uint64_t v, uint64_t matched, uint64_t *esc) {
+    const int64_t d = static_cast<int64_t>(v - matched);
+    if (d > static_cast<int64_t>(kOffEscape) && d <= static_cast<int64_t>(INT32_MAX)) return static_cast<int32_t>(d);
+    *esc = v;
+    return kOffEscape;
+}
+
+// Where one cell's matched and offsets live -- HBM, or a fused kernel's shared-memory rows -- and its index in the
+// arena, which addresses its escape slots (always in HBM).
+struct HotPtrs {
+    uint64_t *matched;
+    int32_t *next_d, *pc_d;
+    size_t cell;
+};
+struct HotVals {
+    uint64_t matched, next_idx, peer_committed;
+};
+__device__ __forceinline__ HotPtrs hot_ptrs(const Columns &c, size_t cell) {
+    return HotPtrs{c.matched + cell, c.next_d + cell, c.pc_d + cell, cell};
+}
+__device__ __forceinline__ HotVals hot_load(const Columns &c, const HotPtrs &p) {
+    HotVals h;
+    h.matched = *p.matched;
+    h.next_idx = off_decode(*p.next_d, h.matched, c.next_idx + p.cell);
+    h.peer_committed = off_decode(*p.pc_d, h.matched, c.peer_committed + p.cell);
+    return h;
+}
+// The cell's new values over its old ones: writes what changed, and both offsets when matched changed.
+__device__ __forceinline__ void hot_write(const Columns &c, const HotPtrs &p, const HotVals &old, const HotVals &v) {
+    const bool m_new = v.matched != old.matched;
+    if (m_new) *p.matched = v.matched;
+    if (m_new || v.next_idx != old.next_idx) *p.next_d = off_encode(v.next_idx, v.matched, c.next_idx + p.cell);
+    if (m_new || v.peer_committed != old.peer_committed)
+        *p.pc_d = off_encode(v.peer_committed, v.matched, c.peer_committed + p.cell);
+}
+// The same from the cell's stored form (matched and the two offsets as loaded): writes what differs.
+__device__ __forceinline__ void hot_write_over(const Columns &c, const HotPtrs &p, uint64_t old_matched, int32_t old_next_d,
+                                               int32_t old_pc_d, const HotVals &v) {
+    if (v.matched != old_matched) *p.matched = v.matched;
+    const int32_t nd = off_encode(v.next_idx, v.matched, c.next_idx + p.cell);
+    if (nd != old_next_d) *p.next_d = nd;
+    const int32_t pd = off_encode(v.peer_committed, v.matched, c.peer_committed + p.cell);
+    if (pd != old_pc_d) *p.pc_d = pd;
+}
+__device__ __forceinline__ void hot_store(const Columns &c, const HotPtrs &p, const HotVals &v) {
+    *p.matched = v.matched;
+    *p.next_d = off_encode(v.next_idx, v.matched, c.next_idx + p.cell);
+    *p.pc_d = off_encode(v.peer_committed, v.matched, c.peer_committed + p.cell);
+}
+__device__ __forceinline__ void hot_set_next(const Columns &c, const HotPtrs &p, uint64_t next_idx) {
+    *p.next_d = off_encode(next_idx, *p.matched, c.next_idx + p.cell);
+}
+// Progress::update_committed (progress.rs:153-157)
+__device__ __forceinline__ void hot_update_committed(const Columns &c, const HotPtrs &p, uint64_t committed) {
+    const uint64_t m = *p.matched;
+    if (committed > off_decode(*p.pc_d, m, c.peer_committed + p.cell))
+        *p.pc_d = off_encode(committed, m, c.peer_committed + p.cell);
+}
+// Column IO of an offset column (raftgpu_column_read / _write): materialize the decoded values of cells [first,
+// first + n) in their u64 column, or encode the values the host has put there.
+__global__ void offset_column_kernel(const uint64_t *__restrict__ matched, int32_t *__restrict__ d,
+                                     uint64_t *__restrict__ esc, size_t first, uint32_t n, bool encode) {
+    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const size_t cell = first + i;
+        if (encode)
+            d[cell] = off_encode(esc[cell], matched[cell], &esc[cell]);
+        else
+            esc[cell] = off_decode(d[cell], matched[cell], &esc[cell]);
+    }
+}
 
 // ---------------------------------------------------------------------------
 // Inflights (src/tracker/inflights.rs) of one cell, when the arena keeps the windows on the device.  The flag bit

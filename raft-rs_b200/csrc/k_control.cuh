@@ -7,8 +7,8 @@
 // a selected group contributes one entry per present peer other than itself that is not paused
 // (progress.rs:210-216).  Lanes count their entries, a warp scan turns the counts into offsets, ONE
 // global atomic per warp reserves the range, each lane writes its 16-byte entries.
-// Algorithmic bytes: 4 per 32 groups (bitmap) + per advanced group 4 (meta) + K x 17 (pflags,
-// next_idx, pending_request_snapshot of its peers) read, 16 written per entry.
+// Algorithmic bytes: 4 per 32 groups (bitmap) + per advanced group 4 (meta) + K x 25 (pflags,
+// matched and the next_idx offset, pending_request_snapshot of its peers) read, 16 written per entry.
 __global__ void __launch_bounds__(256)
 send_list_kernel(Columns c, uint32_t first, uint32_t n, const uint32_t *__restrict__ adv_bitmap,
                  raftgpu_send_entry *__restrict__ out, unsigned long long capacity, unsigned long long *__restrict__ count,
@@ -41,7 +41,7 @@ send_list_kernel(Columns c, uint32_t first, uint32_t n, const uint32_t *__restri
                 if ((peers >> s) & 1u) {
                     const size_t cell = static_cast<size_t>(s) * c.cap + g;
                     f[s] = c.pflags[cell];
-                    nx[s] = c.next_idx[cell];
+                    nx[s] = hot_load(c, hot_ptrs(c, cell)).next_idx;
                     prs[s] = c.pending_req_snapshot[cell];
                 }
             }
@@ -139,7 +139,7 @@ heartbeat_resp_kernel(Columns c, const raftgpu_append_resp *__restrict__ recs, u
                         else if (f0 & RAFTGPU_PF_INS_FULL)
                             ins_free_first_one(c, cell, f);
                     }
-                    if (commit > c.peer_committed[cell]) c.peer_committed[cell] = commit;      // :1791
+                    hot_update_committed(c, hot_ptrs(c, cell), commit);                          // :1791
                     if (f != f0) c.pflags[cell] = static_cast<uint8_t>(f);
                     res = RAFTGPU_RES_OK;
                     if (c.matched[cell] < c.last_index[g] || c.pending_req_snapshot[cell] != RAFTGPU_INVALID_INDEX)
@@ -180,7 +180,7 @@ update_state_kernel(Columns c, const raftgpu_send_entry *__restrict__ e, uint64_
                 if (c.ins_cap && !ins_add(c, cell, last, f)) {
                     res = 0xffu;                                                  // ins.add on a full window panics
                 } else {
-                    c.next_idx[cell] = last + 1;                                  // :233-236 optimistic_update
+                    hot_set_next(c, hot_ptrs(c, cell), last + 1);                    // :233-236 optimistic_update
                     if (f != f0) c.pflags[cell] = static_cast<uint8_t>(f);
                 }
             } else if (state == RAFTGPU_STATE_PROBE)
@@ -261,9 +261,7 @@ __global__ void conf_kernel(Columns c, uint32_t g, uint32_t new_meta, uint32_t a
         const size_t cell = static_cast<size_t>(s) * c.cap + g;
         if (((added | removed) >> s) & 1u) {
             const bool add = (added >> s) & 1u;
-            c.matched[cell] = 0;
-            c.next_idx[cell] = add ? next_idx : 0;  // Progress::new(next_idx, ..), progress.rs:60-73
-            c.peer_committed[cell] = 0;
+            hot_store(c, hot_ptrs(c, cell), HotVals{0, add ? next_idx : 0, 0});  // Progress::new(next_idx, ..), progress.rs:60-73
             c.pending_snapshot[cell] = 0;
             c.pending_req_snapshot[cell] = 0;
             c.commit_group_id[cell] = 0;
@@ -283,18 +281,21 @@ __global__ void reset_kernel(Columns c, uint32_t g, uint64_t term_start, uint64_
     for (int s = 0; s < kSlots; s++) {
         if (!((present >> s) & 1u)) continue;
         const size_t cell = static_cast<size_t>(s) * c.cap + g;
-        // Progress::reset(last_index + 1), progress.rs:82-92
-        c.matched[cell] = 0;
-        c.next_idx[cell] = last_index + 1;
+        // Progress::reset(last_index + 1), progress.rs:82-92 (peer_committed is kept)
+        const HotPtrs hp = hot_ptrs(c, cell);
+        HotVals h = hot_load(c, hp);
+        h.matched = 0;
+        h.next_idx = last_index + 1;
         c.pending_snapshot[cell] = 0;
         c.pending_req_snapshot[cell] = RAFTGPU_INVALID_INDEX;
         c.pflags[cell] = RAFTGPU_STATE_PROBE;
         ins_reset(c, cell);  // progress.rs:91 ins.reset()
         c.votes[cell] = 0;  // prs.reset_votes(), raft.rs:953
         if ((meta & RAFTGPU_META_HAS_SELF) && RAFTGPU_META_SELF(meta) == static_cast<uint32_t>(s)) {
-            c.matched[cell] = persisted;         // raft.rs:967
-            c.peer_committed[cell] = committed;  // raft.rs:968
+            h.matched = persisted;          // raft.rs:967
+            h.peer_committed = committed;   // raft.rs:968
         }
+        hot_store(c, hp, h);
     }
     c.committed[g] = committed;
     c.term_start[g] = term_start;
@@ -312,7 +313,8 @@ __global__ void become_leader_kernel(Columns c, uint32_t g) {
             RAFTGPU_STATE_REPLICATE);
         c.pending_snapshot[cell] = 0;
         ins_reset(c, cell);
-        c.next_idx[cell] = c.matched[cell] + 1;  // progress.rs:110-114
+        const HotPtrs hp = hot_ptrs(c, cell);
+        hot_set_next(c, hp, *hp.matched + 1);  // progress.rs:110-114
     }
     const uint64_t li = c.last_index[g] + 1;  // raft.rs:1192 append_entry(&mut [Entry::default()])
     c.last_index[g] = li;
@@ -324,12 +326,13 @@ __global__ void progress_get_kernel(Columns c, uint32_t g, uint32_t s, raftgpu_p
     const uint32_t f = c.pflags[cell];
     const uint32_t meta = c.meta[g];
     raftgpu_progress p{};
-    p.matched = c.matched[cell];
-    p.next_idx = c.next_idx[cell];
+    const HotVals h = hot_load(c, hot_ptrs(c, cell));
+    p.matched = h.matched;
+    p.next_idx = h.next_idx;
     p.pending_snapshot = c.pending_snapshot[cell];
     p.pending_request_snapshot = c.pending_req_snapshot[cell];
     p.commit_group_id = c.commit_group_id[cell];
-    p.committed_index = c.peer_committed[cell];
+    p.committed_index = h.peer_committed;
     p.state = f & RAFTGPU_PF_STATE_MASK;
     p.paused = (f & RAFTGPU_PF_PAUSED) != 0;
     p.recent_active = (f & RAFTGPU_PF_RECENT_ACTIVE) != 0;
@@ -340,12 +343,10 @@ __global__ void progress_get_kernel(Columns c, uint32_t g, uint32_t s, raftgpu_p
 
 __global__ void progress_set_kernel(Columns c, uint32_t g, uint32_t s, raftgpu_progress p) {
     const size_t cell = static_cast<size_t>(s) * c.cap + g;
-    c.matched[cell] = p.matched;
-    c.next_idx[cell] = p.next_idx;
+    hot_store(c, hot_ptrs(c, cell), HotVals{p.matched, p.next_idx, p.committed_index});
     c.pending_snapshot[cell] = p.pending_snapshot;
     c.pending_req_snapshot[cell] = p.pending_request_snapshot;
     c.commit_group_id[cell] = p.commit_group_id;
-    c.peer_committed[cell] = p.committed_index;
     const bool full = c.ins_cap ? (c.ins_meta[cell] >> 16) == c.ins_cap : p.ins_full != 0;  // device windows: derived
     c.pflags[cell] = static_cast<uint8_t>((p.state & RAFTGPU_PF_STATE_MASK) |
                                           (p.paused ? RAFTGPU_PF_PAUSED : 0) |
@@ -360,7 +361,9 @@ __device__ __forceinline__ uint32_t majority_vote(uint32_t mask, uint32_t yes, u
 __global__ void progress_op_kernel(Columns c, uint32_t g, uint32_t s, int op, uint64_t a0, uint64_t a1,
                                    uint64_t a2, int32_t *out) {
     const size_t cell = static_cast<size_t>(s) * c.cap + g;
-    uint64_t matched = c.matched[cell], next = c.next_idx[cell];
+    const HotPtrs hp = hot_ptrs(c, cell);
+    const HotVals h = hot_load(c, hp);
+    uint64_t matched = h.matched, next = h.next_idx, peer_committed = h.peer_committed;
     uint32_t f = c.pflags[cell];
     const uint32_t state = f & RAFTGPU_PF_STATE_MASK;
     int32_t ret = 0;
@@ -400,7 +403,7 @@ __global__ void progress_op_kernel(Columns c, uint32_t g, uint32_t s, int op, ui
         break;
     }
     case RAFTGPU_POP_UPDATE_COMMITTED:  // progress.rs:153-157
-        if (a0 > c.peer_committed[cell]) c.peer_committed[cell] = a0;
+        if (a0 > peer_committed) peer_committed = a0;
         break;
     case RAFTGPU_POP_OPTIMISTIC_UPDATE:  // progress.rs:160-163
         next = a0 + 1;
@@ -477,8 +480,7 @@ __global__ void progress_op_kernel(Columns c, uint32_t g, uint32_t s, int op, ui
     default:
         ret = -2;
     }
-    c.matched[cell] = matched;
-    c.next_idx[cell] = next;
+    hot_store(c, hp, HotVals{matched, next, peer_committed});
     c.pflags[cell] = static_cast<uint8_t>(f);
     *out = ret;
 }

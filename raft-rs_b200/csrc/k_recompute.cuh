@@ -76,8 +76,7 @@ __device__ __forceinline__ bool commit_group(const Columns &c, uint32_t g, uint3
         c.committed[g] = mci;  // commit_to: mci <= last_index, never the fatal! branch
         if (commit_out) commit_out[g] = mci;
         if (meta & RAFTGPU_META_HAS_SELF) {  // raft.rs:896-900
-            const size_t cell = static_cast<size_t>(RAFTGPU_META_SELF(meta)) * c.cap + g;
-            if (mci > c.peer_committed[cell]) c.peer_committed[cell] = mci;
+            hot_update_committed(c, hot_ptrs(c, static_cast<size_t>(RAFTGPU_META_SELF(meta)) * c.cap + g), mci);
         }
     }
     return advanced;
@@ -105,11 +104,9 @@ __device__ __noinline__ bool commit_wide_group(const Columns &c, uint32_t g, uin
         if (commit_out) commit_out[g] = mci;
         const uint32_t meta_hi = c.meta[g + 1];  // raft.rs:896-900: the leader's own Progress, in whichever half it lives
         if (meta_lo & RAFTGPU_META_HAS_SELF) {
-            const size_t cell = static_cast<size_t>(RAFTGPU_META_SELF(meta_lo)) * c.cap + g;
-            if (mci > c.peer_committed[cell]) c.peer_committed[cell] = mci;
+            hot_update_committed(c, hot_ptrs(c, static_cast<size_t>(RAFTGPU_META_SELF(meta_lo)) * c.cap + g), mci);
         } else if (meta_hi & RAFTGPU_META_HAS_SELF) {
-            const size_t cell = static_cast<size_t>(RAFTGPU_META_SELF(meta_hi)) * c.cap + g + 1;
-            if (mci > c.peer_committed[cell]) c.peer_committed[cell] = mci;
+            hot_update_committed(c, hot_ptrs(c, static_cast<size_t>(RAFTGPU_META_SELF(meta_hi)) * c.cap + g + 1), mci);
         }
     }
     return advanced;

@@ -10,15 +10,15 @@
 // record), which HBM serves at roughly half the efficiency of dense bursts.  When the batch is
 // ordered by group, a tile of kFTile consecutive groups owns a CONTIGUOUS record range, so the
 // whole step becomes dense traffic.  One CTA per SM runs a ring of shared-memory stages:
-//   - the load warp bulk-loads (TMA, cp.async.bulk) the tile's rows of matched / next_idx /
-//     committed_index / pflags / meta / committed / term_start / last_index, plus an optional
+//   - the load warp bulk-loads (TMA, cp.async.bulk) the tile's rows of matched / the next_idx and
+//     committed_index offsets / pflags / meta / committed / term_start / last_index, plus an optional
 //     payload (the compact kernel's units), into one stage;
 //   - consumer group i % kFGroups takes the CTA's tile i, so the phases of kFGroups tiles overlap:
 //     it applies the tile's records to the shared-memory rows (the kernel's own body), then
 //     recomputes the commit index of the tile's groups from the same rows (matched is read from
 //     HBM once per step instead of twice);
 //   - the store warp bulk-stores the rows back (cp.async.bulk.global.shared::cta).
-// Peer slots outside `hint` (learners) and the cold columns are handled through HBM directly.
+// Peer slots outside `hint` (learners), the cold columns and the offset escapes are handled through HBM directly.
 // tile_off[t] = index of the first record (packed kernel) or unit (compact kernel) of tile t.
 constexpr int kFTile = RAFTGPU_TILE_GROUPS;  // groups per tile = threads per consumer group
 constexpr int kFGroups = 3;                  // consumer groups per CTA
@@ -29,7 +29,7 @@ constexpr int kFMaxStages = 8;
 // in neighbouring lanes and touch the SAME column index of DIFFERENT rows: with a 256-element row
 // stride they would all fall on the same shared-memory banks (4-way conflicts on every access).
 // 258 u64 (= 2064 B, still 16-byte aligned for TMA) shifts consecutive rows by 4 banks.
-constexpr uint32_t kFRow64 = (kFTile + 2) * 8;   // bytes per u64 row
+constexpr uint32_t kFRow64 = (kFTile + 2) * 8;   // bytes per u64 row; an offset row (next_d, pc_d) uses its first half
 constexpr uint32_t kFRow8 = kFTile + 16;         // bytes per u8 (pflags) row
 constexpr uint32_t kFDefer = 32;                 // deferred (rare-path) records per warp per tile; more are handled inline
 // dynamic shared memory of the fused kernels: 227 KB per CTA minus their static shared memory (barriers, deferred lists)
@@ -145,11 +145,17 @@ struct TileBarriers {
 
 // One stage's rows in shared memory.  Row r of a per-peer column is the r-th hinted slot.
 struct TileRows {
-    uint64_t *matched, *next, *pc, *committed, *ts, *li;
+    uint64_t *matched;
+    int32_t *next, *pc;  // the offsets next_d / pc_d, rows kFRow64 bytes apart
+    uint64_t *committed, *ts, *li;
     uint32_t *meta;
     uint8_t *flags;
     uint32_t *units;  // the payload
 };
+// matched and the offsets of the cell staged in row r for group gl (arena cell `cell`)
+__device__ __forceinline__ HotPtrs staged_hot(const TileRows &t, uint32_t r, uint32_t gl, size_t cell) {
+    return HotPtrs{&t.matched[r * (kFRow64 / 8) + gl], &t.next[r * (kFRow64 / 4) + gl], &t.pc[r * (kFRow64 / 4) + gl], cell};
+}
 
 // Where a consumer group is in its walk over the CTA's tiles.
 struct TileCursor {
@@ -202,8 +208,8 @@ struct TileRing {
         uint8_t *sb = smem + static_cast<size_t>(it % a.n_stages) * stage_bytes;
         TileRows t;
         t.matched = reinterpret_cast<uint64_t *>(sb);
-        t.next = reinterpret_cast<uint64_t *>(sb + H * kFRow64);
-        t.pc = reinterpret_cast<uint64_t *>(sb + 2u * H * kFRow64);
+        t.next = reinterpret_cast<int32_t *>(sb + H * kFRow64);
+        t.pc = reinterpret_cast<int32_t *>(sb + 2u * H * kFRow64);
         t.committed = reinterpret_cast<uint64_t *>(sb + 3u * H * kFRow64);
         t.ts = t.committed + kFRow64 / 8;
         t.li = t.ts + kFRow64 / 8;
@@ -248,17 +254,17 @@ struct TileRing {
             const uint32_t staged = staged_units(u0, u1);
             if (lane == 0) {
                 mbar_wait(&bar->empty[st], ph ^ 1u);
-                mbar_expect_tx(&bar->full[st], 3u * H * ng16 * 8u + H * ng16 + 3u * ng16 * 8u + ng16 * 4u + staged * 4u);
+                mbar_expect_tx(&bar->full[st], H * ng16 * (8u + 4u + 4u + 1u) + 3u * ng16 * 8u + ng16 * 4u + staged * 4u);
             }
             __syncwarp();
             const TileRows t = rows(it);
             for (uint32_t j = lane; j < n_copies; j += 32) {
                 if (j < 4u * H) {
-                    const uint32_t col = j / H, r = j % H;  // col: 0 matched, 1 next_idx, 2 committed_index, 3 pflags
+                    const uint32_t col = j / H, r = j % H;  // col: 0 matched, 1 next_d, 2 pc_d, 3 pflags
                     const size_t cell = static_cast<size_t>(hinted_slot(r)) * c.cap + g0;
                     if (col == 0) tma_load_1d(t.matched + r * (kFRow64 / 8), c.matched + cell, ng16 * 8u, &bar->full[st]);
-                    if (col == 1) tma_load_1d(t.next + r * (kFRow64 / 8), c.next_idx + cell, ng16 * 8u, &bar->full[st]);
-                    if (col == 2) tma_load_1d(t.pc + r * (kFRow64 / 8), c.peer_committed + cell, ng16 * 8u, &bar->full[st]);
+                    if (col == 1) tma_load_1d(t.next + r * (kFRow64 / 4), c.next_d + cell, ng16 * 4u, &bar->full[st]);
+                    if (col == 2) tma_load_1d(t.pc + r * (kFRow64 / 4), c.pc_d + cell, ng16 * 4u, &bar->full[st]);
                     if (col == 3) tma_load_1d(t.flags + r * kFRow8, c.pflags + cell, ng16, &bar->full[st]);
                 } else if (j == 4u * H) {
                     tma_load_1d(t.committed, c.committed + g0, ng16 * 8u, &bar->full[st]);
@@ -292,8 +298,8 @@ struct TileRing {
                     const uint32_t col = j / H, r = j % H;
                     const size_t cell = static_cast<size_t>(hinted_slot(r)) * c.cap + g0;
                     if (col == 0) tma_store_1d(c.matched + cell, t.matched + r * (kFRow64 / 8), ng16 * 8u);
-                    if (col == 1) tma_store_1d(c.next_idx + cell, t.next + r * (kFRow64 / 8), ng16 * 8u);
-                    if (col == 2) tma_store_1d(c.peer_committed + cell, t.pc + r * (kFRow64 / 8), ng16 * 8u);
+                    if (col == 1) tma_store_1d(c.next_d + cell, t.next + r * (kFRow64 / 4), ng16 * 4u);
+                    if (col == 2) tma_store_1d(c.pc_d + cell, t.pc + r * (kFRow64 / 4), ng16 * 4u);
                     if (col == 3) tma_store_1d(c.pflags + cell, t.flags + r * kFRow8, ng16);
                 } else if (j == 4u * H) {
                     tma_store_1d(c.committed + g0, t.committed, ng16 * 8u);
@@ -387,10 +393,11 @@ struct TileRing {
                 s.committed[gl] = mci;  // (the store warp copies the row to commit_out too)
                 if (meta & RAFTGPU_META_HAS_SELF) {  // raft.rs:896-900
                     const uint32_t self = RAFTGPU_META_SELF(meta);
-                    uint64_t *pc = ((hint >> self) & 1u)
-                                       ? &s.pc[__popc(hint & ((1u << self) - 1u)) * R64 + gl]
-                                       : &c.peer_committed[static_cast<size_t>(self) * c.cap + g];
-                    if (mci > *pc) *pc = mci;
+                    const size_t cell = static_cast<size_t>(self) * c.cap + g;
+                    if ((hint >> self) & 1u)
+                        hot_update_committed(c, staged_hot(s, __popc(hint & ((1u << self) - 1u)), gl, cell), mci);
+                    else
+                        hot_update_committed(c, hot_ptrs(c, cell), mci);
                 }
             }
         }
@@ -432,18 +439,18 @@ struct TileRing {
 __device__ __forceinline__ uint32_t tile_general_apply(const Columns &c, const RecRegs &rec, uint64_t ext_hint,
                                                     uint64_t ext_snapshot, uint32_t gl, uint32_t hint,
                                                     const TileRows &t, uint32_t *local) {
-    constexpr uint32_t R64 = kFRow64 / 8;
     const uint32_t slot = static_cast<uint32_t>(rec.w0 >> 32) & 0xffu;
     if (slot < kSlots && ((hint >> slot) & 1u)) {
         const uint32_t r = __popc(hint & ((1u << slot) - 1u));
+        const CellPtrs sp{staged_hot(t, r, gl, static_cast<size_t>(slot) * c.cap + static_cast<uint32_t>(rec.w0)), &t.li[gl],
+                          &t.flags[r * kFRow8 + gl]};
+        const HotVals h = hot_load(c, sp.hot);
         CellRegs cd;
         cd.meta = t.meta[gl];
-        cd.matched = t.matched[r * R64 + gl];
-        cd.next_idx = t.next[r * R64 + gl];
+        cd.matched = h.matched;
+        cd.next_idx = h.next_idx;
         cd.flags = t.flags[r * kFRow8 + gl];
-        cd.peer_committed = t.pc[r * R64 + gl];
-        const CellPtrs sp{&t.matched[r * R64 + gl], &t.next[r * R64 + gl], &t.pc[r * R64 + gl], &t.li[gl],
-                          &t.flags[r * kFRow8 + gl]};
+        cd.peer_committed = h.peer_committed;
         return apply_one<2>(c, nullptr, ext_hint, ext_snapshot, rec, cd, sp, local);
     }
     CellRegs cd = load_cell(c, rec);
@@ -456,29 +463,33 @@ __device__ __forceinline__ uint32_t tile_general_apply(const Columns &c, const R
 // The common records -- accept, leader-local, rejection without a snapshot request -- for a peer
 // in Replicate or Probe state whose cell is staged in shared memory: statement for statement the
 // branches of apply_one (raft.rs:1674-1677, 1709-1730, 974-991, 1010-1014; progress.rs:95-114,
-// 138-157, 168-206).  Returns false (nothing touched) when the record needs the general path.
+// 138-157, 168-206).  Returns false (nothing touched) when the record needs the general path, which
+// includes a cell whose offsets are escaped: the exact values would be a dependent HBM load.
 // `res` is left alone unless the record makes progress.
 template <bool kSimple5>
 __device__ __forceinline__ bool tile_fast_apply(const Columns &c, const TileRows &t, uint32_t gl, uint32_t g, uint32_t slot,
                                                 uint64_t index, uint64_t commit, bool is_local, bool is_reject,
                                                 uint64_t ext_hint, uint32_t hint, uint32_t present_mask, uint32_t *local,
                                                 uint32_t &res) {
-    constexpr uint32_t R64 = kFRow64 / 8;
+    constexpr uint32_t R64 = kFRow64 / 8, R32 = kFRow64 / 4;
     if (!((hint >> slot) & 1u)) return false;
     const uint32_t r = kSimple5 ? slot : static_cast<uint32_t>(__popc(hint & ((1u << slot) - 1u)));
-    const uint32_t ci = r * R64 + gl;
+    const uint32_t ci = r * R64 + gl, di = r * R32 + gl;
     const uint32_t f0 = t.flags[r * kFRow8 + gl];
     const uint32_t state = f0 & RAFTGPU_PF_STATE_MASK;
-    if (!((present_mask >> slot) & 1u) || state == RAFTGPU_STATE_SNAPSHOT) return false;
-    uint64_t m = t.matched[ci], nx = t.next[ci];
-    const uint64_t m0 = m, nx0 = nx;
+    const int32_t nd = t.next[di], pd = t.pc[di];
+    if (!((present_mask >> slot) & 1u) || state == RAFTGPU_STATE_SNAPSHOT || off_escaped(nd) || off_escaped(pd))
+        return false;
+    uint64_t m = t.matched[ci];
+    const uint64_t m0 = m;
+    uint64_t nx = off_value(nd, m0), pc = off_value(pd, m0);
     uint32_t f = f0;
     local[0]++;
     if (is_local) {
         if (commit != 0) t.li[gl] = commit;
     } else {
         f |= RAFTGPU_PF_RECENT_ACTIVE;
-        if (commit > t.pc[ci]) t.pc[ci] = commit;
+        if (commit > pc) pc = commit;
     }
     if (is_reject) {  // maybe_decr_to without a snapshot request
         local[2]++;
@@ -520,8 +531,7 @@ __device__ __forceinline__ bool tile_fast_apply(const Columns &c, const TileRows
             nx = m + 1;
         }
     }
-    if (m != m0) t.matched[ci] = m;
-    if (nx != nx0) t.next[ci] = nx;
+    hot_write_over(c, staged_hot(t, r, gl, static_cast<size_t>(slot) * c.cap + g), m0, nd, pd, HotVals{m, nx, pc});
     if (f != f0) t.flags[r * kFRow8 + gl] = static_cast<uint8_t>(f);
     return true;
 }

@@ -15,12 +15,14 @@ joint = os.environ.get("JOINT", "0") == "1"
 kernel = os.environ.get("KERNEL", "packed")
 assert kernel in ("packed", "compact"), kernel
 NA = 4
-arenas, rounds = [], []
+arenas, rounds, outs = [], [], []
 pack_buf = np.empty((7 * n + 64, 2), dtype=np.uint64)
 for a in range(NA):
     s = B.Synth(n, 0x5EED0003 + 0x100 * a, k_peers=5, joint=joint)
     ar = B.Arena(n, n_rings=1, ring_records=4096)
     ar.group_alloc_range(n); ar.load_columns(s.initial)
+    # the step's outputs (advanced bitmap, commit index of every group), written as bench.py's fused leg writes them
+    outs.append({"d_adv": ar.device_alloc(4 * ((n + 31) // 32 + 1)), "d_commit": ar.device_alloc(8 * n)})
     rr = []
     for _ in range(R):
         recs = s.next_round()
@@ -50,9 +52,9 @@ snapshots = [ar.read_columns(n) for ar in arenas]
 def launch(a, r):
     args, kw = rounds[a][r]
     if kernel == "packed":
-        arenas[a].step_sorted_device(*args, stream=sh)
+        arenas[a].step_sorted_device(*args, stream=sh, **outs[a])
     else:
-        arenas[a].step_compact_device(*args, stream=sh, **kw)
+        arenas[a].step_compact_device(*args, stream=sh, **outs[a], **kw)
 
 
 with torch.cuda.stream(st):
