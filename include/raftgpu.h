@@ -22,8 +22,10 @@
  *    own compute stream);
  *  - threading follows the reference (raw_node.rs:284 "RawNode is a
  *    thread-unsafe Node", raft.rs:292-294 `Raft: Send`): calls that touch ONE
- *    group may run concurrently for DIFFERENT groups; raftgpu_step* and the
- *    arena lifecycle calls need exclusive access.
+ *    group may run concurrently for DIFFERENT groups; raftgpu_step*,
+ *    raftgpu_control (it may change many groups' configurations, and with them
+ *    the launch plan of the next step) and the arena lifecycle calls need
+ *    exclusive access.
  *
  * Data layout in HBM (struct-of-arrays, see DESIGN.md): per-peer columns are
  * [RAFTGPU_SLOTS][cap] u64 / u8, per-group columns are [cap]; a "group" is one
@@ -722,6 +724,52 @@ int32_t raftgpu_tally_votes(raftgpu_arena *arena, void *stream, uint32_t first, 
 /* Single-group form (synchronous). */
 int32_t raftgpu_vote_result(raftgpu_arena *arena, uint32_t group, int32_t *out_result,
                             uint32_t *out_granted, uint32_t *out_rejected);
+
+/* ---- batched control plane ------------------------------------------------ */
+
+/* One command of a raftgpu_control list: one single-group control call and its arguments.  40 bytes. */
+typedef struct {
+    uint32_t group;     /* group id as the single-group calls take it (the low half of a wide group) */
+    uint8_t op;         /* RAFTGPU_CTL_* */
+    uint8_t peer_slot;  /* 0..15 where the op names a peer; SET_CONF: the self slot, 0xff = none */
+    uint16_t arg;       /* PROGRESS_OP: RAFTGPU_POP_*; RECORD_VOTE: 0 no / 1 yes; SET_GROUP_COMMIT: enable */
+    uint64_t a[4];      /* the single call's u64 arguments, in its order */
+} raftgpu_ctl_cmd;
+
+/* What the command's single call would have returned. */
+typedef struct {
+    int32_t status;     /* exactly the single call's status */
+    int32_t value;      /* its out value: has_quorum / quorum_recently_active / maybe_commit_to 0|1, progress_op's
+                           result, vote_result as VoteResult | granted << 8 | rejected << 16; else 0 */
+} raftgpu_ctl_result;
+
+/* op                                    single call                      arguments */
+#define RAFTGPU_CTL_SET_CONF 0              /* raftgpu_group_set_conf        a = {incoming, outgoing, learners, next_idx}, peer_slot = self */
+#define RAFTGPU_CTL_RESET 1                 /* raftgpu_group_reset           a = {term_start, last_index, committed, persisted} */
+#define RAFTGPU_CTL_BECOME_LEADER 2         /* raftgpu_group_become_leader   - */
+#define RAFTGPU_CTL_SET_LOG_BOUNDS 3        /* raftgpu_group_set_log_bounds  a = {term_start, last_index} */
+#define RAFTGPU_CTL_SET_TERM 4              /* raftgpu_group_set_term        a[0] */
+#define RAFTGPU_CTL_COMMIT_TO 5             /* raftgpu_group_commit_to       a[0] */
+#define RAFTGPU_CTL_MAYBE_COMMIT_TO 6       /* raftgpu_group_maybe_commit_to a[0] */
+#define RAFTGPU_CTL_SET_GROUP_COMMIT 7      /* raftgpu_set_group_commit      arg */
+#define RAFTGPU_CTL_ASSIGN_COMMIT_GROUP 8   /* raftgpu_assign_commit_group   peer_slot, a[0] */
+#define RAFTGPU_CTL_RESET_VOTES 9           /* raftgpu_reset_votes           - */
+#define RAFTGPU_CTL_RECORD_VOTE 10          /* raftgpu_record_vote           peer_slot, arg */
+#define RAFTGPU_CTL_VOTE_RESULT 11          /* raftgpu_vote_result           - */
+#define RAFTGPU_CTL_HAS_QUORUM 12           /* raftgpu_has_quorum            a[0] = slot mask */
+#define RAFTGPU_CTL_QUORUM_RECENTLY_ACTIVE 13 /* raftgpu_quorum_recently_active peer_slot = perspective_of */
+#define RAFTGPU_CTL_PROGRESS_OP 14          /* raftgpu_progress_op           peer_slot, arg = RAFTGPU_POP_*, a[0..2] */
+
+/* Run a list of control commands for many groups in a few launches (the store-wide election after a restart, the
+ * check_quorum sweep, region splits).  The contract: the arena, every results[i], the device counters and the
+ * arena's meta mirror end exactly as calling the single-group entry points one at a time, in list order, would
+ * leave them.  A command its single call would refuse (an unallocated group, the high half of a wide group, an
+ * absent peer, a mask too wide, an unknown RAFTGPU_POP_* code) does nothing and carries that status, and an unknown
+ * op carries RAFTGPU_ERR_INVALID whatever its group; the other commands still run.  Returns RAFTGPU_OK when the list ran (n == 0 included), RAFTGPU_ERR_INVALID for a NULL
+ * cmds / results with n > 0, RAFTGPU_ERR_BUSY while records are enqueued for a step, RAFTGPU_ERR_CUDA on a CUDA
+ * failure.  A list longer than the arena's staging buffer runs in list-order chunks.  Synchronous; needs exclusive
+ * access (see the threading note at the top). */
+int32_t raftgpu_control(raftgpu_arena *arena, const raftgpu_ctl_cmd *cmds, uint64_t n, raftgpu_ctl_result *results);
 
 /* ---- plumbing ------------------------------------------------------------ */
 int32_t raftgpu_counters_read(raftgpu_arena *arena, raftgpu_counters *out);

@@ -54,6 +54,15 @@ SEND_ENTRY_DTYPE = np.dtype([("group", "<u4"), ("peer_slot", "u1"), ("flags", "u
                              ("next_idx", "<u8")])
 assert SEND_ENTRY_DTYPE.itemsize == 16
 SEND_SNAPSHOT = 0x1
+# raftgpu_control (the batched control plane): one command per single-group control call, and its result
+(CTL_SET_CONF, CTL_RESET, CTL_BECOME_LEADER, CTL_SET_LOG_BOUNDS, CTL_SET_TERM, CTL_COMMIT_TO, CTL_MAYBE_COMMIT_TO,
+ CTL_SET_GROUP_COMMIT, CTL_ASSIGN_COMMIT_GROUP, CTL_RESET_VOTES, CTL_RECORD_VOTE, CTL_VOTE_RESULT, CTL_HAS_QUORUM,
+ CTL_QUORUM_RECENTLY_ACTIVE, CTL_PROGRESS_OP) = range(15)
+CTL_NO_SELF = 0xFF
+CTL_CMD_DTYPE = np.dtype([("group", "<u4"), ("op", "u1"), ("peer_slot", "u1"), ("arg", "<u2"), ("a", "<u8", (4,))])
+assert CTL_CMD_DTYPE.itemsize == 40
+CTL_RESULT_DTYPE = np.dtype([("status", "<i4"), ("value", "<i4")])
+assert CTL_RESULT_DTYPE.itemsize == 8
 
 # host column name -> (column id, numpy dtype, per-peer?)
 COLUMNS = {
@@ -268,6 +277,7 @@ def lib() -> C.CDLL:
             "raftgpu_step_send_list": ([vp, vp, u64, C.POINTER(u64)], i32),
             "raftgpu_vote_result": ([vp, u32, C.POINTER(i32), C.POINTER(u32), C.POINTER(u32)], i32),
             "raftgpu_group_set_term": ([vp, u32, u64], i32),
+            "raftgpu_control": ([vp, vp, u64, vp], i32),
             "raftgpu_arena_enable_inflights": ([vp, u32], i32),
             "raftgpu_inflights_get": ([vp, u32, u32, C.POINTER(u32), C.POINTER(u32), vp, u32], i32),
             "raftgpu_heartbeat_resp_device": ([vp, vp, vp, u64, vp, vp], i32),
@@ -562,6 +572,14 @@ class Arena:
 
     def assign_commit_group(self, g, slot, gid):
         self._ck(self._L.raftgpu_assign_commit_group(self._h, g, slot, gid), "assign_commit_group")
+
+    def control(self, cmds: np.ndarray) -> np.ndarray:
+        """raftgpu_control: every command of the list as its single-group call, in list order.  Returns the
+        CTL_RESULT_DTYPE results (a refused command carries its status there; only the call's own failure raises)."""
+        assert cmds.dtype == CTL_CMD_DTYPE and cmds.flags.c_contiguous
+        res = np.zeros(len(cmds), dtype=CTL_RESULT_DTYPE)
+        self._ck(self._L.raftgpu_control(self._h, cmds.ctypes.data, len(cmds), res.ctypes.data), "control")
+        return res
 
     # -- bulk columns
     def column_write(self, col: int, slot: int, first: int, arr: np.ndarray):

@@ -241,6 +241,9 @@ struct raftgpu_arena {
     int n_inflight = 0;
     // control plane: single-group calls share the scratch buffers and the meta mirror
     std::mutex ctl_mu;
+    // raftgpu_control scratch, kept between calls: per group (pair), the commands staged in the current chunk and
+    // its running meta; per command of the chunk, its wave (kCtlSkip = not staged) and, in wave order, its index
+    std::vector<uint32_t> ctl_count, ctl_meta, ctl_wave, ctl_order;
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -812,11 +815,21 @@ void wait_submitter(raftgpu_arena *a) {
     }
 }
 
-template <typename T, typename F>
-int32_t host_batch_op(raftgpu_arena *a, const T *in, uint64_t n, uint8_t *results, F &&launch, uint32_t *out_dups) {
+// The admission rule of every host batch call: the fill set's staging is idle (no records enqueued for a step).
+int32_t host_batch_admit(raftgpu_arena *a, StagingSet **out) {
     wait_submitter(a);
     StagingSet &s = a->sets[a->fill];
     if (s.in_flight || s.next_chunk.load() != 0) return fail(a, RAFTGPU_ERR_BUSY, "records are staged for a step: step first");
+    *out = &s;
+    return RAFTGPU_OK;
+}
+
+template <typename T, typename F>
+int32_t host_batch_op(raftgpu_arena *a, const T *in, uint64_t n, uint8_t *results, F &&launch, uint32_t *out_dups) {
+    StagingSet *sp = nullptr;
+    const int32_t adm = host_batch_admit(a, &sp);
+    if (adm != RAFTGPU_OK) return adm;
+    StagingSet &s = *sp;
     const uint64_t room = rec_slots(a) * sizeof(PackedRec);
     if (n * sizeof(T) > room || n > 4 * (room / sizeof(PackedRec))) return fail(a, RAFTGPU_ERR_FULL, "batch larger than the staging buffer");
     CK(a, cudaSetDevice(a->device));
@@ -947,6 +960,7 @@ int32_t run_step(raftgpu_arena *a, const char *form, uint32_t flags, Queue &&que
 extern "C" {
 
 #include "abi_control.inc"
+#include "abi_control_batch.inc"
 #include "abi_device.inc"
 #include "abi_staging.inc"
 #include "abi_compact.inc"

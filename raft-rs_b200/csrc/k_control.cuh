@@ -205,58 +205,61 @@ __device__ __forceinline__ uint32_t majority_vote(uint32_t mask, uint32_t yes, u
     return RAFTGPU_VOTE_LOST;
 }
 
+// One group's tally: VoteResult | granted << 8 | rejected << 16.
+__device__ __forceinline__ uint32_t tally_group(const Columns &c, uint32_t g) {
+    uint32_t meta = c.meta[g];
+    uint32_t in = RAFTGPU_META_IN(meta), outm = RAFTGPU_META_OUT(meta);
+    uint32_t yes = 0, no = 0;
+#pragma unroll
+    for (int s = 0; s < kSlots; s++) {
+        const uint32_t v = c.votes[static_cast<size_t>(s) * c.cap + g];
+        yes |= (v == 2u) << s;
+        no |= (v == 1u) << s;
+    }
+    if (meta & (RAFTGPU_META_WIDE_LO | RAFTGPU_META_WIDE_HI)) {  // a wide group: both halves get the result over 16 peers
+        const uint32_t other = (meta & RAFTGPU_META_WIDE_LO) ? g + 1 : g - 1, sh_me = (meta & RAFTGPU_META_WIDE_LO) ? 0u : 8u;
+        const uint32_t mo = c.meta[other];
+        uint32_t yo = 0, no2 = 0;
+        for (int s = 0; s < kSlots; s++) {
+            const uint32_t v = c.votes[static_cast<size_t>(s) * c.cap + other];
+            yo |= (v == 2u) << s;
+            no2 |= (v == 1u) << s;
+        }
+        in = (in << sh_me) | (RAFTGPU_META_IN(mo) << (8u - sh_me));
+        outm = (outm << sh_me) | (RAFTGPU_META_OUT(mo) << (8u - sh_me));
+        yes = (yes << sh_me) | (yo << (8u - sh_me));
+        no = (no << sh_me) | (no2 << (8u - sh_me));
+    }
+    const uint32_t i = majority_vote(in, yes, no), o = majority_vote(outm, yes, no);
+    uint32_t r;
+    if (i == RAFTGPU_VOTE_WON && o == RAFTGPU_VOTE_WON)
+        r = RAFTGPU_VOTE_WON;
+    else if (i == RAFTGPU_VOTE_LOST || o == RAFTGPU_VOTE_LOST)
+        r = RAFTGPU_VOTE_LOST;
+    else
+        r = RAFTGPU_VOTE_PENDING;
+    const uint32_t voters = in | outm;  // tracker.rs:320-322
+    return r | (__popc(yes & voters) << 8) | (__popc(no & voters) << 16);
+}
+
 __global__ void __launch_bounds__(256)
 tally_kernel(Columns c, uint32_t first, uint32_t n, uint32_t *__restrict__ out,
              unsigned long long *__restrict__ counters) {
     const uint64_t t = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     const bool active = t < n;
-    if (active) {
-        const uint32_t g = first + static_cast<uint32_t>(t);
-        uint32_t meta = c.meta[g];
-        uint32_t in = RAFTGPU_META_IN(meta), outm = RAFTGPU_META_OUT(meta);
-        uint32_t yes = 0, no = 0;
-#pragma unroll
-        for (int s = 0; s < kSlots; s++) {
-            const uint32_t v = c.votes[static_cast<size_t>(s) * c.cap + g];
-            yes |= (v == 2u) << s;
-            no |= (v == 1u) << s;
-        }
-        if (meta & (RAFTGPU_META_WIDE_LO | RAFTGPU_META_WIDE_HI)) {  // a wide group: both halves get the result over 16 peers
-            const uint32_t other = (meta & RAFTGPU_META_WIDE_LO) ? g + 1 : g - 1, sh_me = (meta & RAFTGPU_META_WIDE_LO) ? 0u : 8u;
-            const uint32_t mo = c.meta[other];
-            uint32_t yo = 0, no2 = 0;
-            for (int s = 0; s < kSlots; s++) {
-                const uint32_t v = c.votes[static_cast<size_t>(s) * c.cap + other];
-                yo |= (v == 2u) << s;
-                no2 |= (v == 1u) << s;
-            }
-            in = (in << sh_me) | (RAFTGPU_META_IN(mo) << (8u - sh_me));
-            outm = (outm << sh_me) | (RAFTGPU_META_OUT(mo) << (8u - sh_me));
-            yes = (yes << sh_me) | (yo << (8u - sh_me));
-            no = (no << sh_me) | (no2 << (8u - sh_me));
-        }
-        const uint32_t i = majority_vote(in, yes, no), o = majority_vote(outm, yes, no);
-        uint32_t r;
-        if (i == RAFTGPU_VOTE_WON && o == RAFTGPU_VOTE_WON)
-            r = RAFTGPU_VOTE_WON;
-        else if (i == RAFTGPU_VOTE_LOST || o == RAFTGPU_VOTE_LOST)
-            r = RAFTGPU_VOTE_LOST;
-        else
-            r = RAFTGPU_VOTE_PENDING;
-        const uint32_t voters = in | outm;  // tracker.rs:320-322
-        out[g] = r | (__popc(yes & voters) << 8) | (__popc(no & voters) << 16);
-    }
+    if (active) out[first + static_cast<uint32_t>(t)] = tally_group(c, first + static_cast<uint32_t>(t));
     const uint32_t local[1] = {active ? 1u : 0u};
     const int which[1] = {kCntVotes};
     block_flush_counts<1>(local, which, counters, nullptr);
 }
 
 // ---------------------------------------------------------------------------
-// Control-plane helpers (single thread; launched <<<1,1>>>).
+// Control-plane helpers: one group each, as __device__ functions that the single-group <<<1,1>>> kernels below and
+// control_kernel (one thread per command) share.
 
 // ProgressTracker::apply_conf (tracker.rs:380-397)
-__global__ void conf_kernel(Columns c, uint32_t g, uint32_t new_meta, uint32_t added,
-                            uint32_t removed, uint64_t next_idx) {
+__device__ __forceinline__ void conf_group(const Columns &c, uint32_t g, uint32_t new_meta, uint32_t added,
+                                           uint32_t removed, uint64_t next_idx) {
     for (int s = 0; s < kSlots; s++) {
         const size_t cell = static_cast<size_t>(s) * c.cap + g;
         if (((added | removed) >> s) & 1u) {
@@ -272,10 +275,14 @@ __global__ void conf_kernel(Columns c, uint32_t g, uint32_t new_meta, uint32_t a
     }
     c.meta[g] = new_meta;
 }
+__global__ void conf_kernel(Columns c, uint32_t g, uint32_t new_meta, uint32_t added,
+                            uint32_t removed, uint64_t next_idx) {
+    conf_group(c, g, new_meta, added, removed, next_idx);
+}
 
 // Raft::reset (raft.rs:942-971) for the tracker + log bookkeeping of one group.
-__global__ void reset_kernel(Columns c, uint32_t g, uint64_t term_start, uint64_t last_index,
-                             uint64_t committed, uint64_t persisted) {
+__device__ __forceinline__ void reset_group(const Columns &c, uint32_t g, uint64_t term_start, uint64_t last_index,
+                                            uint64_t committed, uint64_t persisted) {
     const uint32_t meta = c.meta[g];
     const uint32_t present = RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta);
     for (int s = 0; s < kSlots; s++) {
@@ -301,10 +308,14 @@ __global__ void reset_kernel(Columns c, uint32_t g, uint64_t term_start, uint64_
     c.term_start[g] = term_start;
     c.last_index[g] = last_index;
 }
+__global__ void reset_kernel(Columns c, uint32_t g, uint64_t term_start, uint64_t last_index,
+                             uint64_t committed, uint64_t persisted) {
+    reset_group(c, g, term_start, last_index, committed, persisted);
+}
 
 // Raft::become_leader's tracker side (raft.rs:1176-1192): self.become_replicate(),
 // then the empty entry of the new term is appended at last_index + 1.
-__global__ void become_leader_kernel(Columns c, uint32_t g) {
+__device__ __forceinline__ void become_leader_group(const Columns &c, uint32_t g) {
     const uint32_t meta = c.meta[g];
     if (meta & RAFTGPU_META_HAS_SELF) {
         const size_t cell = static_cast<size_t>(RAFTGPU_META_SELF(meta)) * c.cap + g;
@@ -320,6 +331,7 @@ __global__ void become_leader_kernel(Columns c, uint32_t g) {
     c.last_index[g] = li;
     c.term_start[g] = li;
 }
+__global__ void become_leader_kernel(Columns c, uint32_t g) { become_leader_group(c, g); }
 
 __global__ void progress_get_kernel(Columns c, uint32_t g, uint32_t s, raftgpu_progress *out) {
     const size_t cell = static_cast<size_t>(s) * c.cap + g;
@@ -357,9 +369,9 @@ __global__ void progress_set_kernel(Columns c, uint32_t g, uint32_t s, raftgpu_p
 __device__ __forceinline__ uint32_t majority_vote(uint32_t mask, uint32_t yes, uint32_t no);
 
 // Every method of Progress (src/tracker/progress.rs:75-243) on one cell, literally, for the
-// host mirror's ProgressRef: op codes are RAFTGPU_POP_*.  *out gets the bool / status result.
-__global__ void progress_op_kernel(Columns c, uint32_t g, uint32_t s, int op, uint64_t a0, uint64_t a1,
-                                   uint64_t a2, int32_t *out) {
+// host mirror's ProgressRef: op codes are RAFTGPU_POP_*.  Returns the bool / status result.
+__device__ __forceinline__ int32_t progress_op_cell(const Columns &c, uint32_t g, uint32_t s, int op, uint64_t a0,
+                                                    uint64_t a1, uint64_t a2) {
     const size_t cell = static_cast<size_t>(s) * c.cap + g;
     const HotPtrs hp = hot_ptrs(c, cell);
     const HotVals h = hot_load(c, hp);
@@ -482,12 +494,16 @@ __global__ void progress_op_kernel(Columns c, uint32_t g, uint32_t s, int op, ui
     }
     hot_store(c, hp, HotVals{matched, next, peer_committed});
     c.pflags[cell] = static_cast<uint8_t>(f);
-    *out = ret;
+    return ret;
+}
+__global__ void progress_op_kernel(Columns c, uint32_t g, uint32_t s, int op, uint64_t a0, uint64_t a1,
+                                   uint64_t a2, int32_t *out) {
+    *out = progress_op_cell(c, g, s, op, a0, a1, a2);
 }
 
 // ProgressTracker::has_quorum (tracker.rs:367-372): vote_result(|id| set.get(id).map(|_| true)) == Won,
 // and quorum_recently_active (tracker.rs:346-361), which also clears recent_active.
-__global__ void quorum_kernel(Columns c, uint32_t g, int op, uint32_t arg, int32_t *out) {
+__device__ __forceinline__ int32_t quorum_group(const Columns &c, uint32_t g, int op, uint32_t arg) {
     const uint32_t meta = c.meta[g];
     const bool wide = (meta & RAFTGPU_META_WIDE_LO) != 0;  // peers 8..15 live in group g + 1
     const uint32_t meta_hi = wide ? c.meta[g + 1] : 0u;
@@ -511,12 +527,13 @@ __global__ void quorum_kernel(Columns c, uint32_t g, int op, uint32_t arg, int32
     }
     // members of the set vote yes, everyone else is missing (None)
     const uint32_t i = majority_vote(in, active, 0), o = majority_vote(outm, active, 0);
-    *out = (i == RAFTGPU_VOTE_WON && o == RAFTGPU_VOTE_WON) ? 1 : 0;
+    return (i == RAFTGPU_VOTE_WON && o == RAFTGPU_VOTE_WON) ? 1 : 0;
 }
+__global__ void quorum_kernel(Columns c, uint32_t g, int op, uint32_t arg, int32_t *out) { *out = quorum_group(c, g, op, arg); }
 
 // The two halves of a wide group share the group's log / commit columns: make them agree (a LOCAL record or a
 // single-half control-plane call may have touched one half only).
-__global__ void wide_sync_kernel(Columns c, uint32_t g) {
+__device__ __forceinline__ void wide_sync(const Columns &c, uint32_t g) {
     const uint64_t li = umax64(c.last_index[g], c.last_index[g + 1]);
     const uint64_t cm = umax64(c.committed[g], c.committed[g + 1]);
     c.last_index[g] = c.last_index[g + 1] = li;
@@ -524,6 +541,7 @@ __global__ void wide_sync_kernel(Columns c, uint32_t g) {
     c.term_start[g + 1] = c.term_start[g];
     c.term[g + 1] = c.term[g];
 }
+__global__ void wide_sync_kernel(Columns c, uint32_t g) { wide_sync(c, g); }
 
 __global__ void group_get_kernel(Columns c, uint32_t g, raftgpu_group_state *out) {
     raftgpu_group_state s{};
@@ -536,9 +554,10 @@ __global__ void group_get_kernel(Columns c, uint32_t g, raftgpu_group_state *out
 
 // op 0: set_log_bounds; op 1: commit_to (status in *out: 0 ok, 1 out of range);
 // op 2: meta bit set/clear (a = mask, b = enable); op 3: assign commit group (a = slot, b = id);
-// op 4: reset votes; op 5: record vote (a = slot, b = vote+1), first vote wins (tracker.rs:308-310)
-__global__ void group_op_kernel(Columns c, uint32_t g, int op, uint64_t a, uint64_t b,
-                                uint32_t *out) {
+// op 4: reset votes; op 5: record vote (a = slot, b = vote+1), first vote wins (tracker.rs:308-310);
+// op 6: maybe_commit (1 = advanced).  Returns the status / flag of ops 1 and 6, 0 for the others.
+__device__ __forceinline__ uint32_t group_op(const Columns &c, uint32_t g, int op, uint64_t a, uint64_t b) {
+    uint32_t out = 0;
     switch (op) {
     case 0:
         c.term_start[g] = a;
@@ -546,12 +565,12 @@ __global__ void group_op_kernel(Columns c, uint32_t g, int op, uint64_t a, uint6
         break;
     case 1:  // RaftLog::commit_to, raft_log.rs:286-300
         if (c.committed[g] >= a) {
-            *out = 0;
+            out = 0;
         } else if (c.last_index[g] < a) {
-            *out = 1;
+            out = 1;
         } else {
             c.committed[g] = a;
-            *out = 0;
+            out = 0;
         }
         break;
     case 2:
@@ -571,10 +590,99 @@ __global__ void group_op_kernel(Columns c, uint32_t g, int op, uint64_t a, uint6
     case 6:  // RaftLog::maybe_commit(max_index = a, term = the leader's), raft_log.rs:487-499, range form
         if (a > c.committed[g] && a >= c.term_start[g] && a <= c.last_index[g]) {
             c.committed[g] = a;
-            *out = 1;
+            out = 1;
         } else {
-            *out = 0;
+            out = 0;
         }
         break;
     }
+    return out;
+}
+__global__ void group_op_kernel(Columns c, uint32_t g, int op, uint64_t a, uint64_t b, uint32_t *out) {
+    const uint32_t r = group_op(c, g, op, a, b);
+    if (op == 1 || op == 6) *out = r;
+}
+
+// ---------------------------------------------------------------------------
+// control_kernel: one wave of a raftgpu_control list, one thread per command (DESIGN 3.8).  The host has validated
+// every command against its meta mirror and put at most one command of each group (of each wide pair) in the wave,
+// so the threads touch disjoint cells.  It has also resolved the commands: `group` is the half that holds the named
+// peer, `peer_slot` the slot within that half, and a SET_CONF's a[0] carries the new meta words of the low half
+// (bits 0..31) and the high half (bits 32..63).  Every op runs the device function of its single-group call;
+// res[i] = {status, value} of cmds[i].
+__global__ void __launch_bounds__(256)
+control_kernel(Columns c, const raftgpu_ctl_cmd *__restrict__ cmds, uint32_t n, int2 *__restrict__ res,
+               unsigned long long *__restrict__ counters) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t tallied = 0;
+    if (t < n) {
+        const raftgpu_ctl_cmd m = cmds[t];
+        const uint32_t g = m.group;
+        const uint32_t halves = (m.op != RAFTGPU_CTL_SET_TERM && (c.meta[g] & RAFTGPU_META_WIDE_LO)) ? 2u : 1u;
+        int32_t status = RAFTGPU_OK, value = 0;
+        switch (m.op) {
+        case RAFTGPU_CTL_SET_CONF:
+            for (uint32_t k = 0; k < halves; k++) {
+                const uint32_t meta = static_cast<uint32_t>(m.a[0] >> (32 * k)), was = c.meta[g + k];
+                const uint32_t p_was = RAFTGPU_META_IN(was) | RAFTGPU_META_OUT(was) | RAFTGPU_META_LEARN(was);
+                const uint32_t p_now = RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta);
+                conf_group(c, g + k, meta, p_now & ~p_was, p_was & ~p_now, m.a[3]);
+            }
+            break;
+        case RAFTGPU_CTL_RESET:
+            for (uint32_t k = 0; k < halves; k++) reset_group(c, g + k, m.a[0], m.a[1], m.a[2], m.a[3]);
+            break;
+        case RAFTGPU_CTL_BECOME_LEADER:
+            for (uint32_t k = 0; k < halves; k++) become_leader_group(c, g + k);
+            break;
+        case RAFTGPU_CTL_SET_LOG_BOUNDS:
+            for (uint32_t k = 0; k < halves; k++) group_op(c, g + k, 0, m.a[0], m.a[1]);
+            break;
+        case RAFTGPU_CTL_SET_TERM:  // a high half alone when named alone, as raftgpu_group_set_term
+            c.term[g] = m.a[0];
+            if (c.meta[g] & RAFTGPU_META_WIDE_LO) c.term[g + 1] = m.a[0];
+            break;
+        case RAFTGPU_CTL_COMMIT_TO:
+            if (halves == 2) wide_sync(c, g);
+            status = group_op(c, g, 1, m.a[0], 0) ? RAFTGPU_ERR_COMMIT_RANGE : RAFTGPU_OK;
+            if (halves == 2) group_op(c, g + 1, 1, m.a[0], 0);
+            break;
+        case RAFTGPU_CTL_MAYBE_COMMIT_TO:
+            if (halves == 2) {
+                wide_sync(c, g);
+                group_op(c, g + 1, 6, m.a[0], 0);
+            }
+            value = static_cast<int32_t>(group_op(c, g, 6, m.a[0], 0));
+            break;
+        case RAFTGPU_CTL_SET_GROUP_COMMIT:
+            for (uint32_t k = 0; k < halves; k++) group_op(c, g + k, 2, RAFTGPU_META_GROUP_COMMIT, m.arg ? 1 : 0);
+            break;
+        case RAFTGPU_CTL_ASSIGN_COMMIT_GROUP:
+            group_op(c, g, 3, m.peer_slot, m.a[0]);
+            break;
+        case RAFTGPU_CTL_RESET_VOTES:
+            for (uint32_t k = 0; k < halves; k++) group_op(c, g + k, 4, 0, 0);
+            break;
+        case RAFTGPU_CTL_RECORD_VOTE:
+            group_op(c, g, 5, m.peer_slot, m.arg ? 2 : 1);
+            break;
+        case RAFTGPU_CTL_VOTE_RESULT:
+            value = static_cast<int32_t>(tally_group(c, g));
+            tallied = 1;
+            break;
+        case RAFTGPU_CTL_HAS_QUORUM:
+            value = quorum_group(c, g, 0, static_cast<uint32_t>(m.a[0]) & (halves == 2 ? 0xffffu : 0xffu));
+            break;
+        case RAFTGPU_CTL_QUORUM_RECENTLY_ACTIVE:
+            value = quorum_group(c, g, 1, m.peer_slot);
+            break;
+        case RAFTGPU_CTL_PROGRESS_OP:
+            value = progress_op_cell(c, g, m.peer_slot, m.arg, m.a[0], m.a[1], m.a[2]);
+            break;
+        }
+        res[t] = make_int2(status, value);
+    }
+    const uint32_t local[1] = {tallied};
+    const int which[1] = {kCntVotes};
+    block_flush_counts<1>(local, which, counters, nullptr);
 }
