@@ -675,8 +675,8 @@ int32_t raftgpu_step_wire_status(raftgpu_arena *arena, const uint8_t **status, u
  * records: pr.update_committed(m.commit), recent_active = true, resume(), a full inflights window of a
  * Replicate peer frees its first entry (INS_FULL clears), and the result byte says whether the reference would
  * call send_append: RAFTGPU_RES_OK | RAFTGPU_RES_SEND when pr.matched < last_index or a snapshot was requested
- * (raft.rs:1800-1803); RAFTGPU_RES_NO_PROGRESS for an unknown peer.  The read-index tail (:1806-1818) is not
- * on this path.  A heartbeat batch is its own pass, ordered by the caller between steps (it reads last_index,
+ * (raft.rs:1800-1803); RAFTGPU_RES_NO_PROGRESS for an unknown peer.  The read-index tail (:1806-1818) is
+ * raftgpu_read_index_ack over the same records (RAFTGPU_REC_READ_CTX, ignored here).  A heartbeat batch is its own pass, ordered by the caller between steps (it reads last_index,
  * which a step's LOCAL records write): "all heartbeat responses of the tick after its append responses" is
  * one of the delivery orders raft allows.  One record per (group, peer) cell; a second one is not applied,
  * gets result 0 and -- in the host form -- makes the call return RAFTGPU_ERR_INVALID.
@@ -711,6 +711,102 @@ int32_t raftgpu_arena_enable_inflights(raftgpu_arena *arena, uint32_t max_inflig
 /* One peer's window: *start, *count (inflights.rs:21-23) and, when buffer != NULL, its `capacity` ring entries. */
 int32_t raftgpu_inflights_get(raftgpu_arena *arena, uint32_t group, uint32_t peer_slot, uint32_t *start, uint32_t *count,
                               uint64_t *buffer, uint32_t capacity);
+
+/* ---- ReadIndex, ReadOnlyOption::Safe (SURVEY 8(f) rank 3, read side) -------- */
+
+/* The leader side of MsgReadIndex (raft.rs:2056-2091) and the read-index tail of Raft::handle_heartbeat_response
+ * (raft.rs:1805-1818) as batched device passes: each group's ReadOnly (read_only.rs:86-139) is a queue in HBM.
+ * Contexts are opaque bytes in the reference; here they are u64 context ids the caller assigns (equal bytes, equal
+ * id; 0 = no context, m.context.is_empty()), and the caller keeps id -> (bytes, original Message) for
+ * handle_ready_read_index (raft.rs:2790-2805).  A pending read's acks are a 16-bit peer-slot mask (a wide group's
+ * peer 8 + s is bit 8 + s); the self bit is set when it is queued.  Deviations from the reference, both documented
+ * in DESIGN.md 3.9: the queue holds at most max_pending reads (RAFTGPU_READ_FULL; the reference's is unbounded),
+ * and a peer removed by a configuration change loses its acks (a peer removed and re-added while a read is
+ * pending must ack again; this can delay a read, never release one early).  The queue of a wide group lives on
+ * its low half.
+ *
+ * Opt-in, like device-side Inflights: call before groups are allocated.  Memory: max_pending x 18 bytes + 16 per
+ * group slot (8 pending reads: about 160 bytes).  Arenas that do not call it behave exactly as without the feature;
+ * the step kernels never read the queues, so every step form (the fused tile kernels included) stays available. */
+#define RAFTGPU_READ_MAX_PENDING 64u
+int32_t raftgpu_arena_enable_read_index(raftgpu_arena *arena, uint32_t max_pending);
+
+/* RAFTGPU_REC_HEARTBEAT records with this flag carry the response's context id in `index` (0 = none).
+ * raftgpu_heartbeat_resp[_device] ignores the bit, so the tracker pass and the read pass can run over the same
+ * device buffer. */
+#define RAFTGPU_REC_READ_CTX 0x08u
+
+/* One MsgReadIndex at the leader: 16 bytes. */
+typedef struct {
+    uint32_t group;     /* the group id (the low half of a wide group) */
+    uint32_t reserved;
+    uint64_t ctx;       /* context id, non-zero */
+} raftgpu_read_req;
+/* One released read (ReadIndexStatus minus the message, read_only.rs:58-63): 24 bytes. */
+typedef struct {
+    uint32_t group;
+    uint32_t reserved;
+    uint64_t ctx;
+    uint64_t index;     /* the commit index the read was queued with */
+} raftgpu_read_state;
+
+/* per-request result byte */
+#define RAFTGPU_READ_QUEUED 1u   /* add_request: a new entry at the back of the queue, acks = {self} */
+#define RAFTGPU_READ_READY 2u    /* is_singleton(): released at once with index = committed (raft.rs:2064-2070) */
+#define RAFTGPU_READ_DUP 3u      /* the ctx is already pending: nothing changes (read_only.rs:89-91); the reference
+                                    still broadcasts the heartbeat */
+#define RAFTGPU_READ_DROPPED 4u  /* !commit_to_current_term() (raft.rs:2057-2062): term_start <= committed <=
+                                    last_index does not hold (a non-leader's requests are always dropped) */
+#define RAFTGPU_READ_FULL 5u     /* the queue already holds max_pending reads: resubmit after a release */
+#define RAFTGPU_READ_NO_GROUP 6u /* an unallocated group, or the high half of a wide group */
+#define RAFTGPU_READ_NO_CTX 7u   /* ctx == 0: 0 is "no context" and cannot be acked */
+
+/* Requests (raft.rs:2056-2091) for many groups: d_reqs in non-decreasing group order (queue order is arrival
+ * order), verified on the device before anything is applied -- on a violation nothing is applied, every result
+ * is 0 and *d_bad (u32, nullable) is bumped once.  d_results (n bytes, nullable) gets RAFTGPU_READ_*; READY reads
+ * go to d_released, *d_count (u64) = how many (zeroed here first).  capacity must be at least n
+ * (RAFTGPU_ERR_INVALID before any launch otherwise): a release cannot be regenerated.  Asynchronous on `stream`. */
+int32_t raftgpu_read_index_request_device(raftgpu_arena *arena, void *stream, const raftgpu_read_req *d_reqs, uint64_t n,
+                                          uint8_t *d_results, raftgpu_read_state *d_released, uint64_t capacity,
+                                          uint64_t *d_count, uint32_t *d_bad);
+/* Host form: copies, runs and waits; RAFTGPU_ERR_INVALID (nothing applied) when the requests are out of group
+ * order; *out_n = released reads copied to `released`. */
+int32_t raftgpu_read_index_request(raftgpu_arena *arena, const raftgpu_read_req *reqs, uint64_t n, uint8_t *results,
+                                   raftgpu_read_state *released, uint64_t capacity, uint64_t *out_n);
+
+/* The read-index tail of handle_heartbeat_response (raft.rs:1805-1818) for a batch of RAFTGPU_REC_HEARTBEAT |
+ * RAFTGPU_REC_READ_CTX records (every other record is ignored, and so is a responder without Progress or ctx 0):
+ * recv_ack (read_only.rs:104-110) ORs the responder's bit into its ctx's pending entry, then per group the last
+ * entry that a record named and whose acks have a quorum (ProgressTracker::has_quorum, tracker.rs:367-372) is
+ * advanced to (read_only.rs:115-129): it and every entry in front of it are released, contiguously and in queue
+ * order.
+ * Any number of records per cell, in any order: the result is what applying them one at a time in any order
+ * gives (DESIGN.md 3.9).  *d_count (u64) = released reads, zeroed here first.  capacity must be at least
+ * min(n, allocated groups) x max_pending (RAFTGPU_ERR_INVALID before any launch otherwise), so a release is never
+ * lost.  Asynchronous on `stream`. */
+int32_t raftgpu_read_index_ack_device(raftgpu_arena *arena, void *stream, const raftgpu_append_resp *d_records, uint64_t n,
+                                      raftgpu_read_state *d_released, uint64_t capacity, uint64_t *d_count);
+int32_t raftgpu_read_index_ack(raftgpu_arena *arena, const raftgpu_append_resp *records, uint64_t n,
+                               raftgpu_read_state *released, uint64_t capacity, uint64_t *out_n);
+
+/* The tail of post_conf_change (raft.rs:2648-2664) for the listed groups (a group listed twice counts once):
+ * recv_ack(self, last pending ctx) and, when the new configuration gives that entry a quorum, every pending read
+ * is released.  List only groups whose configuration just changed: on any other group it could release a read
+ * the reference would not.  capacity must be at least n x max_pending.  Synchronous. */
+int32_t raftgpu_read_index_recheck(raftgpu_arena *arena, const uint32_t *groups, uint64_t n, raftgpu_read_state *out,
+                                   uint64_t capacity, uint64_t *out_n);
+
+/* ReadOnly::last_pending_request_ctx (read_only.rs:132-135) for groups [first, first + n): the ctx bcast_heartbeat
+ * attaches (raft.rs:876), d_out[g - first] = 0 for none.  Asynchronous on `stream`. */
+int32_t raftgpu_read_index_last_ctx_device(raftgpu_arena *arena, void *stream, uint32_t first, uint32_t n, uint64_t *d_out);
+
+/* Inspection: one group's pending reads in queue order (*count = pending_read_count, raft.rs:437; up to
+ * `capacity` entries of ctx / index / acks, each nullable), and the same for groups [first, first + n) at once:
+ * counts[n], and ctx / index / acks as [n][max_pending] (group i's entry k at i * max_pending + k). */
+int32_t raftgpu_read_index_get(raftgpu_arena *arena, uint32_t group, uint32_t *count, uint64_t *ctx, uint64_t *index,
+                               uint16_t *acks, uint32_t capacity);
+int32_t raftgpu_read_index_read(raftgpu_arena *arena, uint32_t first, uint32_t n, uint32_t *counts, uint64_t *ctx,
+                                uint64_t *index, uint16_t *acks);
 
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 

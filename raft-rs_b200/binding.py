@@ -63,6 +63,14 @@ CTL_CMD_DTYPE = np.dtype([("group", "<u4"), ("op", "u1"), ("peer_slot", "u1"), (
 assert CTL_CMD_DTYPE.itemsize == 40
 CTL_RESULT_DTYPE = np.dtype([("status", "<i4"), ("value", "<i4")])
 assert CTL_RESULT_DTYPE.itemsize == 8
+# ReadIndex (ReadOnlyOption::Safe): requests, released reads, result bytes, the heartbeat record flag
+READ_REQ_DTYPE = np.dtype([("group", "<u4"), ("reserved", "<u4"), ("ctx", "<u8")])
+assert READ_REQ_DTYPE.itemsize == 16
+READ_STATE_DTYPE = np.dtype([("group", "<u4"), ("reserved", "<u4"), ("ctx", "<u8"), ("index", "<u8")])
+assert READ_STATE_DTYPE.itemsize == 24
+REC_READ_CTX = 0x08
+READ_QUEUED, READ_READY, READ_DUP, READ_DROPPED, READ_FULL, READ_NO_GROUP, READ_NO_CTX = range(1, 8)
+READ_MAX_PENDING = 64
 
 # host column name -> (column id, numpy dtype, per-peer?)
 COLUMNS = {
@@ -282,6 +290,15 @@ def lib() -> C.CDLL:
             "raftgpu_inflights_get": ([vp, u32, u32, C.POINTER(u32), C.POINTER(u32), vp, u32], i32),
             "raftgpu_heartbeat_resp_device": ([vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_heartbeat_resp": ([vp, vp, u64, vp], i32),
+            "raftgpu_arena_enable_read_index": ([vp, u32], i32),
+            "raftgpu_read_index_request_device": ([vp, vp, vp, u64, vp, vp, u64, vp, vp], i32),
+            "raftgpu_read_index_request": ([vp, vp, u64, vp, vp, u64, C.POINTER(u64)], i32),
+            "raftgpu_read_index_ack_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
+            "raftgpu_read_index_ack": ([vp, vp, u64, vp, u64, C.POINTER(u64)], i32),
+            "raftgpu_read_index_recheck": ([vp, vp, u64, vp, u64, C.POINTER(u64)], i32),
+            "raftgpu_read_index_last_ctx_device": ([vp, vp, u32, u32, vp], i32),
+            "raftgpu_read_index_get": ([vp, u32, C.POINTER(u32), vp, vp, vp, u32], i32),
+            "raftgpu_read_index_read": ([vp, u32, u32, vp, vp, vp, vp], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -720,6 +737,63 @@ class Arena:
         res = np.zeros(len(recs), dtype=np.uint8)
         self._ck(self._L.raftgpu_heartbeat_resp(self._h, recs.ctypes.data, len(recs), res.ctypes.data), "heartbeat_resp")
         return res
+
+    # -- ReadIndex, ReadOnlyOption::Safe (include/raftgpu.h)
+    def enable_read_index(self, max_pending: int = 8):
+        self._ck(self._L.raftgpu_arena_enable_read_index(self._h, max_pending), "arena_enable_read_index")
+        self.read_max_pending = max_pending
+
+    def read_index_request(self, reqs: np.ndarray):
+        """raftgpu_read_index_request: READ_REQ_DTYPE requests in group order -> (result bytes, released reads)."""
+        assert reqs.dtype == READ_REQ_DTYPE and reqs.flags.c_contiguous
+        res = np.zeros(len(reqs), dtype=np.uint8)
+        out = np.zeros(max(1, len(reqs)), dtype=READ_STATE_DTYPE)
+        n = C.c_uint64()
+        self._ck(self._L.raftgpu_read_index_request(self._h, reqs.ctypes.data, len(reqs), res.ctypes.data, out.ctypes.data,
+                                                    len(reqs), C.byref(n)), "read_index_request")
+        return res, out[: n.value]
+
+    def read_index_ack(self, recs: np.ndarray) -> np.ndarray:
+        """raftgpu_read_index_ack: HEARTBEAT | READ_CTX records (index = ctx id) -> released reads."""
+        assert recs.dtype == APPEND_RESP_DTYPE and recs.flags.c_contiguous
+        cap = min(len(recs), self.get_info().n_alloc) * self.read_max_pending
+        out = np.zeros(max(1, cap), dtype=READ_STATE_DTYPE)
+        n = C.c_uint64()
+        self._ck(self._L.raftgpu_read_index_ack(self._h, recs.ctypes.data, len(recs), out.ctypes.data, cap, C.byref(n)),
+                 "read_index_ack")
+        return out[: n.value]
+
+    def read_index_recheck(self, groups) -> np.ndarray:
+        """raftgpu_read_index_recheck: post_conf_change's read tail for the listed groups -> released reads."""
+        g = np.ascontiguousarray(groups, dtype=np.uint32)
+        cap = len(g) * self.read_max_pending
+        out = np.zeros(max(1, cap), dtype=READ_STATE_DTYPE)
+        n = C.c_uint64()
+        self._ck(self._L.raftgpu_read_index_recheck(self._h, g.ctypes.data, len(g), out.ctypes.data, cap, C.byref(n)),
+                 "read_index_recheck")
+        return out[: n.value]
+
+    def read_index_last_ctx_device(self, first, n, d_out, stream=None):
+        self._ck(self._L.raftgpu_read_index_last_ctx_device(self._h, stream, first, n, d_out), "read_index_last_ctx_device")
+
+    def read_index_get(self, g):
+        """One group's pending reads in queue order: (ctx u64[], index u64[], acks u16[])."""
+        P = self.read_max_pending
+        cnt = C.c_uint32()
+        ctx, idx, acks = np.zeros(P, np.uint64), np.zeros(P, np.uint64), np.zeros(P, np.uint16)
+        self._ck(self._L.raftgpu_read_index_get(self._h, g, C.byref(cnt), ctx.ctypes.data, idx.ctypes.data, acks.ctypes.data, P),
+                 "read_index_get")
+        k = cnt.value
+        return ctx[:k], idx[:k], acks[:k]
+
+    def read_index_read(self, first, n):
+        """Groups [first, first + n) at once: (counts u32[n], ctx / index u64[n][P], acks u16[n][P]), queue order."""
+        P = self.read_max_pending
+        cnt = np.zeros(n, np.uint32)
+        ctx, idx, acks = np.zeros((n, P), np.uint64), np.zeros((n, P), np.uint64), np.zeros((n, P), np.uint16)
+        self._ck(self._L.raftgpu_read_index_read(self._h, first, n, cnt.ctypes.data, ctx.ctypes.data, idx.ctypes.data,
+                                                 acks.ctypes.data), "read_index_read")
+        return cnt, ctx, idx, acks
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

@@ -244,6 +244,11 @@ struct raftgpu_arena {
     // raftgpu_control scratch, kept between calls: per group (pair), the commands staged in the current chunk and
     // its running meta; per command of the chunk, its wave (kCtlSkip = not staged) and, in wave order, its index
     std::vector<uint32_t> ctl_count, ctl_meta, ctl_wave, ctl_order;
+    // ReadIndex (raftgpu_arena_enable_read_index): the ack pass's per-group mask of the ring positions its acks named
+    // [cap] (zero between passes) and touched-group list [cap]; rq_flag[0] = the request pass's order violation,
+    // rq_flag[1] = the touched list's length
+    unsigned long long *rq_hit = nullptr;
+    uint32_t *rq_list = nullptr, *rq_flag = nullptr;
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -569,6 +574,13 @@ void destroy(raftgpu_arena *a) {
     cudaFree(c.term);
     cudaFree(c.ins_meta);
     cudaFree(c.ins_buf);
+    cudaFree(c.rq_hc);
+    cudaFree(c.rq_ctx);
+    cudaFree(c.rq_index);
+    cudaFree(c.rq_acks);
+    cudaFree(a->rq_hit);
+    cudaFree(a->rq_list);
+    cudaFree(a->rq_flag);
     cudaFree(a->d_wire_first);
     cudaFree(a->d_counters);
     cudaFree(a->d_scratch);
@@ -724,6 +736,14 @@ int32_t sync_op(raftgpu_arena *a, F &&launch) {
     CKL(a);
     CK(a, cudaStreamSynchronize(a->s_compute));
     return RAFTGPU_OK;
+}
+
+// ReadIndex queues (arenas with raftgpu_arena_enable_read_index only): groups [first, first + n) become allocated with
+// an empty queue (value = kRqAlloc) or free (0).
+int32_t read_mark(raftgpu_arena *a, uint32_t first, uint32_t n, uint32_t value) {
+    if (!a->cols.rq_cap || n == 0) return RAFTGPU_OK;
+    const uint32_t blocks = std::min<uint32_t>(div_up(n, 256), 8u * static_cast<uint32_t>(a->sm_count));
+    return sync_op(a, [&](cudaStream_t st) { read_mark_kernel<<<blocks, 256, 0, st>>>(a->cols.rq_hc, first, n, value); });
 }
 
 struct ColumnDesc {
@@ -966,5 +986,6 @@ extern "C" {
 #include "abi_compact.inc"
 #include "abi_wire.inc"
 #include "abi_results.inc"
+#include "abi_read.inc"
 
 }  // extern "C"

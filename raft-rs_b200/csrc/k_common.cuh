@@ -29,6 +29,13 @@ struct Columns {
     uint32_t ins_cap;
     uint32_t *ins_meta;
     uint64_t *ins_buf;
+    // ReadIndex queues (raftgpu_arena_enable_read_index, k_read.cuh): rq_cap = max_pending, 0 = off; rq_hc [cap] =
+    // head | count << 8 | kRqAlloc; rq_ctx / rq_index / rq_acks [rq_cap][cap] the ring entries (read_only.rs:58-63)
+    uint32_t rq_cap;
+    uint32_t *rq_hc;
+    uint64_t *rq_ctx;
+    uint64_t *rq_index;
+    uint16_t *rq_acks;
 };
 
 enum Counter : int {
@@ -182,6 +189,35 @@ __device__ __forceinline__ bool ins_add(const Columns &c, size_t cell, uint64_t 
     c.ins_meta[cell] = start | ((count + 1) << 16);
     if (count + 1 == c.ins_cap) flags |= RAFTGPU_PF_INS_FULL;
     return true;
+}
+
+// ---------------------------------------------------------------------------
+// ReadIndex queues (src/read_only.rs), when the arena keeps them (Columns::rq_cap != 0).  A group's queue is a ring
+// of rq_cap entries; its word rq_hc holds the front's position, the entry count and kRqAlloc (the group slot is
+// allocated: group alloc / free set and clear it).  The kernels are in k_read.cuh; the control-plane hooks below.
+constexpr uint32_t kRqAlloc = 0x80000000u;
+__device__ __forceinline__ uint32_t rq_count(uint32_t hc) { return (hc >> 8) & 0xffu; }
+// the cell of queue entry k (0 = the front) of group g
+__device__ __forceinline__ size_t rq_at(const Columns &c, uint32_t g, uint32_t hc, uint32_t k) {
+    uint32_t p = (hc & 0xffu) + k;
+    if (p >= c.rq_cap) p -= c.rq_cap;
+    return static_cast<size_t>(p) * c.cap + g;
+}
+// Raft::reset replaces the ReadOnly (raft.rs:957): the queue is emptied
+__device__ __forceinline__ void rq_reset(const Columns &c, uint32_t g) {
+    if (c.rq_cap) c.rq_hc[g] &= kRqAlloc;
+}
+// apply_conf removed the peers `removed` of half g (new meta `meta`): their bits leave every pending read's acks, so
+// that a slot reused for a new peer does not inherit an old ack (DESIGN 3.9)
+__device__ __forceinline__ void rq_conf_removed(const Columns &c, uint32_t g, uint32_t meta, uint32_t removed) {
+    if (!c.rq_cap || !removed) return;
+    const bool hi = (meta & RAFTGPU_META_WIDE_HI) != 0;
+    const uint32_t qg = hi ? g - 1 : g, keep = ~(removed << (hi ? 8 : 0));
+    const uint32_t hc = c.rq_hc[qg];
+    for (uint32_t k = 0; k < rq_count(hc); k++) {
+        uint16_t *p = &c.rq_acks[rq_at(c, qg, hc, k)];
+        *p = static_cast<uint16_t>(*p & keep);
+    }
 }
 
 // ---------------------------------------------------------------------------

@@ -274,6 +274,7 @@ __device__ __forceinline__ void conf_group(const Columns &c, uint32_t g, uint32_
         }
     }
     c.meta[g] = new_meta;
+    rq_conf_removed(c, g, new_meta, removed);
 }
 __global__ void conf_kernel(Columns c, uint32_t g, uint32_t new_meta, uint32_t added,
                             uint32_t removed, uint64_t next_idx) {
@@ -307,6 +308,7 @@ __device__ __forceinline__ void reset_group(const Columns &c, uint32_t g, uint64
     c.committed[g] = committed;
     c.term_start[g] = term_start;
     c.last_index[g] = last_index;
+    rq_reset(c, g);  // raft.rs:957 read_only = ReadOnly::new(..)
 }
 __global__ void reset_kernel(Columns c, uint32_t g, uint64_t term_start, uint64_t last_index,
                              uint64_t committed, uint64_t persisted) {

@@ -21,6 +21,7 @@ namespace raftgpu {
 #include "k_tile.cuh"
 #include "k_tile_compact.cuh"
 #include "k_control.cuh"
+#include "k_read.cuh"
 #include "k_wire.cuh"
 
 }  // namespace raftgpu
