@@ -643,6 +643,8 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
 #define RAFTGPU_WIRE_MALFORMED 4u  /* not a protobuf message, a bad frame, or a group that is not allocated */
 #define RAFTGPU_WIRE_DUP 5u        /* a later frame of a (group, peer) cell that already has one in this batch: cells are
                                       applied in arrival order, one message per step -- resubmit it with the next batch */
+#define RAFTGPU_WIRE_CONTEXT 6u    /* (raftgpu_heartbeat_wire only) a context that is not an 8-byte read id, or any context
+                                      on an arena without read queues: the host's own ReadOnly handles the frame */
 typedef struct raftgpu_wire_batch {
     const uint8_t *bytes;    /* the frames, back to back */
     uint64_t n_bytes;
@@ -807,6 +809,38 @@ int32_t raftgpu_read_index_get(raftgpu_arena *arena, uint32_t group, uint32_t *c
                                uint16_t *acks, uint32_t capacity);
 int32_t raftgpu_read_index_read(raftgpu_arena *arena, uint32_t first, uint32_t n, uint32_t *counts, uint64_t *ctx,
                                 uint64_t *index, uint16_t *acks);
+
+/* ---- heartbeat responses from the wire ---------------------------------------- */
+
+/* Raft::handle_heartbeat_response (raft.rs:1777-1819) for the MsgHeartbeatResponse frames (msg_type 9) of a wire
+ * batch, in the format of raftgpu_wire_batch (u32 LE group << 4 | peer_slot, then the serialized Message; peer
+ * 8 + s of a wide group is cell (g + 1, s)).  The context of a heartbeat that carries read id x is the 8 bytes of x,
+ * little-endian (the caller builds the heartbeat; the follower echoes its context, raft.rs:2461).  Field 12 decodes
+ * as a parser does: the last length-delimited occurrence wins, a varint field 12 is skipped.  Per frame:
+ *   - no context: the tracker part, exactly raftgpu_heartbeat_resp for a RAFTGPU_REC_HEARTBEAT record with
+ *     commit = m.commit;
+ *   - an 8-byte context on an arena with read queues: the tracker part, and the read part, exactly
+ *     raftgpu_read_index_ack for the same record with RAFTGPU_REC_READ_CTX and the id in `index` (id 0 acks nothing);
+ *   - any other context, or any context on an arena without read queues: RAFTGPU_WIRE_CONTEXT, nothing applied.
+ * status[i] = RAFTGPU_WIRE_* << 4 | RAFTGPU_RES_* (RAFTGPU_RES_OK [| RAFTGPU_RES_SEND] or RAFTGPU_RES_NO_PROGRESS for
+ * an applied frame).  RAFTGPU_WIRE_SKIP_TYPE for every other message type (MsgAppendResponse included: the same
+ * bytes can go through raftgpu_wire_apply_device as well, and each frame is applied by exactly one of the two),
+ * RAFTGPU_WIRE_TERM, RAFTGPU_WIRE_MALFORMED and RAFTGPU_WIRE_DUP (a later frame of a cell that already has one in the
+ * batch) as for the AppendResponse path.  A frame is applied whole or not at all: a DUP, TERM, CONTEXT or MALFORMED
+ * frame touches neither the tracker nor the read queue; the host may deliver it later.  Like raftgpu_heartbeat_resp,
+ * the pass runs between steps (it reads last_index).
+ * Released reads go to d_released, *d_count (u64) = how many, zeroed here first; capacity must be at least
+ * min(n, allocated groups) x max_pending (RAFTGPU_ERR_INVALID before any launch otherwise).  On an arena without read
+ * queues d_released / capacity / d_count may be NULL / 0.  d_bytes 16-byte aligned, n and n_bytes below 4 GiB.
+ * Asynchronous on `stream`.  The pass keeps its own decode scratch (not a staging set's) and shares the read
+ * passes' per-group scratch: run it on one stream with the other read-index passes. */
+int32_t raftgpu_heartbeat_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                      const uint32_t *d_offsets, uint64_t n, uint8_t *d_status,
+                                      raftgpu_read_state *d_released, uint64_t capacity, uint64_t *d_count);
+/* Host form: copies, runs and waits; status (n bytes) nullable; *out_n = released reads copied to `released`
+ * (released / capacity / out_n may be NULL / 0 on an arena without read queues). */
+int32_t raftgpu_heartbeat_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets, uint64_t n,
+                               uint8_t *status, raftgpu_read_state *released, uint64_t capacity, uint64_t *out_n);
 
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 

@@ -48,6 +48,13 @@ int32_t raftgpu_synth_wire_encode(const raftgpu_append_resp *recs, uint64_t n, c
                                   uint64_t bytes_cap, uint32_t *out_offsets, uint64_t *out_n_frames, uint64_t *out_n_bytes,
                                   raftgpu_append_resp *out_local, uint64_t *out_n_local);
 
+/* RAFTGPU_REC_HEARTBEAT records -> MsgHeartbeatResponse frames, one per such record in record order (others are
+ * skipped): msg_type 9, term (term[group], NULL = 1), commit, and for a RAFTGPU_REC_READ_CTX record with a non-zero
+ * ctx id (`index`) the context = the id's 8 bytes, little-endian.  out_offsets has room for n + 1 entries. */
+int32_t raftgpu_synth_wire_encode_heartbeats(const raftgpu_append_resp *recs, uint64_t n, const uint64_t *term,
+                                             uint8_t *out_bytes, uint64_t bytes_cap, uint32_t *out_offsets,
+                                             uint64_t *out_n_frames, uint64_t *out_n_bytes);
+
 #ifdef __cplusplus
 }
 #endif

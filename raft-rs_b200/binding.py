@@ -43,7 +43,7 @@ BULK_SORTED = 0x1
 (COL_MATCHED, COL_NEXT_IDX, COL_PEER_COMMITTED, COL_PENDING_SNAPSHOT, COL_PENDING_REQ_SNAPSHOT,
  COL_COMMIT_GROUP_ID, COL_PFLAGS, COL_VOTES, COL_META, COL_COMMITTED, COL_TERM_START,
  COL_LAST_INDEX, COL_TERM, COL_INS_META) = range(14)
-WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP = range(6)
+WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WIRE_CONTEXT = range(7)
 
 APPEND_RESP_DTYPE = np.dtype(
     [("group", "<u4"), ("peer_slot", "u1"), ("flags", "u1"), ("reserved", "<u2"),
@@ -299,6 +299,8 @@ def lib() -> C.CDLL:
             "raftgpu_read_index_last_ctx_device": ([vp, vp, u32, u32, vp], i32),
             "raftgpu_read_index_get": ([vp, u32, C.POINTER(u32), vp, vp, vp, u32], i32),
             "raftgpu_read_index_read": ([vp, u32, u32, vp, vp, vp, vp], i32),
+            "raftgpu_heartbeat_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, u64, vp], i32),
+            "raftgpu_heartbeat_wire": ([vp, vp, u64, vp, u64, vp, vp, u64, C.POINTER(u64)], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -337,6 +339,8 @@ def synth_lib() -> C.CDLL:
         L.raftgpu_synth_round.restype = i32
         L.raftgpu_synth_wire_encode.argtypes = [vp, u64, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64), vp, C.POINTER(u64)]
         L.raftgpu_synth_wire_encode.restype = i32
+        L.raftgpu_synth_wire_encode_heartbeats.argtypes = [vp, u64, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+        L.raftgpu_synth_wire_encode_heartbeats.restype = i32
         _synth_lib = L
     return _synth_lib
 
@@ -794,6 +798,24 @@ class Arena:
         self._ck(self._L.raftgpu_read_index_read(self._h, first, n, cnt.ctypes.data, ctx.ctypes.data, idx.ctypes.data,
                                                  acks.ctypes.data), "read_index_read")
         return cnt, ctx, idx, acks
+
+    def heartbeat_wire(self, batch):
+        """raftgpu_heartbeat_wire: the MsgHeartbeatResponse frames of a wire batch (.bytes, .n_bytes, .offsets, .n, e.g.
+        wire.WireBuffers) -> (status bytes WIRE_* << 4 | RES_*, released reads; empty without read queues)."""
+        status = np.zeros(batch.n, dtype=np.uint8)
+        P = getattr(self, "read_max_pending", 0)
+        cap = min(batch.n, self.get_info().n_alloc) * P
+        out = np.zeros(max(1, cap), dtype=READ_STATE_DTYPE)
+        n = C.c_uint64()
+        self._ck(self._L.raftgpu_heartbeat_wire(self._h, batch.bytes.ctypes.data, batch.n_bytes, batch.offsets.ctypes.data,
+                                                batch.n, status.ctypes.data, out.ctypes.data if cap else None, cap,
+                                                C.byref(n)), "heartbeat_wire")
+        return status, out[: n.value]
+
+    def heartbeat_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_status, d_released=None, capacity=0, d_count=None,
+                              stream=None):
+        self._ck(self._L.raftgpu_heartbeat_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_status, d_released,
+                                                       capacity, d_count), "heartbeat_wire_device")
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

@@ -249,6 +249,10 @@ struct raftgpu_arena {
     // rq_flag[1] = the touched list's length
     unsigned long long *rq_hit = nullptr;
     uint32_t *rq_list = nullptr, *rq_flag = nullptr;
+    // raftgpu_heartbeat_wire (allocated on first use): first frame of every cell [kSlots][cap], one record per frame
+    uint32_t *hbw_first = nullptr;
+    raftgpu_append_resp *hbw_recs = nullptr;
+    uint64_t hbw_recs_cap = 0;
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -582,6 +586,8 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->rq_list);
     cudaFree(a->rq_flag);
     cudaFree(a->d_wire_first);
+    cudaFree(a->hbw_first);
+    cudaFree(a->hbw_recs);
     cudaFree(a->d_counters);
     cudaFree(a->d_scratch);
     cudaFreeHost(a->h_scratch);
@@ -987,5 +993,6 @@ extern "C" {
 #include "abi_wire.inc"
 #include "abi_results.inc"
 #include "abi_read.inc"
+#include "abi_hb_wire.inc"
 
 }  // extern "C"

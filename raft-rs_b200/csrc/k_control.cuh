@@ -109,6 +109,35 @@ heartbeat_commit_kernel(Columns c, uint32_t first, uint32_t n, uint64_t *__restr
 // pr.matched < last_index || pending_request_snapshot != INVALID_INDEX (:1800-1803).  A scatter pass by
 // nature (the records name the cells); one record per cell, verified through `touched` like the other
 // zero-copy paths (a second record for a cell is not applied and bumps *dup_count).
+//
+// heartbeat_resp_one is the body for one response from (g, slot) with commit = m.commit, shared with the wire form
+// (k_hb_wire.cuh).  `claim()` runs once the responder is known to have a Progress and says whether this response
+// may take the cell (false: a second response of the batch, not applied, result 0).
+template <typename Claim>
+__device__ __forceinline__ uint32_t heartbeat_resp_one(const Columns &c, uint32_t g, uint32_t slot, uint64_t commit,
+                                                       Claim &&claim) {
+    const bool in_range = g < c.cap && slot < kSlots;
+    const uint32_t meta = in_range ? c.meta[g] : 0u;
+    const uint32_t present = RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta);
+    if (!in_range || !((present >> slot) & 1u)) return RAFTGPU_RES_NO_PROGRESS;  // raft.rs:1779-1789
+    if (!claim()) return 0u;
+    const size_t cell = static_cast<size_t>(slot) * c.cap + g;
+    const uint32_t f0 = c.pflags[cell];
+    uint32_t f = (f0 | RAFTGPU_PF_RECENT_ACTIVE) & ~RAFTGPU_PF_PAUSED;          // :1792-1793
+    if ((f0 & RAFTGPU_PF_STATE_MASK) == RAFTGPU_STATE_REPLICATE) {  // :1796-1798
+        if (!c.ins_cap)
+            f &= ~RAFTGPU_PF_INS_FULL;  // host-side windows: a full one that loses an entry is not full
+        else if (f0 & RAFTGPU_PF_INS_FULL)
+            ins_free_first_one(c, cell, f);
+    }
+    hot_update_committed(c, hot_ptrs(c, cell), commit);                          // :1791
+    if (f != f0) c.pflags[cell] = static_cast<uint8_t>(f);
+    uint32_t res = RAFTGPU_RES_OK;
+    if (c.matched[cell] < c.last_index[g] || c.pending_req_snapshot[cell] != RAFTGPU_INVALID_INDEX)
+        res |= RAFTGPU_RES_SEND;                                                // :1800-1803
+    return res;
+}
+
 __global__ void __launch_bounds__(256)
 heartbeat_resp_kernel(Columns c, const raftgpu_append_resp *__restrict__ recs, uint64_t n, uint8_t *__restrict__ results,
                       uint32_t *__restrict__ touched, uint32_t *__restrict__ dup_count) {
@@ -120,32 +149,14 @@ heartbeat_resp_kernel(Columns c, const raftgpu_append_resp *__restrict__ recs, u
         const uint32_t rflags = static_cast<uint32_t>(w0 >> 40) & 0xffu;
         uint32_t res = 0;
         if (rflags & RAFTGPU_REC_HEARTBEAT) {
-            const bool in_range = g < c.cap && slot < kSlots;
-            const uint32_t meta = in_range ? c.meta[g] : 0u;
-            const uint32_t present = RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta);
-            if (!in_range || !((present >> slot) & 1u)) {
-                res = RAFTGPU_RES_NO_PROGRESS;  // raft.rs:1779-1789
-            } else {
+            res = heartbeat_resp_one(c, g, slot, commit, [&]() {
                 const uint32_t bit = 1u << (8 * (g & 3u) + slot);
                 if (touched && (atomicOr(&touched[g >> 2], bit) & bit)) {
                     if (dup_count) atomicAdd(dup_count, 1u);
-                } else {
-                    const size_t cell = static_cast<size_t>(slot) * c.cap + g;
-                    const uint32_t f0 = c.pflags[cell];
-                    uint32_t f = (f0 | RAFTGPU_PF_RECENT_ACTIVE) & ~RAFTGPU_PF_PAUSED;          // :1792-1793
-                    if ((f0 & RAFTGPU_PF_STATE_MASK) == RAFTGPU_STATE_REPLICATE) {  // :1796-1798
-                        if (!c.ins_cap)
-                            f &= ~RAFTGPU_PF_INS_FULL;  // host-side windows: a full one that loses an entry is not full
-                        else if (f0 & RAFTGPU_PF_INS_FULL)
-                            ins_free_first_one(c, cell, f);
-                    }
-                    hot_update_committed(c, hot_ptrs(c, cell), commit);                          // :1791
-                    if (f != f0) c.pflags[cell] = static_cast<uint8_t>(f);
-                    res = RAFTGPU_RES_OK;
-                    if (c.matched[cell] < c.last_index[g] || c.pending_req_snapshot[cell] != RAFTGPU_INVALID_INDEX)
-                        res |= RAFTGPU_RES_SEND;                                                // :1800-1803
+                    return false;
                 }
-            }
+                return true;
+            });
         }
         if (results) results[i] = static_cast<uint8_t>(res);
     }

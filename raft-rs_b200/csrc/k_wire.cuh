@@ -33,6 +33,7 @@ struct WireMsg {  // the scalar fields this path looks at
     uint32_t msg_type;
     bool reject;
     uint64_t term, log_term, index, commit, reject_hint, request_snapshot;
+    uint32_t ctx_off, ctx_len;  // wire_decode<true> only: bytes [ctx_off, ctx_off + ctx_len) are the last context (12)
 };
 
 constexpr uint32_t kWireThreads = 256;
@@ -52,11 +53,14 @@ __device__ __forceinline__ bool wire_varint(const uint8_t *p, uint32_t &pos, uin
     return false;
 }
 
-// One serialized Message -> WireMsg.  false = not a well-formed protobuf message.
+// One serialized Message -> WireMsg.  false = not a well-formed protobuf message.  kContext: also the context's
+// position (the heartbeat-response path, k_hb_wire.cuh); the AppendResponse kernels instantiate it without.
+template <bool kContext = false>
 __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, WireMsg &m) {
     m.msg_type = 0;
     m.reject = false;
     m.term = m.log_term = m.index = m.commit = m.reject_hint = m.request_snapshot = 0;
+    if constexpr (kContext) m.ctx_off = m.ctx_len = 0;
     uint32_t pos = 0;
     while (pos < len) {
         uint64_t tag;
@@ -84,6 +88,12 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
         } else if (wt == 2) {
             uint64_t l;
             if (!wire_varint(p, pos, len, 10, l) || l > len - pos) return false;
+            if constexpr (kContext) {
+                if (field == 12) {  // bytes context = 12; a repeated one keeps its last value, as a parser does
+                    m.ctx_off = pos;
+                    m.ctx_len = static_cast<uint32_t>(l);
+                }
+            }
             pos += static_cast<uint32_t>(l);
         } else {
             return false;  // groups (3, 4) are not proto3; 6, 7 do not exist
@@ -119,17 +129,27 @@ __device__ __forceinline__ WireStage wire_stage_block(const WireSrc &w, uint32_t
     return s;
 }
 
+// Frame i's bytes (from the stage when they are there), its length and its u32 LE header; nullptr = not a frame
+// (offsets out of order or past the batch, shorter than the header).
+__device__ __forceinline__ const uint8_t *wire_frame_at(const WireSrc &w, const WireStage &s, const uint8_t *stage, uint32_t i,
+                                                        uint32_t &hdr, uint32_t &len) {
+    const uint32_t a = w.offsets[i], b = w.offsets[i + 1];
+    if (b < a || b > w.n_bytes || b - a < 4u) return nullptr;
+    const uint8_t *p = (s.staged && a >= s.lo && b <= s.hi) ? stage + (a - s.base) : w.bytes + a;
+    hdr = p[0] | (static_cast<uint32_t>(p[1]) << 8) | (static_cast<uint32_t>(p[2]) << 16) | (static_cast<uint32_t>(p[3]) << 24);
+    len = b - a;
+    return p;
+}
+
 // Frame i: its status before the duplicate rule, the record, the REJECT's hint / request_snapshot.
 __device__ __forceinline__ uint32_t wire_frame(const Columns &c, const WireSrc &w, const WireStage &s, const uint8_t *stage,
                                                uint32_t i, RecRegs &rec, uint64_t &hint, uint64_t &request_snapshot) {
-    const uint32_t a = w.offsets[i], b = w.offsets[i + 1];
-    if (b < a || b > w.n_bytes || b - a < 4u) return RAFTGPU_WIRE_MALFORMED;
-    const uint8_t *p = (s.staged && a >= s.lo && b <= s.hi) ? stage + (a - s.base) : w.bytes + a;
-    const uint32_t hdr = p[0] | (static_cast<uint32_t>(p[1]) << 8) | (static_cast<uint32_t>(p[2]) << 16) |
-                         (static_cast<uint32_t>(p[3]) << 24);
+    uint32_t hdr, len;
+    const uint8_t *p = wire_frame_at(w, s, stage, i, hdr, len);
+    if (!p) return RAFTGPU_WIRE_MALFORMED;
     const uint32_t group = hdr >> 4, slot = hdr & 15u;
     WireMsg m;
-    if (group >= w.n_groups || !wire_decode(p + 4, b - a - 4u, m)) return RAFTGPU_WIRE_MALFORMED;
+    if (group >= w.n_groups || !wire_decode(p + 4, len - 4u, m)) return RAFTGPU_WIRE_MALFORMED;
     if (m.msg_type != 4u) return RAFTGPU_WIRE_SKIP_TYPE;  // MsgAppendResponse, eraftpb.proto:54
     const uint64_t gterm = c.term[group];
     if (gterm != 0 && m.term != gterm) return RAFTGPU_WIRE_TERM;

@@ -23,5 +23,6 @@ namespace raftgpu {
 #include "k_control.cuh"
 #include "k_read.cuh"
 #include "k_wire.cuh"
+#include "k_hb_wire.cuh"
 
 }  // namespace raftgpu

@@ -218,4 +218,38 @@ int32_t raftgpu_synth_wire_encode(const raftgpu_append_resp *recs, uint64_t n, c
     return RAFTGPU_OK;
 }
 
+// Heartbeat responses as a transport holds them: every RAFTGPU_REC_HEARTBEAT record becomes a MsgHeartbeatResponse
+// (handle_heartbeat, raft.rs:2452-2464: term, commit, the heartbeat's context echoed); the ctx id of a
+// RAFTGPU_REC_READ_CTX record is the context, 8 bytes little-endian, when it is non-zero.
+int32_t raftgpu_synth_wire_encode_heartbeats(const raftgpu_append_resp *recs, uint64_t n, const uint64_t *term,
+                                             uint8_t *out_bytes, uint64_t bytes_cap, uint32_t *out_offsets,
+                                             uint64_t *out_n_frames, uint64_t *out_n_bytes) {
+    if ((!recs && n) || !out_bytes || !out_offsets || !out_n_frames || !out_n_bytes) return RAFTGPU_ERR_INVALID;
+    uint64_t nf = 0;
+    uint8_t *p = out_bytes;
+    out_offsets[0] = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        const raftgpu_append_resp &r = recs[i];
+        if (!(r.flags & RAFTGPU_REC_HEARTBEAT)) continue;
+        if (static_cast<uint64_t>(p - out_bytes) + 64 > bytes_cap) return RAFTGPU_ERR_FULL;
+        const uint32_t hdr = (r.group << 4) | (r.peer_slot & 15u);
+        memcpy(p, &hdr, 4);
+        p += 4;
+        p = put_field(p, 1, 9);                                     // msg_type = MsgHeartbeatResponse
+        p = put_field(p, 2, 1);                                     // to: the leader
+        p = put_field(p, 3, static_cast<uint64_t>(r.peer_slot) + 1); // from
+        p = put_field(p, 4, term ? term[r.group] : 1);              // term
+        p = put_field(p, 8, r.commit);                              // commit
+        if ((r.flags & RAFTGPU_REC_READ_CTX) && r.index) {
+            *p++ = (12u << 3) | 2u;                                 // context, length-delimited
+            *p++ = 8;
+            for (int k = 0; k < 8; k++) *p++ = static_cast<uint8_t>(r.index >> (8 * k));
+        }
+        out_offsets[++nf] = static_cast<uint32_t>(p - out_bytes);
+    }
+    *out_n_frames = nf;
+    *out_n_bytes = static_cast<uint64_t>(p - out_bytes);
+    return RAFTGPU_OK;
+}
+
 }  // extern "C"

@@ -40,6 +40,18 @@ class WireBuffers:
         self.n, self.n_bytes, self.n_records = nf.value, nb.value, nl.value
         return self
 
+    def encode_heartbeats(self, recs: np.ndarray, term: np.ndarray | None = None):
+        """REC_HEARTBEAT records -> MsgHeartbeatResponse frames, one per record in order (term, commit, and the ctx id of a
+        REC_READ_CTX record as an 8-byte little-endian context when it is non-zero); returns self."""
+        nf, nb = C.c_uint64(), C.c_uint64()
+        rc = B.synth_lib().raftgpu_synth_wire_encode_heartbeats(
+            recs.ctypes.data, len(recs), None if term is None else term.ctypes.data, self.bytes.ctypes.data,
+            len(self.bytes), self.offsets.ctypes.data, C.byref(nf), C.byref(nb))
+        if rc != B.OK:
+            raise B.RaftGpuError(rc, "raftgpu_synth_wire_encode_heartbeats")
+        self.n, self.n_bytes, self.n_records = nf.value, nb.value, 0
+        return self
+
     def set_frames(self, frames: list[bytes], records: np.ndarray | None = None):
         """Arbitrary frames (tests): each already starts with its 4-byte header."""
         blob = b"".join(frames)
