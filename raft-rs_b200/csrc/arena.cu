@@ -985,8 +985,8 @@ int32_t run_step(raftgpu_arena *a, const char *form, uint32_t flags, Queue &&que
 // ===========================================================================
 extern "C" {
 
-#include "abi_control.inc"
 #include "abi_control_batch.inc"
+#include "abi_control.inc"
 #include "abi_device.inc"
 #include "abi_staging.inc"
 #include "abi_compact.inc"

@@ -1,4 +1,5 @@
-// k_control.cuh -- send_list_kernel, tally_kernel and the single-group control-plane kernels.
+// k_control.cuh -- send_list_kernel, the heartbeat and update_state passes, tally_kernel, and the control plane:
+// control_cmd, run by control_kernel (a list) and control_one_kernel (a single-group call).
 // Part of kernels.cuh (included there, inside namespace raftgpu; not a standalone header).
 
 // ---------------------------------------------------------------------------
@@ -265,8 +266,7 @@ tally_kernel(Columns c, uint32_t first, uint32_t n, uint32_t *__restrict__ out,
 }
 
 // ---------------------------------------------------------------------------
-// Control-plane helpers: one group each, as __device__ functions that the single-group <<<1,1>>> kernels below and
-// control_kernel (one thread per command) share.
+// Control-plane helpers: one group each, as __device__ functions that control_cmd (below) dispatches to.
 
 // ProgressTracker::apply_conf (tracker.rs:380-397)
 __device__ __forceinline__ void conf_group(const Columns &c, uint32_t g, uint32_t new_meta, uint32_t added,
@@ -286,10 +286,6 @@ __device__ __forceinline__ void conf_group(const Columns &c, uint32_t g, uint32_
     }
     c.meta[g] = new_meta;
     rq_conf_removed(c, g, new_meta, removed);
-}
-__global__ void conf_kernel(Columns c, uint32_t g, uint32_t new_meta, uint32_t added,
-                            uint32_t removed, uint64_t next_idx) {
-    conf_group(c, g, new_meta, added, removed, next_idx);
 }
 
 // Raft::reset (raft.rs:942-971) for the tracker + log bookkeeping of one group.
@@ -321,10 +317,6 @@ __device__ __forceinline__ void reset_group(const Columns &c, uint32_t g, uint64
     c.last_index[g] = last_index;
     rq_reset(c, g);  // raft.rs:957 read_only = ReadOnly::new(..)
 }
-__global__ void reset_kernel(Columns c, uint32_t g, uint64_t term_start, uint64_t last_index,
-                             uint64_t committed, uint64_t persisted) {
-    reset_group(c, g, term_start, last_index, committed, persisted);
-}
 
 // Raft::become_leader's tracker side (raft.rs:1176-1192): self.become_replicate(),
 // then the empty entry of the new term is appended at last_index + 1.
@@ -344,7 +336,6 @@ __device__ __forceinline__ void become_leader_group(const Columns &c, uint32_t g
     c.last_index[g] = li;
     c.term_start[g] = li;
 }
-__global__ void become_leader_kernel(Columns c, uint32_t g) { become_leader_group(c, g); }
 
 __global__ void progress_get_kernel(Columns c, uint32_t g, uint32_t s, raftgpu_progress *out) {
     const size_t cell = static_cast<size_t>(s) * c.cap + g;
@@ -509,10 +500,6 @@ __device__ __forceinline__ int32_t progress_op_cell(const Columns &c, uint32_t g
     c.pflags[cell] = static_cast<uint8_t>(f);
     return ret;
 }
-__global__ void progress_op_kernel(Columns c, uint32_t g, uint32_t s, int op, uint64_t a0, uint64_t a1,
-                                   uint64_t a2, int32_t *out) {
-    *out = progress_op_cell(c, g, s, op, a0, a1, a2);
-}
 
 // ProgressTracker::has_quorum (tracker.rs:367-372): vote_result(|id| set.get(id).map(|_| true)) == Won,
 // and quorum_recently_active (tracker.rs:346-361), which also clears recent_active.
@@ -542,7 +529,6 @@ __device__ __forceinline__ int32_t quorum_group(const Columns &c, uint32_t g, in
     const uint32_t i = majority_vote(in, active, 0), o = majority_vote(outm, active, 0);
     return (i == RAFTGPU_VOTE_WON && o == RAFTGPU_VOTE_WON) ? 1 : 0;
 }
-__global__ void quorum_kernel(Columns c, uint32_t g, int op, uint32_t arg, int32_t *out) { *out = quorum_group(c, g, op, arg); }
 
 // The two halves of a wide group share the group's log / commit columns: make them agree (a LOCAL record or a
 // single-half control-plane call may have touched one half only).
@@ -554,9 +540,10 @@ __device__ __forceinline__ void wide_sync(const Columns &c, uint32_t g) {
     c.term_start[g + 1] = c.term_start[g];
     c.term[g + 1] = c.term[g];
 }
-__global__ void wide_sync_kernel(Columns c, uint32_t g) { wide_sync(c, g); }
 
+// group_get: a wide group's halves agree first (wide_sync), as every command on the pair does.
 __global__ void group_get_kernel(Columns c, uint32_t g, raftgpu_group_state *out) {
+    if (c.meta[g] & RAFTGPU_META_WIDE_LO) wide_sync(c, g);
     raftgpu_group_state s{};
     s.meta = c.meta[g];
     s.committed = c.committed[g];
@@ -565,137 +552,122 @@ __global__ void group_get_kernel(Columns c, uint32_t g, raftgpu_group_state *out
     *out = s;
 }
 
-// op 0: set_log_bounds; op 1: commit_to (status in *out: 0 ok, 1 out of range);
-// op 2: meta bit set/clear (a = mask, b = enable); op 3: assign commit group (a = slot, b = id);
-// op 4: reset votes; op 5: record vote (a = slot, b = vote+1), first vote wins (tracker.rs:308-310);
-// op 6: maybe_commit (1 = advanced).  Returns the status / flag of ops 1 and 6, 0 for the others.
-__device__ __forceinline__ uint32_t group_op(const Columns &c, uint32_t g, int op, uint64_t a, uint64_t b) {
-    uint32_t out = 0;
-    switch (op) {
-    case 0:
-        c.term_start[g] = a;
-        c.last_index[g] = b;
-        break;
-    case 1:  // RaftLog::commit_to, raft_log.rs:286-300
-        if (c.committed[g] >= a) {
-            out = 0;
-        } else if (c.last_index[g] < a) {
-            out = 1;
-        } else {
-            c.committed[g] = a;
-            out = 0;
-        }
-        break;
-    case 2:
-        c.meta[g] = b ? (c.meta[g] | static_cast<uint32_t>(a)) : (c.meta[g] & ~static_cast<uint32_t>(a));
-        break;
-    case 3:
-        c.commit_group_id[static_cast<size_t>(a) * c.cap + g] = b;
-        break;
-    case 4:
-        for (int s = 0; s < kSlots; s++) c.votes[static_cast<size_t>(s) * c.cap + g] = 0;
-        break;
-    case 5: {
-        uint8_t *v = &c.votes[static_cast<size_t>(a) * c.cap + g];
-        if (*v == 0) *v = static_cast<uint8_t>(b);  // entry(id).or_insert(vote)
-        break;
-    }
-    case 6:  // RaftLog::maybe_commit(max_index = a, term = the leader's), raft_log.rs:487-499, range form
-        if (a > c.committed[g] && a >= c.term_start[g] && a <= c.last_index[g]) {
-            c.committed[g] = a;
-            out = 1;
-        } else {
-            out = 0;
-        }
-        break;
-    }
-    return out;
+// RaftLog::commit_to (raft_log.rs:286-300): false when to_commit is beyond last_index (the reference panics).
+__device__ __forceinline__ bool commit_to_group(const Columns &c, uint32_t g, uint64_t to_commit) {
+    if (c.committed[g] >= to_commit) return true;
+    if (c.last_index[g] < to_commit) return false;
+    c.committed[g] = to_commit;
+    return true;
 }
-__global__ void group_op_kernel(Columns c, uint32_t g, int op, uint64_t a, uint64_t b, uint32_t *out) {
-    const uint32_t r = group_op(c, g, op, a, b);
-    if (op == 1 || op == 6) *out = r;
+
+// RaftLog::maybe_commit(max_index, term = the leader's) (raft_log.rs:487-499), range form: true when it advanced.
+__device__ __forceinline__ bool maybe_commit_group(const Columns &c, uint32_t g, uint64_t max_index) {
+    if (max_index > c.committed[g] && max_index >= c.term_start[g] && max_index <= c.last_index[g]) {
+        c.committed[g] = max_index;
+        return true;
+    }
+    return false;
 }
 
 // ---------------------------------------------------------------------------
-// control_kernel: one wave of a raftgpu_control list, one thread per command (DESIGN 3.8).  The host has validated
-// every command against its meta mirror and put at most one command of each group (of each wide pair) in the wave,
-// so the threads touch disjoint cells.  It has also resolved the commands: `group` is the half that holds the named
-// peer, `peer_slot` the slot within that half, and a SET_CONF's a[0] carries the new meta words of the low half
-// (bits 0..31) and the high half (bits 32..63).  Every op runs the device function of its single-group call;
-// res[i] = {status, value} of cmds[i].
+// control_cmd: one command of the control plane (DESIGN 3.8), which every single-group call is too.  The host has
+// validated it against its meta mirror and resolved it: `group` is the half that holds the named peer, `peer_slot` the
+// slot within that half, and a SET_CONF's a[0] carries the new meta words of the low half (bits 0..31) and the high
+// half (bits 32..63).  Both halves of a wide group where the single call does both.  Returns {status, value};
+// *tallied = 1 for a VOTE_RESULT.
+__device__ __forceinline__ int2 control_cmd(const Columns &c, const raftgpu_ctl_cmd &m, uint32_t *tallied) {
+    const uint32_t g = m.group;
+    const uint32_t halves = (m.op != RAFTGPU_CTL_SET_TERM && (c.meta[g] & RAFTGPU_META_WIDE_LO)) ? 2u : 1u;
+    int32_t status = RAFTGPU_OK, value = 0;
+    switch (m.op) {
+    case RAFTGPU_CTL_SET_CONF:
+        for (uint32_t k = 0; k < halves; k++) {
+            const uint32_t meta = static_cast<uint32_t>(m.a[0] >> (32 * k)), was = c.meta[g + k];
+            const uint32_t p_was = RAFTGPU_META_IN(was) | RAFTGPU_META_OUT(was) | RAFTGPU_META_LEARN(was);
+            const uint32_t p_now = RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta);
+            conf_group(c, g + k, meta, p_now & ~p_was, p_was & ~p_now, m.a[3]);
+        }
+        break;
+    case RAFTGPU_CTL_RESET:
+        for (uint32_t k = 0; k < halves; k++) reset_group(c, g + k, m.a[0], m.a[1], m.a[2], m.a[3]);
+        break;
+    case RAFTGPU_CTL_BECOME_LEADER:
+        for (uint32_t k = 0; k < halves; k++) become_leader_group(c, g + k);
+        break;
+    case RAFTGPU_CTL_SET_LOG_BOUNDS:
+        for (uint32_t k = 0; k < halves; k++) {
+            c.term_start[g + k] = m.a[0];
+            c.last_index[g + k] = m.a[1];
+        }
+        break;
+    case RAFTGPU_CTL_SET_TERM:  // a high half alone when named alone
+        c.term[g] = m.a[0];
+        if (c.meta[g] & RAFTGPU_META_WIDE_LO) c.term[g + 1] = m.a[0];
+        break;
+    case RAFTGPU_CTL_COMMIT_TO:
+        if (halves == 2) wide_sync(c, g);
+        status = commit_to_group(c, g, m.a[0]) ? RAFTGPU_OK : RAFTGPU_ERR_COMMIT_RANGE;
+        if (halves == 2) commit_to_group(c, g + 1, m.a[0]);
+        break;
+    case RAFTGPU_CTL_MAYBE_COMMIT_TO:
+        if (halves == 2) {
+            wide_sync(c, g);
+            maybe_commit_group(c, g + 1, m.a[0]);
+        }
+        value = maybe_commit_group(c, g, m.a[0]) ? 1 : 0;
+        break;
+    case RAFTGPU_CTL_SET_GROUP_COMMIT:
+        for (uint32_t k = 0; k < halves; k++)
+            c.meta[g + k] = m.arg ? (c.meta[g + k] | RAFTGPU_META_GROUP_COMMIT) : (c.meta[g + k] & ~RAFTGPU_META_GROUP_COMMIT);
+        break;
+    case RAFTGPU_CTL_ASSIGN_COMMIT_GROUP:
+        c.commit_group_id[static_cast<size_t>(m.peer_slot) * c.cap + g] = m.a[0];
+        break;
+    case RAFTGPU_CTL_RESET_VOTES:
+        for (uint32_t k = 0; k < halves; k++)
+            for (int s = 0; s < kSlots; s++) c.votes[static_cast<size_t>(s) * c.cap + g + k] = 0;
+        break;
+    case RAFTGPU_CTL_RECORD_VOTE: {  // the first vote wins: entry(id).or_insert(vote), tracker.rs:308-310
+        uint8_t *v = &c.votes[static_cast<size_t>(m.peer_slot) * c.cap + g];
+        if (*v == 0) *v = m.arg ? 2 : 1;
+        break;
+    }
+    case RAFTGPU_CTL_VOTE_RESULT:
+        value = static_cast<int32_t>(tally_group(c, g));
+        *tallied = 1;
+        break;
+    case RAFTGPU_CTL_HAS_QUORUM:
+        value = quorum_group(c, g, 0, static_cast<uint32_t>(m.a[0]) & (halves == 2 ? 0xffffu : 0xffu));
+        break;
+    case RAFTGPU_CTL_QUORUM_RECENTLY_ACTIVE:
+        value = quorum_group(c, g, 1, m.peer_slot);
+        break;
+    case RAFTGPU_CTL_PROGRESS_OP:
+        value = progress_op_cell(c, g, m.peer_slot, m.arg, m.a[0], m.a[1], m.a[2]);
+        break;
+    }
+    return make_int2(status, value);
+}
+
+// control_kernel: one wave of a raftgpu_control list, one thread per command.  The host has put at most one command
+// of each group (of each wide pair) in the wave, so the threads touch disjoint cells; res[i] = {status, value} of
+// cmds[i].
 __global__ void __launch_bounds__(256)
 control_kernel(Columns c, const raftgpu_ctl_cmd *__restrict__ cmds, uint32_t n, int2 *__restrict__ res,
                unsigned long long *__restrict__ counters) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t tallied = 0;
-    if (t < n) {
-        const raftgpu_ctl_cmd m = cmds[t];
-        const uint32_t g = m.group;
-        const uint32_t halves = (m.op != RAFTGPU_CTL_SET_TERM && (c.meta[g] & RAFTGPU_META_WIDE_LO)) ? 2u : 1u;
-        int32_t status = RAFTGPU_OK, value = 0;
-        switch (m.op) {
-        case RAFTGPU_CTL_SET_CONF:
-            for (uint32_t k = 0; k < halves; k++) {
-                const uint32_t meta = static_cast<uint32_t>(m.a[0] >> (32 * k)), was = c.meta[g + k];
-                const uint32_t p_was = RAFTGPU_META_IN(was) | RAFTGPU_META_OUT(was) | RAFTGPU_META_LEARN(was);
-                const uint32_t p_now = RAFTGPU_META_IN(meta) | RAFTGPU_META_OUT(meta) | RAFTGPU_META_LEARN(meta);
-                conf_group(c, g + k, meta, p_now & ~p_was, p_was & ~p_now, m.a[3]);
-            }
-            break;
-        case RAFTGPU_CTL_RESET:
-            for (uint32_t k = 0; k < halves; k++) reset_group(c, g + k, m.a[0], m.a[1], m.a[2], m.a[3]);
-            break;
-        case RAFTGPU_CTL_BECOME_LEADER:
-            for (uint32_t k = 0; k < halves; k++) become_leader_group(c, g + k);
-            break;
-        case RAFTGPU_CTL_SET_LOG_BOUNDS:
-            for (uint32_t k = 0; k < halves; k++) group_op(c, g + k, 0, m.a[0], m.a[1]);
-            break;
-        case RAFTGPU_CTL_SET_TERM:  // a high half alone when named alone, as raftgpu_group_set_term
-            c.term[g] = m.a[0];
-            if (c.meta[g] & RAFTGPU_META_WIDE_LO) c.term[g + 1] = m.a[0];
-            break;
-        case RAFTGPU_CTL_COMMIT_TO:
-            if (halves == 2) wide_sync(c, g);
-            status = group_op(c, g, 1, m.a[0], 0) ? RAFTGPU_ERR_COMMIT_RANGE : RAFTGPU_OK;
-            if (halves == 2) group_op(c, g + 1, 1, m.a[0], 0);
-            break;
-        case RAFTGPU_CTL_MAYBE_COMMIT_TO:
-            if (halves == 2) {
-                wide_sync(c, g);
-                group_op(c, g + 1, 6, m.a[0], 0);
-            }
-            value = static_cast<int32_t>(group_op(c, g, 6, m.a[0], 0));
-            break;
-        case RAFTGPU_CTL_SET_GROUP_COMMIT:
-            for (uint32_t k = 0; k < halves; k++) group_op(c, g + k, 2, RAFTGPU_META_GROUP_COMMIT, m.arg ? 1 : 0);
-            break;
-        case RAFTGPU_CTL_ASSIGN_COMMIT_GROUP:
-            group_op(c, g, 3, m.peer_slot, m.a[0]);
-            break;
-        case RAFTGPU_CTL_RESET_VOTES:
-            for (uint32_t k = 0; k < halves; k++) group_op(c, g + k, 4, 0, 0);
-            break;
-        case RAFTGPU_CTL_RECORD_VOTE:
-            group_op(c, g, 5, m.peer_slot, m.arg ? 2 : 1);
-            break;
-        case RAFTGPU_CTL_VOTE_RESULT:
-            value = static_cast<int32_t>(tally_group(c, g));
-            tallied = 1;
-            break;
-        case RAFTGPU_CTL_HAS_QUORUM:
-            value = quorum_group(c, g, 0, static_cast<uint32_t>(m.a[0]) & (halves == 2 ? 0xffffu : 0xffu));
-            break;
-        case RAFTGPU_CTL_QUORUM_RECENTLY_ACTIVE:
-            value = quorum_group(c, g, 1, m.peer_slot);
-            break;
-        case RAFTGPU_CTL_PROGRESS_OP:
-            value = progress_op_cell(c, g, m.peer_slot, m.arg, m.a[0], m.a[1], m.a[2]);
-            break;
-        }
-        res[t] = make_int2(status, value);
-    }
+    if (t < n) res[t] = control_cmd(c, cmds[t], &tallied);
     const uint32_t local[1] = {tallied};
     const int which[1] = {kCntVotes};
     block_flush_counts<1>(local, which, counters, nullptr);
+}
+
+// control_one_kernel: the command of a single-group call, passed by value (no staging, no H2D); one thread.
+// *res = {status, value}; a VOTE_RESULT adds one to votes_tallied.
+__global__ void control_one_kernel(Columns c, raftgpu_ctl_cmd m, int2 *__restrict__ res,
+                                   unsigned long long *__restrict__ counters) {
+    uint32_t tallied = 0;
+    *res = control_cmd(c, m, &tallied);
+    if (tallied) atomicAdd(&counters[kCntVotes], 1ull);
 }
