@@ -842,6 +842,50 @@ int32_t raftgpu_heartbeat_wire_device(raftgpu_arena *arena, void *stream, const 
 int32_t raftgpu_heartbeat_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets, uint64_t n,
                                uint8_t *status, raftgpu_read_state *released, uint64_t capacity, uint64_t *out_n);
 
+/* ---- heartbeats to the wire ---------------------------------------------------- */
+
+/* Raft::ping / MsgBeat -> bcast_heartbeat (raft.rs:868-889) -> send_heartbeat (raft.rs:822-844) -> send (raft.rs:602-661)
+ * for groups [first, first + n), as serialized MsgHeartbeat frames ready for the transport.  A read-only pass: the
+ * tracker and the read queues are not changed.
+ *
+ * Selection.  d_select is a bitmap in the layout of d_adv_bitmap (bit g = group g, words counted from group 0); NULL =
+ * every group of the range.  A selected group sends only when it is allocated, a leader (term_start !=
+ * RAFTGPU_NO_TERM_START) and its term (raftgpu_group_set_term) is non-zero.  A leader whose term is 0 sends nothing --
+ * a term-less heartbeat would be read as a local message -- and is counted in totals[2], so a missing
+ * raftgpu_group_set_term shows; a non-leader is skipped silently, as `ping` skips it.
+ * Peers.  One MsgHeartbeat per present peer (voter of either half of a joint configuration, or learner) other than
+ * the group's own slot.  The ids are the caller's (the arena keeps slots): d_ids is u64 [RAFTGPU_SLOTS + 1][n], row
+ * s < 8 = the id of the peer in slot s of group first + i, row 8 = that group's Raft::id, the `from` (a leader that
+ * has removed itself has no self slot and still sends).
+ * Wide groups.  Peer 8 + s is cell (g + 1, s), as in the wire batches.  Selection bit, term, term_start, the `from`
+ * (row 8) and the context are the low half's; commit uses committed = max of both halves (what raftgpu_group_get
+ * reports).  A range that splits a wide group is RAFTGPU_ERR_INVALID before any launch.
+ * The message: msg_type = MsgHeartbeat (8), to, from, term = Raft::term, commit = min(pr.matched, committed) and, on
+ * an arena with read queues whose queue is not empty, context = the 8 little-endian bytes of the last pending ctx id
+ * (read_only.rs:132-135: what raftgpu_heartbeat_wire decodes); no context otherwise.  Canonical proto3 encoding of
+ * eraftpb.Message, fields in number order, zero scalars omitted: at most 56 bytes.
+ * Output.  The frames of raftgpu_wire_batch: u32 LE (group << 4 | peer_slot), then the Message; in ascending
+ * (group, slot) order, so the output is deterministic.  d_bytes (16-byte aligned, so the blob can go to the wire
+ * entry points as is) holds the frames back to back; d_offsets [frames + 1] their starts and the end, d_offsets[0] =
+ * 0.  d_totals (u64[3]) = {frames, bytes, leaders without a term}, always the full need.  When frames >
+ * frames_capacity (d_offsets has room for frames_capacity + 1 values) or bytes > bytes_capacity, NOTHING is written to
+ * d_bytes or d_offsets; the pass only reads state, so calling again with larger buffers is always safe.
+ * raftgpu_heartbeat_frames_bound(n) is enough for any n groups; a range whose bound exceeds what u32 offsets address
+ * is RAFTGPU_ERR_INVALID.
+ * Ordering.  The pass reads matched and committed, which steps write: order it against steps on the stream, as for
+ * raftgpu_heartbeat_commits_device.  _device: asynchronous on `stream`, with its own scratch in the arena (run it on
+ * one stream at a time).  The host form copies select / ids, runs and waits: RAFTGPU_ERR_FULL with *out_totals filled
+ * in when a capacity is short. */
+/* Worst-case bytes of raftgpu_heartbeat_frames* output for n group slots (8 frames x 60 bytes per slot). */
+uint64_t raftgpu_heartbeat_frames_bound(uint32_t n);
+int32_t raftgpu_heartbeat_frames_device(raftgpu_arena *arena, void *stream, uint32_t first, uint32_t n,
+                                        const uint32_t *d_select, const uint64_t *d_ids,
+                                        uint8_t *d_bytes, uint64_t bytes_capacity,
+                                        uint32_t *d_offsets, uint64_t frames_capacity, uint64_t *d_totals);
+int32_t raftgpu_heartbeat_frames(raftgpu_arena *arena, uint32_t first, uint32_t n, const uint32_t *select,
+                                 const uint64_t *ids, uint8_t *bytes, uint64_t bytes_capacity, uint32_t *offsets,
+                                 uint64_t frames_capacity, uint64_t *out_totals);
+
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 
 /* ProgressTracker::reset_votes / record_vote (tracker.rs:301-310). */

@@ -301,6 +301,9 @@ def lib() -> C.CDLL:
             "raftgpu_read_index_read": ([vp, u32, u32, vp, vp, vp, vp], i32),
             "raftgpu_heartbeat_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, u64, vp], i32),
             "raftgpu_heartbeat_wire": ([vp, vp, u64, vp, u64, vp, vp, u64, C.POINTER(u64)], i32),
+            "raftgpu_heartbeat_frames_bound": ([u32], u64),
+            "raftgpu_heartbeat_frames_device": ([vp, vp, u32, u32, vp, vp, vp, u64, vp, u64, vp], i32),
+            "raftgpu_heartbeat_frames": ([vp, u32, u32, vp, vp, vp, u64, vp, u64, vp], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -350,6 +353,11 @@ def strerror(status: int) -> str:
 
 
 TILE_GROUPS = 256
+
+
+def heartbeat_frames_bound(n: int) -> int:
+    """raftgpu_heartbeat_frames_bound: bytes enough for the heartbeat frames of any n group slots."""
+    return int(lib().raftgpu_heartbeat_frames_bound(n))
 
 
 def tile_groups() -> int:
@@ -816,6 +824,37 @@ class Arena:
                               stream=None):
         self._ck(self._L.raftgpu_heartbeat_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_status, d_released,
                                                        capacity, d_count), "heartbeat_wire_device")
+
+    def heartbeat_frames(self, first, n, ids, select=None, bytes_out=None, offsets_out=None, bytes_capacity=None,
+                         frames_capacity=None):
+        """raftgpu_heartbeat_frames: bcast_heartbeat for groups [first, first + n) as MsgHeartbeat frames.  ids: u64 [9][n]
+        (peer ids by slot, row 8 = the group's own id); select: u32 bitmap words from group 0, or None for all.  The
+        output goes to bytes_out / offsets_out (allocated at the bound when None) with the given capacities (default:
+        the arrays' sizes) -> (status, blob, offsets, totals u64[3]): status OK with the frames as views of the output
+        arrays, or ERR_FULL with empty views (the totals still say what is needed); any other status raises."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        assert ids.shape == (SLOTS + 1, n)
+        sel = None if select is None else np.ascontiguousarray(select, dtype=np.uint32)
+        if bytes_out is None:
+            bytes_out = np.zeros(max(16, heartbeat_frames_bound(n)), dtype=np.uint8)
+        if offsets_out is None:
+            offsets_out = np.zeros(SLOTS * n + 1, dtype=np.uint32)
+        assert bytes_out.dtype == np.uint8 and offsets_out.dtype == np.uint32 and len(offsets_out) >= 1
+        bcap = len(bytes_out) if bytes_capacity is None else bytes_capacity
+        fcap = len(offsets_out) - 1 if frames_capacity is None else frames_capacity
+        assert bcap <= len(bytes_out) and fcap < len(offsets_out)
+        totals = np.zeros(3, dtype=np.uint64)
+        rc = self._L.raftgpu_heartbeat_frames(self._h, first, n, None if sel is None else sel.ctypes.data, ids.ctypes.data,
+                                              bytes_out.ctypes.data, bcap, offsets_out.ctypes.data, fcap, totals.ctypes.data)
+        if rc == ERR_FULL:
+            return rc, bytes_out[:0], offsets_out[:0], totals
+        self._ck(rc, "heartbeat_frames")
+        return rc, bytes_out[: int(totals[1])], offsets_out[: int(totals[0]) + 1], totals
+
+    def heartbeat_frames_device(self, first, n, d_select, d_ids, d_bytes, bytes_capacity, d_offsets, frames_capacity,
+                                d_totals, stream=None):
+        self._ck(self._L.raftgpu_heartbeat_frames_device(self._h, stream, first, n, d_select, d_ids, d_bytes, bytes_capacity,
+                                                         d_offsets, frames_capacity, d_totals), "heartbeat_frames_device")
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

@@ -253,6 +253,9 @@ struct raftgpu_arena {
     uint32_t *hbw_first = nullptr;
     raftgpu_append_resp *hbw_recs = nullptr;
     uint64_t hbw_recs_cap = 0;
+    // raftgpu_heartbeat_frames (grown on demand): {frames, bytes} per group slot, the block sums, the fit flag
+    uint32_t *hbf_scratch = nullptr;
+    uint64_t hbf_scratch_cap = 0;
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -588,6 +591,7 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->d_wire_first);
     cudaFree(a->hbw_first);
     cudaFree(a->hbw_recs);
+    cudaFree(a->hbf_scratch);
     cudaFree(a->d_counters);
     cudaFree(a->d_scratch);
     cudaFreeHost(a->h_scratch);
@@ -663,6 +667,7 @@ int32_t create(int32_t device, uint32_t max_groups, uint32_t slots, uint32_t n_r
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
+    TRYC(cudaFuncSetAttribute(hbf_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kHbfSmem)));
     {
         const char *f = getenv("RAFTGPU_FORCE_GENERAL");
         a->force_general = f && f[0] == '1';
@@ -994,5 +999,6 @@ extern "C" {
 #include "abi_results.inc"
 #include "abi_read.inc"
 #include "abi_hb_wire.inc"
+#include "abi_hb_frames.inc"
 
 }  // extern "C"

@@ -24,5 +24,6 @@ namespace raftgpu {
 #include "k_read.cuh"
 #include "k_wire.cuh"
 #include "k_hb_wire.cuh"
+#include "k_hb_frames.cuh"
 
 }  // namespace raftgpu
