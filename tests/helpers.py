@@ -126,16 +126,24 @@ def random_state(n, shape, rng):
     return c
 
 
-def random_batch(ref, rng, per_cell, keep=None):
+def random_batch(ref, rng, per_cell, keep=None, edge=False, with_kinds=False):
     """A batch in group order for the groups of `ref`: 70 % of the groups (of those `keep` selects) get
     records for 1-5 random peer slots, the group's peers or not, each cell up to `per_cell` records.  The
     leader's own slot gets LOCAL records; other slots accepts (stale ones, commits above the index, commits
-    far below it) or rejections, 85 % of them with a hint (EXT), a fifth of those with a snapshot request."""
+    far below it) or rejections, 85 % of them with a hint (EXT), a fifth of those with a snapshot request.
+
+    With `edge`, records are drawn from the state to put cells exactly on either side of the offset window of
+    next_idx and peer_committed (_edge_records; groups whose eight cells are all escaped get records on all eight
+    slots).  With `with_kinds` the result is (records, kind of every record: K_*)."""
     n = ref.n_groups
     on = rng.random(n) >= 0.3
     if keep is not None:
         on &= keep
     k = rng.integers(1, 6, n)
+    if edge:
+        crowd = (escaped_cells(ref).sum(axis=0) == O.SLOTS) & (True if keep is None else keep)
+        on |= crowd
+        k = np.where(crowd, O.SLOTS, k)
     perm = rng.random((n, O.SLOTS)).argsort(axis=1)           # every group's peer slots in a random order
     g, j = np.nonzero(on[:, None] & (np.arange(O.SLOTS) < k[:, None]))
     cnt = rng.integers(1, per_cell + 1, len(g))
@@ -162,6 +170,10 @@ def random_batch(ref, rng, per_cell, keep=None):
     ext = reject & (rng.random(r) < 0.85)
     ext_index = np.maximum(0, ri + rng.integers(-5, 3, r))
     ext_snapshot = np.where(rng.random(r) < 0.2, rng.integers(1, 1 << 30, r), 0)
+    kind = np.zeros(r, dtype=np.uint8)
+    if edge:
+        rank = np.arange(r) - np.repeat(np.cumsum(cnt) - cnt, cnt)    # a record's place among its cell's
+        _edge_records(ref, rng, g, s, rank, local, accept, reject, ext, index, commit, ext_index, ext_snapshot, kind)
 
     pos = np.arange(r) + np.cumsum(ext) - ext                 # each EXT right behind its REJECT
     out = np.zeros(r + int(ext.sum()), dtype=O.APPEND_RESP_DTYPE)
@@ -171,7 +183,165 @@ def random_batch(ref, rng, per_cell, keep=None):
     pe = pos[ext] + 1
     out["group"][pe], out["peer_slot"][pe], out["flags"][pe] = g[ext], s[ext], O.REC_EXT
     out["index"][pe], out["commit"][pe] = ext_index[ext], ext_snapshot[ext]
-    return out
+    if not with_kinds:
+        return out
+    kinds = np.zeros(len(out), dtype=np.uint8)
+    kinds[pos], kinds[pe] = kind, kind[ext]
+    return out, kinds
+
+
+# --------------------------------------------------------------------------- the offset window of next_idx / peer_committed
+# On the device next_idx and peer_committed are int32 offsets from the cell's matched; an offset outside
+# (INT32_MIN, INT32_MAX] is stored as the escape code INT32_MIN with the exact value beside it (k_common.cuh).
+
+I32_MIN, I32_MAX = -(2 ** 31), 2 ** 31 - 1
+EDGE_FITS = (0, 1, -1, I32_MAX, I32_MIN + 1)                         # distances value - matched stored as offsets
+EDGE_ESCAPES = (I32_MAX + 1, I32_MIN, I32_MIN - 1, 1 << 40, -(1 << 40))  # and the ones that escape
+RESET_LAST = (2 ** 31 - 2, 2 ** 31 - 1, 2 ** 31, 2 ** 32 + 5, 2 ** 48 + 3)  # last indexes of the Raft::reset shape
+_BELOW = np.array([I32_MIN + 1, I32_MIN, I32_MIN - 1])             # landing distances at the lower bound
+_ABOVE = np.array([I32_MAX, I32_MAX + 1, I32_MAX - 1])             # and at the upper one
+# indexes the edge records stay below: a compact run header holds a 48-bit base, and a batch must stay tileable for
+# the fused compact kernels to take it (one with several records per cell has no other way in)
+_INDEX_LIMIT = 1 << 48
+
+# record kinds of random_batch(edge=True)
+(K_RANDOM, K_LOCAL_JUMP, K_PROBE_REJECT, K_WIDE_RAISE, K_COMMIT_UP, K_RESET_RETURN, K_ESCAPED, K_PAIR) = range(8)
+
+
+def offset_of(value, matched):
+    """value - matched as a signed 64-bit distance (mod 2^64)."""
+    return (np.asarray(value, dtype=np.uint64) - np.asarray(matched, dtype=np.uint64)).view(np.int64)
+
+
+def fits(value, matched):
+    """The host model of off_encode: True where `value` is stored as an offset from `matched`, False where it
+    escapes."""
+    d = offset_of(value, matched)
+    return (d > I32_MIN) & (d <= I32_MAX)
+
+
+def escaped_cells(c, n=None):
+    """[SLOTS][n] bool: cells whose next_idx or peer_committed escapes."""
+    n = c.n_groups if n is None else n
+    m = c.matched[:, :n]
+    return ~fits(c.next_idx[:, :n], m) | ~fits(c.peer_committed[:, :n], m)
+
+
+def edge_state(c, rng, frac=0.3, n=None, escape_groups=None):
+    """Moves next_idx and peer_committed of a fraction `frac` of the cells of groups [0, n) to the edges of the
+    offset window, in place.  A chosen cell gets both values at distances from EDGE_FITS + EDGE_ESCAPES (drawn
+    independently); a fifth of the chosen cells instead get the shape Raft::reset leaves (matched 0, next_idx =
+    last_index + 1 for a last index from RESET_LAST, Probe, peer_committed kept).  Cells are drawn from every
+    slot alike, so hinted slots, learners outside the hint, the self slot and Snapshot-state peers all get them.
+    Every peer cell of the groups `escape_groups` selects gets escaping distances for both values (whole tiles of
+    them overflow the fused kernels' per-warp lists of deferred records).  Values stay in [0, 2^63)."""
+    n = c.n_groups if n is None else n
+    shape = (O.SLOTS, n)
+    m = c.matched[:, :n].astype(np.int64)
+    pick = rng.random(shape) < frac
+    all_d, esc_d = np.array(EDGE_FITS + EDGE_ESCAPES), np.array(EDGE_ESCAPES)
+
+    def place(full):
+        d = np.where(full, esc_d[rng.integers(0, len(esc_d), shape)], all_d[rng.integers(0, len(all_d), shape)])
+        v = m + d
+        return np.where((v < 0) | (v >= _INDEX_LIMIT), m - d, v)
+
+    full = np.zeros(shape, dtype=bool) if escape_groups is None else np.broadcast_to(escape_groups[:n], shape)
+    pick |= full
+    nx, pc = place(full), place(full)
+    c.next_idx[:, :n] = np.where(pick, nx, c.next_idx[:, :n])
+    c.peer_committed[:, :n] = np.where(pick, pc, c.peer_committed[:, :n])
+    reset = pick & (rng.random(shape) < 0.2)
+    last = np.array(RESET_LAST)[rng.integers(0, len(RESET_LAST), shape)]
+    c.matched[:, :n][reset] = 0
+    c.next_idx[:, :n][reset] = last[reset] + 1
+    c.pflags[:, :n][reset] = O.STATE_PROBE
+    c.pending_snapshot[:, :n][reset] = 0
+    c.pending_request_snapshot[:, :n][reset] = 0
+    return c
+
+
+def _edge_records(ref, rng, g, s, rank, local, accept, reject, ext, index, commit, ext_index, ext_snapshot, kind):
+    """random_batch(edge=True): overwrites some of the drawn records (arrays edited in place) with records that land
+    a cell on either side of a bound of the offset window, from the cell's state in `ref`:
+    - K_LOCAL_JUMP: a LOCAL record raising the self slot's matched so that peer_committed - matched lands at
+      -(2^31 - 1), -2^31 or -2^31 - 1 (or next_idx - matched at 2^31 - 1, 2^31 or 2^31 - 2 under a high next_idx);
+      no commit or one within the packed 24-bit delta, so the fused fast path takes it.
+    - K_PROBE_REJECT: a REJECT of a Probe-state peer at next_idx - 1 with an EXT hint landing next_idx at matched -
+      2^31 + 1, matched - 2^31 or one below (the fast path takes these too).
+    - K_WIDE_RAISE: an accept raising matched by 2^31 or more with a commit far below (packed WIDE), landing
+      peer_committed (or next_idx of a Replicate peer) like the LOCAL jumps.
+    - K_COMMIT_UP: an accept whose commit is 2^31 - 1, 2^31 or 2^31 + 1 above the new matched.
+    - K_RESET_RETURN: an accept at last_index of a peer in the reset shape, with and without a commit.
+    - K_ESCAPED: the ordinary records left on cells that are escaped already (the fast path must decline them).
+    - K_PAIR: the first two records of a cell with several: escape, then return (or the reverse for a cell that
+      is escaped), within one batch."""
+    r = len(g)
+    m = ref.matched[s, g].astype(np.int64)
+    nx = ref.next_idx[s, g].astype(np.int64)
+    pc = ref.peer_committed[s, g].astype(np.int64)
+    state = ref.pflags[s, g] & O.PF_STATE_MASK
+    esc = ~fits(nx, m) | ~fits(pc, m)
+    u = rng.random(r)
+    free = np.ones(r, dtype=bool)
+
+    def take(mask, k, is_accept, is_reject=False, new_index=None):
+        mask &= free
+        if new_index is not None:
+            mask &= new_index < _INDEX_LIMIT
+        free[mask] = False
+        kind[mask] = k
+        accept[mask], reject[mask] = is_accept, is_reject
+        ext[mask] = is_reject
+        return mask
+
+    # escape and return within one batch (several records per cell)
+    step = 1 << 31
+    cell = g.astype(np.int64) * 8 + s
+    coin = rng.random(r)[np.arange(r) - rank]                          # one draw per cell
+    pair = ~local & (rank <= 1) & np.isin(cell, cell[rank == 1]) & (coin < 0.6)
+    pair &= np.where(esc, np.maximum(np.maximum(m, pc), nx - 1) + 2, m + 6 + step)[np.arange(r) - rank] < _INDEX_LIMIT
+    pc_up = rng.integers(0, 2, r)
+    x = np.maximum(np.maximum(m, pc), nx - 1) + 1
+    a = take(pair & ~esc & (rank == 0), K_PAIR, True, new_index=m + 6 + step)                 # escape (commit 2^31 + above), then return
+    index[a], commit[a] = (m + 1)[a], (m + 1 + step + pc_up)[a]
+    a = take(pair & ~esc & (rank == 1), K_PAIR, True, new_index=m + 6 + step)
+    index[a], commit[a] = (m + 6 + step)[a], (m + 5 + step)[a]
+    a = take(pair & esc & (rank == 0), K_PAIR, True, new_index=x + 1)                  # return, then escape
+    index[a], commit[a] = x[a], x[a]
+    a = take(pair & esc & (rank == 1), K_PAIR, True, new_index=x + 1)
+    index[a], commit[a] = (x + 1)[a], (x + 1 + step + pc_up)[a]
+
+    below = _BELOW[rng.integers(0, 3, r)]
+    above = _ABOVE[rng.integers(0, 3, r)]
+    lift_pc = pc - m - below                                           # raise matched by this: pc lands at `below`
+    lift_nx = nx - above                                               # matched to land next_idx at `above`
+    to_nx = (lift_nx > m) & (local | (state == O.STATE_REPLICATE)) & (rng.random(r) < 0.7)
+    lifted = np.where(to_nx, lift_nx, m + lift_pc)
+    ok = to_nx | (lift_pc > 0)
+    a = take(local & ok & (u < 0.7), K_LOCAL_JUMP, False, new_index=lifted)
+    index[a] = lifted[a]
+    commit[a] = np.where(rng.random(r) < 0.4, 0, lifted + rng.integers(0, 1000, r))[a]
+
+    a = take(~local & (state == O.STATE_PROBE) & (m >= step + 4) & (nx >= 1) & (u < 0.35), K_PROBE_REJECT, False, True,
+             new_index=nx)
+    index[a] = (nx - 1)[a]
+    commit[a] = np.maximum(0, nx - 1 - rng.integers(0, 4, r))[a]
+    ext_index[a], ext_snapshot[a] = (m + below - 1)[a], 0
+
+    a = take(~local & ok & (u < 0.5), K_WIDE_RAISE, True, new_index=lifted)
+    index[a], commit[a] = lifted[a], np.maximum(0, np.minimum(pc, m) - 1 - rng.integers(0, 4, r))[a]
+
+    a = take(~local & (m == 0) & (nx >= 1) & (u < 0.8), K_RESET_RETURN, True)
+    li = nx - 1
+    index[a] = li[a]
+    commit[a] = np.where(rng.random(r) < 0.5, 0, li - rng.integers(0, 3, r).clip(0, li))[a]
+
+    a = take(~local & (u < 0.65), K_COMMIT_UP, True)
+    top = m + rng.integers(0, 3, r)
+    index[a], commit[a] = top[a], (top + above)[a]
+
+    kind[free & esc] = K_ESCAPED
 
 
 # --------------------------------------------------------------------------- checked fused steps
@@ -215,7 +385,10 @@ def fused_round(arena, n, recs, ref, pk, d_bufs):
     want_adv, want_bm, _, _ = O.arena_recompute(ref)
     main_pk = (pk[:k, 0] & np.uint64(1 << 37)) == 0           # packed records that are not EXT payloads
     main_orig = (recs["flags"] & B.REC_EXT) == 0
-    assert np.array_equal(res[main_pk], want_res[main_orig]), "per-record results differ"
+    if not np.array_equal(res[main_pk], want_res[main_orig]):
+        i = int(np.flatnonzero(res[main_pk] != want_res[main_orig])[0])
+        raise AssertionError(f"per-record results differ: record {recs[main_orig][i]} got {res[main_pk][i]} "
+                             f"want {want_res[main_orig][i]}")
     assert not res[~main_pk].any()
     _check_outputs(arena, n, ref, want_adv, want_bm, bm, com, before, "fused step")
     return want_adv, res[main_pk]
@@ -267,3 +440,94 @@ def compact_bufs(arena, n, per_group):
          arena.device_alloc(3 * per_group * n + 64), arena.device_alloc(arena.cap // 8),
          arena.device_alloc(8 * arena.cap), arena.device_alloc(4))
     return blob, d
+
+
+# --------------------------------------------------------------------------- every way into the fused kernels
+
+def ring_wrapping_groups():
+    """A group count at which the fused kernels' stage ring wraps: 18 tiles per SM plus a ragged one: the grid is one CTA per SM (fewer only with fewer tiles), and consumer
+    group cg of a CTA takes the CTA's tiles cg, cg + 3, ...; a stage is used again n_stages tiles later."""
+    a = B.Arena(256)
+    sm = a.info.sm_count
+    a.close()
+    tg = B.tile_groups()
+    n = 18 * sm * tg + 77
+    tiles = -(-n // tg)
+    assert tiles > sm and n % tg
+    assert tiles // sm >= 2 * 8 + 1       # every CTA wraps an 8-stage ring twice
+    assert tiles // sm // 3 >= 5          # every consumer group gets at least 5 tiles
+    return n
+
+
+class Paths:
+    """One arena per way into the fused kernels, loaded with the same state, each with its oracle copy."""
+
+    def __init__(self, n, init, records_api):
+        self.n = n
+        names = ["packed", "compact", "ordered"] + (["records"] if records_api else [])
+        self.arenas, self.refs = {}, {}
+        for name in names:
+            a = B.Arena(n)
+            assert a.group_alloc_range(n) == 0
+            a.load_columns(init)
+            self.arenas[name], self.refs[name] = a, O.copy_columns(init)
+        pa = self.arenas["packed"]
+        self.pk = np.zeros((16 * n, 2), dtype=np.uint64)
+        self.d_packed = (pa.device_alloc(self.pk.nbytes), pa.device_alloc(4 * (n // B.tile_groups() + 2)),
+                         pa.device_alloc(8 * n), pa.device_alloc(pa.cap // 8), pa.device_alloc(8 * pa.cap))
+        self.blob, self.d_compact = compact_bufs(self.arenas["compact"], n, 12)
+        _, self.d_ordered = compact_bufs(self.arenas["ordered"], n, 12)
+
+    def round(self, recs, per_cell, what):
+        """One batch through every path that takes it; returns the per-record result bytes of each."""
+        assert len(recs) <= 6 * self.n
+        out = {}
+        B.pack_compact(recs, self.blob)
+        if not self.blob[:64].view(B.COMPACT_HDR_DTYPE)[0]["flags"] & B.COMPACT_TILEABLE:
+            # a unit block of the compact stream holds runs of groups at most 4095 past its first: a batch spread
+            # thinner than that is not tileable (the library steps it with the scatter kernel)
+            out["packed"] = fused_round(self.arenas["packed"], self.n, recs, self.refs["packed"], self.pk, self.d_packed)[1]
+            for name in self.arenas:
+                if name != "packed":
+                    self.arenas[name].load_columns(self.refs["packed"])
+                    self.refs[name] = O.copy_columns(self.refs["packed"])
+            return out
+        if per_cell == 1:
+            out["packed"] = fused_round(self.arenas["packed"], self.n, recs, self.refs["packed"], self.pk, self.d_packed)[1]
+            out["compact"] = compact_round(self.arenas["compact"], self.n, recs, self.refs["compact"], self.blob,
+                                           self.d_compact)[1]
+        out["ordered"] = compact_round(self.arenas["ordered"], self.n, recs, self.refs["ordered"], self.blob,
+                                       self.d_ordered, ordered=True)[1]
+        if "records" in self.arenas:
+            records_round(self.arenas["records"], self.n, recs, self.refs["records"], what)
+        if per_cell > 1:       # the packed and per-unit kernels promise one record per cell: catch them up
+            for name in ("packed", "compact"):
+                self.arenas[name].load_columns(self.refs["ordered"])
+                self.refs[name] = O.copy_columns(self.refs["ordered"])
+        return out
+
+    def reload(self, state):
+        """Every arena and oracle copy to `state` (host columns)."""
+        for name, a in self.arenas.items():
+            a.load_columns(state)
+            self.refs[name] = O.copy_columns(state)
+
+    def close(self):
+        for a in self.arenas.values():
+            a.close()
+
+
+def records_round(arena, n, recs, ref, what):
+    """raftgpu_step_begin_records: the library packs the batch and picks the kernel and its plan itself."""
+    arena.step_begin_records(recs, B.STEP_READ_COMMITTED)
+    r = arena.step_wait()
+    O.arena_apply(ref, recs, mode=0)
+    want_adv, want_bm, _, _ = O.arena_recompute(ref)
+    assert r.n_advanced == want_adv and r.n_duplicates == 0, what
+    # the fused kernel counts records without their EXT payloads (the scatter fallback counts both)
+    assert r.n_records == np.count_nonzero((recs["flags"] & B.REC_EXT) == 0), what
+    bm, com = arena.step_results(n)
+    assert np.array_equal(bm, want_bm[: len(bm)]), what
+    adv = bitmap_to_bool(bm, n)
+    assert np.array_equal(com[adv], ref.committed[:n][adv]), what
+    assert_columns_equal(arena.read_columns(n), ref, n, f"records API, {what}")

@@ -12,7 +12,8 @@ import random
 import numpy as np
 import pytest
 
-from helpers import B, O, assert_columns_equal, bitmap_to_bool, checksum, compact_bufs, compact_round, fused_round
+from helpers import (B, O, assert_columns_equal, bitmap_to_bool, checksum, compact_bufs, compact_round, edge_state, fused_round,
+                     random_batch)
 from oracle import datadriven as dd
 
 pytestmark = pytest.mark.gpu
@@ -911,22 +912,28 @@ def _random_batch(ref, n, rng, per_cell):
     return np.array(rows, dtype=B.APPEND_RESP_DTYPE) if rows else np.zeros(0, dtype=B.APPEND_RESP_DTYPE)
 
 
-@pytest.mark.parametrize("seed", [1, 2, 3])
+@pytest.mark.parametrize("seed", [1, 2, 3, "edges"])
 def test_every_ingest_path_agrees_with_the_oracle_on_random_states(seed):
     """Differential test: arbitrary configurations / peer states, random group-ordered batches (accepts,
     stale acks, commits above the index, leader-local records, rejections with and without hint and
     snapshot request, peers the group does not have), through EVERY way of handing a batch to the
     engine -- rings + waves, bulk staging, zero-copy packed, zero-copy compact (fused), the records
-    API, the device-resident fused kernels -- each compared with the oracle column by column."""
-    rng = np.random.default_rng(seed)
+    API, the device-resident fused kernels -- each compared with the oracle column by column.  "edges":
+    next_idx and peer_committed at the edges of their offset window (helpers.edge_state) and batches that
+    move cells across it (random_batch(edge=True))."""
+    edges = seed == "edges"
+    rng = np.random.default_rng(4 if edges else seed)
     n = 2500
     init = _random_state(n, rng)
+    if edges:
+        edge_state(init, rng)
     ref = O.copy_columns(init)
     names = ["enqueue", "bulk", "packed", "compact", "records", "fused16", "fusedc"]
     arenas = {}
     for name in names:
-        # (the wave-splitting paths keep later waves in an overflow area sized from the arena capacity)
-        a = B.Arena(32 * n if name in ("enqueue", "bulk") else n)
+        # (the wave-splitting paths keep later waves in an overflow area sized from the arena capacity; the records
+        # API takes them for batches too hostile for the compact stream, as the edge batches can be)
+        a = B.Arena(32 * n if name in ("enqueue", "bulk") or (edges and name == "records") else n)
         a.group_alloc_range(n)
         a.load_columns(init)
         arenas[name] = a
@@ -938,7 +945,7 @@ def test_every_ingest_path_agrees_with_the_oracle_on_random_states(seed):
     blob, dc = compact_bufs(arenas["fusedc"], n, 40)
     for rnd in range(5):
         per_cell = 3 if rnd >= 3 else 1          # the last rounds: several records per (group, peer)
-        recs = _random_batch(ref, n, rng, per_cell)
+        recs = random_batch(ref, rng, per_cell, edge=True) if edges else _random_batch(ref, n, rng, per_cell)
         O.arena_apply(ref, recs, mode=0)
         want_adv, want_bm, _, _ = O.arena_recompute(ref)
         words = (n + 31) // 32

@@ -10,8 +10,8 @@ with the oracle: result bytes, advanced bitmap, commit_out, counters and every c
 import numpy as np
 import pytest
 
-from helpers import (B, O, TILE_SHAPES, assert_columns_equal, bitmap_to_bool, compact_bufs, compact_round,
-                     fused_round, is_simple5, random_batch, random_state)
+from helpers import (B, O, TILE_SHAPES, Paths, compact_bufs, compact_round, fused_round, is_simple5, random_batch,
+                     random_state, ring_wrapping_groups)
 
 pytestmark = pytest.mark.gpu
 
@@ -20,86 +20,7 @@ RECORDS_API_SHAPES = ("v3", "sparse_a", "joint7")
 
 @pytest.fixture(scope="module")
 def n_groups():
-    """18 tiles per SM plus a ragged one: the grid is one CTA per SM (fewer only with fewer tiles), and consumer
-    group cg of a CTA takes the CTA's tiles cg, cg + 3, ...; a stage is used again n_stages tiles later."""
-    a = B.Arena(256)
-    sm = a.info.sm_count
-    a.close()
-    tg = B.tile_groups()
-    n = 18 * sm * tg + 77
-    tiles = -(-n // tg)
-    assert tiles > sm and n % tg
-    assert tiles // sm >= 2 * 8 + 1       # every CTA wraps an 8-stage ring twice
-    assert tiles // sm // 3 >= 5          # every consumer group gets at least 5 tiles
-    return n
-
-
-class Paths:
-    """One arena per way into the fused kernels, loaded with the same state, each with its oracle copy."""
-
-    def __init__(self, n, init, records_api):
-        self.n = n
-        names = ["packed", "compact", "ordered"] + (["records"] if records_api else [])
-        self.arenas, self.refs = {}, {}
-        for name in names:
-            a = B.Arena(n)
-            assert a.group_alloc_range(n) == 0
-            a.load_columns(init)
-            self.arenas[name], self.refs[name] = a, O.copy_columns(init)
-        pa = self.arenas["packed"]
-        self.pk = np.zeros((8 * n, 2), dtype=np.uint64)
-        self.d_packed = (pa.device_alloc(self.pk.nbytes), pa.device_alloc(4 * (n // B.tile_groups() + 2)),
-                         pa.device_alloc(8 * n), pa.device_alloc(pa.cap // 8), pa.device_alloc(8 * pa.cap))
-        self.blob, self.d_compact = compact_bufs(self.arenas["compact"], n, 12)
-        _, self.d_ordered = compact_bufs(self.arenas["ordered"], n, 12)
-
-    def round(self, recs, per_cell, what):
-        """One batch through every path that takes it; returns the per-record result bytes of each."""
-        assert len(recs) <= 6 * self.n
-        out = {}
-        B.pack_compact(recs, self.blob)
-        if not self.blob[:64].view(B.COMPACT_HDR_DTYPE)[0]["flags"] & B.COMPACT_TILEABLE:
-            # a unit block of the compact stream holds runs of groups at most 4095 past its first: a batch spread
-            # thinner than that is not tileable (the library steps it with the scatter kernel)
-            out["packed"] = fused_round(self.arenas["packed"], self.n, recs, self.refs["packed"], self.pk, self.d_packed)[1]
-            for name in self.arenas:
-                if name != "packed":
-                    self.arenas[name].load_columns(self.refs["packed"])
-                    self.refs[name] = O.copy_columns(self.refs["packed"])
-            return out
-        if per_cell == 1:
-            out["packed"] = fused_round(self.arenas["packed"], self.n, recs, self.refs["packed"], self.pk, self.d_packed)[1]
-            out["compact"] = compact_round(self.arenas["compact"], self.n, recs, self.refs["compact"], self.blob,
-                                           self.d_compact)[1]
-        out["ordered"] = compact_round(self.arenas["ordered"], self.n, recs, self.refs["ordered"], self.blob,
-                                       self.d_ordered, ordered=True)[1]
-        if "records" in self.arenas:
-            records_round(self.arenas["records"], self.n, recs, self.refs["records"], what)
-        if per_cell > 1:       # the packed and per-unit kernels promise one record per cell: catch them up
-            for name in ("packed", "compact"):
-                self.arenas[name].load_columns(self.refs["ordered"])
-                self.refs[name] = O.copy_columns(self.refs["ordered"])
-        return out
-
-    def close(self):
-        for a in self.arenas.values():
-            a.close()
-
-
-def records_round(arena, n, recs, ref, what):
-    """raftgpu_step_begin_records: the library packs the batch and picks the kernel and its plan itself."""
-    arena.step_begin_records(recs, B.STEP_READ_COMMITTED)
-    r = arena.step_wait()
-    O.arena_apply(ref, recs, mode=0)
-    want_adv, want_bm, _, _ = O.arena_recompute(ref)
-    assert r.n_advanced == want_adv and r.n_duplicates == 0, what
-    # the fused kernel counts records without their EXT payloads (the scatter fallback counts both)
-    assert r.n_records == np.count_nonzero((recs["flags"] & B.REC_EXT) == 0), what
-    bm, com = arena.step_results(n)
-    assert np.array_equal(bm, want_bm[: len(bm)]), what
-    adv = bitmap_to_bool(bm, n)
-    assert np.array_equal(com[adv], ref.committed[:n][adv]), what
-    assert_columns_equal(arena.read_columns(n), ref, n, f"records API, {what}")
+    return ring_wrapping_groups()
 
 
 def run_shape(name, n, monkeypatch):
