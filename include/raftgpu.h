@@ -645,6 +645,10 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
                                       applied in arrival order, one message per step -- resubmit it with the next batch */
 #define RAFTGPU_WIRE_CONTEXT 6u    /* (raftgpu_heartbeat_wire only) a context that is not an 8-byte read id, or any context
                                       on an arena without read queues: the host's own ReadOnly handles the frame */
+#define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat only) the group is not selected as a follower, or is a
+                                      leader: Raft::step on the host */
+#define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat only) m.commit beyond max(committed, last_index):
+                                        commit_to would be fatal! (raft_log.rs:291-298) */
 typedef struct raftgpu_wire_batch {
     const uint8_t *bytes;    /* the frames, back to back */
     uint64_t n_bytes;
@@ -885,6 +889,53 @@ int32_t raftgpu_heartbeat_frames_device(raftgpu_arena *arena, void *stream, uint
 int32_t raftgpu_heartbeat_frames(raftgpu_arena *arena, uint32_t first, uint32_t n, const uint32_t *select,
                                  const uint64_t *ids, uint8_t *bytes, uint64_t bytes_capacity, uint32_t *offsets,
                                  uint64_t frames_capacity, uint64_t *out_totals);
+
+/* ---- heartbeats at the follower ------------------------------------------------ */
+
+/* RawNode::step -> Raft::step (raft.rs:1280-1411) -> step_follower (raft.rs:2276-2280) -> handle_heartbeat
+ * (raft.rs:2452-2464) for the MsgHeartbeat frames (msg_type 8) of a wire batch that reach this arena's followers:
+ * commit_to(m.commit) (raft_log.rs:286-300: never decreases) and one MsgHeartbeatResponse through send (raft.rs:602-661).
+ * Input.  The frames of raftgpu_wire_batch, but the header is u32 LE (group << 4 | x) with `group` the follower's own
+ * group slot in this arena (the transport rewrites the leader's header on the way in); x is not read and is copied
+ * into the response's header.  d_bytes 16-byte aligned, n and n_bytes below 4 GiB.
+ * Role.  d_select (required) is a bitmap in the layout of d_adv_bitmap: bit g set when the caller's Raft of group g is
+ * a Follower (not a Candidate or PreCandidate) without a pending_request_snapshot -- host state the arena does not
+ * keep.  d_self_ids (u64, indexed by group slot) holds each group's Raft::id, the `from` of its response (send takes
+ * it from self.id, not from m.to).
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4, | RAFTGPU_RES_OK when a response was written; the first failing check decides:
+ *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot (on an arena with read queues:
+ *                any unallocated group), or the high half of a wide pair (a pair is addressed by its low half);
+ *   SKIP_TYPE    any type but MsgHeartbeat;
+ *   ROLE         the select bit is clear, or the group is a leader (term_start != RAFTGPU_NO_TERM_START);
+ *   TERM         the group's term (raftgpu_group_set_term) is 0 or m.term differs: a higher term is become_follower, a
+ *                lower one may need a MsgAppendResponse (raft.rs:1349-1376), m.term 0 is a local message;
+ *   CONTEXT      a context that is present and not 8 bytes;
+ *   COMMIT_RANGE m.commit > max(committed, last_index) (both halves of a wide pair);
+ *   DUP          a later frame of a group whose first passing frame is applied here.
+ * A frame that does not pass changes nothing: run RawNode::step on it.  d_from (u64[n], nullable) = m.from of every
+ * applied frame (0 for the others), for step_follower's leader_id = m.from and election_elapsed = 0.
+ * Apply.  committed = max(committed, m.commit), on both halves of a wide pair (as raftgpu_group_commit_to).
+ * Output.  One MsgHeartbeatResponse per applied frame, in frame order: the input frame's header, then msg_type 9, to =
+ * m.from, from = the group's id, term, commit = the new committed and, when the heartbeat had one, its 8 context bytes;
+ * canonical proto3 as raftgpu_heartbeat_frames writes (at most 56 bytes + the header).  d_resp_bytes (16-byte aligned)
+ * holds them back to back, d_resp_offsets (n + 1 values) their starts and the end; d_totals (u64[2]) = {responses,
+ * bytes}.  A response cannot be regenerated once committed has moved, so resp_bytes_capacity must be at least
+ * raftgpu_follower_heartbeat_bound(n) and that bound must be addressable by u32 offsets: RAFTGPU_ERR_INVALID before
+ * any launch otherwise.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  The
+ * host form copies (select and self_ids cover the arena's max_groups; only the groups below the highest allocated one
+ * are read), runs and waits; status, from, resp_bytes / resp_offsets as above, totals u64[2]. */
+/* 60 bytes per frame: enough for the responses to any n frames. */
+uint64_t raftgpu_follower_heartbeat_bound(uint64_t n);
+int32_t raftgpu_follower_heartbeat_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                          const uint32_t *d_offsets, uint64_t n, const uint32_t *d_select,
+                                          const uint64_t *d_self_ids, uint8_t *d_status, uint64_t *d_from,
+                                          uint8_t *d_resp_bytes, uint64_t resp_bytes_capacity, uint32_t *d_resp_offsets,
+                                          uint64_t *d_totals);
+int32_t raftgpu_follower_heartbeat(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets,
+                                   uint64_t n, const uint32_t *select, const uint64_t *self_ids, uint8_t *status,
+                                   uint64_t *from, uint8_t *resp_bytes, uint64_t resp_bytes_capacity,
+                                   uint32_t *resp_offsets, uint64_t *totals);
 
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 

@@ -44,6 +44,7 @@ BULK_SORTED = 0x1
  COL_COMMIT_GROUP_ID, COL_PFLAGS, COL_VOTES, COL_META, COL_COMMITTED, COL_TERM_START,
  COL_LAST_INDEX, COL_TERM, COL_INS_META) = range(14)
 WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WIRE_CONTEXT = range(7)
+WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat only
 
 APPEND_RESP_DTYPE = np.dtype(
     [("group", "<u4"), ("peer_slot", "u1"), ("flags", "u1"), ("reserved", "<u2"),
@@ -304,6 +305,9 @@ def lib() -> C.CDLL:
             "raftgpu_heartbeat_frames_bound": ([u32], u64),
             "raftgpu_heartbeat_frames_device": ([vp, vp, u32, u32, vp, vp, vp, u64, vp, u64, vp], i32),
             "raftgpu_heartbeat_frames": ([vp, u32, u32, vp, vp, vp, u64, vp, u64, vp], i32),
+            "raftgpu_follower_heartbeat_bound": ([u64], u64),
+            "raftgpu_follower_heartbeat_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_follower_heartbeat": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -353,6 +357,11 @@ def strerror(status: int) -> str:
 
 
 TILE_GROUPS = 256
+
+
+def follower_heartbeat_bound(n: int) -> int:
+    """raftgpu_follower_heartbeat_bound: response bytes enough for any n heartbeat frames."""
+    return int(lib().raftgpu_follower_heartbeat_bound(n))
 
 
 def heartbeat_frames_bound(n: int) -> int:
@@ -855,6 +864,31 @@ class Arena:
                                 d_totals, stream=None):
         self._ck(self._L.raftgpu_heartbeat_frames_device(self._h, stream, first, n, d_select, d_ids, d_bytes, bytes_capacity,
                                                          d_offsets, frames_capacity, d_totals), "heartbeat_frames_device")
+
+    def follower_heartbeat(self, frames, self_ids, select):
+        """raftgpu_follower_heartbeat: handle_heartbeat at this arena's followers for the MsgHeartbeat frames of a wire
+        batch (.bytes, .n_bytes, .offsets, .n; headers name the follower's group slot).  self_ids: u64 per group slot
+        (Raft::id, the responses' `from`), select: u32 bitmap words from group 0 of the groups that are Followers; both
+        cover the arena's capacity -> (status u8[n], from u64[n], response blob, response offsets u32[responses + 1],
+        totals u64[2])."""
+        ids = np.ascontiguousarray(self_ids, dtype=np.uint64)
+        sel = np.ascontiguousarray(select, dtype=np.uint32)
+        assert len(ids) >= self.cap and len(sel) * 32 >= self.cap
+        n = frames.n
+        status, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
+        resp = np.zeros(max(16, follower_heartbeat_bound(n)), np.uint8)
+        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        self._ck(self._L.raftgpu_follower_heartbeat(self._h, frames.bytes.ctypes.data, frames.n_bytes,
+                                                    frames.offsets.ctypes.data, n, sel.ctypes.data, ids.ctypes.data,
+                                                    status.ctypes.data, frm.ctypes.data, resp.ctypes.data, len(resp),
+                                                    roff.ctypes.data, totals.ctypes.data), "follower_heartbeat")
+        return status, frm, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+
+    def follower_heartbeat_device(self, d_bytes, n_bytes, d_offsets, n, d_select, d_self_ids, d_status, d_from, d_resp_bytes,
+                                  resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
+        self._ck(self._L.raftgpu_follower_heartbeat_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_select,
+                                                           d_self_ids, d_status, d_from, d_resp_bytes, resp_bytes_capacity,
+                                                           d_resp_offsets, d_totals), "follower_heartbeat_device")
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

@@ -256,6 +256,11 @@ struct raftgpu_arena {
     // raftgpu_heartbeat_frames (grown on demand): {frames, bytes} per group slot, the block sums, the fit flag
     uint32_t *hbf_scratch = nullptr;
     uint64_t hbf_scratch_cap = 0;
+    // raftgpu_follower_heartbeat: first passing frame of every group slot [cap] (allocated on first use); grown on
+    // demand, in u64 words: one record per frame, the block sums, the fit flag
+    uint32_t *hfw_first = nullptr;
+    uint64_t *hfw_scratch = nullptr;
+    uint64_t hfw_scratch_cap = 0;
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -592,6 +597,8 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->hbw_first);
     cudaFree(a->hbw_recs);
     cudaFree(a->hbf_scratch);
+    cudaFree(a->hfw_first);
+    cudaFree(a->hfw_scratch);
     cudaFree(a->d_counters);
     cudaFree(a->d_scratch);
     cudaFreeHost(a->h_scratch);
@@ -1000,5 +1007,6 @@ extern "C" {
 #include "abi_read.inc"
 #include "abi_hb_wire.inc"
 #include "abi_hb_frames.inc"
+#include "abi_hb_follow.inc"
 
 }  // extern "C"

@@ -64,11 +64,15 @@ __device__ __forceinline__ HbfGroup hbf_group(const Columns &c, const HbfSrc &s,
     return r;
 }
 
+// Bytes of a heartbeat-kind frame (MsgHeartbeat here, MsgHeartbeatResponse in k_hb_follow.cuh) before its `to` and
+// `commit`: header, msg_type, from, term (never 0 on this path) and the 8-byte context when there is one.
+__device__ __forceinline__ uint32_t hb_msg_fixed(uint64_t from, uint64_t term, bool has_ctx) {
+    return 4u + 2u + (from ? 1u + hbf_vlen(from) : 0u) + 1u + hbf_vlen(term) + (has_ctx ? 10u : 0u);
+}
+
 // Bytes of the frame to a peer with id `to` and commit `commit`, after the fields its group's frames share (`fixed`:
 // header, msg_type, from, term, context).
-__device__ __forceinline__ uint32_t hbf_fixed(const HbfGroup &h) {
-    return 4u + 2u + (h.from ? 1u + hbf_vlen(h.from) : 0u) + 1u + hbf_vlen(h.term) + (h.ctx ? 10u : 0u);
-}
+__device__ __forceinline__ uint32_t hbf_fixed(const HbfGroup &h) { return hb_msg_fixed(h.from, h.term, h.ctx != 0); }
 __device__ __forceinline__ uint32_t hbf_len(uint32_t fixed, uint64_t to, uint64_t commit) {
     return fixed + (to ? 1u + hbf_vlen(to) : 0u) + (commit ? 1u + hbf_vlen(commit) : 0u);
 }
@@ -82,40 +86,47 @@ __device__ __forceinline__ uint8_t *hbf_varint(uint8_t *p, uint64_t v) {
     return p;
 }
 
-// One frame: u32 LE (group << 4 | slot), then eraftpb.Message (eraftpb.proto:71-92) in field-number order with zero
-// scalars omitted: 1 msg_type = MsgHeartbeat (8), 2 to, 3 from, 4 term, 8 commit, 12 context.
-__device__ __forceinline__ uint8_t *hbf_frame(uint8_t *p, uint32_t g, uint32_t slot, const HbfGroup &h, uint64_t to,
-                                              uint64_t commit) {
-    const uint32_t hdr = (g << 4) | slot;
+// One heartbeat-kind frame: u32 LE header, then eraftpb.Message (eraftpb.proto:71-92) in field-number order with zero
+// scalars omitted: 1 msg_type = kType (MsgHeartbeat 8, MsgHeartbeatResponse 9, eraftpb.proto:58-59), 2 to, 3 from,
+// 4 term (never 0 on this path), 8 commit, 12 context (the 8 little-endian bytes of ctx when has_ctx).
+template <uint8_t kType>
+__device__ __forceinline__ uint8_t *hb_msg_frame(uint8_t *p, uint32_t hdr, uint64_t to, uint64_t from, uint64_t term,
+                                                 uint64_t commit, bool has_ctx, uint64_t ctx) {
     p[0] = static_cast<uint8_t>(hdr);
     p[1] = static_cast<uint8_t>(hdr >> 8);
     p[2] = static_cast<uint8_t>(hdr >> 16);
     p[3] = static_cast<uint8_t>(hdr >> 24);
     p[4] = 0x08;  // field 1, varint
-    p[5] = 8;     // MsgHeartbeat, eraftpb.proto:58
+    p[5] = kType;
     p += 6;
     if (to) {
         *p++ = 0x10;
         p = hbf_varint(p, to);
     }
-    if (h.from) {
+    if (from) {
         *p++ = 0x18;
-        p = hbf_varint(p, h.from);
+        p = hbf_varint(p, from);
     }
     *p++ = 0x20;
-    p = hbf_varint(p, h.term);
+    p = hbf_varint(p, term);
     if (commit) {
         *p++ = 0x40;
         p = hbf_varint(p, commit);
     }
-    if (h.ctx) {  // the read id as 8 little-endian bytes (DESIGN 3.10)
+    if (has_ctx) {
         p[0] = 0x62;
         p[1] = 8;
 #pragma unroll
-        for (int k = 0; k < 8; k++) p[2 + k] = static_cast<uint8_t>(h.ctx >> (8 * k));
+        for (int k = 0; k < 8; k++) p[2 + k] = static_cast<uint8_t>(ctx >> (8 * k));
         p += 10;
     }
     return p;
+}
+
+// One MsgHeartbeat frame with header (group << 4 | slot); the read id travels as the context (DESIGN 3.10), id 0 as none.
+__device__ __forceinline__ uint8_t *hbf_frame(uint8_t *p, uint32_t g, uint32_t slot, const HbfGroup &h, uint64_t to,
+                                              uint64_t commit) {
+    return hb_msg_frame<8>(p, (g << 4) | slot, to, h.from, h.term, commit, h.ctx != 0, h.ctx);
 }
 
 // Exclusive scan of two u32 counts over a block of W warps; *tot_a / *tot_b = the block's sums (every thread).
@@ -201,43 +212,65 @@ __global__ void __launch_bounds__(kHbfThreads) hbf_size_kernel(Columns c, HbfSrc
     }
 }
 
-// Pass 2, one block: blk's frames and bytes become each block's exclusive starts; totals = {frames, bytes, leaders
-// without a term}.  flag[0] = the output fits (d_offsets given, frames <= frames_cap, bytes <= bytes_cap); then
-// offsets[frames] = bytes, the end of the last frame.
+// Pass 2, one block: blk's frames and bytes become each block's exclusive starts.  K = u32 per block in blk: {frames,
+// bytes} (K = 2, k_hb_follow.cuh) or {frames, bytes, leaders without a term} (K = 3); totals = the K sums.  flag[0] =
+// the output fits (d_offsets given, frames <= frames_cap, bytes <= bytes_cap); then offsets[frames] = bytes, the end of
+// the last frame.
+template <uint32_t K>
 __global__ void __launch_bounds__(kHbfScanThreads) hbf_scan_kernel(uint32_t *__restrict__ blk, uint32_t nb, uint64_t bytes_cap,
                                                                    uint64_t frames_cap, uint64_t *__restrict__ totals,
                                                                    uint32_t *__restrict__ offsets, uint32_t *__restrict__ flag) {
+    static_assert(K == 2 || K == 3, "blk holds {frames, bytes[, leaders without a term]} per block");
     uint32_t carry_f = 0, carry_b = 0, no_term = 0;
     for (uint32_t j0 = 0; j0 < nb; j0 += kHbfScanThreads) {  // (uniform trip count: every thread reaches the scan)
         const uint32_t j = j0 + threadIdx.x;
         uint32_t f = 0, b = 0;
         if (j < nb) {
-            f = blk[3 * j];
-            b = blk[3 * j + 1];
-            no_term += blk[3 * j + 2];
+            f = blk[K * j];
+            b = blk[K * j + 1];
+            if constexpr (K == 3) no_term += blk[K * j + 2];
         }
         uint32_t tf, tb;
         hbf_block_scan<kHbfScanThreads / 32>(f, b, tf, tb);
         if (j < nb) {
-            blk[3 * j] = carry_f + f;
-            blk[3 * j + 1] = carry_b + b;
+            blk[K * j] = carry_f + f;
+            blk[K * j + 1] = carry_b + b;
         }
         carry_f += tf;
         carry_b += tb;
     }
-    no_term = __reduce_add_sync(0xffffffffu, no_term);
-    __shared__ uint32_t nt[kHbfScanThreads / 32];
-    if ((threadIdx.x & 31u) == 0) nt[threadIdx.x >> 5] = no_term;
-    __syncthreads();
+    uint64_t t = 0;
+    if constexpr (K == 3) {
+        no_term = __reduce_add_sync(0xffffffffu, no_term);
+        __shared__ uint32_t nt[kHbfScanThreads / 32];
+        if ((threadIdx.x & 31u) == 0) nt[threadIdx.x >> 5] = no_term;
+        __syncthreads();
+        if (threadIdx.x == 0)
+            for (uint32_t w = 0; w < kHbfScanThreads / 32; w++) t += nt[w];
+    }
     if (threadIdx.x == 0) {
-        uint64_t t = 0;
-        for (uint32_t w = 0; w < kHbfScanThreads / 32; w++) t += nt[w];
         totals[0] = carry_f;
         totals[1] = carry_b;
-        totals[2] = t;
+        if constexpr (K == 3) totals[2] = t;
         const bool fits = offsets && carry_f <= frames_cap && carry_b <= bytes_cap;
         flag[0] = fits;
         if (fits) offsets[carry_f] = carry_b;
+    }
+}
+
+// A block's contiguous output [b0, b0 + nbytes) from shared memory, where it was assembled at buf + (b0 & 15): whole
+// 16-byte chunks go out as uint4 stores, only the two chunks shared with the neighbouring blocks byte by byte.
+template <uint32_t kThreads>
+__device__ __forceinline__ void hbf_store_block(uint8_t *__restrict__ out, const uint8_t *buf, uint32_t b0, uint32_t nbytes) {
+    const uint32_t a0 = b0 & ~15u, end = b0 + nbytes;
+    for (uint32_t q = a0 + 16u * threadIdx.x; q < end; q += 16u * kThreads) {
+        const uint8_t *src = buf + (q - a0);
+        if (q >= b0 && q + 16u <= end) {
+            *reinterpret_cast<uint4 *>(out + q) = *reinterpret_cast<const uint4 *>(src);
+        } else {
+            for (uint32_t k = 0; k < 16u; k++)
+                if (q + k >= b0 && q + k < end) out[q + k] = src[k];
+        }
     }
 }
 
@@ -273,14 +306,5 @@ __global__ void __launch_bounds__(kHbfThreads) hbf_write_kernel(Columns c, HbfSr
     }
     __syncthreads();
     for (uint32_t j = threadIdx.x; j < nf; j += kHbfThreads) offsets[f0 + j] = offs[j];
-    const uint32_t a0 = b0 - pad, end = b0 + nbytes;
-    for (uint32_t q = a0 + 16u * threadIdx.x; q < end; q += 16u * kHbfThreads) {
-        const uint8_t *src = buf + (q - a0);
-        if (q >= b0 && q + 16u <= end) {
-            *reinterpret_cast<uint4 *>(out + q) = *reinterpret_cast<const uint4 *>(src);
-        } else {
-            for (uint32_t k = 0; k < 16u; k++)
-                if (q + k >= b0 && q + k < end) out[q + k] = src[k];
-        }
-    }
+    hbf_store_block<kHbfThreads>(out, buf, b0, nbytes);
 }

@@ -34,6 +34,7 @@ struct WireMsg {  // the scalar fields this path looks at
     bool reject;
     uint64_t term, log_term, index, commit, reject_hint, request_snapshot;
     uint32_t ctx_off, ctx_len;  // wire_decode<true> only: bytes [ctx_off, ctx_off + ctx_len) are the last context (12)
+    uint64_t from;              // wire_decode<true, true> only: field 3
 };
 
 constexpr uint32_t kWireThreads = 256;
@@ -54,13 +55,15 @@ __device__ __forceinline__ bool wire_varint(const uint8_t *p, uint32_t &pos, uin
 }
 
 // One serialized Message -> WireMsg.  false = not a well-formed protobuf message.  kContext: also the context's
-// position (the heartbeat-response path, k_hb_wire.cuh); the AppendResponse kernels instantiate it without.
-template <bool kContext = false>
+// position (the heartbeat-response path, k_hb_wire.cuh); the AppendResponse kernels instantiate it without.  kFrom:
+// also `from` (the follower's heartbeat path, k_hb_follow.cuh).
+template <bool kContext = false, bool kFrom = false>
 __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, WireMsg &m) {
     m.msg_type = 0;
     m.reject = false;
     m.term = m.log_term = m.index = m.commit = m.reject_hint = m.request_snapshot = 0;
     if constexpr (kContext) m.ctx_off = m.ctx_len = 0;
+    if constexpr (kFrom) m.from = 0;
     uint32_t pos = 0;
     while (pos < len) {
         uint64_t tag;
@@ -79,6 +82,9 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
             else if (field == 10) m.reject = v != 0;
             else if (field == 11) m.reject_hint = v;
             else if (field == 13) m.request_snapshot = v;
+            if constexpr (kFrom) {
+                if (field == 3) m.from = v;
+            }
         } else if (wt == 1) {
             if (len - pos < 8) return false;
             pos += 8;

@@ -25,5 +25,6 @@ namespace raftgpu {
 #include "k_wire.cuh"
 #include "k_hb_wire.cuh"
 #include "k_hb_frames.cuh"
+#include "k_hb_follow.cuh"
 
 }  // namespace raftgpu

@@ -1,0 +1,45 @@
+"""Helpers for the follower heartbeat tests: frame headers read and rewritten in place (the transport's part: a leader's
+(group << 4 | slot) becomes the follower's (group << 4 | x) and back), selection bitmaps, and the columns the pass may
+write."""
+import numpy as np
+
+GROUP_STATE = ("committed", "last_index", "term", "term_start", "meta")
+
+
+def headers(blob, offsets) -> np.ndarray:
+    """The u32 LE header of every frame."""
+    o = np.asarray(offsets[:-1], dtype=np.int64)
+    b = np.asarray(blob, dtype=np.uint32)
+    return b[o] | (b[o + 1] << 8) | (b[o + 2] << 16) | (b[o + 3] << 24)
+
+
+def with_headers(blob, offsets, hdrs) -> np.ndarray:
+    """A copy of blob with every frame's header replaced by hdrs."""
+    out = np.array(blob, dtype=np.uint8, copy=True)
+    o = np.asarray(offsets[:-1], dtype=np.int64)
+    h = np.asarray(hdrs, dtype=np.uint32)
+    for k in range(4):
+        out[o + k] = (h >> (8 * k)) & 0xFF
+    return out
+
+
+def bitmap(bits) -> np.ndarray:
+    """u32 words from group 0 of a bool per group slot (padded to whole words)."""
+    bits = np.asarray(bits, dtype=bool)
+    pad = np.zeros((-len(bits)) % 32, dtype=bool)
+    return np.packbits(np.concatenate([bits, pad]), bitorder="little").view(np.uint32).copy()
+
+
+def frames_of(blob, offsets):
+    """[(header, body bytes)] of a blob."""
+    return [(int.from_bytes(bytes(blob[lo:lo + 4]), "little"), bytes(blob[lo + 4:hi]))
+            for lo, hi in zip(np.asarray(offsets[:-1]).tolist(), np.asarray(offsets[1:]).tolist())]
+
+
+def state(c, n):
+    """The group columns of groups [0, n) (what the pass may write), copied."""
+    return {k: getattr(c, k)[:n].copy() for k in GROUP_STATE}
+
+
+def same_state(x, y) -> bool:
+    return all(np.array_equal(x[k], y[k]) for k in GROUP_STATE)
