@@ -1,43 +1,19 @@
 """ctypes front-end of the follower heartbeat oracle (oracle/hb_follow_oracle.c).
 
-TEST INFRASTRUCTURE ONLY, like oracle.py.  hb_follow_oracle.c is compiled together with hb_frames_oracle.c,
-hb_wire_oracle.c, wire_oracle.c, read_oracle.c, control_oracle.c and raft_oracle.c into its own library,
-libhb_follow_oracle.so: next to the sources when that directory is writable, else in a per-user temporary directory.
+TEST INFRASTRUCTURE ONLY, like oracle.py.  hb_follow_oracle.c is part of libraft_oracle.so; lib() declares its functions
+on oracle.lib().
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import oracle as O
-from oracle import control_oracle as CO
 from oracle import read_oracle as RO
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SOURCES = ("hb_follow_oracle.c", "hb_frames_oracle.c", "hb_wire_oracle.c", "wire_oracle.c", "read_oracle.c",
-            "control_oracle.c", "raft_oracle.c")
-_HEADERS = ("hb_follow_oracle.h", "hb_frames_oracle.h", "hb_wire_oracle.h", "wire_oracle.h", "read_oracle.h",
-            "control_oracle.h", "raft_oracle.h")
 FRAME_MAX = 60  # 4-byte header + at most 56 bytes of Message
 WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8
-
-
-def build(force: bool = False) -> str:
-    """Compile libhb_follow_oracle.so when it is missing or older than its sources; returns its path."""
-    out_dir = _HERE if os.access(_HERE, os.W_OK) else os.path.join(tempfile.gettempdir(), f"hb_follow_oracle_{os.getuid()}")
-    os.makedirs(out_dir, exist_ok=True)
-    path = os.path.join(out_dir, "libhb_follow_oracle.so")
-    newest = max(os.path.getmtime(os.path.join(_HERE, f)) for f in _SOURCES + _HEADERS)
-    if force or not os.path.exists(path) or os.path.getmtime(path) < newest:
-        tmp = f"{path}.{os.getpid()}"
-        subprocess.run([os.environ.get("CC", "gcc"), *CO.CFLAGS, "-shared", "-o", tmp,
-                        *[os.path.join(_HERE, f) for f in _SOURCES]], check=True)
-        os.replace(tmp, path)
-    return path
 
 
 _lib = None
@@ -46,7 +22,7 @@ _lib = None
 def lib() -> C.CDLL:
     global _lib
     if _lib is None:
-        L = C.CDLL(build())
+        L = O.lib()
         u64, vp, sz = C.c_uint64, C.c_void_p, C.c_size_t
         L.hfl_encode_response.argtypes, L.hfl_encode_response.restype = [u64, u64, u64, u64, vp, vp], sz
         args = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, sz, vp, vp, vp, vp, vp, vp, vp]

@@ -1,40 +1,18 @@
 """ctypes front-end of the heartbeat-response wire oracle (oracle/hb_wire_oracle.c).
 
-TEST INFRASTRUCTURE ONLY, like oracle.py.  hb_wire_oracle.c is compiled together with wire_oracle.c, read_oracle.c,
-control_oracle.c and raft_oracle.c into its own library, libhb_wire_oracle.so: next to the sources when that directory
-is writable, else in a per-user temporary directory.
+TEST INFRASTRUCTURE ONLY, like oracle.py.  hb_wire_oracle.c is part of libraft_oracle.so; lib() declares its functions
+on oracle.lib().
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import oracle as O
-from oracle import control_oracle as CO
 from oracle import read_oracle as RO
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SOURCES = ("hb_wire_oracle.c", "wire_oracle.c", "read_oracle.c", "control_oracle.c", "raft_oracle.c")
-_HEADERS = ("hb_wire_oracle.h", "wire_oracle.h", "read_oracle.h", "control_oracle.h", "raft_oracle.h")
 WIRE_CONTEXT = 6
-
-
-def build(force: bool = False) -> str:
-    """Compile libhb_wire_oracle.so when it is missing or older than its sources; returns its path."""
-    out_dir = _HERE if os.access(_HERE, os.W_OK) else os.path.join(tempfile.gettempdir(), f"hb_wire_oracle_{os.getuid()}")
-    os.makedirs(out_dir, exist_ok=True)
-    path = os.path.join(out_dir, "libhb_wire_oracle.so")
-    newest = max(os.path.getmtime(os.path.join(_HERE, f)) for f in _SOURCES + _HEADERS)
-    if force or not os.path.exists(path) or os.path.getmtime(path) < newest:
-        tmp = f"{path}.{os.getpid()}"
-        subprocess.run([os.environ.get("CC", "gcc"), *CO.CFLAGS, "-shared", "-o", tmp,
-                        *[os.path.join(_HERE, f) for f in _SOURCES]], check=True)
-        os.replace(tmp, path)
-    return path
 
 
 class Message(C.Structure):
@@ -47,7 +25,7 @@ _lib = None
 def lib() -> C.CDLL:
     global _lib
     if _lib is None:
-        L = C.CDLL(build())
+        L = O.lib()
         vp, sz = C.c_void_p, C.c_size_t
         L.hwo_decode_message.argtypes, L.hwo_decode_message.restype = [vp, sz, C.POINTER(Message)], C.c_int
         L.hwo_decode_batch.argtypes, L.hwo_decode_batch.restype = [vp, vp, sz, vp, C.c_uint32, C.c_int, vp, vp], None

@@ -7,6 +7,7 @@ path.  See oracle/raft_oracle.h for the reference file:line of every function.
 from __future__ import annotations
 
 import ctypes as C
+import glob
 import os
 import subprocess
 import types
@@ -95,10 +96,11 @@ class WireMessage(C.Structure):
 
 
 def build(force: bool = False) -> str:
-    """Compile oracle/libraft_oracle.so with the committed Makefile."""
+    """Compile oracle/libraft_oracle.so, the whole C oracle (every *.c here), with the committed Makefile
+    when it is missing or older than any C source or header."""
+    sources = glob.glob(os.path.join(_HERE, "*.[ch]"))
     if force or not os.path.exists(_LIB_PATH) or \
-            os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(os.path.join(_HERE, f))
-                                              for f in ("raft_oracle.c", "wire_oracle.c", "raft_oracle.h", "wire_oracle.h")):
+            os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(f) for f in sources):
         subprocess.run(["make", "-C", _HERE, "-s"], check=True)
     return _LIB_PATH
 

@@ -1,43 +1,22 @@
 """ctypes front-end of the ReadIndex oracle (oracle/read_oracle.c).
 
-TEST INFRASTRUCTURE ONLY, like oracle.py.  read_oracle.c is compiled together with control_oracle.c and raft_oracle.c
-into its own library, libread_oracle.so: next to the sources when that directory is writable, else in a per-user
-temporary directory.
+TEST INFRASTRUCTURE ONLY, like oracle.py.  read_oracle.c is part of libraft_oracle.so; lib() declares its functions
+on oracle.lib().
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import oracle as O
 from oracle import control_oracle as CO
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SOURCES = ("read_oracle.c", "control_oracle.c", "raft_oracle.c")
-_HEADERS = ("read_oracle.h", "control_oracle.h", "raft_oracle.h")
 
 READ_REQ_DTYPE = np.dtype([("group", "<u4"), ("reserved", "<u4"), ("ctx", "<u8")])
 READ_STATE_DTYPE = np.dtype([("group", "<u4"), ("reserved", "<u4"), ("ctx", "<u8"), ("index", "<u8")])
 REC_HEARTBEAT, REC_READ_CTX = 0x04, 0x08
 QUEUED, READY, DUP, DROPPED, FULL, NO_GROUP, NO_CTX = range(1, 8)
-
-
-def build(force: bool = False) -> str:
-    """Compile libread_oracle.so when it is missing or older than its sources; returns its path."""
-    out_dir = _HERE if os.access(_HERE, os.W_OK) else os.path.join(tempfile.gettempdir(), f"read_oracle_{os.getuid()}")
-    os.makedirs(out_dir, exist_ok=True)
-    path = os.path.join(out_dir, "libread_oracle.so")
-    newest = max(os.path.getmtime(os.path.join(_HERE, f)) for f in _SOURCES + _HEADERS)
-    if force or not os.path.exists(path) or os.path.getmtime(path) < newest:
-        tmp = f"{path}.{os.getpid()}"
-        subprocess.run([os.environ.get("CC", "gcc"), *CO.CFLAGS, "-shared", "-o", tmp,
-                        *[os.path.join(_HERE, f) for f in _SOURCES]], check=True)
-        os.replace(tmp, path)
-    return path
 
 
 class Queues(C.Structure):
@@ -51,7 +30,7 @@ _lib = None
 def lib() -> C.CDLL:
     global _lib
     if _lib is None:
-        L = C.CDLL(build())
+        L = O.lib()
         V, vp, sz = C.POINTER(O.ArenaView), C.c_void_p, C.c_size_t
         Q = C.POINTER(Queues)
         for name in ("ro_read_request",):

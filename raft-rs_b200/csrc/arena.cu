@@ -36,6 +36,7 @@ namespace {
 
 constexpr int kNumSets = 3;        // staging sets: one filling, up to two steps in flight
 constexpr uint32_t kChunk = 2048;  // records per staging chunk (48 KiB)
+constexpr size_t kScratchBytes = 256;  // d_scratch / h_scratch
 
 // A record moved to a later wave: its packed form (1..4 PackedRec) plus where its result goes.
 struct OverflowRec {
@@ -231,7 +232,7 @@ struct raftgpu_arena {
     Columns cols{};
     uint32_t *d_wire_first = nullptr;  // [kSlots][cap] wire steps: first frame of every cell (allocated on first use)
     unsigned long long *d_counters = nullptr;
-    void *d_scratch = nullptr;  // 256 B for single-group queries
+    void *d_scratch = nullptr;  // kScratchBytes for the small results of single calls (scratch<T>)
     void *h_scratch = nullptr;  // pinned mirror
     cudaStream_t s_compute = nullptr, s_h2d = nullptr, s_d2h = nullptr;
     StagingSet sets[kNumSets];
@@ -407,6 +408,13 @@ inline cudaStream_t pick_stream(raftgpu_arena *a, void *stream) {
 
 inline uint32_t div_up(uint64_t a, uint32_t b) { return static_cast<uint32_t>((a + b - 1) / b); }
 
+// d_scratch or h_scratch as N values of T, from offset 0 (the rule is at their allocation in raftgpu_arena_create)
+template <typename T, size_t N = 1>
+T *scratch(void *p) {
+    static_assert(sizeof(T) * N <= kScratchBytes, "d_scratch / h_scratch hold kScratchBytes");
+    return static_cast<T *>(p);
+}
+
 // True when every group of [first, first+n) is the plain 5-voter configuration in slots 0..4
 // (no joint half, no group commit): the host's meta mirror is authoritative, so the kernels
 // specialised for that case need no per-group check.
@@ -520,16 +528,55 @@ int32_t launch_verified_apply(raftgpu_arena *a, StagingSet &s, Src src, uint64_t
     return RAFTGPU_OK;
 }
 
-// d_wire holds at least `need` bytes (+ a quarter: a batch that grows slowly is not reallocated on every step)
-int32_t grow_wire(raftgpu_arena *a, StagingSet &s, uint64_t need) {
-    if (s.d_wire_cap >= need) return RAFTGPU_OK;
-    CK(a, cudaStreamSynchronize(a->s_compute));  // nothing may still read the old buffer
-    CK(a, cudaFree(s.d_wire));
-    s.d_wire = nullptr;
-    s.d_wire_cap = 0;
-    const int32_t rc = dev_alloc(a, &s.d_wire, need + need / 4, false);
+// A device buffer grown on demand (*ptr, *cap elements of T) holds at least `need`: when it does not, st is synchronised
+// (nothing may still read the old buffer), the buffer freed and need + a quarter allocated (a batch that grows slowly
+// is not reallocated on every call).
+template <typename T>
+int32_t grow_scratch(raftgpu_arena *a, cudaStream_t st, T **ptr, uint64_t *cap, uint64_t need) {
+    if (*cap >= need) return RAFTGPU_OK;
+    CK(a, cudaStreamSynchronize(st));
+    CK(a, cudaFree(*ptr));
+    *ptr = nullptr;
+    *cap = 0;
+    const uint64_t want = need + need / 4;
+    const int32_t rc = dev_alloc(a, ptr, want, false);
     if (rc != RAFTGPU_OK) return rc;
-    s.d_wire_cap = need + need / 4;
+    *cap = want;
+    return RAFTGPU_OK;
+}
+
+// d_wire holds at least `need` bytes
+int32_t grow_wire(raftgpu_arena *a, StagingSet &s, uint64_t need) {
+    return grow_scratch(a, a->s_compute, &s.d_wire, &s.d_wire_cap, need);
+}
+
+// Consecutive regions of a staging set's d_wire, each from a 16-byte boundary: take(bytes) returns the next region's
+// offset; `end` is where the last region ends (what grow_wire needs).
+struct WireLayout {
+    uint64_t end = 0;
+    uint64_t take(uint64_t bytes) {
+        const uint64_t at = (end + 15u) & ~15ull;
+        end = at + bytes;
+        return at;
+    }
+};
+
+// A wire pass's first-frame table (`n` u32, allocated on first use) filled with 0xff on st: no frame yet.  Every pass
+// keeps its own table (DESIGN 3.10).
+int32_t reset_first_frames(raftgpu_arena *a, cudaStream_t st, uint32_t **table, size_t n) {
+    if (!*table) {
+        const int32_t rc = dev_alloc(a, table, n, false);
+        if (rc != RAFTGPU_OK) return rc;
+    }
+    CK(a, cudaMemsetAsync(*table, 0xff, n * sizeof(uint32_t), st));
+    return RAFTGPU_OK;
+}
+
+// The limits of every wire batch: frame offsets and counts are u32 on the device, and the staging kernels read the
+// bytes with 16-byte loads (d_bytes = nullptr: not checked here, for a form that copies the bytes to d_wire itself).
+int32_t wire_batch_check(raftgpu_arena *a, uint64_t n_bytes, uint64_t n, const void *d_bytes) {
+    if (n > 0xfffffff0ull || n_bytes > 0xfffffff0ull) return fail(a, RAFTGPU_ERR_INVALID, "wire batch larger than 4 GiB");
+    if (reinterpret_cast<uintptr_t>(d_bytes) & 15u) return fail(a, RAFTGPU_ERR_INVALID, "wire bytes must be 16-byte aligned");
     return RAFTGPU_OK;
 }
 
@@ -703,8 +750,11 @@ int32_t create(int32_t device, uint32_t max_groups, uint32_t slots, uint32_t n_r
     TRY(dev_alloc(a, &c.term, a->cap));
     TRYC(cudaMemset(c.term_start, 0xff, sizeof(uint64_t) * a->cap));  // RAFTGPU_NO_TERM_START
     TRY(dev_alloc(a, &a->d_counters, kCntCount + 8));  // + 8 diagnostic slots (fused kernel phase cycles)
-    TRY(dev_alloc(a, reinterpret_cast<uint8_t **>(&a->d_scratch), 256));
-    TRY(pin_alloc(a, reinterpret_cast<uint8_t **>(&a->h_scratch), 256));
+    // d_scratch / h_scratch: every user sees them as its own type at offset 0 (scratch<T>), because no two users are
+    // ever live at once: each holds ctl_mu and synchronises s_compute before it returns, and no step kernel touches
+    // d_scratch.
+    TRY(dev_alloc(a, reinterpret_cast<uint8_t **>(&a->d_scratch), kScratchBytes));
+    TRY(pin_alloc(a, reinterpret_cast<uint8_t **>(&a->h_scratch), kScratchBytes));
 
     const uint64_t wave0_total = static_cast<uint64_t>(a->n_chunks) * kChunk;
     const uint64_t rec_total = rec_slots(a);

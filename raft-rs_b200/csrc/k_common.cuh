@@ -1,4 +1,5 @@
-// k_common.cuh -- the arena columns, counters, the quorum selection (MajorityConfig / JointConfig::committed_index), block-level counter flush.
+// k_common.cuh -- the arena columns, counters, the quorum selection (MajorityConfig / JointConfig::committed_index), block-level
+// counter flush and sums, the warp-level reservation of output slots.
 // Part of kernels.cuh (included there, inside namespace raftgpu; not a standalone header).
 
 constexpr int kSlots = RAFTGPU_SLOTS;
@@ -437,4 +438,43 @@ __device__ __forceinline__ void block_flush_counts(const uint32_t (&local)[kN], 
         atomicAdd(&counters[which[threadIdx.x]], static_cast<unsigned long long>(s_cnt[threadIdx.x]));
         if (extra_u32 && threadIdx.x == 1) atomicAdd(extra_u32, s_cnt[1]);
     }
+}
+
+// Per-thread u32 values -> the block's K sums at out[K * blockIdx.x + k]: a warp reduce, one shared word per warp and
+// value, then thread k adds the warps' words of value k.  Every thread of the block (kThreads of them) calls it.
+template <uint32_t K, uint32_t kThreads>
+__device__ __forceinline__ void block_sums(const uint32_t (&v)[K], uint32_t *__restrict__ out) {
+    __shared__ uint32_t sum[K][kThreads / 32];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    uint32_t r[K];
+#pragma unroll
+    for (uint32_t k = 0; k < K; k++) r[k] = __reduce_add_sync(0xffffffffu, v[k]);
+    if (lane == 0) {
+#pragma unroll
+        for (uint32_t k = 0; k < K; k++) sum[k][warp] = r[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        uint32_t t = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < kThreads / 32; w++) t += sum[threadIdx.x][w];
+        out[K * blockIdx.x + threadIdx.x] = t;
+    }
+}
+
+// Every lane of a full warp asks for `want` consecutive slots of *count: a warp scan, ONE atomic per warp (a million
+// same-address atomics, one per group, would serialise in L2), and each lane gets the first of its slots.
+template <typename T>
+__device__ __forceinline__ T warp_reserve(T *count, uint32_t want) {
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t incl = want;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= static_cast<uint32_t>(d)) incl += v;
+    }
+    const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+    T base = 0;
+    if (lane == 31 && total) base = atomicAdd(count, static_cast<T>(total));
+    return __shfl_sync(0xffffffffu, base, 31) + static_cast<T>(incl - want);
 }

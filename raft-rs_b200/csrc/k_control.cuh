@@ -54,18 +54,7 @@ send_list_kernel(Columns c, uint32_t first, uint32_t n, const uint32_t *__restri
                 if (((peers >> s) & 1u) && !paused) send |= 1u << s;
             }
         }
-        const uint32_t cnt = __popc(send);
-        uint32_t incl = cnt;  // inclusive warp scan
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
-            if (lane >= static_cast<uint32_t>(d)) incl += v;
-        }
-        const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
-        if (total == 0) continue;
-        unsigned long long pos = 0;
-        if (lane == 31) pos = atomicAdd(count, static_cast<unsigned long long>(total));
-        pos = __shfl_sync(0xffffffffu, pos, 31) + (incl - cnt);
+        unsigned long long pos = warp_reserve(count, __popc(send));
 #pragma unroll
         for (int s = 0; s < kSlots; s++) {
             if (!((send >> s) & 1u)) continue;

@@ -9,8 +9,8 @@
 //
 // Four kernels and no waiting between blocks: hfw_scan_kernel stages and decodes every frame once, classifies it and
 // writes a 48-byte record per passing frame; hfw_apply_kernel marks the later frames of a group DUP, runs commit_to
-// on the first one and sums the responses per block; hbf_scan_kernel<2> (k_hb_frames.cuh) turns the sums into block
-// starts; hfw_write_kernel encodes the responses (hb_msg_frame<9>) and stores them through shared memory.
+// on the first one and sums the responses per block; hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block
+// starts; hfw_write_kernel encodes the responses (wire_put_hb_frame<9>) and stores them through shared memory.
 
 constexpr uint32_t kHfwThreads = kWireThreads;  // frames per block of every kernel here: one block sum per scan block
 
@@ -27,19 +27,18 @@ struct __align__(16) HfwRec {
 };
 
 __device__ __forceinline__ uint32_t hfw_len(const HfwRec &r) {
-    return hbf_len(hb_msg_fixed(r.from, r.term, (r.w0 >> 32) & 1u), r.to, r.commit);
+    return wire_hb_len(wire_hb_fixed_len(r.from, r.term, (r.w0 >> 32) & 1u), r.to, r.commit);
 }
 
 // Frame i: its status before the duplicate rule (checks in the order of raftgpu.h) and, for RAFTGPU_WIRE_OK, its
 // record.
 __device__ __forceinline__ uint32_t hfw_frame(const Columns &c, const WireSrc &w, const HfwSrc &f, const WireStage &s,
                                               const uint8_t *stage, uint32_t i, HfwRec &r) {
-    uint32_t hdr, len;
-    const uint8_t *p = wire_frame_at(w, s, stage, i, hdr, len);
-    if (!p) return RAFTGPU_WIRE_MALFORMED;
-    const uint32_t g = hdr >> 4;
+    uint32_t hdr;
+    const uint8_t *msg;
     WireMsg m;
-    if (g >= w.n_groups || !wire_decode<true, true>(p + 4, len - 4u, m)) return RAFTGPU_WIRE_MALFORMED;
+    if (wire_open<true, true>(w, s, stage, i, hdr, msg, m) != RAFTGPU_WIRE_OK) return RAFTGPU_WIRE_MALFORMED;
+    const uint32_t g = hdr >> 4;
     const uint32_t meta = c.meta[g];
     if ((meta & RAFTGPU_META_WIDE_HI) || (c.rq_cap && !(c.rq_hc[g] & kRqAlloc))) return RAFTGPU_WIRE_MALFORMED;
     if (m.msg_type != 8u) return RAFTGPU_WIRE_SKIP_TYPE;  // MsgHeartbeat, eraftpb.proto:58
@@ -56,12 +55,7 @@ __device__ __forceinline__ uint32_t hfw_frame(const Columns &c, const WireSrc &w
     r.from = f.self_ids[g];                    // send: from = self.id (raft.rs:612)
     r.term = term;                             // send: term = self.term (raft.rs:650)
     r.commit = m.commit;
-    r.ctx = 0;
-    if (m.ctx_len) {
-        const uint8_t *q = p + 4 + m.ctx_off;
-#pragma unroll
-        for (int k = 0; k < 8; k++) r.ctx |= static_cast<uint64_t>(q[k]) << (8 * k);
-    }
+    r.ctx = m.ctx_len ? wire_ctx_u64(msg + m.ctx_off) : 0;
     return RAFTGPU_WIRE_OK;
 }
 
@@ -71,12 +65,9 @@ __device__ __forceinline__ uint32_t hfw_frame(const Columns &c, const WireSrc &w
 __global__ void __maxnreg__(40) hfw_scan_kernel(Columns c, WireSrc w, HfwSrc f, uint8_t *__restrict__ status,
                                                                HfwRec *__restrict__ recs, uint32_t *__restrict__ first_frame) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
-    const uint32_t first = blockIdx.x * kHfwThreads;
-    if (first >= w.n) return;
-    const uint32_t last = min(first + kHfwThreads, w.n);
-    const WireStage s = wire_stage_block(w, first, last, stage);
-    const uint32_t i = first + threadIdx.x;
-    if (i >= last) return;
+    WireStage s;
+    const uint32_t i = wire_block_frame(w, stage, s);
+    if (i == kNoFrame) return;
     HfwRec r;
     const uint32_t st = hfw_frame(c, w, f, s, stage, i, r);
     status[i] = static_cast<uint8_t>(st << 4);
@@ -120,45 +111,31 @@ __global__ void __launch_bounds__(kHfwThreads) hfw_apply_kernel(Columns c, uint3
         }
         if (from_out) from_out[i] = from;
     }
-    __shared__ uint32_t sum[2][kHfwThreads / 32];
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    resp = __reduce_add_sync(0xffffffffu, resp);
-    bytes = __reduce_add_sync(0xffffffffu, bytes);
-    if (lane == 0) {
-        sum[0][warp] = resp;
-        sum[1][warp] = bytes;
-    }
-    __syncthreads();
-    if (threadIdx.x < 2) {
-        uint32_t t = 0;
-#pragma unroll
-        for (uint32_t k = 0; k < kHfwThreads / 32; k++) t += sum[threadIdx.x][k];
-        blk[2 * blockIdx.x + threadIdx.x] = t;
-    }
+    block_sums<2, kHfwThreads>({resp, bytes}, blk);
 }
 
-// Pass 4 (after hbf_scan_kernel<2> turned blk into block starts): every block encodes its responses, in frame order,
+// Pass 4 (after hbf_scan_kernel<2>, k_wire.cuh, turned blk into block starts): every block encodes its responses, in frame order,
 // into shared memory at their offset from the 16-byte boundary below the block's start and stores them with
-// hbf_store_block; offsets [blk start, + its responses).  Reads 1 per frame + 48 per response; writes the responses
+// wire_store_block; offsets [blk start, + its responses).  Reads 1 per frame + 48 per response; writes the responses
 // and 4 per response.
 __global__ void __launch_bounds__(kHfwThreads) hfw_write_kernel(uint32_t n, const uint8_t *__restrict__ status,
                                                                 const HfwRec *__restrict__ recs, const uint32_t *__restrict__ blk,
                                                                 uint8_t *__restrict__ out, uint32_t *__restrict__ offsets) {
-    __shared__ __align__(16) uint8_t buf[kHfwThreads * kHbfFrameMax + 16];
+    __shared__ __align__(16) uint8_t buf[kHfwThreads * kWireHbFrameMax + 16];
     __shared__ uint32_t offs[kHfwThreads];
     const uint32_t i = blockIdx.x * kHfwThreads + threadIdx.x;
     const bool has = i < n && (status[i] & RAFTGPU_RES_OK);
     HfwRec r{};
     if (has) r = recs[i];
     uint32_t lf = has, lb = has ? hfw_len(r) : 0u, nf, nbytes;
-    hbf_block_scan<kHfwThreads / 32>(lf, lb, nf, nbytes);
+    wire_block_scan<kHfwThreads / 32>(lf, lb, nf, nbytes);
     const uint32_t f0 = blk[2 * blockIdx.x], b0 = blk[2 * blockIdx.x + 1], pad = b0 & 15u;
     if (has) {
         offs[lf] = b0 + lb;
-        hb_msg_frame<9>(buf + pad + lb, static_cast<uint32_t>(r.w0), r.to, r.from, r.term, r.commit, (r.w0 >> 32) & 1u,
+        wire_put_hb_frame<9>(buf + pad + lb, static_cast<uint32_t>(r.w0), r.to, r.from, r.term, r.commit, (r.w0 >> 32) & 1u,
                         r.ctx);  // MsgHeartbeatResponse, raft.rs:2458-2463
     }
     __syncthreads();
     for (uint32_t j = threadIdx.x; j < nf; j += kHfwThreads) offsets[f0 + j] = offs[j];
-    hbf_store_block<kHfwThreads>(out, buf, b0, nbytes);
+    wire_store_block<kHfwThreads>(out, buf, b0, nbytes);
 }

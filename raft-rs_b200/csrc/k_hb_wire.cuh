@@ -15,21 +15,18 @@
 // (w0 = group | slot << 32 | flags << 40, ctx, commit = m.commit).
 __device__ __forceinline__ uint32_t hb_wire_frame(const Columns &c, const WireSrc &w, const WireStage &s, const uint8_t *stage,
                                                   uint32_t i, uint64_t &w0, uint64_t &ctx, uint64_t &commit) {
-    uint32_t hdr, len;
-    const uint8_t *p = wire_frame_at(w, s, stage, i, hdr, len);
-    if (!p) return RAFTGPU_WIRE_MALFORMED;
-    const uint32_t group = hdr >> 4, slot = hdr & 15u;
+    uint32_t hdr;
+    const uint8_t *msg;
     WireMsg m;
-    if (group >= w.n_groups || !wire_decode<true>(p + 4, len - 4u, m)) return RAFTGPU_WIRE_MALFORMED;
+    if (wire_open<true>(w, s, stage, i, hdr, msg, m) != RAFTGPU_WIRE_OK) return RAFTGPU_WIRE_MALFORMED;
+    const uint32_t group = hdr >> 4, slot = hdr & 15u;
     if (m.msg_type != 9u) return RAFTGPU_WIRE_SKIP_TYPE;  // MsgHeartbeatResponse, eraftpb.proto:59
     const uint64_t gterm = c.term[group];
     if (gterm != 0 && m.term != gterm) return RAFTGPU_WIRE_TERM;
     uint32_t flags = RAFTGPU_REC_HEARTBEAT;
     if (m.ctx_len) {
         if (m.ctx_len != 8u || !c.rq_cap) return RAFTGPU_WIRE_CONTEXT;
-        const uint8_t *q = p + 4 + m.ctx_off;
-#pragma unroll
-        for (int k = 0; k < 8; k++) ctx |= static_cast<uint64_t>(q[k]) << (8 * k);
+        ctx = wire_ctx_u64(msg + m.ctx_off);
         flags |= RAFTGPU_REC_READ_CTX;  // raft.rs:1805-1818 runs for this response
     }
     w0 = static_cast<uint64_t>(group) | (static_cast<uint64_t>(slot) << 32) | (static_cast<uint64_t>(flags) << 40);
@@ -44,12 +41,9 @@ __global__ void __maxnreg__(40) hb_wire_scan_kernel(Columns c, WireSrc w, uint8_
                                                                     raftgpu_append_resp *__restrict__ recs,
                                                                     uint32_t *__restrict__ first_frame) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
-    const uint32_t first = blockIdx.x * kWireThreads;
-    if (first >= w.n) return;
-    const uint32_t last = min(first + kWireThreads, w.n);
-    const WireStage s = wire_stage_block(w, first, last, stage);
-    const uint32_t i = first + threadIdx.x;
-    if (i >= last) return;
+    WireStage s;
+    const uint32_t i = wire_block_frame(w, stage, s);
+    if (i == kNoFrame) return;
     uint64_t w0 = 0, ctx = 0, commit = 0;
     const uint32_t st = hb_wire_frame(c, w, s, stage, i, w0, ctx, commit);
     status[i] = static_cast<uint8_t>(st << 4);

@@ -49,23 +49,6 @@ __device__ __forceinline__ void rq_release(const Columns &c, uint32_t g, uint32_
     c.rq_hc[g] = (hc & kRqAlloc) | ((rq_count(hc) - m) << 8) | head;
 }
 
-// Every lane of a full warp asks for `want` consecutive slots of *count: a warp scan, ONE atomic per warp (a million
-// same-address atomics, one per group, would serialise in L2), and each lane gets the first of its slots.
-template <typename T>
-__device__ __forceinline__ T warp_reserve(T *count, uint32_t want) {
-    const uint32_t lane = threadIdx.x & 31;
-    uint32_t incl = want;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
-        if (lane >= static_cast<uint32_t>(d)) incl += v;
-    }
-    const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
-    T base = 0;
-    if (lane == 31 && total) base = atomicAdd(count, static_cast<T>(total));
-    return __shfl_sync(0xffffffffu, base, 31) + static_cast<T>(incl - want);
-}
-
 // ---------------------------------------------------------------------------
 // read_order_kernel: the requests must be in non-decreasing group order (queue order is arrival order).  A violation
 // sets *flag (which read_request_kernel reads before it applies anything) and bumps *bad once.

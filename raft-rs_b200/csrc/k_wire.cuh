@@ -20,6 +20,10 @@
 //
 // HBM-bound byte work: every block stages the contiguous byte range of its 256 frames into shared memory
 // with 16-byte loads (frames are ~26 bytes, unaligned) and the threads parse from there.
+//
+// The file holds the frame format in both directions: the decoder and the block staging every wire pass uses
+// (wire_open, wire_block_frame), and the heartbeat-kind encoder with the block-output code that the leader's
+// MsgHeartbeat frames (k_hb_frames.cuh) and the follower's MsgHeartbeatResponse frames (k_hb_follow.cuh) share.
 
 struct WireSrc {
     const uint8_t *bytes;     // 16-byte aligned
@@ -108,6 +112,15 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
     return true;
 }
 
+// The context convention of the heartbeat paths (DESIGN 3.10): a read id travels as the 8 bytes of the context,
+// little-endian.  q = the context's first byte (WireMsg::ctx_off from the Message's start).
+__device__ __forceinline__ uint64_t wire_ctx_u64(const uint8_t *q) {
+    uint64_t x = 0;
+#pragma unroll
+    for (int k = 0; k < 8; k++) x |= static_cast<uint64_t>(q[k]) << (8 * k);
+    return x;
+}
+
 // The block's frames -> shared memory (when their byte range is sane and fits); returns through smem.
 struct WireStage {
     uint32_t base, lo, hi;
@@ -135,27 +148,43 @@ __device__ __forceinline__ WireStage wire_stage_block(const WireSrc &w, uint32_t
     return s;
 }
 
-// Frame i's bytes (from the stage when they are there), its length and its u32 LE header; nullptr = not a frame
-// (offsets out of order or past the batch, shorter than the header).
-__device__ __forceinline__ const uint8_t *wire_frame_at(const WireSrc &w, const WireStage &s, const uint8_t *stage, uint32_t i,
-                                                        uint32_t &hdr, uint32_t &len) {
+// The prologue of every staging kernel (kWireThreads frames per block): stages the block's frames and returns the
+// thread's frame index, or kNoFrame past the batch.  A block past the batch returns at once, without staging.
+constexpr uint32_t kNoFrame = 0xffffffffu;  // (a frame index is below w.n <= 0xfffffff0)
+
+__device__ __forceinline__ uint32_t wire_block_frame(const WireSrc &w, uint8_t *stage, WireStage &s) {
+    const uint32_t first = blockIdx.x * kWireThreads;
+    if (first >= w.n) return kNoFrame;
+    const uint32_t last = min(first + kWireThreads, w.n);
+    s = wire_stage_block(w, first, last, stage);
+    const uint32_t i = first + threadIdx.x;
+    return i < last ? i : kNoFrame;
+}
+
+// Frame i opened: its u32 LE header, its Message (msg, from the stage when the bytes are there) decoded into m.
+// RAFTGPU_WIRE_MALFORMED when it is not a frame (offsets out of order or past the batch, shorter than the header),
+// names a group >= n_groups or is not a well-formed protobuf message; RAFTGPU_WIRE_OK otherwise.  The flags are
+// wire_decode's.
+template <bool kContext = false, bool kFrom = false>
+__device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage &s, const uint8_t *stage, uint32_t i,
+                                              uint32_t &hdr, const uint8_t *&msg, WireMsg &m) {
     const uint32_t a = w.offsets[i], b = w.offsets[i + 1];
-    if (b < a || b > w.n_bytes || b - a < 4u) return nullptr;
+    if (b < a || b > w.n_bytes || b - a < 4u) return RAFTGPU_WIRE_MALFORMED;
     const uint8_t *p = (s.staged && a >= s.lo && b <= s.hi) ? stage + (a - s.base) : w.bytes + a;
     hdr = p[0] | (static_cast<uint32_t>(p[1]) << 8) | (static_cast<uint32_t>(p[2]) << 16) | (static_cast<uint32_t>(p[3]) << 24);
-    len = b - a;
-    return p;
+    msg = p + 4;
+    if ((hdr >> 4) >= w.n_groups || !wire_decode<kContext, kFrom>(msg, b - a - 4u, m)) return RAFTGPU_WIRE_MALFORMED;
+    return RAFTGPU_WIRE_OK;
 }
 
 // Frame i: its status before the duplicate rule, the record, the REJECT's hint / request_snapshot.
 __device__ __forceinline__ uint32_t wire_frame(const Columns &c, const WireSrc &w, const WireStage &s, const uint8_t *stage,
                                                uint32_t i, RecRegs &rec, uint64_t &hint, uint64_t &request_snapshot) {
-    uint32_t hdr, len;
-    const uint8_t *p = wire_frame_at(w, s, stage, i, hdr, len);
-    if (!p) return RAFTGPU_WIRE_MALFORMED;
-    const uint32_t group = hdr >> 4, slot = hdr & 15u;
+    uint32_t hdr;
+    const uint8_t *msg;
     WireMsg m;
-    if (group >= w.n_groups || !wire_decode(p + 4, len - 4u, m)) return RAFTGPU_WIRE_MALFORMED;
+    if (wire_open(w, s, stage, i, hdr, msg, m) != RAFTGPU_WIRE_OK) return RAFTGPU_WIRE_MALFORMED;
+    const uint32_t group = hdr >> 4, slot = hdr & 15u;
     if (m.msg_type != 4u) return RAFTGPU_WIRE_SKIP_TYPE;  // MsgAppendResponse, eraftpb.proto:54
     const uint64_t gterm = c.term[group];
     if (gterm != 0 && m.term != gterm) return RAFTGPU_WIRE_TERM;
@@ -173,12 +202,9 @@ __device__ __forceinline__ uint32_t wire_frame(const Columns &c, const WireSrc &
 __global__ void __launch_bounds__(kWireThreads) wire_scan_kernel(Columns c, WireSrc w, uint8_t *__restrict__ status,
                                                                  uint32_t *__restrict__ first_frame) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
-    const uint32_t first = blockIdx.x * kWireThreads;
-    if (first >= w.n) return;
-    const uint32_t last = min(first + kWireThreads, w.n);
-    const WireStage s = wire_stage_block(w, first, last, stage);
-    const uint32_t i = first + threadIdx.x;
-    if (i >= last) return;
+    WireStage s;
+    const uint32_t i = wire_block_frame(w, stage, s);
+    if (i == kNoFrame) return;
     RecRegs rec;
     uint64_t hint, snap;
     const uint32_t st = wire_frame(c, w, s, stage, i, rec, hint, snap);
@@ -197,8 +223,9 @@ __global__ void __launch_bounds__(kWireThreads) wire_apply_kernel(Columns c, Wir
                                                                   uint32_t *__restrict__ dup_count) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
     uint32_t local[5] = {0, 0, 0, 0, 0};  // records, updates, rejects, decrements, no_progress
+    // the prologue of wire_block_frame written out: through the helper, ptxas spills in this kernel
     const uint32_t first = blockIdx.x * kWireThreads;
-    if (first < w.n) {
+    if (first < w.n) {  // (every thread goes on to block_flush_counts)
         const uint32_t last = min(first + kWireThreads, w.n);
         const WireStage s = wire_stage_block(w, first, last, stage);
         const uint32_t i = first + threadIdx.x;
@@ -220,4 +247,180 @@ __global__ void __launch_bounds__(kWireThreads) wire_apply_kernel(Columns c, Wir
     }
     const int which[5] = {kCntRecords, kCntUpdates, kCntRejects, kCntDecrements, kCntNoProgress};
     block_flush_counts<5>(local, which, counters, nullptr);
+}
+
+// ---------------------------------------------------------------------------
+// The encoder: heartbeat-kind frames (MsgHeartbeat at the leader, MsgHeartbeatResponse at the follower), and the
+// block-output code of the passes that write them -- a block scan of {frames, bytes}, the one-block scan of the block
+// sums (hbf_scan_kernel) and the 16-byte store of a block's contiguous output.
+
+constexpr uint32_t kWireHbFrameMax = 60;  // 4-byte header + at most 56 bytes of Message
+constexpr uint32_t kHbfScanThreads = 1024;
+
+// bytes of v as a base-128 varint
+__device__ __forceinline__ uint32_t wire_varint_len(uint64_t v) {
+    return v ? (70u - static_cast<uint32_t>(__clzll(static_cast<long long>(v)))) / 7u : 1u;
+}
+
+// Bytes of a heartbeat-kind frame (MsgHeartbeat, k_hb_frames.cuh; MsgHeartbeatResponse, k_hb_follow.cuh) before its
+// `to` and `commit`: header, msg_type, from, term (never 0 on these paths) and the 8-byte context when there is one.
+__device__ __forceinline__ uint32_t wire_hb_fixed_len(uint64_t from, uint64_t term, bool has_ctx) {
+    return 4u + 2u + (from ? 1u + wire_varint_len(from) : 0u) + 1u + wire_varint_len(term) + (has_ctx ? 10u : 0u);
+}
+
+// Bytes of the frame to a peer with id `to` and commit `commit`, after the fields its group's frames share (`fixed`,
+// wire_hb_fixed_len).
+__device__ __forceinline__ uint32_t wire_hb_len(uint32_t fixed, uint64_t to, uint64_t commit) {
+    return fixed + (to ? 1u + wire_varint_len(to) : 0u) + (commit ? 1u + wire_varint_len(commit) : 0u);
+}
+
+__device__ __forceinline__ uint8_t *wire_put_varint(uint8_t *p, uint64_t v) {
+    while (v >= 0x80u) {
+        *p++ = static_cast<uint8_t>(v | 0x80u);
+        v >>= 7;
+    }
+    *p++ = static_cast<uint8_t>(v);
+    return p;
+}
+
+// One heartbeat-kind frame: u32 LE header, then eraftpb.Message (eraftpb.proto:71-92) in field-number order with zero
+// scalars omitted: 1 msg_type = kType (MsgHeartbeat 8, MsgHeartbeatResponse 9, eraftpb.proto:58-59), 2 to, 3 from,
+// 4 term (never 0 on these paths), 8 commit, 12 context (the 8 little-endian bytes of ctx when has_ctx).
+template <uint8_t kType>
+__device__ __forceinline__ uint8_t *wire_put_hb_frame(uint8_t *p, uint32_t hdr, uint64_t to, uint64_t from, uint64_t term,
+                                                 uint64_t commit, bool has_ctx, uint64_t ctx) {
+    p[0] = static_cast<uint8_t>(hdr);
+    p[1] = static_cast<uint8_t>(hdr >> 8);
+    p[2] = static_cast<uint8_t>(hdr >> 16);
+    p[3] = static_cast<uint8_t>(hdr >> 24);
+    p[4] = 0x08;  // field 1, varint
+    p[5] = kType;
+    p += 6;
+    if (to) {
+        *p++ = 0x10;
+        p = wire_put_varint(p, to);
+    }
+    if (from) {
+        *p++ = 0x18;
+        p = wire_put_varint(p, from);
+    }
+    *p++ = 0x20;
+    p = wire_put_varint(p, term);
+    if (commit) {
+        *p++ = 0x40;
+        p = wire_put_varint(p, commit);
+    }
+    if (has_ctx) {
+        p[0] = 0x62;
+        p[1] = 8;
+#pragma unroll
+        for (int k = 0; k < 8; k++) p[2 + k] = static_cast<uint8_t>(ctx >> (8 * k));
+        p += 10;
+    }
+    return p;
+}
+
+// Exclusive scan of two u32 counts over a block of W warps; *tot_a / *tot_b = the block's sums (every thread).
+template <uint32_t W>
+__device__ __forceinline__ void wire_block_scan(uint32_t &a, uint32_t &b, uint32_t &tot_a, uint32_t &tot_b) {
+    __shared__ uint32_t wa[W], wb[W];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    uint32_t ia = a, ib = b;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t va = __shfl_up_sync(0xffffffffu, ia, d), vb = __shfl_up_sync(0xffffffffu, ib, d);
+        if (lane >= static_cast<uint32_t>(d)) {
+            ia += va;
+            ib += vb;
+        }
+    }
+    if (lane == 31) {
+        wa[warp] = ia;
+        wb[warp] = ib;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t xa = lane < W ? wa[lane] : 0u, xb = lane < W ? wb[lane] : 0u;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t va = __shfl_up_sync(0xffffffffu, xa, d), vb = __shfl_up_sync(0xffffffffu, xb, d);
+            if (lane >= static_cast<uint32_t>(d)) {
+                xa += va;
+                xb += vb;
+            }
+        }
+        if (lane < W) {  // inclusive -> the warps' exclusive starts, the sums behind them
+            wa[lane] = xa;
+            wb[lane] = xb;
+        }
+    }
+    __syncthreads();
+    tot_a = wa[W - 1];
+    tot_b = wb[W - 1];
+    const uint32_t sa = warp ? wa[warp - 1] : 0u, sb = warp ? wb[warp - 1] : 0u;
+    a = sa + ia - a;
+    b = sb + ib - b;
+    __syncthreads();  // wa / wb may be reused by the caller's next scan
+}
+
+// Pass 2, one block: blk's frames and bytes become each block's exclusive starts.  K = u32 per block in blk: {frames,
+// bytes} (K = 2, k_hb_follow.cuh) or {frames, bytes, leaders without a term} (K = 3); totals = the K sums.  flag[0] =
+// the output fits (d_offsets given, frames <= frames_cap, bytes <= bytes_cap); then offsets[frames] = bytes, the end of
+// the last frame.
+template <uint32_t K>
+__global__ void __launch_bounds__(kHbfScanThreads) hbf_scan_kernel(uint32_t *__restrict__ blk, uint32_t nb, uint64_t bytes_cap,
+                                                                   uint64_t frames_cap, uint64_t *__restrict__ totals,
+                                                                   uint32_t *__restrict__ offsets, uint32_t *__restrict__ flag) {
+    static_assert(K == 2 || K == 3, "blk holds {frames, bytes[, leaders without a term]} per block");
+    uint32_t carry_f = 0, carry_b = 0, no_term = 0;
+    for (uint32_t j0 = 0; j0 < nb; j0 += kHbfScanThreads) {  // (uniform trip count: every thread reaches the scan)
+        const uint32_t j = j0 + threadIdx.x;
+        uint32_t f = 0, b = 0;
+        if (j < nb) {
+            f = blk[K * j];
+            b = blk[K * j + 1];
+            if constexpr (K == 3) no_term += blk[K * j + 2];
+        }
+        uint32_t tf, tb;
+        wire_block_scan<kHbfScanThreads / 32>(f, b, tf, tb);
+        if (j < nb) {
+            blk[K * j] = carry_f + f;
+            blk[K * j + 1] = carry_b + b;
+        }
+        carry_f += tf;
+        carry_b += tb;
+    }
+    uint64_t t = 0;
+    if constexpr (K == 3) {
+        no_term = __reduce_add_sync(0xffffffffu, no_term);
+        __shared__ uint32_t nt[kHbfScanThreads / 32];
+        if ((threadIdx.x & 31u) == 0) nt[threadIdx.x >> 5] = no_term;
+        __syncthreads();
+        if (threadIdx.x == 0)
+            for (uint32_t w = 0; w < kHbfScanThreads / 32; w++) t += nt[w];
+    }
+    if (threadIdx.x == 0) {
+        totals[0] = carry_f;
+        totals[1] = carry_b;
+        if constexpr (K == 3) totals[2] = t;
+        const bool fits = offsets && carry_f <= frames_cap && carry_b <= bytes_cap;
+        flag[0] = fits;
+        if (fits) offsets[carry_f] = carry_b;
+    }
+}
+
+// A block's contiguous output [b0, b0 + nbytes) from shared memory, where it was assembled at buf + (b0 & 15): whole
+// 16-byte chunks go out as uint4 stores, only the two chunks shared with the neighbouring blocks byte by byte.
+template <uint32_t kThreads>
+__device__ __forceinline__ void wire_store_block(uint8_t *__restrict__ out, const uint8_t *buf, uint32_t b0, uint32_t nbytes) {
+    const uint32_t a0 = b0 & ~15u, end = b0 + nbytes;
+    for (uint32_t q = a0 + 16u * threadIdx.x; q < end; q += 16u * kThreads) {
+        const uint8_t *src = buf + (q - a0);
+        if (q >= b0 && q + 16u <= end) {
+            *reinterpret_cast<uint4 *>(out + q) = *reinterpret_cast<const uint4 *>(src);
+        } else {
+            for (uint32_t k = 0; k < 16u; k++)
+                if (q + k >= b0 && q + k < end) out[q + k] = src[k];
+        }
+    }
 }
