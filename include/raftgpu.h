@@ -645,10 +645,13 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
                                       applied in arrival order, one message per step -- resubmit it with the next batch */
 #define RAFTGPU_WIRE_CONTEXT 6u    /* (raftgpu_heartbeat_wire only) a context that is not an 8-byte read id, or any context
                                       on an arena without read queues: the host's own ReadOnly handles the frame */
-#define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat only) the group is not selected as a follower, or is a
-                                      leader: Raft::step on the host */
+#define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat, raftgpu_vote_wire) the group is not selected for the
+                                      role the pass serves, or is a leader; at raftgpu_vote_wire also a response type
+                                      that is not the candidate's own (step_candidate ignores it): Raft::step on the host */
 #define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat only) m.commit beyond max(committed, last_index):
                                         commit_to would be fatal! (raft_log.rs:291-298) */
+#define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire only) m.commit != 0, m.commit_term != 0 and m.commit beyond
+                                        committed: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
 typedef struct raftgpu_wire_batch {
     const uint8_t *bytes;    /* the frames, back to back */
     uint64_t n_bytes;
@@ -936,6 +939,53 @@ int32_t raftgpu_follower_heartbeat(raftgpu_arena *arena, const void *bytes, uint
                                    uint64_t n, const uint32_t *select, const uint64_t *self_ids, uint8_t *status,
                                    uint64_t *from, uint8_t *resp_bytes, uint64_t resp_bytes_capacity,
                                    uint32_t *resp_offsets, uint64_t *totals);
+
+/* ---- vote responses at a candidate ---------------------------------------------- */
+
+/* RawNode::step -> Raft::step (raft.rs:1280-1349) -> step_candidate (raft.rs:2230-2243) -> poll's record_vote and
+ * tally_votes (raft.rs:2166-2168, tracker.rs:308-340) for the MsgRequestVoteResponse (6) and MsgRequestPreVoteResponse
+ * (18) frames of a wire batch.  The transitions poll makes on a decided tally are NOT applied: become_leader appends to
+ * the caller's log, and role, leader_id and vote are the caller's.  The pass lists the decided groups instead, and the
+ * caller runs its control lists for them (INTEGRATION.md section 6).
+ * Input.  The frames of raftgpu_wire_batch (u32 LE group << 4 | peer_slot, then the Message; peer 8 + s of a wide pair
+ * is cell (g + 1, s)).  d_bytes 16-byte aligned, n and n_bytes below 4 GiB.
+ * Role.  d_select (required) and d_pre (nullable: no PreCandidates) are bitmaps in the layout of d_adv_bitmap: d_select
+ * marks the groups whose Raft is a PreCandidate or a Candidate, d_pre the PreCandidates among them.  A frame addressed
+ * to the high half of a wide pair is checked against the low half's bits, term, term_start and committed (the larger
+ * of both halves', as raftgpu_group_get reports).
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4 | RAFTGPU_RES_*; the first failing check decides:
+ *   MALFORMED    a bad frame or protobuf, or a group at or past the highest allocated slot;
+ *   SKIP_TYPE    any type but 6 and 18 (append and heartbeat responses are left to their own passes);
+ *   ROLE         the select bit is clear, the group is a leader (term_start != RAFTGPU_NO_TERM_START), the pair has no
+ *                voter (a freed slot, or a group not configured yet), or type 6 at a PreCandidate / 18 at a Candidate;
+ *   TERM         the group's term (raftgpu_group_set_term) or m.term is 0; at a Candidate m.term != term; at a
+ *                PreCandidate m.term < term, or a rejection with m.term > term (become_follower).  A granted pre-vote
+ *                with m.term > term passes and leaves the term alone (raft.rs:1319-1330);
+ *   COMMIT_VOTE  m.commit != 0, m.commit_term != 0 and m.commit > committed;
+ *   DUP          a later frame of a (group, peer) cell whose first passing frame is applied here.
+ * A frame that does not pass changes nothing: run RawNode::step on it.  An applied frame's low nibble: RAFTGPU_RES_OK
+ * when its vote was recorded, 0 when the cell already held a vote (record_vote is or_insert, as RAFTGPU_CTL_RECORD_VOTE),
+ * RAFTGPU_RES_NO_PROGRESS for a header slot of 8 or more (nothing recorded).  A vote of a non-voter slot is recorded
+ * and the tally ignores it, as in the reference.
+ * Output.  One raftgpu_vote_outcome per group (pair: the low half) that an applied frame names and whose tally after the
+ * pass is RAFTGPU_VOTE_WON or RAFTGPU_VOTE_LOST, in ascending group order; *d_count (u64) = how many.  Every touched
+ * group adds one to votes_tallied.  Votes only accumulate, so one tally after the batch is the first decided result
+ * that applying the frames one at a time would reach, in any order (DESIGN.md 3.13).  capacity must be at least
+ * min(n, allocated groups), which bounds the outcomes: RAFTGPU_ERR_INVALID before any launch otherwise, as are a missing
+ * d_count, d_select, d_status, d_bytes or d_offsets.  No outcome is written at or past capacity.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  The
+ * host form copies (select and pre cover the groups below the highest allocated one), runs and waits; status (n bytes)
+ * nullable, *out_n = the outcomes copied to `out`. */
+typedef struct raftgpu_vote_outcome {
+    uint32_t group;  /* low half for a wide pair */
+    uint32_t result; /* VoteResult | granted << 8 | rejected << 16, raftgpu_tally_votes' word */
+} raftgpu_vote_outcome;
+int32_t raftgpu_vote_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                 const uint32_t *d_offsets, uint64_t n, const uint32_t *d_select, const uint32_t *d_pre,
+                                 uint8_t *d_status, raftgpu_vote_outcome *d_out, uint64_t capacity, uint64_t *d_count);
+int32_t raftgpu_vote_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets, uint64_t n,
+                          const uint32_t *select, const uint32_t *pre, uint8_t *status, raftgpu_vote_outcome *out,
+                          uint64_t capacity, uint64_t *out_n);
 
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 

@@ -55,6 +55,21 @@ int32_t raftgpu_synth_wire_encode_heartbeats(const raftgpu_append_resp *recs, ui
                                              uint8_t *out_bytes, uint64_t bytes_cap, uint32_t *out_offsets,
                                              uint64_t *out_n_frames, uint64_t *out_n_bytes);
 
+/* One vote response as raftgpu_synth_wire_encode_votes writes it (56 bytes). */
+typedef struct raftgpu_synth_vote {
+    uint32_t hdr;      /* the frame's u32 header: group << 4 | peer_slot */
+    uint32_t msg_type; /* MsgRequestVoteResponse (6) or MsgRequestPreVoteResponse (18) */
+    uint64_t to, from, term, commit, commit_term;
+    uint32_t reject;   /* 0 or 1 */
+    uint32_t reserved;
+} raftgpu_synth_vote;
+
+/* Vote responses -> frames, one per entry in order: the header, then eraftpb.Message with msg_type, to, from, term,
+ * commit, reject and commit_term, fields in number order and zero scalars omitted (the canonical proto3 encoding:
+ * at most 63 bytes a frame, header included).  out_offsets has room for n + 1 entries.  RAFTGPU_ERR_FULL when bytes_cap is short. */
+int32_t raftgpu_synth_wire_encode_votes(const raftgpu_synth_vote *votes, uint64_t n, uint8_t *out_bytes, uint64_t bytes_cap,
+                                        uint32_t *out_offsets, uint64_t *out_n_bytes);
+
 #ifdef __cplusplus
 }
 #endif

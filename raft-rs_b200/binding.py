@@ -44,7 +44,11 @@ BULK_SORTED = 0x1
  COL_COMMIT_GROUP_ID, COL_PFLAGS, COL_VOTES, COL_META, COL_COMMITTED, COL_TERM_START,
  COL_LAST_INDEX, COL_TERM, COL_INS_META) = range(14)
 WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WIRE_CONTEXT = range(7)
-WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat only
+WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat (ROLE also raftgpu_vote_wire)
+WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire only
+# raftgpu_vote_wire's outcome: the group (a pair's low half) and its tally word (VoteResult | granted << 8 | rejected << 16)
+VOTE_OUTCOME_DTYPE = np.dtype([("group", "<u4"), ("result", "<u4")])
+assert VOTE_OUTCOME_DTYPE.itemsize == 8
 
 APPEND_RESP_DTYPE = np.dtype(
     [("group", "<u4"), ("peer_slot", "u1"), ("flags", "u1"), ("reserved", "<u2"),
@@ -308,6 +312,8 @@ def lib() -> C.CDLL:
             "raftgpu_follower_heartbeat_bound": ([u64], u64),
             "raftgpu_follower_heartbeat_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_heartbeat": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_vote_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp], i32),
+            "raftgpu_vote_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, C.POINTER(u64)], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -348,6 +354,8 @@ def synth_lib() -> C.CDLL:
         L.raftgpu_synth_wire_encode.restype = i32
         L.raftgpu_synth_wire_encode_heartbeats.argtypes = [vp, u64, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
         L.raftgpu_synth_wire_encode_heartbeats.restype = i32
+        L.raftgpu_synth_wire_encode_votes.argtypes = [vp, u64, vp, u64, vp, C.POINTER(u64)]
+        L.raftgpu_synth_wire_encode_votes.restype = i32
         _synth_lib = L
     return _synth_lib
 
@@ -357,6 +365,24 @@ def strerror(status: int) -> str:
 
 
 TILE_GROUPS = 256
+
+
+# raftgpu_synth_vote: one vote response for raftgpu_synth_wire_encode_votes
+SYNTH_VOTE_DTYPE = np.dtype([("hdr", "<u4"), ("msg_type", "<u4"), ("to", "<u8"), ("from", "<u8"), ("term", "<u8"),
+                             ("commit", "<u8"), ("commit_term", "<u8"), ("reject", "<u4"), ("reserved", "<u4")])
+assert SYNTH_VOTE_DTYPE.itemsize == 56
+
+
+def synth_encode_votes(votes: np.ndarray):
+    """raftgpu_synth_wire_encode_votes: SYNTH_VOTE_DTYPE entries -> (blob padded to 16 bytes, offsets u32[n + 1])."""
+    votes = np.ascontiguousarray(votes, dtype=SYNTH_VOTE_DTYPE)
+    n = len(votes)
+    blob, off, nb = np.zeros(64 * n + 16, np.uint8), np.zeros(n + 1, np.uint32), C.c_uint64()
+    rc = synth_lib().raftgpu_synth_wire_encode_votes(votes.ctypes.data, n, blob.ctypes.data, len(blob), off.ctypes.data,
+                                                     C.byref(nb))
+    if rc != OK:
+        raise RaftGpuError(rc, "synth_wire_encode_votes")
+    return blob[: (nb.value + 15) // 16 * 16 + 16].copy(), off
 
 
 def follower_heartbeat_bound(n: int) -> int:
@@ -889,6 +915,30 @@ class Arena:
         self._ck(self._L.raftgpu_follower_heartbeat_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_select,
                                                            d_self_ids, d_status, d_from, d_resp_bytes, resp_bytes_capacity,
                                                            d_resp_offsets, d_totals), "follower_heartbeat_device")
+
+    def vote_wire(self, frames, select, pre=None):
+        """raftgpu_vote_wire: poll's record_vote + tally_votes for the MsgRequestVoteResponse / MsgRequestPreVoteResponse
+        frames of a wire batch (.bytes, .n_bytes, .offsets, .n).  select: u32 bitmap words from group 0 of the groups that
+        are PreCandidates or Candidates, pre: those that are PreCandidates (None: none); both cover the groups below the
+        highest allocated one -> (status u8[n], outcomes VOTE_OUTCOME_DTYPE[k] in ascending group order)."""
+        sel = np.ascontiguousarray(select, dtype=np.uint32)
+        pr = None if pre is None else np.ascontiguousarray(pre, dtype=np.uint32)
+        words = (self.get_info().hi + 31) // 32
+        assert len(sel) >= words and (pr is None or len(pr) >= words)
+        n = frames.n
+        status = np.zeros(n, np.uint8)
+        cap = min(n, self.get_info().n_alloc)
+        out = np.zeros(max(1, cap), VOTE_OUTCOME_DTYPE)
+        k = C.c_uint64()
+        self._ck(self._L.raftgpu_vote_wire(self._h, frames.bytes.ctypes.data, frames.n_bytes, frames.offsets.ctypes.data, n,
+                                           sel.ctypes.data, None if pr is None else pr.ctypes.data, status.ctypes.data,
+                                           out.ctypes.data, cap, C.byref(k)), "vote_wire")
+        return status, out[: k.value].copy()
+
+    def vote_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_select, d_pre, d_status, d_out, capacity, d_count,
+                         stream=None):
+        self._ck(self._L.raftgpu_vote_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_select, d_pre, d_status,
+                                                  d_out, capacity, d_count), "vote_wire_device")
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

@@ -262,6 +262,11 @@ struct raftgpu_arena {
     uint32_t *hfw_first = nullptr;
     uint64_t *hfw_scratch = nullptr;
     uint64_t hfw_scratch_cap = 0;
+    // raftgpu_vote_wire: first passing frame of every cell [kSlots][cap] (allocated on first use); grown on demand, in
+    // u64 words: one record per frame, the touched bitmap, the tally words [cap], the block sums
+    uint32_t *vw_first = nullptr;
+    uint64_t *vw_scratch = nullptr;
+    uint64_t vw_scratch_cap = 0;
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -646,6 +651,8 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->hbf_scratch);
     cudaFree(a->hfw_first);
     cudaFree(a->hfw_scratch);
+    cudaFree(a->vw_first);
+    cudaFree(a->vw_scratch);
     cudaFree(a->d_counters);
     cudaFree(a->d_scratch);
     cudaFreeHost(a->h_scratch);
@@ -1058,5 +1065,6 @@ extern "C" {
 #include "abi_hb_wire.inc"
 #include "abi_hb_frames.inc"
 #include "abi_hb_follow.inc"
+#include "abi_vote_wire.inc"
 
 }  // extern "C"

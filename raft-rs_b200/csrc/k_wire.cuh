@@ -39,6 +39,7 @@ struct WireMsg {  // the scalar fields this path looks at
     uint64_t term, log_term, index, commit, reject_hint, request_snapshot;
     uint32_t ctx_off, ctx_len;  // wire_decode<true> only: bytes [ctx_off, ctx_off + ctx_len) are the last context (12)
     uint64_t from;              // wire_decode<true, true> only: field 3
+    uint64_t commit_term;       // wire_decode<.., .., true> only: field 15
 };
 
 constexpr uint32_t kWireThreads = 256;
@@ -60,14 +61,16 @@ __device__ __forceinline__ bool wire_varint(const uint8_t *p, uint32_t &pos, uin
 
 // One serialized Message -> WireMsg.  false = not a well-formed protobuf message.  kContext: also the context's
 // position (the heartbeat-response path, k_hb_wire.cuh); the AppendResponse kernels instantiate it without.  kFrom:
-// also `from` (the follower's heartbeat path, k_hb_follow.cuh).
-template <bool kContext = false, bool kFrom = false>
+// also `from` (the follower's heartbeat path, k_hb_follow.cuh).  kCommitTerm: also commit_term (the vote responses,
+// k_vote_wire.cuh).
+template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false>
 __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, WireMsg &m) {
     m.msg_type = 0;
     m.reject = false;
     m.term = m.log_term = m.index = m.commit = m.reject_hint = m.request_snapshot = 0;
     if constexpr (kContext) m.ctx_off = m.ctx_len = 0;
     if constexpr (kFrom) m.from = 0;
+    if constexpr (kCommitTerm) m.commit_term = 0;
     uint32_t pos = 0;
     while (pos < len) {
         uint64_t tag;
@@ -88,6 +91,9 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
             else if (field == 13) m.request_snapshot = v;
             if constexpr (kFrom) {
                 if (field == 3) m.from = v;
+            }
+            if constexpr (kCommitTerm) {
+                if (field == 15) m.commit_term = v;
             }
         } else if (wt == 1) {
             if (len - pos < 8) return false;
@@ -165,7 +171,7 @@ __device__ __forceinline__ uint32_t wire_block_frame(const WireSrc &w, uint8_t *
 // RAFTGPU_WIRE_MALFORMED when it is not a frame (offsets out of order or past the batch, shorter than the header),
 // names a group >= n_groups or is not a well-formed protobuf message; RAFTGPU_WIRE_OK otherwise.  The flags are
 // wire_decode's.
-template <bool kContext = false, bool kFrom = false>
+template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false>
 __device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage &s, const uint8_t *stage, uint32_t i,
                                               uint32_t &hdr, const uint8_t *&msg, WireMsg &m) {
     const uint32_t a = w.offsets[i], b = w.offsets[i + 1];
@@ -173,7 +179,8 @@ __device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage 
     const uint8_t *p = (s.staged && a >= s.lo && b <= s.hi) ? stage + (a - s.base) : w.bytes + a;
     hdr = p[0] | (static_cast<uint32_t>(p[1]) << 8) | (static_cast<uint32_t>(p[2]) << 16) | (static_cast<uint32_t>(p[3]) << 24);
     msg = p + 4;
-    if ((hdr >> 4) >= w.n_groups || !wire_decode<kContext, kFrom>(msg, b - a - 4u, m)) return RAFTGPU_WIRE_MALFORMED;
+    if ((hdr >> 4) >= w.n_groups || !wire_decode<kContext, kFrom, kCommitTerm>(msg, b - a - 4u, m))
+        return RAFTGPU_WIRE_MALFORMED;
     return RAFTGPU_WIRE_OK;
 }
 
@@ -366,29 +373,34 @@ __device__ __forceinline__ void wire_block_scan(uint32_t &a, uint32_t &b, uint32
 // Pass 2, one block: blk's frames and bytes become each block's exclusive starts.  K = u32 per block in blk: {frames,
 // bytes} (K = 2, k_hb_follow.cuh) or {frames, bytes, leaders without a term} (K = 3); totals = the K sums.  flag[0] =
 // the output fits (d_offsets given, frames <= frames_cap, bytes <= bytes_cap); then offsets[frames] = bytes, the end of
-// the last frame.
+// the last frame.  K = 1 (k_vote_wire.cuh): blk holds one count per block, totals[0] = their sum; the capacities,
+// offsets and flag are not used.
 template <uint32_t K>
 __global__ void __launch_bounds__(kHbfScanThreads) hbf_scan_kernel(uint32_t *__restrict__ blk, uint32_t nb, uint64_t bytes_cap,
                                                                    uint64_t frames_cap, uint64_t *__restrict__ totals,
                                                                    uint32_t *__restrict__ offsets, uint32_t *__restrict__ flag) {
-    static_assert(K == 2 || K == 3, "blk holds {frames, bytes[, leaders without a term]} per block");
+    static_assert(K >= 1 && K <= 3, "blk holds {count} or {frames, bytes[, leaders without a term]} per block");
     uint32_t carry_f = 0, carry_b = 0, no_term = 0;
     for (uint32_t j0 = 0; j0 < nb; j0 += kHbfScanThreads) {  // (uniform trip count: every thread reaches the scan)
         const uint32_t j = j0 + threadIdx.x;
         uint32_t f = 0, b = 0;
         if (j < nb) {
             f = blk[K * j];
-            b = blk[K * j + 1];
+            if constexpr (K >= 2) b = blk[K * j + 1];
             if constexpr (K == 3) no_term += blk[K * j + 2];
         }
         uint32_t tf, tb;
         wire_block_scan<kHbfScanThreads / 32>(f, b, tf, tb);
         if (j < nb) {
             blk[K * j] = carry_f + f;
-            blk[K * j + 1] = carry_b + b;
+            if constexpr (K >= 2) blk[K * j + 1] = carry_b + b;
         }
         carry_f += tf;
         carry_b += tb;
+    }
+    if constexpr (K == 1) {
+        if (threadIdx.x == 0) totals[0] = carry_f;
+        return;
     }
     uint64_t t = 0;
     if constexpr (K == 3) {

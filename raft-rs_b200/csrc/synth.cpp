@@ -252,4 +252,27 @@ int32_t raftgpu_synth_wire_encode_heartbeats(const raftgpu_append_resp *recs, ui
     return RAFTGPU_OK;
 }
 
+int32_t raftgpu_synth_wire_encode_votes(const raftgpu_synth_vote *votes, uint64_t n, uint8_t *out_bytes, uint64_t bytes_cap,
+                                        uint32_t *out_offsets, uint64_t *out_n_bytes) {
+    if ((!votes && n) || !out_bytes || !out_offsets || !out_n_bytes) return RAFTGPU_ERR_INVALID;
+    uint8_t *p = out_bytes;
+    out_offsets[0] = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        const raftgpu_synth_vote &v = votes[i];
+        if (static_cast<uint64_t>(p - out_bytes) + 64 > bytes_cap) return RAFTGPU_ERR_FULL;
+        memcpy(p, &v.hdr, 4);
+        p += 4;
+        p = put_field(p, 1, v.msg_type);
+        p = put_field(p, 2, v.to);
+        p = put_field(p, 3, v.from);
+        p = put_field(p, 4, v.term);
+        p = put_field(p, 8, v.commit);
+        p = put_field(p, 10, v.reject != 0);
+        p = put_field(p, 15, v.commit_term);
+        out_offsets[i + 1] = static_cast<uint32_t>(p - out_bytes);
+    }
+    *out_n_bytes = static_cast<uint64_t>(p - out_bytes);
+    return RAFTGPU_OK;
+}
+
 }  // extern "C"

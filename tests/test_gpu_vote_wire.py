@@ -1,0 +1,327 @@
+"""Vote responses at a candidate on the GPU (raftgpu_vote_wire[_device]) against the batch oracle
+(oracle/vote_wire_oracle.c): the reference's election table, every status, random 100K-group elections with joint
+configurations, learners, wide pairs and hostile frames, a 1M-group storm against INTEGRATION.md section 6's control
+list on a twin arena, one buffer through all three response passes, and the refusals.  Run with -m gpu."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+from oracle import oracle as O
+from oracle import control_oracle as CO
+from oracle import vote_wire_oracle as VW
+from helpers import B
+from control_cmds import cmds
+import hb_frames as F
+import vote_frames as V
+import test_oracle_vote_wire as T
+
+pytestmark = pytest.mark.gpu
+
+
+def _arena(e):
+    a = B.Arena(e.n + 64)
+    if e.n_narrow:
+        assert a.group_alloc_range(e.n_narrow) == 0
+    for k in range(e.n_wide):
+        assert a.group_alloc_wide() == e.n_narrow + 2 * k
+    assert np.all(a.control(e.setup)["status"] == 0)
+    a.control(e.campaign)
+    return a
+
+
+def _votes(a, n):
+    return np.stack([a.column_read(B.COL_VOTES, s, 0, n, np.uint8) for s in range(O.SLOTS)])
+
+
+def _device(a, blob, off, sel, pre, cap=None):
+    """The device form over buffers from raftgpu_device_alloc -> (status, outcomes)."""
+    n = len(off) - 1
+    cap = min(n, a.get_info().n_alloc) if cap is None else cap
+    bufs = [a.device_alloc(x) for x in (max(16, len(blob)), 4 * (n + 1), sel.nbytes, pre.nbytes, max(1, n), 8 * max(1, cap), 8)]
+    d_b, d_o, d_s, d_p, d_st, d_out, d_cnt = bufs
+    for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_p, pre)):
+        a.h2d(p, x)
+    a.vote_wire_device(d_b, len(blob), d_o, n, d_s, d_p, d_st, d_out, cap, d_cnt)
+    a.synchronize()
+    cnt = np.zeros(1, np.uint64)
+    a.d2h(cnt, d_cnt)
+    st, out = np.zeros(n, np.uint8), np.zeros(int(cnt[0]), B.VOTE_OUTCOME_DTYPE)
+    a.d2h(st, d_st)
+    if len(out):
+        a.d2h(out, d_out)
+    for p in bufs:
+        a.device_free(p)
+    return st, out
+
+
+# --------------------------------------------------------------------------- 1. the table and the statuses
+
+
+@pytest.mark.parametrize("case", range(len(T.ONE_ROUND)))
+def test_leader_election_in_one_round_rpc(case):
+    size, votes, state = T.ONE_ROUND[case]
+    a = B.Arena(64)
+    assert a.group_alloc_range(1) == 0
+    a.control(cmds((B.CTL_SET_CONF, 0, 0, 0, ((1 << size) - 1, 0, 0, 11)), (B.CTL_RESET, 0, 0, 0, (B.NO_TERM_START, 10, 5, 10))))
+    camp = cmds((B.CTL_RESET, 0, 0, 0, (B.NO_TERM_START, 10, 5, 10)), (B.CTL_SET_TERM, 0, 0, 0, (1,)),
+                (B.CTL_RESET_VOTES, 0), (B.CTL_RECORD_VOTE, 0, 0, 1), (B.CTL_VOTE_RESULT, 0))
+    first = int(a.control(camp)["value"][-1])
+    frames = [F.frame(0, k - 1, V.message(6, 1, not v, to=1, frm=k)) for k, v in votes.items()]
+    st, outs = a.vote_wire(F.Frames(frames), V.bitmap([True]))
+    assert np.all(st == (B.WIRE_OK << 4 | B.RES_OK))
+    assert T.expected_state(first, outs) == state and len(outs) == (state != "Candidate" and bool(frames))
+    a.close()
+
+
+def test_statuses_match_the_oracle():
+    """test_statuses_in_order's frames and arena through the C ABI (host form) and the device form."""
+    meta = B.make_meta(0x1F, 0, 0, 0)
+    for device in (False, True):
+        a = B.Arena(64)
+        assert a.group_alloc_range(4) == 0
+        a.control(cmds(*[(B.CTL_SET_CONF, g, 0, 0, (0x1F, 0, 0, 11)) for g in range(4)],
+                       *[(B.CTL_RESET, g, 0, 0, (11 if g == 2 else B.NO_TERM_START, 10, 5, 10)) for g in range(4)],
+                       *[(B.CTL_SET_TERM, g, 0, 0, (7,)) for g in range(4)]))
+        c, vt = T._arena([meta] * 4, [7] * 4)
+        c.term_start[2] = 11
+        frames = [F.frame(9, 1, V.message(6, 7)), F.frame(0, 1, b"\x08"), F.frame(0, 1, V.message(4, 7)),
+                  F.frame(3, 1, V.message(6, 7)), F.frame(2, 1, V.message(6, 7)), F.frame(0, 1, V.message(18, 7)),
+                  F.frame(1, 1, V.message(6, 7)), F.frame(0, 1, V.message(6, 0)), F.frame(0, 1, V.message(6, 8)),
+                  F.frame(1, 1, V.message(18, 6)), F.frame(1, 1, V.message(18, 8, True)),
+                  F.frame(0, 2, V.message(6, 7, commit=6, commit_term=7)), F.frame(0, 2, V.message(6, 7, commit=6)),
+                  F.frame(0, 3, V.message(6, 7, True)), F.frame(0, 2, V.message(6, 7, True)), F.frame(1, 1, V.message(18, 8)),
+                  F.frame(1, 9, V.message(18, 7)), F.frame(0, 4, V.message(6, 7))]
+        sel, pre = V.bitmap([True, True, True, False]), V.bitmap([False, True, False, False])
+        want_st, want_out, _ = T._run(c, vt, frames, [True, True, True, False], [False, True, False, False])
+        blob, off = F.batch(frames)
+        got = _device(a, np.concatenate([blob, np.zeros(16, np.uint8)]), off, sel, pre) if device else \
+            a.vote_wire(F.Frames(frames), sel, pre)
+        assert np.array_equal(got[0], want_st) and np.array_equal(got[1], want_out), (device, got, want_st, want_out)
+        assert np.array_equal(_votes(a, 4), vt[:, :4]) and np.count_nonzero(vt[:, :4]) == 4
+        a.close()
+
+
+# --------------------------------------------------------------------------- 2. random 100K-group elections
+
+
+@pytest.mark.parametrize("device", [False, True], ids=["host", "device"])
+def test_random_elections_vs_oracle(device):
+    rng = np.random.default_rng(0x7077 + device)
+    e = V.Election(rng, 96_000, 2_000)
+    a = _arena(e)
+    c, vt = T._state(e)
+    assert np.array_equal(_votes(a, e.n), vt[:, :e.n])
+    kinds = np.zeros(16, np.int64)
+    for rnd in range(2):
+        frames = e.frames(rng, commit_vote=True)
+        frames = [frames[i] for i in rng.permutation(len(frames))]
+        blob, off = F.batch(frames)
+        sel = V.bitmap(np.isin(e.role, (V.PRE_CANDIDATE, V.CANDIDATE)) & (rng.random(e.n) < 0.95))  # some unselected
+        sel = np.concatenate([sel, np.zeros(4, np.uint32)])
+        pre = np.concatenate([e.pre(), np.zeros(4, np.uint32)])
+        before = a.counters()["votes_tallied"]
+        want_st, want_out, tallied = VW.batch(c, vt, blob, off, sel, pre)
+        got_st, got_out = _device(a, np.concatenate([blob, np.zeros(16, np.uint8)]), off, sel, pre) if device else \
+            a.vote_wire(F.Frames(frames), sel, pre)
+        assert np.array_equal(got_st, want_st), (rnd, np.flatnonzero(got_st != want_st)[:5])
+        assert np.array_equal(got_out, want_out), rnd
+        assert np.array_equal(_votes(a, e.n), vt[:, :e.n]), rnd
+        assert a.counters()["votes_tallied"] - before == tallied
+        kinds += np.bincount(got_st >> 4, minlength=16)
+        assert len(want_out) > 10_000
+    for k in (B.WIRE_OK, B.WIRE_DUP, B.WIRE_ROLE, B.WIRE_TERM, B.WIRE_SKIP_TYPE, B.WIRE_MALFORMED, B.WIRE_COMMIT_VOTE):
+        assert kinds[k] > 100, (k, kinds)
+    a.close()
+
+
+# --------------------------------------------------------------------------- 3. the 1M-group storm
+
+
+def _storm_list(groups, slots, granted):
+    """Section 6 step 2: RECORD_VOTE + VOTE_RESULT per response."""
+    out = np.zeros(2 * len(groups), B.CTL_CMD_DTYPE)
+    out["group"] = np.repeat(groups, 2)
+    out["op"][0::2], out["op"][1::2] = B.CTL_RECORD_VOTE, B.CTL_VOTE_RESULT
+    out["peer_slot"][0::2], out["arg"][0::2] = slots, granted
+    return out
+
+
+def test_1m_storm_against_the_control_list():
+    rng = np.random.default_rng(0x7078)
+    n = 1_000_000
+    arenas = []
+    for _ in range(2):
+        a = B.Arena(n)
+        assert a.group_alloc_range(n) == 0
+        arenas.append(a)
+    g = np.arange(n, dtype=np.uint32)
+    last = rng.integers(10, 1 << 30, n).astype(np.uint64)
+    com = last - rng.integers(0, 10, n).astype(np.uint64)
+    term = rng.integers(1, 1 << 30, n).astype(np.uint64)
+    setup = np.zeros(5 * n, B.CTL_CMD_DTYPE)
+    setup["group"] = np.tile(g, 5)
+    setup["op"][:n], setup["peer_slot"][:n] = B.CTL_SET_CONF, 0
+    setup["a"][:n, 0], setup["a"][:n, 3] = 0x1F, last + 1
+    setup["op"][n:2 * n] = B.CTL_RESET                                        # section 6 step 1: the campaign
+    setup["a"][n:2 * n] = np.stack([np.full(n, B.NO_TERM_START, np.uint64), last, com, last], 1)
+    setup["op"][2 * n:3 * n], setup["a"][2 * n:3 * n, 0] = B.CTL_SET_TERM, term
+    setup["op"][3 * n:4 * n] = B.CTL_RESET_VOTES
+    setup["op"][4 * n:], setup["arg"][4 * n:] = B.CTL_RECORD_VOTE, 1
+    for a in arenas:
+        assert np.all(a.control(setup)["status"] == 0)
+    # 4M responses, shuffled: each peer of every group answers once
+    gs = np.repeat(g, 4)
+    slots = np.tile(np.arange(1, 5, dtype=np.uint32), n)
+    granted = (rng.random(4 * n) < 0.55).astype(np.uint32)
+    perm = rng.permutation(4 * n)
+    gs, slots, granted = gs[perm], slots[perm], granted[perm]
+    e = np.zeros(4 * n, B.SYNTH_VOTE_DTYPE)
+    e["hdr"], e["msg_type"], e["to"], e["from"] = gs << 4 | slots, 6, 1, slots + 1
+    e["term"], e["reject"] = term[gs], 1 - granted
+    blob, off = B.synth_encode_votes(e)
+    st, out = _device(arenas[0], blob, off, V.bitmap(np.ones(n, bool)), V.bitmap(np.zeros(n, bool)))
+    assert np.all(st == (B.WIRE_OK << 4 | B.RES_OK))
+    res = arenas[1].control(_storm_list(gs, slots, granted))
+    assert np.all(res["status"] == 0)
+    last_word = np.zeros(n, np.uint32)
+    last_word[gs] = res["value"][1::2].astype(np.uint32)                     # (the last write of a group wins)
+    decided = np.flatnonzero(last_word & 0xFF != B.VOTE_PENDING)
+    assert np.array_equal(out["group"], decided) and np.array_equal(out["result"], last_word[decided])
+    assert len(out) == n                                                     # 5 voters, every vote in: all decided
+    assert np.array_equal(_votes(arenas[0], n), _votes(arenas[1], n))
+    won = out["group"][(out["result"] & 0xFF) == B.VOTE_WON]
+    win = np.zeros(2 * len(won), B.CTL_CMD_DTYPE)                            # section 6 step 3 on both arenas
+    win["group"] = np.repeat(won, 2)
+    win["op"][0::2], win["op"][1::2] = B.CTL_RESET, B.CTL_BECOME_LEADER
+    win["a"][0::2] = np.stack([last[won] + 1, last[won], com[won], last[won]], 1)
+    for a in arenas:
+        assert np.all(a.control(win)["status"] == 0)
+    c0, c1 = arenas[0].read_columns(n), arenas[1].read_columns(n)
+    for name in B.COLUMNS:
+        assert np.array_equal(getattr(c0, name), getattr(c1, name)), name
+    assert np.array_equal(_votes(arenas[0], n), _votes(arenas[1], n))
+    for a in arenas:
+        a.close()
+
+
+# --------------------------------------------------------------------------- 4. one buffer, three passes
+
+
+def test_mixed_buffer_each_frame_applied_once():
+    """Append, heartbeat and vote responses in one buffer through raftgpu_step_begin_wire, raftgpu_heartbeat_wire and
+    raftgpu_vote_wire: every frame is applied (status OK) by at most one pass, and by exactly the one of its type when
+    the frame is well-formed for it."""
+    rng = np.random.default_rng(0x7079)
+    e = V.Election(rng, 4000, 0, p_role=(0.1, 0.4, 0.25, 0.25))
+    a = _arena(e)
+    frames, kind = [], []
+    for f in e.frames(rng, noise=False):
+        frames.append(f)
+        kind.append(6)
+    for g in range(e.n):
+        if e.role[g] != V.LEADER:
+            continue
+        for s in range(1, 5):
+            if not (int(e.present[g]) >> s & 1) or s == e.self_slot[g]:
+                continue
+            t = int(e.term[g])
+            frames.append(F.frame(g, s, F.message(4, term=t, index=int(e.last[g]))))
+            kind.append(4)
+            frames.append(F.frame(g, s, F.message(9, term=t, commit=int(e.committed[g]))))
+            kind.append(9)
+    order = rng.permutation(len(frames))
+    frames, kind = [frames[i] for i in order], np.array(kind)[order]
+    fb = F.Frames(frames)
+    vst, _ = a.vote_wire(fb, e.select(), e.pre())
+    hst, _ = a.heartbeat_wire(fb)
+    a.step_begin_wire(fb)
+    a.step_wait()
+    ast = a.wire_status().copy()
+    ok = np.stack([(x >> 4) == B.WIRE_OK for x in (ast, hst, vst)])
+    assert np.all(ok.sum(0) <= 1)
+    for row, k in enumerate((4, 9, 6)):
+        assert np.all(ok[row] <= (kind == k)) and ok[row][kind == k].mean() > 0.5, k
+        others = np.stack([ast, hst, vst])[row][kind != k] >> 4
+        assert np.all(others == B.WIRE_SKIP_TYPE), k
+    a.close()
+
+
+# --------------------------------------------------------------------------- 5. freed slots and the outcome bound
+
+
+def test_freed_selected_groups_stay_within_capacity():
+    """100 group slots of which 99 are freed (raftgpu_group_free leaves their term behind) but still selected, each hit
+    by a response at that term: only the allocated group is recorded and listed, and with capacity = min(n, allocated)
+    = 1 nothing is written past the first outcome, in either form."""
+    a = B.Arena(128)
+    assert a.group_alloc_range(100) == 0
+    a.control(cmds(*[(B.CTL_SET_CONF, g, 0, 0, (0b11, 0, 0, 11)) for g in range(100)],
+                   *[(B.CTL_SET_TERM, g, 0, 0, (4,)) for g in range(100)], (B.CTL_RECORD_VOTE, 0, 0, 1)))
+    for g in range(1, 100):
+        a.group_free(g)
+    info = a.get_info()
+    assert (info.hi, info.n_alloc) == (100, 1)
+    assert np.all(a.column_read(B.COL_TERM, 0, 0, 100, np.uint64) == 4)
+    frames = [F.frame(g, 1, V.message(6, 4)) for g in range(99, -1, -1)]
+    blob, off = F.batch(frames)
+    blob = np.concatenate([blob, np.zeros(16, np.uint8)])
+    n, sel = len(frames), V.bitmap(np.ones(128, bool))
+    want = [B.WIRE_ROLE << 4] * 99 + [B.WIRE_OK << 4 | B.RES_OK]
+    # the device form, with a guard entry after the one outcome the capacity allows
+    bufs = [a.device_alloc(x) for x in (len(blob), 4 * (n + 1), sel.nbytes, n, 16, 8)]
+    d_b, d_o, d_s, d_st, d_out, d_c = bufs
+    for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_out, np.full(16, 0xEE, np.uint8))):
+        a.h2d(p, x)
+    a.vote_wire_device(d_b, len(blob) - 16, d_o, n, d_s, None, d_st, d_out, 1, d_c)
+    a.synchronize()
+    st, out, cnt = np.zeros(n, np.uint8), np.zeros(16, np.uint8), np.zeros(1, np.uint64)
+    a.d2h(st, d_st), a.d2h(out, d_out), a.d2h(cnt, d_c)
+    assert st.tolist() == want and cnt.tolist() == [1]
+    assert out[:8].view(B.VOTE_OUTCOME_DTYPE).tolist() == [(0, B.VOTE_WON | 2 << 8)] and np.all(out[8:] == 0xEE)
+    v = _votes(a, 100)
+    assert v[1, 0] == 2 and np.count_nonzero(v[:, 1:]) == 0
+    for p in bufs:
+        a.device_free(p)
+    # the host form, on the same votes (or_insert: the second frame of group 0 finds its vote, result 0)
+    st, outs = a.vote_wire(F.Frames(frames), sel)
+    assert st.tolist() == want[:-1] + [B.WIRE_OK << 4] and outs.tolist() == [(0, B.VOTE_WON | 2 << 8)]
+    a.close()
+
+
+# --------------------------------------------------------------------------- 6. refusals
+
+
+def test_refusals_before_any_launch():
+    a = B.Arena(64)
+    assert a.group_alloc_range(16) == 0
+    a.control(cmds(*[(B.CTL_SET_CONF, g, 0, 0, (0x1F, 0, 0, 11)) for g in range(16)], *[(B.CTL_SET_TERM, g, 0, 0, (3,)) for g in range(16)]))
+    L, h = a._L, a._h
+    n = 16
+    blob, off = F.batch([F.frame(g, 1, V.message(6, 3)) for g in range(n)])
+    sel = V.bitmap(np.ones(64, bool))
+    d_b, d_o, d_s = a.device_alloc(1024), a.device_alloc(4 * (n + 1)), a.device_alloc(sel.nbytes)
+    d_st, d_out, d_c = a.device_alloc(n), a.device_alloc(8 * n), a.device_alloc(8)
+    for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_st, np.full(n, 0xEE, np.uint8)), (d_c, np.full(1, 77, np.uint64))):
+        a.h2d(p, x)
+    nb = len(blob)
+    dev = lambda **k: L.raftgpu_vote_wire_device(h, None, k.get("b", d_b), k.get("nb", nb), k.get("o", d_o), k.get("n", n),
+                                                 k.get("s", d_s), None, k.get("st", d_st), k.get("out", d_out),
+                                                 k.get("cap", n), k.get("c", d_c))
+    refused = [dev(cap=n - 1), dev(cap=0, out=None), dev(b=d_b + 4), dev(nb=1 << 32), dev(n=1 << 32, cap=1 << 32),
+               dev(s=None), dev(c=None), dev(st=None), dev(o=None), dev(b=None), dev(out=None)]
+    assert refused == [B.ERR_INVALID] * len(refused), refused
+    a.synchronize()
+    gst, gc = np.zeros(n, np.uint8), np.zeros(1, np.uint64)
+    a.d2h(gst, d_st), a.d2h(gc, d_c)
+    assert np.all(gst == 0xEE) and gc.tolist() == [77]                       # nothing was launched
+    assert np.all(_votes(a, 16) == 0)
+    cnt, outs = C.c_uint64(), np.zeros(n, B.VOTE_OUTCOME_DTYPE)
+    assert L.raftgpu_vote_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, sel.ctypes.data, None, None, outs.ctypes.data,
+                               n - 1, C.byref(cnt)) == B.ERR_INVALID
+    # the capacity rule counts allocated groups: 16 of them, so 16 frames need 16
+    assert dev(cap=16) == B.OK
+    a.synchronize()
+    a.d2h(gc, d_c)
+    assert gc.tolist() == [0] and np.all(_votes(a, 16)[1] == 2)
+    a.close()
