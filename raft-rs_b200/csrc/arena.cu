@@ -6,6 +6,7 @@
 // RAFTGPU_ERR_NO_DEVICE and nothing else can be called.
 #include <algorithm>
 #include <atomic>
+#include <cassert>
 #include <chrono>
 #include <condition_variable>
 #include <functional>
@@ -399,7 +400,7 @@ inline double trace_us(const raftgpu_arena *a) {
 inline bool group_ok(const raftgpu_arena *a, uint32_t g) { return g < a->cap && a->allocated[g]; }
 
 // PackedRec slots of a staging set's device record buffer (d_recs): wave 0 + the later waves.  Between steps the
-// buffer also stages the other forms' batches and the host calls' (host_batch_op, raftgpu_step_send_list).
+// buffer also stages the other forms' batches and the host calls' (HostFrame, raftgpu_step_send_list).
 inline uint64_t rec_slots(const raftgpu_arena *a) { return static_cast<uint64_t>(a->n_chunks) * kChunk + a->overflow_records; }
 
 inline uint32_t present_mask(uint32_t meta) {
@@ -554,17 +555,6 @@ int32_t grow_scratch(raftgpu_arena *a, cudaStream_t st, T **ptr, uint64_t *cap, 
 int32_t grow_wire(raftgpu_arena *a, StagingSet &s, uint64_t need) {
     return grow_scratch(a, a->s_compute, &s.d_wire, &s.d_wire_cap, need);
 }
-
-// Consecutive regions of a staging set's d_wire, each from a 16-byte boundary: take(bytes) returns the next region's
-// offset; `end` is where the last region ends (what grow_wire needs).
-struct WireLayout {
-    uint64_t end = 0;
-    uint64_t take(uint64_t bytes) {
-        const uint64_t at = (end + 15u) & ~15ull;
-        end = at + bytes;
-        return at;
-    }
-};
 
 // A wire pass's first-frame table (`n` u32, allocated on first use) filled with 0xff on st: no frame yet.  Every pass
 // keeps its own table (DESIGN 3.10).
@@ -919,25 +909,120 @@ int32_t host_batch_admit(raftgpu_arena *a, StagingSet **out) {
     return RAFTGPU_OK;
 }
 
-template <typename T, typename F>
-int32_t host_batch_op(raftgpu_arena *a, const T *in, uint64_t n, uint8_t *results, F &&launch, uint32_t *out_dups) {
-    StagingSet *sp = nullptr;
-    const int32_t adm = host_batch_admit(a, &sp);
-    if (adm != RAFTGPU_OK) return adm;
-    StagingSet &s = *sp;
-    const uint64_t room = rec_slots(a) * sizeof(PackedRec);
-    if (n * sizeof(T) > room || n > 4 * (room / sizeof(PackedRec))) return fail(a, RAFTGPU_ERR_FULL, "batch larger than the staging buffer");
-    CK(a, cudaSetDevice(a->device));
-    CK(a, cudaMemcpyAsync(s.d_recs, in, n * sizeof(T), cudaMemcpyHostToDevice, a->s_compute));
-    CK(a, cudaMemsetAsync(s.d_step_adv, 0, 8, a->s_compute));
-    const int32_t rc = launch(reinterpret_cast<const T *>(s.d_recs), s.d_results, s.d_step_adv + 1);
-    if (rc != RAFTGPU_OK) return rc;
-    if (results) CK(a, cudaMemcpyAsync(results, s.d_results, n, cudaMemcpyDeviceToHost, a->s_compute));
-    CK(a, cudaMemcpyAsync(s.h_step_adv, s.d_step_adv, 8, cudaMemcpyDeviceToHost, a->s_compute));
-    CK(a, cudaStreamSynchronize(a->s_compute));
-    if (out_dups) *out_dups = s.h_step_adv[1];
-    return RAFTGPU_OK;
-}
+// ---- the host frame: every host form of a batch pass (raftgpu_heartbeat_resp, raftgpu_update_state, the three
+// raftgpu_read_index_* passes, raftgpu_heartbeat_wire, raftgpu_heartbeat_frames, raftgpu_follower_heartbeat,
+// raftgpu_vote_wire) stages its host buffers in the fill set, idle between steps, runs its `_device` form on s_compute
+// and copies the outputs back through one HostFrame:
+//   open   admission (host_batch_admit), and the record batch if the form has one: the batch goes to d_recs and one
+//          result byte per item to d_results, so it is refused with ERR_FULL past their room;
+//   in     a region of d_wire copied from a host buffer; out: a region only reserved; rest: the last region, which
+//          takes what d_wire has room for (at least `min` bytes) until enlarge gives it an exact size;
+//   run    d_wire grown to hold the regions, the H2D copies (the batch, then the inputs in order), then the pass;
+//   back   a D2H copy from d_results, d_wire or the arena's scratch (where the counts go, scratch<T>);
+//   wait   the synchronise of s_compute that ends a phase, when the frame queued anything since the last one.
+// A null host pointer or a zero length copies nothing.  Regions are offsets: only the pass sees device pointers into
+// d_wire, made after the growth that may move it.  The regions start on 16-byte boundaries.
+struct WireRegion {
+    uint64_t at;
+};
+
+// What a frame's pass sees: the batch, the result bytes, d_wire as it is after the growth and the rest region's bytes.
+struct Staged {
+    const void *recs;
+    uint8_t *results;
+    uint8_t *wire;
+    uint64_t rest;
+    template <typename T>
+    T *at(WireRegion r) const {
+        return reinterpret_cast<T *>(wire + r.at);
+    }
+};
+
+class HostFrame {
+  public:
+    explicit HostFrame(raftgpu_arena *a) : a_(a) {}
+
+    int32_t open(const void *recs = nullptr, uint64_t n = 0, size_t elem = 0) {
+        const int32_t rc = host_batch_admit(a_, &s_);
+        if (rc != RAFTGPU_OK) return rc;
+        if (n * elem > rec_slots(a_) * sizeof(PackedRec) || n > 4 * rec_slots(a_))
+            return fail(a_, RAFTGPU_ERR_FULL, "batch larger than the staging buffer");
+        recs_ = recs;
+        rec_bytes_ = n * elem;
+        CK(a_, cudaSetDevice(a_->device));
+        return RAFTGPU_OK;
+    }
+
+    WireRegion in(const void *src, uint64_t bytes) {
+        const WireRegion r = take(bytes);
+        assert(n_in_ < kInputs);
+        in_[n_in_++] = {r.at, src, bytes};
+        return r;
+    }
+    WireRegion out(uint64_t bytes) { return take(bytes); }
+    WireRegion rest(uint64_t min) {
+        rest_ = take(min);
+        return rest_;
+    }
+    void enlarge(uint64_t bytes) {
+        end_ = rest_.at + bytes;
+        rest_bytes_ = bytes;
+    }
+
+    template <typename Pass>
+    int32_t run(Pass &&pass) {
+        StagingSet &s = *s_;
+        int32_t rc = grow_wire(a_, s, end_);
+        if (rc != RAFTGPU_OK) return rc;
+        if (recs_ && rec_bytes_) CK(a_, cudaMemcpyAsync(s.d_recs, recs_, rec_bytes_, cudaMemcpyHostToDevice, a_->s_compute));
+        for (uint32_t i = 0; i < n_in_; i++)
+            if (in_[i].src && in_[i].bytes)
+                CK(a_, cudaMemcpyAsync(s.d_wire + in_[i].at, in_[i].src, in_[i].bytes, cudaMemcpyHostToDevice, a_->s_compute));
+        queued_ = true;
+        const Staged d{s.d_recs, s.d_results, s.d_wire, std::min(rest_bytes_, s.d_wire_cap - rest_.at)};
+        return pass(d);
+    }
+
+    const uint8_t *results() const { return s_->d_results; }
+    int32_t back(void *dst, const void *d_src, uint64_t bytes) {
+        if (!dst || !bytes) return RAFTGPU_OK;
+        CK(a_, cudaMemcpyAsync(dst, d_src, bytes, cudaMemcpyDeviceToHost, a_->s_compute));
+        queued_ = true;
+        return RAFTGPU_OK;
+    }
+    int32_t back(void *dst, WireRegion src, uint64_t bytes) { return back(dst, s_->d_wire + src.at, bytes); }
+
+    int32_t wait() {
+        if (!queued_) return RAFTGPU_OK;
+        queued_ = false;
+        CK(a_, cudaStreamSynchronize(a_->s_compute));
+        return RAFTGPU_OK;
+    }
+
+  private:
+    static constexpr uint32_t kInputs = 4;
+    struct Input {
+        uint64_t at;
+        const void *src;
+        uint64_t bytes;
+    };
+    WireRegion take(uint64_t bytes) {
+        const uint64_t at = (end_ + 15u) & ~15ull;
+        end_ = at + bytes;
+        return {at};
+    }
+
+    raftgpu_arena *a_;
+    StagingSet *s_ = nullptr;
+    const void *recs_ = nullptr;
+    uint64_t rec_bytes_ = 0;
+    Input in_[kInputs] = {};
+    uint32_t n_in_ = 0;
+    uint64_t end_ = 0;               // where the last region ends: what d_wire must hold
+    WireRegion rest_ = {0};
+    uint64_t rest_bytes_ = UINT64_MAX;  // the rest region's size once enlarged (until then: to the end of d_wire)
+    bool queued_ = false;               // copies or a pass queued since the last wait
+};
 
 // ---- the step frame: every raftgpu_step_begin* form is step_admit -> the form's own function, which queues its H2D
 // copies on s_h2d and its apply kernels on s_compute and says what it queued (StepWork) -> step_finish -> step_book.
