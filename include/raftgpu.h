@@ -645,13 +645,17 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
                                       applied in arrival order, one message per step -- resubmit it with the next batch */
 #define RAFTGPU_WIRE_CONTEXT 6u    /* (raftgpu_heartbeat_wire only) a context that is not an 8-byte read id, or any context
                                       on an arena without read queues: the host's own ReadOnly handles the frame */
-#define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat, raftgpu_vote_wire) the group is not selected for the
-                                      role the pass serves, or is a leader; at raftgpu_vote_wire also a response type
-                                      that is not the candidate's own (step_candidate ignores it): Raft::step on the host */
+#define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat, raftgpu_vote_wire, raftgpu_vote_request_wire) the group
+                                      is not selected for the role the pass serves, or is a leader; at raftgpu_vote_wire
+                                      also a response type that is not the candidate's own (step_candidate ignores it):
+                                      Raft::step on the host */
 #define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat only) m.commit beyond max(committed, last_index):
                                         commit_to would be fatal! (raft_log.rs:291-298) */
-#define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire only) m.commit != 0, m.commit_term != 0 and m.commit beyond
-                                        committed: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
+#define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire, raftgpu_vote_request_wire) m.commit != 0, m.commit_term != 0
+                                        and m.commit beyond committed -- at raftgpu_vote_request_wire for a rejected
+                                        request: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
+#define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire only) the reference drops the frame: a vote request
+                                        in lease (raft.rs:1288-1316) or a MsgRequestVote at a lower term (:1399-1409) */
 typedef struct raftgpu_wire_batch {
     const uint8_t *bytes;    /* the frames, back to back */
     uint64_t n_bytes;
@@ -986,6 +990,77 @@ int32_t raftgpu_vote_wire_device(raftgpu_arena *arena, void *stream, const void 
 int32_t raftgpu_vote_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets, uint64_t n,
                           const uint32_t *select, const uint32_t *pre, uint8_t *status, raftgpu_vote_outcome *out,
                           uint64_t capacity, uint64_t *out_n);
+
+/* ---- vote requests at a voter -------------------------------------------------- */
+
+/* RawNode::step -> Raft::step (raft.rs:1280-1411, then the MsgRequestVote | MsgRequestPreVote arm at :1418-1462, with
+ * send at :602-661) for the MsgRequestVote (5) and MsgRequestPreVote (17) frames of a wire batch: the term rules, the
+ * grant decision and one response per decided frame.
+ * Input.  The frames of raftgpu_wire_batch, but the header is u32 LE (group << 4 | x) with `group` the voter's own group
+ * slot in this arena (the transport rewrites the header on the way in); x is not read and is copied into the response's
+ * header.  d_bytes 16-byte aligned, n and n_bytes below 4 GiB.  d_voters (16-byte aligned, read only) has one
+ * raftgpu_voter per group slot below the highest allocated one: the per-group facts the arena does not keep.  term,
+ * term_start, committed and last_index come from the arena; for a wide pair (addressed by its low half) committed and
+ * last_index are the larger of both halves', as raftgpu_group_get reports.
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4 | RAFTGPU_VREQ_* for an applied frame; the first failing check decides:
+ *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot, or a wide pair's high half;
+ *   SKIP_TYPE    any type but 5 and 17;
+ *   ROLE         RAFTGPU_VOTER_SELECT is clear, or the group is a leader (term_start != RAFTGPU_NO_TERM_START): a leader
+ *                that steps down has host-side consequences;
+ *   TERM         the group's term (raftgpu_group_set_term) is 0, or m.term is 0 (a local message);
+ * then the first frame of each group in frame order that got this far is decided by the term rules:
+ *   IGNORED      m.term > term in lease (RAFTGPU_VOTER_LEASE, and the context is not "CampaignTransfer"), or a
+ *                MsgRequestVote with m.term < term: the reference drops it;
+ *   COMMIT_VOTE  a rejection with m.commit != 0, m.commit_term != 0 and m.commit > committed (maybe_commit_by_vote
+ *                needs the log);
+ *   OK           decided and applied: a MsgRequestVote with m.term > term first runs become_follower(m.term,
+ *                INVALID_ID)'s arena part (term = m.term, and RAFTGPU_CTL_RESET's reset on both halves with term_start
+ *                RAFTGPU_NO_TERM_START, last_index, committed and the table's persisted) and is decided with vote 0 and no
+ *                leader; a MsgRequestPreVote at a lower term is rejected at the group's term (raft.rs:1395-1398); else
+ *                can_vote, is_up_to_date(m.index, m.log_term) and the priority rule (:1420-1428) grant or reject;
+ *   DUP          every later frame of a group whose first frame reached the term rules in this batch: its decision
+ *                depends on what the first one changes; resubmit DUP frames, in order, with the next batch.
+ * A frame that is not OK changes nothing: run RawNode::step on it (IGNORED ones may be dropped).  d_out (nullable,
+ * u64[2 n]) = {m.from, the group's term after the frame} per applied frame, zero for the others.
+ * Output.  One response per applied frame, in frame order: the input header, then eraftpb.Message with msg_type 6 or 18,
+ * to = m.from, from = the table's id, term (m.term on a grant, the group's term otherwise), reject, and on a rejection
+ * of the vote arm commit and commit_term; canonical proto3 as raftgpu_synth_wire_encode_votes writes (at most 63 bytes
+ * with the header).  d_resp_bytes (16-byte aligned) holds them back to back, d_resp_offsets (n + 1 values) their starts
+ * and the end, d_totals (u64[2]) = {responses, bytes}.  The pass writes terms and resets groups, so a response cannot be
+ * produced again: resp_bytes_capacity must be at least raftgpu_vote_request_wire_bound(n), and that bound addressable
+ * by u32 offsets: RAFTGPU_ERR_INVALID before any launch otherwise, as are a missing d_voters, d_status, d_bytes or
+ * d_offsets with n > 0 and misaligned buffers.  The caller sends the responses only after it has made the changed
+ * HardState (term, vote) durable.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  The
+ * host form copies (voters covers the groups below the highest allocated one), runs and waits; status, out,
+ * resp_bytes / resp_offsets as above, totals u64[2]. */
+#define RAFTGPU_VOTER_SELECT 0x1u /* the pass decides this group: a Follower, PreCandidate or Candidate */
+#define RAFTGPU_VOTER_LEADER 0x2u /* leader_id != INVALID_ID */
+#define RAFTGPU_VOTER_LEASE 0x4u  /* check_quorum && leader_id != INVALID_ID && election_elapsed < election_timeout */
+#define RAFTGPU_VREQ_GRANTED 0x1u /* the response has reject = false */
+#define RAFTGPU_VREQ_VOTED 0x2u   /* a granted MsgRequestVote: the caller sets vote = m.from, election_elapsed = 0 */
+#define RAFTGPU_VREQ_BUMPED 0x4u  /* the term was raised: the caller runs become_follower(m.term, INVALID_ID)'s host side */
+typedef struct raftgpu_voter {
+    uint64_t id;          /* Raft::id: the response's from */
+    uint64_t vote;        /* Raft::vote, 0 = INVALID_ID */
+    uint64_t last_term;   /* raft_log.last_term() */
+    uint64_t commit_term; /* raft_log.commit_info().1, the term of `committed` */
+    uint64_t persisted;   /* raft_log.persisted: the self cell's matched after a term bump's reset (raft.rs:967) */
+    uint64_t priority;    /* Raft::priority */
+    uint32_t flags;       /* RAFTGPU_VOTER_* */
+    uint32_t reserved;    /* 0 */
+    uint64_t reserved2;   /* 0 */
+} raftgpu_voter;
+/* 64 bytes per frame: enough for the responses to any n frames. */
+uint64_t raftgpu_vote_request_wire_bound(uint64_t n);
+int32_t raftgpu_vote_request_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                         const uint32_t *d_offsets, uint64_t n, const raftgpu_voter *d_voters,
+                                         uint8_t *d_status, uint64_t *d_out, uint8_t *d_resp_bytes,
+                                         uint64_t resp_bytes_capacity, uint32_t *d_resp_offsets, uint64_t *d_totals);
+int32_t raftgpu_vote_request_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets,
+                                  uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
+                                  uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
+                                  uint64_t *totals);
 
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 

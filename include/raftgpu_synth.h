@@ -70,6 +70,23 @@ typedef struct raftgpu_synth_vote {
 int32_t raftgpu_synth_wire_encode_votes(const raftgpu_synth_vote *votes, uint64_t n, uint8_t *out_bytes, uint64_t bytes_cap,
                                         uint32_t *out_offsets, uint64_t *out_n_bytes);
 
+/* One vote request as raftgpu_synth_wire_encode_vote_requests writes it (104 bytes). */
+typedef struct raftgpu_synth_vote_request {
+    uint32_t hdr;      /* the frame's u32 header: group << 4 | x */
+    uint32_t msg_type; /* MsgRequestVote (5) or MsgRequestPreVote (17) */
+    uint64_t to, from, term, log_term, index, commit, commit_term, priority;
+    uint8_t context[24];  /* the first context_len bytes are the context */
+    uint32_t context_len; /* 0 (none) .. 24 */
+    uint32_t reserved;
+} raftgpu_synth_vote_request;
+
+/* Vote requests -> frames, one per entry in order: the header, then eraftpb.Message with msg_type, to, from, term,
+ * log_term, index, commit, context, priority and commit_term, fields in number order and zero scalars and an empty
+ * context omitted (the canonical proto3 encoding: at most 120 bytes a frame, header included).  out_offsets has room for
+ * n + 1 entries.  RAFTGPU_ERR_FULL when bytes_cap is short, RAFTGPU_ERR_INVALID for a context_len past 24. */
+int32_t raftgpu_synth_wire_encode_vote_requests(const raftgpu_synth_vote_request *reqs, uint64_t n, uint8_t *out_bytes,
+                                                uint64_t bytes_cap, uint32_t *out_offsets, uint64_t *out_n_bytes);
+
 #ifdef __cplusplus
 }
 #endif

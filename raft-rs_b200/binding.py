@@ -45,7 +45,15 @@ BULK_SORTED = 0x1
  COL_LAST_INDEX, COL_TERM, COL_INS_META) = range(14)
 WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WIRE_CONTEXT = range(7)
 WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat (ROLE also raftgpu_vote_wire)
-WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire only
+WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire, raftgpu_vote_request_wire
+WIRE_IGNORED = 10  # raftgpu_vote_request_wire only
+# raftgpu_vote_request_wire: the caller's table (raftgpu_voter), its flags, and the low nibble of an applied frame
+VOTER_SELECT, VOTER_LEADER, VOTER_LEASE = 0x1, 0x2, 0x4
+VREQ_GRANTED, VREQ_VOTED, VREQ_BUMPED = 0x1, 0x2, 0x4
+VOTER_DTYPE = np.dtype([("id", "<u8"), ("vote", "<u8"), ("last_term", "<u8"), ("commit_term", "<u8"),
+                        ("persisted", "<u8"), ("priority", "<u8"), ("flags", "<u4"), ("reserved", "<u4"),
+                        ("reserved2", "<u8")])
+assert VOTER_DTYPE.itemsize == 64
 # raftgpu_vote_wire's outcome: the group (a pair's low half) and its tally word (VoteResult | granted << 8 | rejected << 16)
 VOTE_OUTCOME_DTYPE = np.dtype([("group", "<u4"), ("result", "<u4")])
 assert VOTE_OUTCOME_DTYPE.itemsize == 8
@@ -314,6 +322,9 @@ def lib() -> C.CDLL:
             "raftgpu_follower_heartbeat": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_vote_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp], i32),
             "raftgpu_vote_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, C.POINTER(u64)], i32),
+            "raftgpu_vote_request_wire_bound": ([u64], u64),
+            "raftgpu_vote_request_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_vote_request_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -356,6 +367,8 @@ def synth_lib() -> C.CDLL:
         L.raftgpu_synth_wire_encode_heartbeats.restype = i32
         L.raftgpu_synth_wire_encode_votes.argtypes = [vp, u64, vp, u64, vp, C.POINTER(u64)]
         L.raftgpu_synth_wire_encode_votes.restype = i32
+        L.raftgpu_synth_wire_encode_vote_requests.argtypes = [vp, u64, vp, u64, vp, C.POINTER(u64)]
+        L.raftgpu_synth_wire_encode_vote_requests.restype = i32
         _synth_lib = L
     return _synth_lib
 
@@ -383,6 +396,32 @@ def synth_encode_votes(votes: np.ndarray):
     if rc != OK:
         raise RaftGpuError(rc, "synth_wire_encode_votes")
     return blob[: (nb.value + 15) // 16 * 16 + 16].copy(), off
+
+
+# raftgpu_synth_vote_request: one vote request for raftgpu_synth_wire_encode_vote_requests
+SYNTH_VOTE_REQUEST_DTYPE = np.dtype([("hdr", "<u4"), ("msg_type", "<u4"), ("to", "<u8"), ("from", "<u8"), ("term", "<u8"),
+                                     ("log_term", "<u8"), ("index", "<u8"), ("commit", "<u8"), ("commit_term", "<u8"),
+                                     ("priority", "<u8"), ("context", "u1", (24,)), ("context_len", "<u4"),
+                                     ("reserved", "<u4")])
+assert SYNTH_VOTE_REQUEST_DTYPE.itemsize == 104
+
+
+def synth_encode_vote_requests(reqs: np.ndarray):
+    """raftgpu_synth_wire_encode_vote_requests: SYNTH_VOTE_REQUEST_DTYPE entries -> (blob padded to 16 bytes, offsets
+    u32[n + 1])."""
+    reqs = np.ascontiguousarray(reqs, dtype=SYNTH_VOTE_REQUEST_DTYPE)
+    n = len(reqs)
+    blob, off, nb = np.zeros(128 * n + 16, np.uint8), np.zeros(n + 1, np.uint32), C.c_uint64()
+    rc = synth_lib().raftgpu_synth_wire_encode_vote_requests(reqs.ctypes.data, n, blob.ctypes.data, len(blob),
+                                                             off.ctypes.data, C.byref(nb))
+    if rc != OK:
+        raise RaftGpuError(rc, "synth_wire_encode_vote_requests")
+    return blob[: (nb.value + 15) // 16 * 16 + 16].copy(), off
+
+
+def vote_request_wire_bound(n: int) -> int:
+    """raftgpu_vote_request_wire_bound: response bytes enough for any n vote-request frames."""
+    return int(lib().raftgpu_vote_request_wire_bound(n))
 
 
 def follower_heartbeat_bound(n: int) -> int:
@@ -939,6 +978,29 @@ class Arena:
                          stream=None):
         self._ck(self._L.raftgpu_vote_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_select, d_pre, d_status,
                                                   d_out, capacity, d_count), "vote_wire_device")
+
+    def vote_request_wire(self, frames, voters):
+        """raftgpu_vote_request_wire: Raft::step's term rules and the vote arm for the MsgRequestVote /
+        MsgRequestPreVote frames of a wire batch (.bytes, .n_bytes, .offsets, .n; headers name the voter's group slot).
+        voters: VOTER_DTYPE rows covering the groups below the highest allocated one -> (status u8[n], out u64[n][2] =
+        {m.from, term after} of the applied frames, response blob, response offsets u32[responses + 1], totals u64[2])."""
+        vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
+        assert len(vt) >= self.get_info().hi
+        n = frames.n
+        status, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
+        resp = np.zeros(max(16, vote_request_wire_bound(n)), np.uint8)
+        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        self._ck(self._L.raftgpu_vote_request_wire(self._h, frames.bytes.ctypes.data, frames.n_bytes,
+                                                   frames.offsets.ctypes.data, n, vt.ctypes.data, status.ctypes.data,
+                                                   out.ctypes.data, resp.ctypes.data, len(resp), roff.ctypes.data,
+                                                   totals.ctypes.data), "vote_request_wire")
+        return status, out, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+
+    def vote_request_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_voters, d_status, d_out, d_resp_bytes,
+                                 resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
+        self._ck(self._L.raftgpu_vote_request_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters, d_status,
+                                                          d_out, d_resp_bytes, resp_bytes_capacity, d_resp_offsets, d_totals),
+                 "vote_request_wire_device")
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

@@ -268,6 +268,11 @@ struct raftgpu_arena {
     uint32_t *vw_first = nullptr;
     uint64_t *vw_scratch = nullptr;
     uint64_t vw_scratch_cap = 0;
+    // raftgpu_vote_request_wire: first frame of every group slot that reached the term rules [cap] (allocated on first
+    // use); grown on demand, in u64 words: one record per frame, the block sums, the fit flag
+    uint32_t *vrq_first = nullptr;
+    uint64_t *vrq_scratch = nullptr;
+    uint64_t vrq_scratch_cap = 0;
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -643,6 +648,8 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->hfw_scratch);
     cudaFree(a->vw_first);
     cudaFree(a->vw_scratch);
+    cudaFree(a->vrq_first);
+    cudaFree(a->vrq_scratch);
     cudaFree(a->d_counters);
     cudaFree(a->d_scratch);
     cudaFreeHost(a->h_scratch);
@@ -911,7 +918,7 @@ int32_t host_batch_admit(raftgpu_arena *a, StagingSet **out) {
 
 // ---- the host frame: every host form of a batch pass (raftgpu_heartbeat_resp, raftgpu_update_state, the three
 // raftgpu_read_index_* passes, raftgpu_heartbeat_wire, raftgpu_heartbeat_frames, raftgpu_follower_heartbeat,
-// raftgpu_vote_wire) stages its host buffers in the fill set, idle between steps, runs its `_device` form on s_compute
+// raftgpu_vote_wire, raftgpu_vote_request_wire) stages its host buffers in the fill set, idle between steps, runs its `_device` form on s_compute
 // and copies the outputs back through one HostFrame:
 //   open   admission (host_batch_admit), and the record batch if the form has one: the batch goes to d_recs and one
 //          result byte per item to d_results, so it is refused with ERR_FULL past their room;
@@ -1151,5 +1158,6 @@ extern "C" {
 #include "abi_hb_frames.inc"
 #include "abi_hb_follow.inc"
 #include "abi_vote_wire.inc"
+#include "abi_vote_request.inc"
 
 }  // extern "C"

@@ -23,7 +23,8 @@
 //
 // The file holds the frame format in both directions: the decoder and the block staging every wire pass uses
 // (wire_open, wire_block_frame), and the heartbeat-kind encoder with the block-output code that the leader's
-// MsgHeartbeat frames (k_hb_frames.cuh) and the follower's MsgHeartbeatResponse frames (k_hb_follow.cuh) share.
+// MsgHeartbeat frames (k_hb_frames.cuh) and the follower's MsgHeartbeatResponse frames (k_hb_follow.cuh) share; the
+// voter's vote responses (k_vote_request.cuh) use that block-output code with their own encoder.
 
 struct WireSrc {
     const uint8_t *bytes;     // 16-byte aligned
@@ -40,6 +41,7 @@ struct WireMsg {  // the scalar fields this path looks at
     uint32_t ctx_off, ctx_len;  // wire_decode<true> only: bytes [ctx_off, ctx_off + ctx_len) are the last context (12)
     uint64_t from;              // wire_decode<true, true> only: field 3
     uint64_t commit_term;       // wire_decode<.., .., true> only: field 15
+    uint64_t priority;          // wire_decode<.., .., .., true> only: field 14
 };
 
 constexpr uint32_t kWireThreads = 256;
@@ -62,8 +64,8 @@ __device__ __forceinline__ bool wire_varint(const uint8_t *p, uint32_t &pos, uin
 // One serialized Message -> WireMsg.  false = not a well-formed protobuf message.  kContext: also the context's
 // position (the heartbeat-response path, k_hb_wire.cuh); the AppendResponse kernels instantiate it without.  kFrom:
 // also `from` (the follower's heartbeat path, k_hb_follow.cuh).  kCommitTerm: also commit_term (the vote responses,
-// k_vote_wire.cuh).
-template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false>
+// k_vote_wire.cuh).  kPriority: also priority (the vote requests, k_vote_request.cuh).
+template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false, bool kPriority = false>
 __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, WireMsg &m) {
     m.msg_type = 0;
     m.reject = false;
@@ -71,6 +73,7 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
     if constexpr (kContext) m.ctx_off = m.ctx_len = 0;
     if constexpr (kFrom) m.from = 0;
     if constexpr (kCommitTerm) m.commit_term = 0;
+    if constexpr (kPriority) m.priority = 0;
     uint32_t pos = 0;
     while (pos < len) {
         uint64_t tag;
@@ -94,6 +97,9 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
             }
             if constexpr (kCommitTerm) {
                 if (field == 15) m.commit_term = v;
+            }
+            if constexpr (kPriority) {
+                if (field == 14) m.priority = v;
             }
         } else if (wt == 1) {
             if (len - pos < 8) return false;
@@ -171,7 +177,7 @@ __device__ __forceinline__ uint32_t wire_block_frame(const WireSrc &w, uint8_t *
 // RAFTGPU_WIRE_MALFORMED when it is not a frame (offsets out of order or past the batch, shorter than the header),
 // names a group >= n_groups or is not a well-formed protobuf message; RAFTGPU_WIRE_OK otherwise.  The flags are
 // wire_decode's.
-template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false>
+template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false, bool kPriority = false>
 __device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage &s, const uint8_t *stage, uint32_t i,
                                               uint32_t &hdr, const uint8_t *&msg, WireMsg &m) {
     const uint32_t a = w.offsets[i], b = w.offsets[i + 1];
@@ -179,7 +185,7 @@ __device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage 
     const uint8_t *p = (s.staged && a >= s.lo && b <= s.hi) ? stage + (a - s.base) : w.bytes + a;
     hdr = p[0] | (static_cast<uint32_t>(p[1]) << 8) | (static_cast<uint32_t>(p[2]) << 16) | (static_cast<uint32_t>(p[3]) << 24);
     msg = p + 4;
-    if ((hdr >> 4) >= w.n_groups || !wire_decode<kContext, kFrom, kCommitTerm>(msg, b - a - 4u, m))
+    if ((hdr >> 4) >= w.n_groups || !wire_decode<kContext, kFrom, kCommitTerm, kPriority>(msg, b - a - 4u, m))
         return RAFTGPU_WIRE_MALFORMED;
     return RAFTGPU_WIRE_OK;
 }
@@ -323,6 +329,49 @@ __device__ __forceinline__ uint8_t *wire_put_hb_frame(uint8_t *p, uint32_t hdr, 
 #pragma unroll
         for (int k = 0; k < 8; k++) p[2 + k] = static_cast<uint8_t>(ctx >> (8 * k));
         p += 10;
+    }
+    return p;
+}
+
+// A vote response (MsgRequestVoteResponse 6, MsgRequestPreVoteResponse 18; k_vote_request.cuh): u32 LE header, then
+// eraftpb.Message in field-number order with zero scalars omitted, as raftgpu_synth_wire_encode_votes writes it:
+// 1 msg_type, 2 to, 3 from, 4 term, 8 commit, 10 reject, 15 commit_term.  At most 4 + 2 + 5 * 11 + 2 = 63 bytes.
+constexpr uint32_t kWireVoteFrameMax = 64;
+
+// bytes of the frame, header included
+__device__ __forceinline__ uint32_t wire_vote_len(uint64_t to, uint64_t from, uint64_t term, uint64_t commit, bool reject,
+                                                  uint64_t commit_term) {
+    return 6u + (to ? 1u + wire_varint_len(to) : 0u) + (from ? 1u + wire_varint_len(from) : 0u) +
+           (term ? 1u + wire_varint_len(term) : 0u) + (commit ? 1u + wire_varint_len(commit) : 0u) + (reject ? 2u : 0u) +
+           (commit_term ? 1u + wire_varint_len(commit_term) : 0u);
+}
+
+__device__ __forceinline__ uint8_t *wire_put_vote_frame(uint8_t *p, uint32_t hdr, uint8_t type, uint64_t to, uint64_t from,
+                                                        uint64_t term, uint64_t commit, bool reject, uint64_t commit_term) {
+    p[0] = static_cast<uint8_t>(hdr);
+    p[1] = static_cast<uint8_t>(hdr >> 8);
+    p[2] = static_cast<uint8_t>(hdr >> 16);
+    p[3] = static_cast<uint8_t>(hdr >> 24);
+    p[4] = 0x08;  // field 1, varint
+    p[5] = type;
+    p += 6;
+    const uint8_t tags[4] = {0x10, 0x18, 0x20, 0x40};  // fields 2, 3, 4, 8
+    const uint64_t vals[4] = {to, from, term, commit};
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        if (vals[k]) {
+            *p++ = tags[k];
+            p = wire_put_varint(p, vals[k]);
+        }
+    }
+    if (reject) {
+        p[0] = 0x50;  // field 10
+        p[1] = 1;
+        p += 2;
+    }
+    if (commit_term) {
+        *p++ = 0x78;  // field 15
+        p = wire_put_varint(p, commit_term);
     }
     return p;
 }

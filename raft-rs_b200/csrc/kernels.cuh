@@ -27,5 +27,6 @@ namespace raftgpu {
 #include "k_hb_frames.cuh"
 #include "k_hb_follow.cuh"
 #include "k_vote_wire.cuh"
+#include "k_vote_request.cuh"
 
 }  // namespace raftgpu

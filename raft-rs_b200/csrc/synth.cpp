@@ -275,4 +275,36 @@ int32_t raftgpu_synth_wire_encode_votes(const raftgpu_synth_vote *votes, uint64_
     return RAFTGPU_OK;
 }
 
+int32_t raftgpu_synth_wire_encode_vote_requests(const raftgpu_synth_vote_request *reqs, uint64_t n, uint8_t *out_bytes,
+                                                uint64_t bytes_cap, uint32_t *out_offsets, uint64_t *out_n_bytes) {
+    if ((!reqs && n) || !out_bytes || !out_offsets || !out_n_bytes) return RAFTGPU_ERR_INVALID;
+    uint8_t *p = out_bytes;
+    out_offsets[0] = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        const raftgpu_synth_vote_request &r = reqs[i];
+        if (r.context_len > sizeof(r.context)) return RAFTGPU_ERR_INVALID;
+        if (static_cast<uint64_t>(p - out_bytes) + 120 > bytes_cap) return RAFTGPU_ERR_FULL;
+        memcpy(p, &r.hdr, 4);
+        p += 4;
+        p = put_field(p, 1, r.msg_type);
+        p = put_field(p, 2, r.to);
+        p = put_field(p, 3, r.from);
+        p = put_field(p, 4, r.term);
+        p = put_field(p, 5, r.log_term);
+        p = put_field(p, 6, r.index);
+        p = put_field(p, 8, r.commit);
+        if (r.context_len) {
+            *p++ = (12u << 3) | 2u;  // context, length-delimited
+            *p++ = static_cast<uint8_t>(r.context_len);
+            memcpy(p, r.context, r.context_len);
+            p += r.context_len;
+        }
+        p = put_field(p, 14, r.priority);
+        p = put_field(p, 15, r.commit_term);
+        out_offsets[i + 1] = static_cast<uint32_t>(p - out_bytes);
+    }
+    *out_n_bytes = static_cast<uint64_t>(p - out_bytes);
+    return RAFTGPU_OK;
+}
+
 }  // extern "C"
