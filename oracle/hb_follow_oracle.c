@@ -25,7 +25,7 @@ size_t hfl_encode_response(uint64_t to, uint64_t from, uint64_t term, uint64_t c
 static uint64_t max64(uint64_t x, uint64_t y) { return x > y ? x : y; }
 
 void hfl_follower_heartbeats(ro_arena_view *a, const ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets,
-                             size_t n, const uint32_t *select, const uint64_t *self_ids, uint8_t *status, uint64_t *from,
+                             size_t n, uint64_t n_bytes, const uint32_t *select, const uint64_t *self_ids, uint8_t *status, uint64_t *from,
                              uint8_t *resp, uint32_t *resp_offsets, uint64_t *totals) {
     uint8_t *applied = (uint8_t *)calloc(a->n_groups ? a->n_groups : 1, 1);
     uint64_t frames = 0, len = 0;
@@ -33,7 +33,7 @@ void hfl_follower_heartbeats(ro_arena_view *a, const ro_read_queues *q, const ui
         status[i] = WO_WIRE_MALFORMED << 4;
         from[i] = 0;
         const uint32_t lo = offsets[i], hi = offsets[i + 1];
-        if (hi < lo || hi - lo < 4) continue;
+        if (hi < lo || hi > n_bytes || hi - lo < 4) continue;
         uint32_t hdr;
         memcpy(&hdr, bytes + lo, 4);
         const uint32_t g = hdr >> 4;
@@ -89,12 +89,12 @@ void hfl_follower_heartbeats(ro_arena_view *a, const ro_read_queues *q, const ui
     free(applied);
 }
 
-double hfl_bench(ro_arena_view *a, const ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+double hfl_bench(ro_arena_view *a, const ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                  const uint32_t *select, const uint64_t *self_ids, uint8_t *status, uint64_t *from, uint8_t *resp,
                  uint32_t *resp_offsets, uint64_t *totals) {
     struct timespec t0, t1;
     clock_gettime(CLOCK_MONOTONIC, &t0);
-    hfl_follower_heartbeats(a, q, bytes, offsets, n, select, self_ids, status, from, resp, resp_offsets, totals);
+    hfl_follower_heartbeats(a, q, bytes, offsets, n, n_bytes, select, self_ids, status, from, resp, resp_offsets, totals);
     clock_gettime(CLOCK_MONOTONIC, &t1);
     return (double)(t1.tv_sec - t0.tv_sec) + 1e-9 * (double)(t1.tv_nsec - t0.tv_nsec);
 }

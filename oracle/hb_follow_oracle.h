@@ -40,12 +40,12 @@ size_t hfl_encode_response(uint64_t to, uint64_t from, uint64_t term, uint64_t c
  * from[i] = m.from of an applied frame, 0 otherwise.  resp [60 n] / resp_offsets [n + 1]: the responses, in frame
  * order, framed with the input header; totals = {responses, bytes}. */
 void hfl_follower_heartbeats(ro_arena_view *a, const ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets,
-                             size_t n, const uint32_t *select, const uint64_t *self_ids, uint8_t *status, uint64_t *from,
+                             size_t n, uint64_t n_bytes, const uint32_t *select, const uint64_t *self_ids, uint8_t *status, uint64_t *from,
                              uint8_t *resp, uint32_t *resp_offsets, uint64_t *totals);
 
 /* CPU baseline: the same pass over the same inputs, timed with CLOCK_MONOTONIC; returns seconds.  The arena view is
  * changed as hfl_follower_heartbeats changes it. */
-double hfl_bench(ro_arena_view *a, const ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+double hfl_bench(ro_arena_view *a, const ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                  const uint32_t *select, const uint64_t *self_ids, uint8_t *status, uint64_t *from, uint8_t *resp,
                  uint32_t *resp_offsets, uint64_t *totals);
 

@@ -25,7 +25,7 @@ def lib() -> C.CDLL:
         L = O.lib()
         u64, vp, sz = C.c_uint64, C.c_void_p, C.c_size_t
         L.hfl_encode_response.argtypes, L.hfl_encode_response.restype = [u64, u64, u64, u64, vp, vp], sz
-        args = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, sz, vp, vp, vp, vp, vp, vp, vp]
+        args = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, sz, u64, vp, vp, vp, vp, vp, vp, vp]
         L.hfl_follower_heartbeats.argtypes, L.hfl_follower_heartbeats.restype = args, None
         L.hfl_bench.argtypes, L.hfl_bench.restype = args, C.c_double
         _lib = L
@@ -41,10 +41,11 @@ def encode_response(to: int, frm: int, term: int, commit: int, context: bytes | 
     return bytes(buf[:k])
 
 
-def follower_heartbeats(c, q, blob, offsets, select, self_ids, bench: bool = False):
+def follower_heartbeats(c, q, blob, offsets, select, self_ids, bench: bool = False, n_bytes=None):
     """hfl_follower_heartbeats over columns c (c.term = Raft::term of each group; changed in place, as the arena is)
     and read queues q (RO.ReadQueues, or None for an arena without them) -> (status u8[n], from u64[n], response blob,
-    response offsets u32[responses + 1], totals u64[2]); with bench=True also the pass's seconds."""
+    response offsets u32[responses + 1], totals u64[2]); with bench=True also the pass's seconds.
+    n_bytes as in O.wire_decode_batch."""
     blob = np.ascontiguousarray(blob, dtype=np.uint8)
     offsets = np.ascontiguousarray(offsets, dtype=np.uint32)
     sel = np.ascontiguousarray(select, dtype=np.uint32)
@@ -57,7 +58,7 @@ def follower_heartbeats(c, q, blob, offsets, select, self_ids, bench: bool = Fal
     qq = q._q() if q is not None else None
     f = lib().hfl_bench if bench else lib().hfl_follower_heartbeats
     secs = f(C.byref(v), C.byref(qq) if qq is not None else None, blob.ctypes.data, offsets.ctypes.data, n,
-             sel.ctypes.data, ids.ctypes.data, status.ctypes.data, frm.ctypes.data, resp.ctypes.data, roff.ctypes.data,
-             totals.ctypes.data)
+             O.wire_n_bytes(blob, n_bytes), sel.ctypes.data, ids.ctypes.data, status.ctypes.data, frm.ctypes.data,
+             resp.ctypes.data, roff.ctypes.data, totals.ctypes.data)
     out = (status, frm, resp[: int(totals[1])].copy(), roff[: int(totals[0]) + 1].copy(), totals)
     return out + (secs,) if bench else out

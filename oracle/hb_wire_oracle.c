@@ -44,14 +44,14 @@ int hwo_decode_message(const uint8_t *buf, size_t len, hwo_message *out) {
     return 1;
 }
 
-void hwo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, const uint64_t *group_term, uint32_t n_groups,
+void hwo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes, const uint64_t *group_term, uint32_t n_groups,
                       int read_queues, uint8_t *status, ro_append_resp *recs) {
     uint8_t *touched = (uint8_t *)calloc(n_groups ? n_groups : 1, 1); /* 8 slot bits per group */
     for (size_t i = 0; i < n; i++) {
         memset(&recs[i], 0, sizeof(recs[i]));
         const uint32_t lo = offsets[i], hi = offsets[i + 1];
         status[i] = WO_WIRE_MALFORMED;
-        if (hi < lo || hi - lo < 4) continue;
+        if (hi < lo || hi > n_bytes || hi - lo < 4) continue;
         uint32_t hdr;
         memcpy(&hdr, bytes + lo, 4);
         const uint32_t group = hdr >> 4, slot = hdr & 15u;
@@ -90,10 +90,10 @@ void hwo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, c
     free(touched);
 }
 
-void hwo_apply(ro_arena_view *a, ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+void hwo_apply(ro_arena_view *a, ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                const uint64_t *group_term, uint8_t *status, ro_read_state *out, uint64_t *n_out) {
     ro_append_resp *recs = (ro_append_resp *)malloc((n ? n : 1) * sizeof(ro_append_resp));
-    hwo_decode_batch(bytes, offsets, n, group_term, a->n_groups, q != NULL, status, recs);
+    hwo_decode_batch(bytes, offsets, n, n_bytes, group_term, a->n_groups, q != NULL, status, recs);
     size_t m = 0;
     for (size_t i = 0; i < n; i++) {
         if (status[i] == WO_WIRE_OK) {

@@ -39,12 +39,12 @@ enum { HWO_WIRE_CONTEXT = 6 }; /* a context that is not 8 bytes, or any context 
  * records for the others.  read_queues: whether the arena keeps read queues.  Checks in order: frame / group /
  * protobuf (MALFORMED), msg_type 9 (SKIP_TYPE), group_term (TERM; NULL or 0 = not checked), the context (CONTEXT),
  * then the first frame of a (group, slot < 8) cell wins and later ones are DUP. */
-void hwo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, const uint64_t *group_term, uint32_t n_groups,
+void hwo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes, const uint64_t *group_term, uint32_t n_groups,
                       int read_queues, uint8_t *status, ro_append_resp *recs);
 
 /* Decode, then handle_heartbeat_response for the applied frames in frame order: status[i] = WO_WIRE_* << 4 |
  * RO_RES_* of the tracker part; the read part (q != NULL) appends released reads to out. */
-void hwo_apply(ro_arena_view *a, ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+void hwo_apply(ro_arena_view *a, ro_read_queues *q, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                const uint64_t *group_term, uint8_t *status, ro_read_state *out, uint64_t *n_out);
 
 #ifdef __cplusplus

@@ -28,8 +28,10 @@ def lib() -> C.CDLL:
         L = O.lib()
         vp, sz = C.c_void_p, C.c_size_t
         L.hwo_decode_message.argtypes, L.hwo_decode_message.restype = [vp, sz, C.POINTER(Message)], C.c_int
-        L.hwo_decode_batch.argtypes, L.hwo_decode_batch.restype = [vp, vp, sz, vp, C.c_uint32, C.c_int, vp, vp], None
-        L.hwo_apply.argtypes = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, sz, vp, vp, vp, C.POINTER(C.c_uint64)]
+        L.hwo_decode_batch.argtypes = [vp, vp, sz, C.c_uint64, vp, C.c_uint32, C.c_int, vp, vp]
+        L.hwo_decode_batch.restype = None
+        L.hwo_apply.argtypes = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, sz, C.c_uint64, vp, vp, vp,
+                                C.POINTER(C.c_uint64)]
         L.hwo_apply.restype = None
         _lib = L
     return _lib
@@ -56,20 +58,22 @@ def _arrays(blob, offsets, terms):
     return blob, offsets, gt
 
 
-def decode_batch(blob, offsets, n_groups: int, terms=None, read_queues: bool = True):
-    """hwo_decode_batch -> (status u8[n] as WIRE_*, records (APPEND_RESP_DTYPE)[n])."""
+def decode_batch(blob, offsets, n_groups: int, terms=None, read_queues: bool = True, n_bytes=None):
+    """hwo_decode_batch -> (status u8[n] as WIRE_*, records (APPEND_RESP_DTYPE)[n]); n_bytes as in
+    O.wire_decode_batch."""
     blob, offsets, gt = _arrays(blob, offsets, terms)
     n = len(offsets) - 1
     status = np.zeros(n, np.uint8)
     recs = np.zeros(n, O.APPEND_RESP_DTYPE)
-    lib().hwo_decode_batch(blob.ctypes.data, offsets.ctypes.data, n, None if gt is None else gt.ctypes.data, n_groups,
-                           int(read_queues), status.ctypes.data, recs.ctypes.data)
+    lib().hwo_decode_batch(blob.ctypes.data, offsets.ctypes.data, n, O.wire_n_bytes(blob, n_bytes),
+                           None if gt is None else gt.ctypes.data, n_groups, int(read_queues), status.ctypes.data,
+                           recs.ctypes.data)
     return status, recs
 
 
-def apply(c, q, blob, offsets, terms=None):
+def apply(c, q, blob, offsets, terms=None, n_bytes=None):
     """hwo_apply over columns c (groups [0, c.n_groups) are the arena's) and read queues q (RO.ReadQueues, or None for
-    an arena without them) -> (status bytes WIRE_* << 4 | RES_*, released reads)."""
+    an arena without them) -> (status bytes WIRE_* << 4 | RES_*, released reads); n_bytes as in O.wire_decode_batch."""
     blob, offsets, gt = _arrays(blob, offsets, terms)
     n = len(offsets) - 1
     status = np.zeros(n, np.uint8)
@@ -78,5 +82,6 @@ def apply(c, q, blob, offsets, terms=None):
     v = O.view(c)
     qq = q._q() if q is not None else None
     lib().hwo_apply(C.byref(v), C.byref(qq) if qq is not None else None, blob.ctypes.data, offsets.ctypes.data, n,
-                    None if gt is None else gt.ctypes.data, status.ctypes.data, out.ctypes.data, C.byref(cnt))
+                    O.wire_n_bytes(blob, n_bytes), None if gt is None else gt.ctypes.data, status.ctypes.data, out.ctypes.data,
+                    C.byref(cnt))
     return status, out[: cnt.value]

@@ -183,7 +183,7 @@ def lib() -> C.CDLL:
         L.ro_inflights_reset.argtypes, L.ro_inflights_reset.restype = [pi], None
         L.wo_decode_message.argtypes = [C.c_void_p, sz, C.POINTER(WireMessage)]
         L.wo_decode_message.restype = i32
-        L.wo_decode_batch.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+        L.wo_decode_batch.argtypes = [C.c_void_p, C.c_void_p, sz, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p]
         L.wo_decode_batch.restype = None
         _lib = L
@@ -413,8 +413,17 @@ def wire_decode_message(raw: bytes):
             "request_snapshot": m.request_snapshot, "reject_hint": m.reject_hint, "priority": m.priority}
 
 
-def wire_decode_batch(blob: np.ndarray, offsets: np.ndarray, n_groups: int, group_term: np.ndarray | None = None):
-    """wo_decode_batch -> (status u8[n], records (24-byte dtype)[n], hint u64[n], request_snapshot u64[n])."""
+def wire_n_bytes(blob: np.ndarray, n_bytes: int | None) -> int:
+    """A wire batch's length: n_bytes, at most len(blob) (the oracles read no byte past the blob)."""
+    n_bytes = len(blob) if n_bytes is None else int(n_bytes)
+    assert 0 <= n_bytes <= len(blob)
+    return n_bytes
+
+
+def wire_decode_batch(blob: np.ndarray, offsets: np.ndarray, n_groups: int, group_term: np.ndarray | None = None,
+                      n_bytes: int | None = None):
+    """wo_decode_batch -> (status u8[n], records (24-byte dtype)[n], hint u64[n], request_snapshot u64[n]).  n_bytes:
+    the batch's length (default len(blob)); a frame that ends past it is WIRE_MALFORMED."""
     n = len(offsets) - 1
     rec_dtype = np.dtype([("group", "<u4"), ("peer_slot", "u1"), ("flags", "u1"), ("reserved", "<u2"),
                           ("index", "<u8"), ("commit", "<u8")])
@@ -425,6 +434,7 @@ def wire_decode_batch(blob: np.ndarray, offsets: np.ndarray, n_groups: int, grou
     blob = np.ascontiguousarray(blob, dtype=np.uint8)
     offsets = np.ascontiguousarray(offsets, dtype=np.uint32)
     gt = None if group_term is None else np.ascontiguousarray(group_term, dtype=np.uint64)
-    lib().wo_decode_batch(blob.ctypes.data, offsets.ctypes.data, n, None if gt is None else gt.ctypes.data, n_groups,
-                          status.ctypes.data, recs.ctypes.data, hint.ctypes.data, snap.ctypes.data)
+    lib().wo_decode_batch(blob.ctypes.data, offsets.ctypes.data, n, wire_n_bytes(blob, n_bytes),
+                          None if gt is None else gt.ctypes.data, n_groups, status.ctypes.data, recs.ctypes.data,
+                          hint.ctypes.data, snap.ctypes.data)
     return status, recs, hint, snap

@@ -39,10 +39,10 @@ static int transfer(const uint8_t *msg, uint32_t off, uint32_t len) {
 
 /* Frame i opened: its header, Message and context; 0 when it is not a frame, names a group >= n_groups or is not a
  * protobuf message. */
-static int open_frame(const ro_arena_view *a, const uint8_t *bytes, const uint32_t *offsets, size_t i, uint32_t *hdr,
+static int open_frame(const ro_arena_view *a, const uint8_t *bytes, const uint32_t *offsets, uint64_t n_bytes, size_t i, uint32_t *hdr,
                       wo_message *m, int *force) {
     const uint32_t lo = offsets[i], hi = offsets[i + 1];
-    if (hi < lo || hi - lo < 4) return 0;
+    if (hi < lo || hi > n_bytes || hi - lo < 4) return 0;
     memcpy(hdr, bytes + lo, 4); /* little-endian host */
     hwo_message h;
     if ((*hdr >> 4) >= a->n_groups || !hwo_decode_message(bytes + lo + 4, hi - lo - 4, &h)) return 0;
@@ -92,7 +92,7 @@ static void respond(uint8_t *resp, uint32_t *resp_offsets, uint64_t *totals, uin
 }
 
 void vro_batch(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets,
-               size_t n, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
+               size_t n, uint64_t n_bytes, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
                uint64_t *totals) {
     uint8_t *claimed = (uint8_t *)calloc(a->n_groups ? a->n_groups : 1, 1);
     totals[0] = totals[1] = 0;
@@ -103,7 +103,7 @@ void vro_batch(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, const uint8_
         int force;
         status[i] = WO_WIRE_MALFORMED << 4;
         out[2 * i] = out[2 * i + 1] = 0;
-        if (!open_frame(a, bytes, offsets, i, &hdr, &m, &force)) continue;
+        if (!open_frame(a, bytes, offsets, n_bytes, i, &hdr, &m, &force)) continue;
         const uint32_t g = hdr >> 4;
         if (a->meta[g] & RO_META_WIDE_HI) continue;
         if (m.msg_type != 5 && m.msg_type != 17) { /* MsgRequestVote, MsgRequestPreVote */
@@ -161,7 +161,7 @@ void vro_batch(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, const uint8_
 }
 
 void vro_literal(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, uint8_t *role, vro_voter *voters,
-                 const uint8_t *bytes, const uint32_t *offsets, size_t n, uint8_t *resp, uint32_t *resp_offsets,
+                 const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes, uint8_t *resp, uint32_t *resp_offsets,
                  uint64_t *totals) {
     totals[0] = totals[1] = 0;
     resp_offsets[0] = 0;
@@ -169,7 +169,7 @@ void vro_literal(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, uint8_t *r
         uint32_t hdr;
         wo_message m;
         int force;
-        if (!open_frame(a, bytes, offsets, i, &hdr, &m, &force) || (m.msg_type != 5 && m.msg_type != 17)) continue;
+        if (!open_frame(a, bytes, offsets, n_bytes, i, &hdr, &m, &force) || (m.msg_type != 5 && m.msg_type != 17)) continue;
         const uint32_t g = hdr >> 4;
         if (a->meta[g] & RO_META_WIDE_HI) continue; /* a pair is addressed by its low half */
         vro_voter *v = &voters[g];
@@ -204,11 +204,11 @@ void vro_literal(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, uint8_t *r
 }
 
 double vro_bench(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets,
-                 size_t n, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
+                 size_t n, uint64_t n_bytes, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
                  uint64_t *totals) {
     struct timespec t0, t1;
     clock_gettime(CLOCK_MONOTONIC, &t0);
-    vro_batch(a, q, votes, bytes, offsets, n, voters, status, out, resp, resp_offsets, totals);
+    vro_batch(a, q, votes, bytes, offsets, n, n_bytes, voters, status, out, resp, resp_offsets, totals);
     clock_gettime(CLOCK_MONOTONIC, &t1);
     return (double)(t1.tv_sec - t0.tv_sec) + 1e-9 * (double)(t1.tv_nsec - t0.tv_nsec);
 }

@@ -49,19 +49,19 @@ size_t vro_encode_response(uint32_t msg_type, uint64_t to, uint64_t from, uint64
  * otherwise; the responses (header + Message) back to back in resp (64 n bytes), resp_offsets [responses + 1],
  * totals = {responses, bytes}. */
 void vro_batch(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets,
-               size_t n, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
+               size_t n, uint64_t n_bytes, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
                uint64_t *totals);
 
 /* The literal form: every frame in order, as the reference steps it.  role[g] (0 Follower, 1 PreCandidate, 2 Candidate,
  * 3 Leader; the low half's for a pair), voters (vote, flags) and the arena change as the reference would change them;
  * the responses go to resp / resp_offsets / totals as in the batch form (resp: 64 n bytes). */
 void vro_literal(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, uint8_t *role, vro_voter *voters,
-                 const uint8_t *bytes, const uint32_t *offsets, size_t n, uint8_t *resp, uint32_t *resp_offsets,
+                 const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes, uint8_t *resp, uint32_t *resp_offsets,
                  uint64_t *totals);
 
 /* vro_batch's seconds on one core (the micro-benchmark's CPU reference). */
 double vro_bench(ro_arena_view *a, ro_read_queues *q, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets,
-                 size_t n, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
+                 size_t n, uint64_t n_bytes, const vro_voter *voters, uint8_t *status, uint64_t *out, uint8_t *resp, uint32_t *resp_offsets,
                  uint64_t *totals);
 
 #ifdef __cplusplus

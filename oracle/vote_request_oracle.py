@@ -31,10 +31,11 @@ def lib() -> C.CDLL:
         L = O.lib()
         u32, u64, vp, sz = C.c_uint32, C.c_uint64, C.c_void_p, C.c_size_t
         L.vro_encode_response.argtypes, L.vro_encode_response.restype = [u32, u64, u64, u64, u64, C.c_int, u64, vp], sz
-        args = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, vp, sz, vp, vp, vp, vp, vp, vp]
+        args = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, vp, sz, u64, vp, vp, vp, vp, vp, vp]
         L.vro_batch.argtypes, L.vro_batch.restype = args, None
         L.vro_bench.argtypes, L.vro_bench.restype = args, C.c_double
-        L.vro_literal.argtypes = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, vp, vp, vp, sz, vp, vp, vp]
+        L.vro_literal.argtypes = [C.POINTER(O.ArenaView), C.POINTER(RO.Queues), vp, vp, vp, vp, vp, sz, u64, vp, vp,
+                                 vp]
         L.vro_literal.restype = None
         _lib = L
     return _lib
@@ -47,7 +48,7 @@ def encode_response(msg_type, to, frm, term, commit=0, reject=False, commit_term
     return bytes(buf[:k])
 
 
-def _common(c, q, votes, blob, offsets):
+def _common(c, q, votes, blob, offsets, n_bytes):
     assert votes.dtype == np.uint8 and votes.shape == (O.SLOTS, c.cap) and votes.flags.c_contiguous
     blob = np.ascontiguousarray(blob, dtype=np.uint8)
     offsets = np.ascontiguousarray(offsets, dtype=np.uint32)
@@ -55,32 +56,33 @@ def _common(c, q, votes, blob, offsets):
     resp, roff, totals = np.zeros(max(16, n * FRAME_MAX), np.uint8), np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
     v = O.view(c)
     qq = q._q() if q is not None else None
-    return blob, offsets, n, resp, roff, totals, v, qq
+    return blob, offsets, n, O.wire_n_bytes(blob, n_bytes), resp, roff, totals, v, qq
 
 
-def batch(c, q, votes, blob, offsets, voters, bench: bool = False):
+def batch(c, q, votes, blob, offsets, voters, bench: bool = False, n_bytes=None):
     """vro_batch over columns c (c.term = Raft::term; changed in place, as the arena is), read queues q (RO.ReadQueues
     or None) and votes ([SLOTS][cap] u8) with the caller's table voters (VOTER_DTYPE per group slot) -> (status u8[n],
-    out u64[n][2], response blob, response offsets u32[responses + 1], totals u64[2]); with bench=True also seconds."""
-    blob, offsets, n, resp, roff, totals, v, qq = _common(c, q, votes, blob, offsets)
+    out u64[n][2], response blob, response offsets u32[responses + 1], totals u64[2]); with bench=True also seconds.
+    n_bytes as in O.wire_decode_batch."""
+    blob, offsets, n, nb, resp, roff, totals, v, qq = _common(c, q, votes, blob, offsets, n_bytes)
     vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
     assert len(vt) >= c.n_groups
     status, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
     f = lib().vro_bench if bench else lib().vro_batch
     secs = f(C.byref(v), C.byref(qq) if qq is not None else None, votes.ctypes.data, blob.ctypes.data, offsets.ctypes.data,
-             n, vt.ctypes.data, status.ctypes.data, out.ctypes.data, resp.ctypes.data, roff.ctypes.data, totals.ctypes.data)
+             n, nb, vt.ctypes.data, status.ctypes.data, out.ctypes.data, resp.ctypes.data, roff.ctypes.data, totals.ctypes.data)
     res = (status, out, resp[: int(totals[1])].copy(), roff[: int(totals[0]) + 1].copy(), totals)
     return res + (secs,) if bench else res
 
 
-def literal(c, q, votes, role, voters, blob, offsets):
+def literal(c, q, votes, role, voters, blob, offsets, n_bytes=None):
     """vro_literal: the frames one at a time as the reference steps them.  c, q, votes, role (u8 per group slot) and
     voters (VOTER_DTYPE, a contiguous array: its vote and flags change) change in place -> (response blob, response
-    offsets u32[responses + 1], totals u64[2])."""
-    blob, offsets, n, resp, roff, totals, v, qq = _common(c, q, votes, blob, offsets)
+    offsets u32[responses + 1], totals u64[2]).  n_bytes as in O.wire_decode_batch."""
+    blob, offsets, n, nb, resp, roff, totals, v, qq = _common(c, q, votes, blob, offsets, n_bytes)
     assert voters.dtype == VOTER_DTYPE and voters.flags.c_contiguous and len(voters) >= c.n_groups
     assert role.dtype == np.uint8 and role.flags.c_contiguous and len(role) >= c.n_groups
     lib().vro_literal(C.byref(v), C.byref(qq) if qq is not None else None, votes.ctypes.data, role.ctypes.data,
-                      voters.ctypes.data, blob.ctypes.data, offsets.ctypes.data, n, resp.ctypes.data, roff.ctypes.data,
+                      voters.ctypes.data, blob.ctypes.data, offsets.ctypes.data, n, nb, resp.ctypes.data, roff.ctypes.data,
                       totals.ctypes.data)
     return resp[: int(totals[1])].copy(), roff[: int(totals[0]) + 1].copy(), totals

@@ -11,10 +11,10 @@ static inline int bit(const uint32_t *bm, uint32_t g) { return (int)((bm[g / 32]
 static uint64_t max64(uint64_t x, uint64_t y) { return x > y ? x : y; }
 
 /* Frame i: its header and Message; 0 when it is not a frame, names a group >= n_groups or is not a protobuf message. */
-static int open_frame(const ro_arena_view *a, const uint8_t *bytes, const uint32_t *offsets, size_t i, uint32_t *hdr,
+static int open_frame(const ro_arena_view *a, const uint8_t *bytes, const uint32_t *offsets, uint64_t n_bytes, size_t i, uint32_t *hdr,
                       wo_message *m) {
     const uint32_t lo = offsets[i], hi = offsets[i + 1];
-    if (hi < lo || hi - lo < 4) return 0;
+    if (hi < lo || hi > n_bytes || hi - lo < 4) return 0;
     memcpy(hdr, bytes + lo, 4); /* little-endian host */
     return (*hdr >> 4) < a->n_groups && wo_decode_message(bytes + lo + 4, hi - lo - 4, m);
 }
@@ -33,7 +33,7 @@ static uint32_t tally(const ro_arena_view *a, const uint8_t *votes, uint32_t lo)
     return (uint32_t)v | gr << 8 | rj << 16;
 }
 
-void vwo_batch(ro_arena_view *a, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+void vwo_batch(ro_arena_view *a, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                const uint32_t *select, const uint32_t *pre, uint8_t *status, vwo_outcome *out, uint64_t *n_out,
                uint64_t *tallied) {
     uint8_t *applied = (uint8_t *)calloc((size_t)RO_SLOTS * a->cap + 1, 1), *touched = (uint8_t *)calloc(a->cap + 1, 1);
@@ -41,7 +41,7 @@ void vwo_batch(ro_arena_view *a, uint8_t *votes, const uint8_t *bytes, const uin
         uint32_t hdr;
         wo_message m;
         status[i] = WO_WIRE_MALFORMED << 4;
-        if (!open_frame(a, bytes, offsets, i, &hdr, &m)) continue;
+        if (!open_frame(a, bytes, offsets, n_bytes, i, &hdr, &m)) continue;
         if (m.msg_type != 6 && m.msg_type != 18) { /* MsgRequestVoteResponse, MsgRequestPreVoteResponse */
             status[i] = WO_WIRE_SKIP_TYPE << 4;
             continue;
@@ -149,12 +149,12 @@ static void transition(ro_arena_view *a, uint8_t *votes, uint8_t *role, uint32_t
     }
 }
 
-void vwo_literal(ro_arena_view *a, uint8_t *votes, uint8_t *role, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+void vwo_literal(ro_arena_view *a, uint8_t *votes, uint8_t *role, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                  uint32_t *first) {
     for (size_t i = 0; i < n; i++) {
         uint32_t hdr;
         wo_message m;
-        if (!open_frame(a, bytes, offsets, i, &hdr, &m) || (m.msg_type != 6 && m.msg_type != 18)) continue;
+        if (!open_frame(a, bytes, offsets, n_bytes, i, &hdr, &m) || (m.msg_type != 6 && m.msg_type != 18)) continue;
         const uint32_t g = hdr >> 4, slot = hdr & 15u, lo = low_half(a, g);
         const uint64_t term = a->term[lo];
         /* Raft::step's term rules (raft.rs:1280-1349); m.term == 0 is a local message and goes on */

@@ -41,14 +41,14 @@ typedef struct {
 /* The batch form.  select / pre: bitmaps from group 0 (pre nullable); status[i] = WO_WIRE_* / VWO_WIRE_* << 4 | the
  * applied frame's result (1 recorded, 0 the cell had a vote, 4 a slot >= 8); out (room for min(n, n_groups)) gets the
  * decided groups in ascending order, *n_out how many, *tallied the touched groups. */
-void vwo_batch(ro_arena_view *a, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+void vwo_batch(ro_arena_view *a, uint8_t *votes, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                const uint32_t *select, const uint32_t *pre, uint8_t *status, vwo_outcome *out, uint64_t *n_out,
                uint64_t *tallied);
 
 /* The literal form.  role[g] (VWO_*, the low half's for a pair) and the arena (a->term included) change as the reference
  * would change them.  first[g] = the first Won or Lost word poll returned for group g in this batch, left alone where
  * none did (the caller fills it with 0xffffffff). */
-void vwo_literal(ro_arena_view *a, uint8_t *votes, uint8_t *role, const uint8_t *bytes, const uint32_t *offsets, size_t n,
+void vwo_literal(ro_arena_view *a, uint8_t *votes, uint8_t *role, const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes,
                  uint32_t *first);
 
 #ifdef __cplusplus

@@ -74,7 +74,7 @@ int wo_decode_message(const uint8_t *buf, size_t len, wo_message *out) {
     return 1;
 }
 
-void wo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, const uint64_t *group_term,
+void wo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, uint64_t n_bytes, const uint64_t *group_term,
                      uint32_t n_groups, uint8_t *status, wo_record *recs, uint64_t *hint, uint64_t *request_snapshot) {
     uint8_t *touched = (uint8_t *)calloc(n_groups ? n_groups : 1, 2); /* 16 slot bits per group */
     for (size_t i = 0; i < n; i++) {
@@ -82,7 +82,7 @@ void wo_decode_batch(const uint8_t *bytes, const uint32_t *offsets, size_t n, co
         hint[i] = 0;
         request_snapshot[i] = 0;
         const uint32_t lo = offsets[i], hi = offsets[i + 1];
-        if (hi < lo || hi - lo < 4) {
+        if (hi < lo || hi > n_bytes || hi - lo < 4) {
             status[i] = WO_WIRE_MALFORMED;
             continue;
         }

@@ -31,8 +31,9 @@ def _self_ids(rng, n):
     return ids
 
 
-def _device(a, blob, off, sel, ids):
-    """The device form over buffers from raftgpu_device_alloc -> (status, from, response blob, offsets, totals)."""
+def _device(a, blob, off, sel, ids, n_bytes=None):
+    """The device form over buffers from raftgpu_device_alloc (n_bytes: of blob, all of it by default) -> (status, from,
+    response blob, offsets, totals)."""
     n = len(off) - 1
     bound = B.follower_heartbeat_bound(n)
     bufs = [a.device_alloc(x) for x in (max(16, len(blob)), 4 * (n + 1), sel.nbytes, ids.nbytes, max(1, n), 8 * max(1, n),
@@ -40,7 +41,7 @@ def _device(a, blob, off, sel, ids):
     d_b, d_o, d_s, d_i, d_st, d_f, d_rb, d_ro, d_t = bufs
     for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_i, ids)):
         a.h2d(p, x)
-    a.follower_heartbeat_device(d_b, len(blob), d_o, n, d_s, d_i, d_st, d_f, d_rb, bound, d_ro, d_t)
+    a.follower_heartbeat_device(d_b, len(blob) if n_bytes is None else n_bytes, d_o, n, d_s, d_i, d_st, d_f, d_rb, bound, d_ro, d_t)
     a.synchronize()
     tot = np.zeros(2, np.uint64)
     a.d2h(tot, d_t)

@@ -176,9 +176,9 @@ def _mixed_batch(rng, d, n, terms, reads, k):
     return F.batch([frames[j] for j in order])
 
 
-def _oracle_append(c, blob, offsets, n, terms):
+def _oracle_append(c, blob, offsets, n, terms, n_bytes=None):
     """raftgpu_wire_apply_device: the AppendResponse frames, first of every cell, in frame order."""
-    status, recs, hint, snap = O.wire_decode_batch(blob, offsets, n, terms)
+    status, recs, hint, snap = O.wire_decode_batch(blob, offsets, n, terms, n_bytes)
     ok = np.nonzero(status == O.WIRE_OK)[0]
     rows = []
     for i in ok:

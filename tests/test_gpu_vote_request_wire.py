@@ -19,9 +19,11 @@ pytestmark = pytest.mark.gpu
 ARENA_COLUMNS = ("term_start", "committed", "last_index", "matched", "next_idx", "peer_committed", "pflags")
 
 
-def _device(a, blob, off, voters):
-    """The device form over buffers from raftgpu_device_alloc -> (status, out, response blob, offsets, totals)."""
+def _device(a, blob, off, voters, n_bytes=None):
+    """The device form over buffers from raftgpu_device_alloc (n_bytes: of blob, all of it by default) -> (status, out,
+    response blob, offsets, totals)."""
     n = len(off) - 1
+    n_bytes = len(blob) if n_bytes is None else n_bytes
     blob = np.concatenate([blob, np.zeros(16, np.uint8)])
     bound = B.vote_request_wire_bound(n)
     vt = np.ascontiguousarray(voters, B.VOTER_DTYPE)
@@ -30,7 +32,7 @@ def _device(a, blob, off, voters):
     d_b, d_o, d_v, d_st, d_out, d_rb, d_ro, d_t = bufs
     for p, x in ((d_b, blob), (d_o, off), (d_v, vt)):
         a.h2d(p, x)
-    a.vote_request_wire_device(d_b, len(blob) - 16, d_o, n, d_v, d_st, d_out, d_rb, bound, d_ro, d_t)
+    a.vote_request_wire_device(d_b, n_bytes, d_o, n, d_v, d_st, d_out, d_rb, bound, d_ro, d_t)
     a.synchronize()
     tot = np.zeros(2, np.uint64)
     a.d2h(tot, d_t)

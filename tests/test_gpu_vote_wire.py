@@ -1,7 +1,8 @@
 """Vote responses at a candidate on the GPU (raftgpu_vote_wire[_device]) against the batch oracle
 (oracle/vote_wire_oracle.c): the reference's election table, every status, random 100K-group elections with joint
 configurations, learners, wide pairs and hostile frames, a 1M-group storm against INTEGRATION.md section 6's control
-list on a twin arena, one buffer through all three response passes, and the refusals.  Run with -m gpu."""
+list on a twin arena, and the refusals (one buffer through every wire pass: test_gpu_wire_batches.py).  Run with
+-m gpu."""
 import ctypes as C
 
 import numpy as np
@@ -34,15 +35,16 @@ def _votes(a, n):
     return np.stack([a.column_read(B.COL_VOTES, s, 0, n, np.uint8) for s in range(O.SLOTS)])
 
 
-def _device(a, blob, off, sel, pre, cap=None):
-    """The device form over buffers from raftgpu_device_alloc -> (status, outcomes)."""
+def _device(a, blob, off, sel, pre, cap=None, n_bytes=None):
+    """The device form over buffers from raftgpu_device_alloc (n_bytes: of blob, all of it by default) -> (status,
+    outcomes)."""
     n = len(off) - 1
     cap = min(n, a.get_info().n_alloc) if cap is None else cap
     bufs = [a.device_alloc(x) for x in (max(16, len(blob)), 4 * (n + 1), sel.nbytes, pre.nbytes, max(1, n), 8 * max(1, cap), 8)]
     d_b, d_o, d_s, d_p, d_st, d_out, d_cnt = bufs
     for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_p, pre)):
         a.h2d(p, x)
-    a.vote_wire_device(d_b, len(blob), d_o, n, d_s, d_p, d_st, d_out, cap, d_cnt)
+    a.vote_wire_device(d_b, len(blob) if n_bytes is None else n_bytes, d_o, n, d_s, d_p, d_st, d_out, cap, d_cnt)
     a.synchronize()
     cnt = np.zeros(1, np.uint64)
     a.d2h(cnt, d_cnt)
@@ -203,48 +205,6 @@ def test_1m_storm_against_the_control_list():
     assert np.array_equal(_votes(arenas[0], n), _votes(arenas[1], n))
     for a in arenas:
         a.close()
-
-
-# --------------------------------------------------------------------------- 4. one buffer, three passes
-
-
-def test_mixed_buffer_each_frame_applied_once():
-    """Append, heartbeat and vote responses in one buffer through raftgpu_step_begin_wire, raftgpu_heartbeat_wire and
-    raftgpu_vote_wire: every frame is applied (status OK) by at most one pass, and by exactly the one of its type when
-    the frame is well-formed for it."""
-    rng = np.random.default_rng(0x7079)
-    e = V.Election(rng, 4000, 0, p_role=(0.1, 0.4, 0.25, 0.25))
-    a = _arena(e)
-    frames, kind = [], []
-    for f in e.frames(rng, noise=False):
-        frames.append(f)
-        kind.append(6)
-    for g in range(e.n):
-        if e.role[g] != V.LEADER:
-            continue
-        for s in range(1, 5):
-            if not (int(e.present[g]) >> s & 1) or s == e.self_slot[g]:
-                continue
-            t = int(e.term[g])
-            frames.append(F.frame(g, s, F.message(4, term=t, index=int(e.last[g]))))
-            kind.append(4)
-            frames.append(F.frame(g, s, F.message(9, term=t, commit=int(e.committed[g]))))
-            kind.append(9)
-    order = rng.permutation(len(frames))
-    frames, kind = [frames[i] for i in order], np.array(kind)[order]
-    fb = F.Frames(frames)
-    vst, _ = a.vote_wire(fb, e.select(), e.pre())
-    hst, _ = a.heartbeat_wire(fb)
-    a.step_begin_wire(fb)
-    a.step_wait()
-    ast = a.wire_status().copy()
-    ok = np.stack([(x >> 4) == B.WIRE_OK for x in (ast, hst, vst)])
-    assert np.all(ok.sum(0) <= 1)
-    for row, k in enumerate((4, 9, 6)):
-        assert np.all(ok[row] <= (kind == k)) and ok[row][kind == k].mean() > 0.5, k
-        others = np.stack([ast, hst, vst])[row][kind != k] >> 4
-        assert np.all(others == B.WIRE_SKIP_TYPE), k
-    a.close()
 
 
 # --------------------------------------------------------------------------- 5. freed slots and the outcome bound
