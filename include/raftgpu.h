@@ -506,9 +506,14 @@ int32_t raftgpu_step_begin_compact(raftgpu_arena *arena, const void *pinned_blob
  * works through the scatter kernel, one record per cell), then the step is submitted like
  * raftgpu_step_begin_compact.  Nothing may have been enqueued for this step.  `records` can be
  * reused as soon as the call returns.  A batch too hostile for the compact form (every record
- * escaping to the side table) goes through raftgpu_enqueue_bulk + raftgpu_step_begin instead, and so does
- * a batch with several records per cell on an arena that cannot run the fused kernel (device-side
- * Inflights, wide groups; RAFTGPU_STEP_ASYNC is ignored on such arenas).
+ * escaping to the side table) goes through raftgpu_enqueue_bulk + raftgpu_step_begin instead, and
+ * so does a batch with several records per cell that the fused kernel cannot take: one that is
+ * not group-ordered or too sparse to tile (a unit block of the stream spanning more than 4095
+ * groups), or any such batch on an arena that cannot run the fused kernel (device-side Inflights,
+ * wide groups; RAFTGPU_STEP_ASYNC is ignored on such arenas).  With RAFTGPU_STEP_ASYNC the batch
+ * is packed after the call has returned, too late to change paths: a batch that needs the general
+ * path is refused instead, its raftgpu_step_wait returns RAFTGPU_ERR_FULL and nothing of it is
+ * applied; submit it again without RAFTGPU_STEP_ASYNC.
  * raft.rs:1663-1743 + 893-904 for a whole tick, as one call. */
 int32_t raftgpu_step_begin_records(raftgpu_arena *arena, const raftgpu_append_resp *records, uint64_t n,
                                    uint32_t flags);
@@ -529,7 +534,8 @@ int32_t raftgpu_step_compact_device(raftgpu_arena *arena, void *stream, const vo
                                     uint32_t *d_adv_bitmap, uint64_t *d_commit_out, uint32_t *d_dup_count,
                                     uint32_t flags);
 /* Result bytes of the last completed ZERO-COPY step (packed: one per packed record, compact:
- * one per unit; 0 for EXT payloads / headers), valid until the next raftgpu_step_wait.  Needs
+ * one per unit; 0 for EXT payloads / headers), valid until the next raftgpu_step_wait
+ * (RAFTGPU_ERR_INVALID while two steps are in flight, as raftgpu_step_results).  Needs
  * RAFTGPU_STEP_READ_RESULTS.  raft.rs:1663-1743: what handle_append_response decided per message. */
 int32_t raftgpu_step_slot_results(raftgpu_arena *arena, const uint8_t **results, uint64_t *n_slots);
 
@@ -572,7 +578,11 @@ int32_t raftgpu_step_wait(raftgpu_arena *arena, raftgpu_step_result *out);
 int32_t raftgpu_step(raftgpu_arena *arena, uint32_t flags, raftgpu_step_result *out);
 
 /* Results of the last completed step, in arena-owned pinned memory, valid until
- * the next raftgpu_step_wait: adv_bitmap has bit g set iff group g advanced
+ * the next raftgpu_step_wait.  While two steps are in flight the third staging set,
+ * which held them, stages the next batch: from the begin that leaves two in flight
+ * until the next wait this call returns RAFTGPU_ERR_INVALID, as do
+ * raftgpu_step_slot_results, raftgpu_step_record_results and raftgpu_step_send_list.
+ * adv_bitmap has bit g set iff group g advanced
  * (LightReady.commit_index, raw_node.rs:643-650); committed[g] is meaningful
  * for advanced groups when RAFTGPU_STEP_READ_COMMITTED was set. */
 int32_t raftgpu_step_results(raftgpu_arena *arena, const uint32_t **adv_bitmap,
