@@ -30,7 +30,7 @@
  * Data layout in HBM (struct-of-arrays, see DESIGN.md): per-peer columns are
  * [RAFTGPU_SLOTS][cap] u64 / u8, per-group columns are [cap]; a "group" is one
  * raft group (one ProgressTracker), a "peer slot" one Progress of that group.
- * next_idx and peer_committed are held on the device as signed 32-bit offsets
+ * next_idx and peer_committed are held on the device as signed 16-bit offsets
  * from the same cell's matched, with the exact u64 kept aside for a value the
  * offset cannot express; raftgpu_column_read / _write convert, so every column
  * call still sees u64 values (and a write of matched keeps the cells' next_idx

@@ -10,8 +10,8 @@ struct Columns {
     uint64_t *matched;
     // next_idx and peer_committed of a cell are stored as offsets from its matched (next_d, pc_d; off_* below); the
     // u64 columns hold the exact value of the cells whose offset is kOffEscape and are not read for any other cell
-    int32_t *next_d;
-    int32_t *pc_d;
+    int16_t *next_d;
+    int16_t *pc_d;
     uint64_t *next_idx;
     uint64_t *peer_committed;
     uint64_t *pending_snapshot;
@@ -62,25 +62,26 @@ __device__ __forceinline__ uint64_t umax64(uint64_t a, uint64_t b) { return a > 
 
 // ---------------------------------------------------------------------------
 // The offset codec of next_idx and peer_committed.  In a live group both sit within the inflight window of the same
-// cell's matched, so each is stored as a signed 32-bit offset from it (next_d, pc_d): a fused step then moves 8 bytes
-// per cell for the two instead of 16.  A value the offset cannot express (a peer right after Raft::reset, whose
-// matched is 0) is stored as kOffEscape, with the exact value in the u64 column.  The format is lossless for every
-// u64 value.  Offsets are relative to matched, so every write of matched re-encodes both offsets of its cell
+// cell's matched, so each is stored as a signed 16-bit offset from it (next_d, pc_d): a fused step then moves 4 bytes
+// per cell for the two instead of 16.  A value the offset cannot express -- more than 32 767 entries ahead of matched
+// or behind it, or a peer right after Raft::reset, whose matched is 0 -- is stored as kOffEscape, with the
+// exact value in the u64 column; such a cell takes the general path, correct but slower.  The format is lossless for
+// every u64 value.  Offsets are relative to matched, so every write of matched re-encodes both offsets of its cell
 // (hot_write); nothing outside this section does the arithmetic.
-constexpr int32_t kOffEscape = INT32_MIN;
+constexpr int16_t kOffEscape = INT16_MIN;
 
-__device__ __forceinline__ bool off_escaped(int32_t d) { return d == kOffEscape; }
+__device__ __forceinline__ bool off_escaped(int16_t d) { return d == kOffEscape; }
 // the value of an offset that is not kOffEscape
-__device__ __forceinline__ uint64_t off_value(int32_t d, uint64_t matched) {
+__device__ __forceinline__ uint64_t off_value(int16_t d, uint64_t matched) {
     return matched + static_cast<uint64_t>(static_cast<int64_t>(d));
 }
-__device__ __forceinline__ uint64_t off_decode(int32_t d, uint64_t matched, const uint64_t *esc) {
+__device__ __forceinline__ uint64_t off_decode(int16_t d, uint64_t matched, const uint64_t *esc) {
     return off_escaped(d) ? *esc : off_value(d, matched);
 }
 // the offset to store for value v; a value that does not fit goes to *esc (a plain store, no read)
-__device__ __forceinline__ int32_t off_encode(uint64_t v, uint64_t matched, uint64_t *esc) {
-    const int64_t d = static_cast<int64_t>(v - matched);
-    if (d > static_cast<int64_t>(kOffEscape) && d <= static_cast<int64_t>(INT32_MAX)) return static_cast<int32_t>(d);
+__device__ __forceinline__ int16_t off_encode(uint64_t v, uint64_t matched, uint64_t *esc) {
+    const uint64_t d = v - matched;  // in the window (kOffEscape, INT16_MAX] iff d + INT16_MAX <= 2 * INT16_MAX, mod 2^64
+    if (d + static_cast<uint64_t>(INT16_MAX) <= 2u * static_cast<uint64_t>(INT16_MAX)) return static_cast<int16_t>(d);
     *esc = v;
     return kOffEscape;
 }
@@ -89,7 +90,7 @@ __device__ __forceinline__ int32_t off_encode(uint64_t v, uint64_t matched, uint
 // arena, which addresses its escape slots (always in HBM).
 struct HotPtrs {
     uint64_t *matched;
-    int32_t *next_d, *pc_d;
+    int16_t *next_d, *pc_d;
     size_t cell;
 };
 struct HotVals {
@@ -114,12 +115,12 @@ __device__ __forceinline__ void hot_write(const Columns &c, const HotPtrs &p, co
         *p.pc_d = off_encode(v.peer_committed, v.matched, c.peer_committed + p.cell);
 }
 // The same from the cell's stored form (matched and the two offsets as loaded): writes what differs.
-__device__ __forceinline__ void hot_write_over(const Columns &c, const HotPtrs &p, uint64_t old_matched, int32_t old_next_d,
-                                               int32_t old_pc_d, const HotVals &v) {
+__device__ __forceinline__ void hot_write_over(const Columns &c, const HotPtrs &p, uint64_t old_matched, int16_t old_next_d,
+                                               int16_t old_pc_d, const HotVals &v) {
     if (v.matched != old_matched) *p.matched = v.matched;
-    const int32_t nd = off_encode(v.next_idx, v.matched, c.next_idx + p.cell);
+    const int16_t nd = off_encode(v.next_idx, v.matched, c.next_idx + p.cell);
     if (nd != old_next_d) *p.next_d = nd;
-    const int32_t pd = off_encode(v.peer_committed, v.matched, c.peer_committed + p.cell);
+    const int16_t pd = off_encode(v.peer_committed, v.matched, c.peer_committed + p.cell);
     if (pd != old_pc_d) *p.pc_d = pd;
 }
 __device__ __forceinline__ void hot_store(const Columns &c, const HotPtrs &p, const HotVals &v) {
@@ -138,7 +139,7 @@ __device__ __forceinline__ void hot_update_committed(const Columns &c, const Hot
 }
 // Column IO of an offset column (raftgpu_column_read / _write): materialize the decoded values of cells [first,
 // first + n) in their u64 column, or encode the values the host has put there.
-__global__ void offset_column_kernel(const uint64_t *__restrict__ matched, int32_t *__restrict__ d,
+__global__ void offset_column_kernel(const uint64_t *__restrict__ matched, int16_t *__restrict__ d,
                                      uint64_t *__restrict__ esc, size_t first, uint32_t n, bool encode) {
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {

@@ -29,7 +29,7 @@ constexpr int kFMaxStages = 8;
 // in neighbouring lanes and touch the SAME column index of DIFFERENT rows: with a 256-element row
 // stride they would all fall on the same shared-memory banks (4-way conflicts on every access).
 // 258 u64 (= 2064 B, still 16-byte aligned for TMA) shifts consecutive rows by 4 banks.
-constexpr uint32_t kFRow64 = (kFTile + 2) * 8;   // bytes per u64 row; an offset row (next_d, pc_d) uses its first half
+constexpr uint32_t kFRow64 = (kFTile + 2) * 8;   // bytes per u64 row; an offset row (next_d, pc_d) uses its first quarter
 constexpr uint32_t kFRow8 = kFTile + 16;         // bytes per u8 (pflags) row
 constexpr uint32_t kFDefer = 32;                 // deferred (rare-path) records per warp per tile; more are handled inline
 // dynamic shared memory of the fused kernels: 227 KB per CTA minus their static shared memory (barriers, deferred lists)
@@ -146,7 +146,7 @@ struct TileBarriers {
 // One stage's rows in shared memory.  Row r of a per-peer column is the r-th hinted slot.
 struct TileRows {
     uint64_t *matched;
-    int32_t *next, *pc;  // the offsets next_d / pc_d, rows kFRow64 bytes apart
+    int16_t *next, *pc;  // the offsets next_d / pc_d, rows kFRow64 bytes apart
     uint64_t *committed, *ts, *li;
     uint32_t *meta;
     uint8_t *flags;
@@ -154,7 +154,7 @@ struct TileRows {
 };
 // matched and the offsets of the cell staged in row r for group gl (arena cell `cell`)
 __device__ __forceinline__ HotPtrs staged_hot(const TileRows &t, uint32_t r, uint32_t gl, size_t cell) {
-    return HotPtrs{&t.matched[r * (kFRow64 / 8) + gl], &t.next[r * (kFRow64 / 4) + gl], &t.pc[r * (kFRow64 / 4) + gl], cell};
+    return HotPtrs{&t.matched[r * (kFRow64 / 8) + gl], &t.next[r * (kFRow64 / 2) + gl], &t.pc[r * (kFRow64 / 2) + gl], cell};
 }
 
 // Where a consumer group is in its walk over the CTA's tiles.
@@ -208,8 +208,8 @@ struct TileRing {
         uint8_t *sb = smem + static_cast<size_t>(it % a.n_stages) * stage_bytes;
         TileRows t;
         t.matched = reinterpret_cast<uint64_t *>(sb);
-        t.next = reinterpret_cast<int32_t *>(sb + H * kFRow64);
-        t.pc = reinterpret_cast<int32_t *>(sb + 2u * H * kFRow64);
+        t.next = reinterpret_cast<int16_t *>(sb + H * kFRow64);
+        t.pc = reinterpret_cast<int16_t *>(sb + 2u * H * kFRow64);
         t.committed = reinterpret_cast<uint64_t *>(sb + 3u * H * kFRow64);
         t.ts = t.committed + kFRow64 / 8;
         t.li = t.ts + kFRow64 / 8;
@@ -254,7 +254,7 @@ struct TileRing {
             const uint32_t staged = staged_units(u0, u1);
             if (lane == 0) {
                 mbar_wait(&bar->empty[st], ph ^ 1u);
-                mbar_expect_tx(&bar->full[st], H * ng16 * (8u + 4u + 4u + 1u) + 3u * ng16 * 8u + ng16 * 4u + staged * 4u);
+                mbar_expect_tx(&bar->full[st], H * ng16 * (8u + 2u + 2u + 1u) + 3u * ng16 * 8u + ng16 * 4u + staged * 4u);
             }
             __syncwarp();
             const TileRows t = rows(it);
@@ -263,8 +263,8 @@ struct TileRing {
                     const uint32_t col = j / H, r = j % H;  // col: 0 matched, 1 next_d, 2 pc_d, 3 pflags
                     const size_t cell = static_cast<size_t>(hinted_slot(r)) * c.cap + g0;
                     if (col == 0) tma_load_1d(t.matched + r * (kFRow64 / 8), c.matched + cell, ng16 * 8u, &bar->full[st]);
-                    if (col == 1) tma_load_1d(t.next + r * (kFRow64 / 4), c.next_d + cell, ng16 * 4u, &bar->full[st]);
-                    if (col == 2) tma_load_1d(t.pc + r * (kFRow64 / 4), c.pc_d + cell, ng16 * 4u, &bar->full[st]);
+                    if (col == 1) tma_load_1d(t.next + r * (kFRow64 / 2), c.next_d + cell, ng16 * 2u, &bar->full[st]);
+                    if (col == 2) tma_load_1d(t.pc + r * (kFRow64 / 2), c.pc_d + cell, ng16 * 2u, &bar->full[st]);
                     if (col == 3) tma_load_1d(t.flags + r * kFRow8, c.pflags + cell, ng16, &bar->full[st]);
                 } else if (j == 4u * H) {
                     tma_load_1d(t.committed, c.committed + g0, ng16 * 8u, &bar->full[st]);
@@ -298,8 +298,8 @@ struct TileRing {
                     const uint32_t col = j / H, r = j % H;
                     const size_t cell = static_cast<size_t>(hinted_slot(r)) * c.cap + g0;
                     if (col == 0) tma_store_1d(c.matched + cell, t.matched + r * (kFRow64 / 8), ng16 * 8u);
-                    if (col == 1) tma_store_1d(c.next_d + cell, t.next + r * (kFRow64 / 4), ng16 * 4u);
-                    if (col == 2) tma_store_1d(c.pc_d + cell, t.pc + r * (kFRow64 / 4), ng16 * 4u);
+                    if (col == 1) tma_store_1d(c.next_d + cell, t.next + r * (kFRow64 / 2), ng16 * 2u);
+                    if (col == 2) tma_store_1d(c.pc_d + cell, t.pc + r * (kFRow64 / 2), ng16 * 2u);
                     if (col == 3) tma_store_1d(c.pflags + cell, t.flags + r * kFRow8, ng16);
                 } else if (j == 4u * H) {
                     tma_store_1d(c.committed + g0, t.committed, ng16 * 8u);
@@ -471,13 +471,13 @@ __device__ __forceinline__ bool tile_fast_apply(const Columns &c, const TileRows
                                                 uint64_t index, uint64_t commit, bool is_local, bool is_reject,
                                                 uint64_t ext_hint, uint32_t hint, uint32_t present_mask, uint32_t *local,
                                                 uint32_t &res) {
-    constexpr uint32_t R64 = kFRow64 / 8, R32 = kFRow64 / 4;
+    constexpr uint32_t R64 = kFRow64 / 8, R16 = kFRow64 / 2;
     if (!((hint >> slot) & 1u)) return false;
     const uint32_t r = kSimple5 ? slot : static_cast<uint32_t>(__popc(hint & ((1u << slot) - 1u)));
-    const uint32_t ci = r * R64 + gl, di = r * R32 + gl;
+    const uint32_t ci = r * R64 + gl, di = r * R16 + gl;
     const uint32_t f0 = t.flags[r * kFRow8 + gl];
     const uint32_t state = f0 & RAFTGPU_PF_STATE_MASK;
-    const int32_t nd = t.next[di], pd = t.pc[di];
+    const int16_t nd = t.next[di], pd = t.pc[di];
     if (!((present_mask >> slot) & 1u) || state == RAFTGPU_STATE_SNAPSHOT || off_escaped(nd) || off_escaped(pd))
         return false;
     uint64_t m = t.matched[ci];
