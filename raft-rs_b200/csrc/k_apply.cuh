@@ -53,6 +53,48 @@ struct CellPtrs {
 
 // PackedRec and the kPk* / kCu* bit layouts: wire_format.h
 
+// The packed record at position i < n, read through at(j) -> ulonglong2 (one 128-bit load): the record array in HBM,
+// or the fused step's shared-memory copy of a tile's records (step_tile_kernel).
+template <class At>
+__device__ __forceinline__ RecRegs load_packed_rec(const At &at, uint64_t i, uint64_t n) {
+    RecRegs r;
+    const ulonglong2 q = at(i);
+    const uint64_t w0 = q.x;
+    const uint32_t delta = static_cast<uint32_t>(w0 >> 40);
+    const uint32_t flags = ((w0 & kPkReject) ? RAFTGPU_REC_REJECT : 0u) | ((w0 & kPkLocal) ? RAFTGPU_REC_LOCAL : 0u) |
+                           ((w0 & kPkExt) ? RAFTGPU_REC_EXT : 0u);
+    // the public layout: group | slot << 32 | flags << 40
+    r.w0 = (w0 & 0xffffffffull) | (((w0 >> 32) & 7ull) << 32) | (static_cast<uint64_t>(flags) << 40);
+    r.index = q.y;
+    if (w0 & kPkLocal)
+        r.commit = delta == kPkNoCommit ? 0 : q.y + delta;
+    else
+        r.commit = q.y - delta;
+    if ((w0 & kPkWide) && !(w0 & kPkExt)) {  // rare: the exact commit follows in an EXT of kind 3
+        for (uint64_t j = i + 1; j < n && j <= i + 3; j++) {
+            const ulonglong2 e = at(j);
+            if (!(e.x & kPkExt)) break;
+            if ((e.x >> 40) == 3) r.commit = e.y;
+        }
+    }
+    return r;
+}
+
+// next_probe_index / request_snapshot of the packed REJECT at position i, read through at(j) as above
+template <class At>
+__device__ __forceinline__ void load_packed_reject_ext(const At &at, uint64_t i, uint64_t n, uint64_t &hint,
+                                                       uint64_t &request_snapshot) {
+    hint = 0;
+    request_snapshot = RAFTGPU_INVALID_INDEX;
+    for (uint64_t j = i + 1; j < n && j <= i + 3; j++) {
+        const ulonglong2 e = at(j);
+        if (!(e.x & kPkExt)) break;
+        const uint32_t kind = static_cast<uint32_t>(e.x >> 40);
+        if (kind == 1) hint = e.y;
+        if (kind == 2) request_snapshot = e.y;
+    }
+}
+
 template <bool kPacked>
 __device__ __forceinline__ RecRegs load_rec(const void *recs_v, uint64_t i, uint64_t n) {
     RecRegs r;
@@ -68,25 +110,8 @@ __device__ __forceinline__ RecRegs load_rec(const void *recs_v, uint64_t i, uint
         r.index = p[1];
         r.commit = p[2];
     } else {
-        const ulonglong2 q = reinterpret_cast<const ulonglong2 *>(recs_v)[i];  // one 128-bit load
-        const uint64_t w0 = q.x;
-        const uint32_t delta = static_cast<uint32_t>(w0 >> 40);
-        const uint32_t flags = ((w0 & kPkReject) ? RAFTGPU_REC_REJECT : 0u) | ((w0 & kPkLocal) ? RAFTGPU_REC_LOCAL : 0u) |
-                               ((w0 & kPkExt) ? RAFTGPU_REC_EXT : 0u);
-        // the public layout: group | slot << 32 | flags << 40
-        r.w0 = (w0 & 0xffffffffull) | (((w0 >> 32) & 7ull) << 32) | (static_cast<uint64_t>(flags) << 40);
-        r.index = q.y;
-        if (w0 & kPkLocal)
-            r.commit = delta == kPkNoCommit ? 0 : q.y + delta;
-        else
-            r.commit = q.y - delta;
-        if ((w0 & kPkWide) && !(w0 & kPkExt)) {  // rare: the exact commit follows in an EXT of kind 3
-            for (uint64_t j = i + 1; j < n && j <= i + 3; j++) {
-                const ulonglong2 e = reinterpret_cast<const ulonglong2 *>(recs_v)[j];
-                if (!(e.x & kPkExt)) break;
-                if ((e.x >> 40) == 3) r.commit = e.y;
-            }
-        }
+        const ulonglong2 *q = reinterpret_cast<const ulonglong2 *>(recs_v);
+        r = load_packed_rec([q](uint64_t j) { return q[j]; }, i, n);
     }
     return r;
 }
@@ -95,9 +120,9 @@ __device__ __forceinline__ RecRegs load_rec(const void *recs_v, uint64_t i, uint
 template <bool kPacked>
 __device__ __forceinline__ void load_reject_ext(const void *recs_v, uint64_t i, uint64_t n, uint64_t &hint,
                                                 uint64_t &request_snapshot) {
-    hint = 0;
-    request_snapshot = RAFTGPU_INVALID_INDEX;
     if constexpr (!kPacked) {
+        hint = 0;
+        request_snapshot = RAFTGPU_INVALID_INDEX;
         if (i + 1 < n) {
             const uint64_t *e = reinterpret_cast<const uint64_t *>(static_cast<const raftgpu_append_resp *>(recs_v) + i + 1);
             if ((e[0] >> 40) & RAFTGPU_REC_EXT) {
@@ -106,13 +131,8 @@ __device__ __forceinline__ void load_reject_ext(const void *recs_v, uint64_t i, 
             }
         }
     } else {
-        for (uint64_t j = i + 1; j < n && j <= i + 3; j++) {
-            const ulonglong2 e = reinterpret_cast<const ulonglong2 *>(recs_v)[j];
-            if (!(e.x & kPkExt)) break;
-            const uint32_t kind = static_cast<uint32_t>(e.x >> 40);
-            if (kind == 1) hint = e.y;
-            if (kind == 2) request_snapshot = e.y;
-        }
+        const ulonglong2 *q = reinterpret_cast<const ulonglong2 *>(recs_v);
+        load_packed_reject_ext([q](uint64_t j) { return q[j]; }, i, n, hint, request_snapshot);
     }
 }
 

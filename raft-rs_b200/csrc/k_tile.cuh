@@ -14,7 +14,8 @@
 //     committed_index offsets / pflags / meta / committed / term_start / last_index, plus an optional
 //     payload (the compact kernel's units), into one stage;
 //   - consumer group i % kFGroups takes the CTA's tile i, so the phases of kFGroups tiles overlap:
-//     it applies the tile's records to the shared-memory rows (the kernel's own body), then
+//     it applies the tile's records to the shared-memory rows (the kernel's own body; the packed kernel's
+//     records arrive in a double buffer of the consumer group's own, outside the ring), then
 //     recomputes the commit index of the tile's groups from the same rows (matched is read from
 //     HBM once per step instead of twice);
 //   - the store warp bulk-stores the rows back (cp.async.bulk.global.shared::cta).
@@ -29,7 +30,9 @@ constexpr int kFMaxStages = 8;
 // in neighbouring lanes and touch the SAME column index of DIFFERENT rows: with a 256-element row
 // stride they would all fall on the same shared-memory banks (4-way conflicts on every access).
 // 258 u64 (= 2064 B, still 16-byte aligned for TMA) shifts consecutive rows by 4 banks.
-constexpr uint32_t kFRow64 = (kFTile + 2) * 8;   // bytes per u64 row; an offset row (next_d, pc_d) uses its first quarter
+constexpr uint32_t kFRow64 = (kFTile + 2) * 8;   // bytes per u64 row
+// bytes per 16-bit offset row (next_d, pc_d): 264 elements, 16-byte aligned too, consecutive rows 4 banks apart
+constexpr uint32_t kFRow16 = (kFTile + 8) * 2;
 constexpr uint32_t kFRow8 = kFTile + 16;         // bytes per u8 (pflags) row
 constexpr uint32_t kFDefer = 32;                 // deferred (rare-path) records per warp per tile; more are handled inline
 // dynamic shared memory of the fused kernels: 227 KB per CTA minus their static shared memory (barriers, deferred lists)
@@ -37,7 +40,7 @@ constexpr uint32_t kFSmem = 227u * 1024u - 5u * 1024u;
 
 // bytes of one stage for H hinted slots and a payload of payload_bytes (shared by host and device)
 __host__ __device__ constexpr uint32_t tile_stage_bytes(uint32_t H, uint32_t payload_bytes) {
-    return 3u * H * kFRow64 + 3u * kFRow64 + kFTile * 4u + H * kFRow8 + payload_bytes;
+    return H * kFRow64 + 2u * H * kFRow16 + 3u * kFRow64 + kFTile * 4u + H * kFRow8 + payload_bytes;
 }
 // The stage count of both fused kernels: the most stages, at most kFMaxStages, that fit in kFSmem
 // beside extra_bytes of other dynamic shared memory.
@@ -49,19 +52,27 @@ __host__ __device__ constexpr int tile_stages(uint32_t H, uint32_t payload_bytes
 // keeps one u32 run index per group of each consumer group behind the stages.
 constexpr uint32_t kCUnitCap = 1536;
 constexpr uint32_t kCRunBytes = kFGroups * kFTile * 4u;
+// The packed kernel copies up to kRecCap packed records of a tile into shared memory (the rest of a crowded tile is
+// read from HBM): two buffers per consumer group behind the stages, one for its current tile and one that its next
+// tile's records land in meanwhile.  (bench.py's cfg3 stream, 1M groups × 5 peers, has 910 ± 22 records per tile, at
+// most 991; cfg4's, 7 slots under joint consensus, 1 172 ± 32, at most 1 287: a larger cap would cost it a stage.)
+constexpr uint32_t kRecCap = 4u * kFTile;
+constexpr uint32_t kRecBytes = kFGroups * 2u * kRecCap * 16u;
 // Every hint width leaves a stage per consumer group (wait_stage relies on it) ...
-static_assert(tile_stages(kSlots, kCUnitCap * 4u, kCRunBytes) >= kFGroups, "a stage per consumer group");
+static_assert(tile_stages(kSlots, 0, kRecBytes) >= kFGroups && tile_stages(kSlots, kCUnitCap * 4u, kCRunBytes) >= kFGroups,
+              "a stage per consumer group");
 // ... and with 256-group tiles the plans for H = 1..8 hinted slots are
-static_assert(kFTile != 256 || (tile_stages(1, 0, 0) == 8 && tile_stages(2, 0, 0) == 8 && tile_stages(3, 0, 0) == 8 &&
-                                tile_stages(4, 0, 0) == 6 && tile_stages(5, 0, 0) == 5 && tile_stages(6, 0, 0) == 4 &&
-                                tile_stages(7, 0, 0) == 4 && tile_stages(8, 0, 0) == 3),
-              "packed kernel: 39 536 B per stage at H = 5");
+static_assert(kFTile != 256 || (tile_stages(1, 0, kRecBytes) == 8 && tile_stages(2, 0, kRecBytes) == 8 &&
+                                tile_stages(3, 0, kRecBytes) == 7 && tile_stages(4, 0, kRecBytes) == 6 &&
+                                tile_stages(5, 0, kRecBytes) == 5 && tile_stages(6, 0, kRecBytes) == 4 &&
+                                tile_stages(7, 0, kRecBytes) == 4 && tile_stages(8, 0, kRecBytes) == 3),
+              "packed kernel: 24 176 B per stage at H = 5, beside 96 KB of record buffers");
 static_assert(kFTile != 256 || (tile_stages(1, kCUnitCap * 4u, kCRunBytes) == 8 && tile_stages(2, kCUnitCap * 4u, kCRunBytes) == 8 &&
-                                tile_stages(3, kCUnitCap * 4u, kCRunBytes) == 6 && tile_stages(4, kCUnitCap * 4u, kCRunBytes) == 5 &&
-                                tile_stages(5, kCUnitCap * 4u, kCRunBytes) == 4 && tile_stages(6, kCUnitCap * 4u, kCRunBytes) == 4 &&
-                                tile_stages(7, kCUnitCap * 4u, kCRunBytes) == 3 && tile_stages(8, kCUnitCap * 4u, kCRunBytes) == 3),
-              "compact kernel: 45 680 B per stage at H = 5");
-static_assert(kFTile != 256 || (tile_stage_bytes(5, 0) == 39536 && tile_stage_bytes(5, kCUnitCap * 4u) == 45680), "stage sizes");
+                                tile_stages(3, kCUnitCap * 4u, kCRunBytes) == 8 && tile_stages(4, kCUnitCap * 4u, kCRunBytes) == 8 &&
+                                tile_stages(5, kCUnitCap * 4u, kCRunBytes) == 7 && tile_stages(6, kCUnitCap * 4u, kCRunBytes) == 6 &&
+                                tile_stages(7, kCUnitCap * 4u, kCRunBytes) == 6 && tile_stages(8, kCUnitCap * 4u, kCRunBytes) == 5),
+              "compact kernel: 30 320 B per stage at H = 5");
+static_assert(kFTile != 256 || (tile_stage_bytes(5, 0) == 24176 && tile_stage_bytes(5, kCUnitCap * 4u) == 30320), "stage sizes");
 
 // ---- 1-D TMA and mbarrier primitives
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
@@ -140,13 +151,14 @@ struct TileBarriers {
     uint64_t full[kFMaxStages];   // loads landed            (load warp -> consumers)
     uint64_t done[kFMaxStages];   // rows final in smem      (consumers -> store warp)
     uint64_t empty[kFMaxStages];  // rows read by the stores (store warp -> load warp)
+    uint64_t recs[kFGroups][2];   // packed kernel: a consumer group's record buffer filled (its thread 0 -> the group)
     uint32_t clk[kFGroups];       // RAFTGPU_TILE_DEBUG: per consumer group, the end of its wait for the stage
 };
 
 // One stage's rows in shared memory.  Row r of a per-peer column is the r-th hinted slot.
 struct TileRows {
     uint64_t *matched;
-    int16_t *next, *pc;  // the offsets next_d / pc_d, rows kFRow64 bytes apart
+    int16_t *next, *pc;  // the offsets next_d / pc_d, rows kFRow16 bytes apart
     uint64_t *committed, *ts, *li;
     uint32_t *meta;
     uint8_t *flags;
@@ -154,7 +166,7 @@ struct TileRows {
 };
 // matched and the offsets of the cell staged in row r for group gl (arena cell `cell`)
 __device__ __forceinline__ HotPtrs staged_hot(const TileRows &t, uint32_t r, uint32_t gl, size_t cell) {
-    return HotPtrs{&t.matched[r * (kFRow64 / 8) + gl], &t.next[r * (kFRow64 / 2) + gl], &t.pc[r * (kFRow64 / 2) + gl], cell};
+    return HotPtrs{&t.matched[r * (kFRow64 / 8) + gl], &t.next[r * (kFRow16 / 2) + gl], &t.pc[r * (kFRow16 / 2) + gl], cell};
 }
 
 // Where a consumer group is in its walk over the CTA's tiles.
@@ -186,6 +198,10 @@ struct TileRing {
                 mbar_init(&bar->done[s], 1);
                 mbar_init(&bar->empty[s], 1);
             }
+            for (int g = 0; g < kFGroups; g++) {
+                mbar_init(&bar->recs[g][0], 1);
+                mbar_init(&bar->recs[g][1], 1);
+            }
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
         __syncthreads();
@@ -209,8 +225,8 @@ struct TileRing {
         TileRows t;
         t.matched = reinterpret_cast<uint64_t *>(sb);
         t.next = reinterpret_cast<int16_t *>(sb + H * kFRow64);
-        t.pc = reinterpret_cast<int16_t *>(sb + 2u * H * kFRow64);
-        t.committed = reinterpret_cast<uint64_t *>(sb + 3u * H * kFRow64);
+        t.pc = reinterpret_cast<int16_t *>(sb + H * (kFRow64 + kFRow16));
+        t.committed = reinterpret_cast<uint64_t *>(sb + H * (kFRow64 + 2u * kFRow16));
         t.ts = t.committed + kFRow64 / 8;
         t.li = t.ts + kFRow64 / 8;
         t.meta = reinterpret_cast<uint32_t *>(t.li + kFRow64 / 8);
@@ -263,8 +279,8 @@ struct TileRing {
                     const uint32_t col = j / H, r = j % H;  // col: 0 matched, 1 next_d, 2 pc_d, 3 pflags
                     const size_t cell = static_cast<size_t>(hinted_slot(r)) * c.cap + g0;
                     if (col == 0) tma_load_1d(t.matched + r * (kFRow64 / 8), c.matched + cell, ng16 * 8u, &bar->full[st]);
-                    if (col == 1) tma_load_1d(t.next + r * (kFRow64 / 2), c.next_d + cell, ng16 * 2u, &bar->full[st]);
-                    if (col == 2) tma_load_1d(t.pc + r * (kFRow64 / 2), c.pc_d + cell, ng16 * 2u, &bar->full[st]);
+                    if (col == 1) tma_load_1d(t.next + r * (kFRow16 / 2), c.next_d + cell, ng16 * 2u, &bar->full[st]);
+                    if (col == 2) tma_load_1d(t.pc + r * (kFRow16 / 2), c.pc_d + cell, ng16 * 2u, &bar->full[st]);
                     if (col == 3) tma_load_1d(t.flags + r * kFRow8, c.pflags + cell, ng16, &bar->full[st]);
                 } else if (j == 4u * H) {
                     tma_load_1d(t.committed, c.committed + g0, ng16 * 8u, &bar->full[st]);
@@ -298,8 +314,8 @@ struct TileRing {
                     const uint32_t col = j / H, r = j % H;
                     const size_t cell = static_cast<size_t>(hinted_slot(r)) * c.cap + g0;
                     if (col == 0) tma_store_1d(c.matched + cell, t.matched + r * (kFRow64 / 8), ng16 * 8u);
-                    if (col == 1) tma_store_1d(c.next_d + cell, t.next + r * (kFRow64 / 2), ng16 * 2u);
-                    if (col == 2) tma_store_1d(c.pc_d + cell, t.pc + r * (kFRow64 / 2), ng16 * 2u);
+                    if (col == 1) tma_store_1d(c.next_d + cell, t.next + r * (kFRow16 / 2), ng16 * 2u);
+                    if (col == 2) tma_store_1d(c.pc_d + cell, t.pc + r * (kFRow16 / 2), ng16 * 2u);
                     if (col == 3) tma_store_1d(c.pflags + cell, t.flags + r * kFRow8, ng16);
                 } else if (j == 4u * H) {
                     tma_store_1d(c.committed + g0, t.committed, ng16 * 8u);
@@ -471,7 +487,7 @@ __device__ __forceinline__ bool tile_fast_apply(const Columns &c, const TileRows
                                                 uint64_t index, uint64_t commit, bool is_local, bool is_reject,
                                                 uint64_t ext_hint, uint32_t hint, uint32_t present_mask, uint32_t *local,
                                                 uint32_t &res) {
-    constexpr uint32_t R64 = kFRow64 / 8, R16 = kFRow64 / 2;
+    constexpr uint32_t R64 = kFRow64 / 8, R16 = kFRow16 / 2;
     if (!((hint >> slot) & 1u)) return false;
     const uint32_t r = kSimple5 ? slot : static_cast<uint32_t>(__popc(hint & ((1u << slot) - 1u)));
     const uint32_t ci = r * R64 + gl, di = r * R16 + gl;
@@ -542,8 +558,11 @@ __device__ __forceinline__ uint32_t present_of(uint32_t meta) {
 
 // ---------------------------------------------------------------------------
 // step_tile_kernel: the fused step on packed records in group order (tile_off from raftgpu_tile_index).
-// The records are read straight from HBM / L2, not staged: the stage holds rows only, which buys a fifth
-// stage; the records of a tile are prefetched into L2 while the previous tile is processed.
+// The records do not travel through the ring.  Each consumer group owns two record buffers behind the stages: while it
+// works on one tile, its thread 0 bulk-copies (cp.async.bulk) the first kRecCap records of the group's next tile into
+// the other buffer, on that buffer's own mbarrier.  The apply loop then reads its records from shared memory instead
+// of waiting on L2 behind the ring's traffic; the records of a crowded tile past the cap are read from HBM (and
+// prefetched into L2 during the previous tile).
 struct TileArgs {
     TileRingArgs r;
     const PackedRec *recs;  // packed records in group order
@@ -567,19 +586,34 @@ __global__ void __launch_bounds__(kFThreads, 1) step_tile_kernel(Columns c, Tile
     } else if (warp == kFGroups * kFTile / 32) {
         ring.load_warp(c, nullptr);
     } else {
+        const uint32_t cg = warp / (kFTile / 32);
         const uint32_t tid = threadIdx.x % kFTile;
-        for (TileCursor t = ring.first(warp / (kFTile / 32)); t.tile < ring.n_tiles; ring.next(t)) {
+        // buffer b of this consumer group (its address is recomputed where used: a register live across the loop spills)
+        auto rbuf = [&](uint32_t b) { return reinterpret_cast<ulonglong2 *>(ring.extra()) + (cg * 2u + b) * kRecCap; };
+        // (thread 0 of the group) the first kRecCap records of [r0, r1) into buffer b.  Its previous contents were read
+        // in the records phase of the group's tile before last, which ended in the group's barrier, and generic reads
+        // are followed by an async-proxy write: fence.  A record-less tile arrives with 0 bytes, so the wait passes.
+        auto fill = [&](uint32_t b, uint32_t r0, uint32_t r1) {
+            const uint32_t n = r1 > r0 ? min(r1 - r0, kRecCap) : 0u;
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            mbar_expect_tx(&bars.recs[cg][b], n * 16u);
+            if (n) tma_load_1d(rbuf(b), a.recs + r0, n * 16u, &bars.recs[cg][b]);
+        };
+        TileCursor t = ring.first(cg);
+        if (tid == 0 && t.tile < ring.n_tiles) fill(0, t.u0, t.u1);
+        for (; t.tile < ring.n_tiles; ring.next(t)) {
             const uint32_t g0 = t.tile * kFTile;
             const uint32_t ng = ring.groups_of(g0);
             const uint32_t rbeg = t.u0, cnt = t.u1 - t.u0;
-            const ulonglong2 *g_recs = reinterpret_cast<const ulonglong2 *>(a.recs + rbeg);
-            auto rec_at = [&](uint32_t j) -> ulonglong2 { return j < cnt ? g_recs[j] : make_ulonglong2(kPkExt, 0ull); };
-            // this thread's first record is requested BEFORE the wait for the stage (its address does not depend
-            // on it); the loop then fetches one record ahead.  (Two ahead was slower with scripts/micro_tile.py:
-            // the kernel sits near its register ceiling and the consumers are bound by issue latency, not by the
-            // record reads.)
-            ulonglong2 q_next = rec_at(tid);
+            // the group's i-th tile reads buffer i & 1, whose barrier completes one phase per use
+            const uint32_t i = t.it / kFGroups;
+            if (tid == 0 && t.tile + ring.tile_step() < ring.n_tiles) fill((i + 1u) & 1u, t.nx0, t.nx1);
             const TileRows s = ring.wait(t);
+            mbar_wait(&bars.recs[cg][i & 1u], (i >> 1) & 1u);
+            const ulonglong2 *s_recs = rbuf(i & 1u);
+            const ulonglong2 *g_recs = reinterpret_cast<const ulonglong2 *>(a.recs + rbeg);
+            // every read of the tile's record j < cnt: the shared-memory copy, or HBM past the cap
+            auto rec_at = [&](uint32_t j) -> ulonglong2 { return j < kRecCap ? s_recs[j] : g_recs[j]; };
 
             // ---- the tile's records against the shared-memory rows (raft.rs:1663-1743)
             // The main loop handles the records that make up ~98 % of the traffic -- an accept or a leader-local
@@ -592,8 +626,8 @@ __global__ void __launch_bounds__(kFThreads, 1) step_tile_kernel(Columns c, Tile
             if (lane == 0) s_ndefer[warp] = 0;
             __syncwarp();
             auto slow_record = [&](const uint32_t k) {
-                const RecRegs rec = load_rec<true>(g_recs, k, cnt);
-                const uint64_t w0 = g_recs[k].x;
+                const RecRegs rec = load_packed_rec(rec_at, k, cnt);
+                const uint64_t w0 = rec_at(k).x;
                 const uint32_t gl = static_cast<uint32_t>(rec.w0) - g0;
                 uint32_t res = 0;
                 if (gl >= ng) {  // not this tile's group: the batch is not in group order / bad index
@@ -604,7 +638,7 @@ __global__ void __launch_bounds__(kFThreads, 1) step_tile_kernel(Columns c, Tile
                     // (the loop above has taken every accept and leader-local record the fast path can take)
                     uint64_t ext_hint = 0, ext_snapshot = RAFTGPU_INVALID_INDEX;
                     const bool is_reject = (w0 & kPkReject) != 0;
-                    if (is_reject) load_reject_ext<true>(g_recs, k, cnt, ext_hint, ext_snapshot);
+                    if (is_reject) load_packed_reject_ext(rec_at, k, cnt, ext_hint, ext_snapshot);
                     const bool fast = is_reject && !(w0 & kPkWide) && ext_snapshot == RAFTGPU_INVALID_INDEX &&
                                       tile_fast_apply<kSimple5>(c, s, gl, g0 + gl, static_cast<uint32_t>(rec.w0 >> 32) & 7u,
                                                                 rec.index, rec.index - (w0 >> 40), false, true, ext_hint, hint,
@@ -614,8 +648,7 @@ __global__ void __launch_bounds__(kFThreads, 1) step_tile_kernel(Columns c, Tile
                 if (a.r.results) a.r.results[rbeg + k] = static_cast<uint8_t>(res);
             };
             for (uint32_t k = tid; k < cnt; k += kFTile) {
-                const ulonglong2 q = q_next;
-                q_next = rec_at(k + kFTile);
+                const ulonglong2 q = rec_at(k);
                 const uint64_t w0 = q.x;
                 if (w0 & kPkExt) {
                     if (a.r.results) a.r.results[rbeg + k] = 0;
@@ -644,12 +677,13 @@ __global__ void __launch_bounds__(kFThreads, 1) step_tile_kernel(Columns c, Tile
                 const uint32_t nd = s_ndefer[warp] < kFDefer ? s_ndefer[warp] : kFDefer;
                 for (uint32_t j = lane; j < nd; j += 32) slow_record(my_defer[j]);
             }
-            named_bar_sync(1 + static_cast<int>(warp / (kFTile / 32)), kFTile);  // the group's cells are final
+            // the group's cells are final, and its record buffer is read: thread 0 may fill it again
+            named_bar_sync(1 + static_cast<int>(cg), kFTile);
 
             ring.finish(c, t, s, local);
-            if (t.tile + ring.tile_step() < ring.n_tiles) {  // next tile's records -> L2 (one line = 8 records)
+            if (t.tile + ring.tile_step() < ring.n_tiles) {  // next tile's records past the cap -> L2 (one line = 8 records)
                 const uint32_t nn = t.nx1 - t.nx0;
-                for (uint32_t k = tid * 8u; k < nn; k += kFTile * 8u) prefetch_l2(a.recs + t.nx0 + k);
+                for (uint32_t k = kRecCap + tid * 8u; k < nn; k += kFTile * 8u) prefetch_l2(a.recs + t.nx0 + k);
             }
         }
     }
