@@ -214,6 +214,17 @@ struct HostPool {
     }
 };
 
+// The device scratch of one wire pass: `first`, its first-frame table (allocated on first use and refilled with 0xff by
+// every run: no frame yet), and `buf`, a buffer grown on demand (`cap` u64 words) that the pass carves where it runs
+// (its abi_*.inc); pass_scratch prepares both.  Never shared between passes (DESIGN 3.10): a wire step may be in flight
+// on s_compute while another pass runs on the caller's stream.
+struct PassScratch {
+    uint32_t *first = nullptr;
+    uint64_t *buf = nullptr;
+    uint64_t cap = 0;
+};
+enum Pass { kPassWireStep, kPassHbWire, kPassHbFrames, kPassHbFollow, kPassVoteWire, kPassVoteRequest, kPassCount };
+
 }  // namespace
 
 struct raftgpu_arena {
@@ -231,7 +242,6 @@ struct raftgpu_arena {
     uint32_t n_simple5 = 0;                  // groups whose meta is the plain 5-voter configuration
     bool force_general = false;              // RAFTGPU_FORCE_GENERAL=1: never take the simple5 kernels
     Columns cols{};
-    uint32_t *d_wire_first = nullptr;  // [kSlots][cap] wire steps: first frame of every cell (allocated on first use)
     unsigned long long *d_counters = nullptr;
     void *d_scratch = nullptr;  // kScratchBytes for the small results of single calls (scratch<T>)
     void *h_scratch = nullptr;  // pinned mirror
@@ -251,28 +261,7 @@ struct raftgpu_arena {
     // rq_flag[1] = the touched list's length
     unsigned long long *rq_hit = nullptr;
     uint32_t *rq_list = nullptr, *rq_flag = nullptr;
-    // raftgpu_heartbeat_wire (allocated on first use): first frame of every cell [kSlots][cap], one record per frame
-    uint32_t *hbw_first = nullptr;
-    raftgpu_append_resp *hbw_recs = nullptr;
-    uint64_t hbw_recs_cap = 0;
-    // raftgpu_heartbeat_frames (grown on demand): {frames, bytes} per group slot, the block sums, the fit flag
-    uint32_t *hbf_scratch = nullptr;
-    uint64_t hbf_scratch_cap = 0;
-    // raftgpu_follower_heartbeat: first passing frame of every group slot [cap] (allocated on first use); grown on
-    // demand, in u64 words: one record per frame, the block sums, the fit flag
-    uint32_t *hfw_first = nullptr;
-    uint64_t *hfw_scratch = nullptr;
-    uint64_t hfw_scratch_cap = 0;
-    // raftgpu_vote_wire: first passing frame of every cell [kSlots][cap] (allocated on first use); grown on demand, in
-    // u64 words: one record per frame, the touched bitmap, the tally words [cap], the block sums
-    uint32_t *vw_first = nullptr;
-    uint64_t *vw_scratch = nullptr;
-    uint64_t vw_scratch_cap = 0;
-    // raftgpu_vote_request_wire: first frame of every group slot that reached the term rules [cap] (allocated on first
-    // use); grown on demand, in u64 words: one record per frame, the block sums, the fit flag
-    uint32_t *vrq_first = nullptr;
-    uint64_t *vrq_scratch = nullptr;
-    uint64_t vrq_scratch_cap = 0;
+    PassScratch pass[kPassCount];  // the wire passes' scratch, one each
     // group allocation
     std::mutex alloc_mu;
     std::vector<uint32_t> free_list;
@@ -561,8 +550,7 @@ int32_t grow_wire(raftgpu_arena *a, StagingSet &s, uint64_t need) {
     return grow_scratch(a, a->s_compute, &s.d_wire, &s.d_wire_cap, need);
 }
 
-// A wire pass's first-frame table (`n` u32, allocated on first use) filled with 0xff on st: no frame yet.  Every pass
-// keeps its own table (DESIGN 3.10).
+// A wire pass's first-frame table (`n` u32, allocated on first use) filled with 0xff on st: no frame yet.
 int32_t reset_first_frames(raftgpu_arena *a, cudaStream_t st, uint32_t **table, size_t n) {
     if (!*table) {
         const int32_t rc = dev_alloc(a, table, n, false);
@@ -570,6 +558,16 @@ int32_t reset_first_frames(raftgpu_arena *a, cudaStream_t st, uint32_t **table, 
     }
     CK(a, cudaMemsetAsync(*table, 0xff, n * sizeof(uint32_t), st));
     return RAFTGPU_OK;
+}
+
+// What a wire pass does before its first launch on st: its first-frame table of first_n u32 reset (0: the pass keeps
+// none), its buffer holding at least `words` u64.
+int32_t pass_scratch(raftgpu_arena *a, cudaStream_t st, PassScratch &p, size_t first_n, uint64_t words) {
+    if (first_n) {
+        const int32_t rc = reset_first_frames(a, st, &p.first, first_n);
+        if (rc != RAFTGPU_OK) return rc;
+    }
+    return grow_scratch(a, st, &p.buf, &p.cap, words);
 }
 
 // The limits of every wire batch: frame offsets and counts are u32 on the device, and the staging kernels read the
@@ -640,16 +638,10 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->rq_hit);
     cudaFree(a->rq_list);
     cudaFree(a->rq_flag);
-    cudaFree(a->d_wire_first);
-    cudaFree(a->hbw_first);
-    cudaFree(a->hbw_recs);
-    cudaFree(a->hbf_scratch);
-    cudaFree(a->hfw_first);
-    cudaFree(a->hfw_scratch);
-    cudaFree(a->vw_first);
-    cudaFree(a->vw_scratch);
-    cudaFree(a->vrq_first);
-    cudaFree(a->vrq_scratch);
+    for (PassScratch &p : a->pass) {
+        cudaFree(p.first);
+        cudaFree(p.buf);
+    }
     cudaFree(a->d_counters);
     cudaFree(a->d_scratch);
     cudaFreeHost(a->h_scratch);
@@ -1030,6 +1022,104 @@ class HostFrame {
     uint64_t rest_bytes_ = UINT64_MAX;  // the rest region's size once enlarged (until then: to the end of d_wire)
     bool queued_ = false;               // copies or a pass queued since the last wait
 };
+
+// ---- the reply pipeline (DESIGN 3.12): a pass that answers every frame it applies with a frame of its own
+// (raftgpu_follower_heartbeat, raftgpu_vote_request_wire) keeps its decision -- a scan and an apply kernel -- and
+// shares the rest: reply_check, reply_run<P> for the `_device` form, reply_host for the host form.  P is the pass's
+// reply policy (reply_write_kernel, k_wire.cuh).
+
+// The refusals both forms make before any copy or launch; bound_name: the pass's public bound function, n * frame_max.
+int32_t reply_check(raftgpu_arena *a, uint64_t n_bytes, uint64_t n, uint64_t frame_max, uint64_t resp_bytes_capacity,
+                    const char *bound_name) {
+    const int32_t rc = wire_batch_check(a, n_bytes, n, nullptr);  // (the device form checks the alignment after)
+    if (rc != RAFTGPU_OK) return rc;
+    if (n * frame_max > 0xffffffffull)
+        return fail(a, RAFTGPU_ERR_INVALID, "the responses of this batch may not be addressable by u32 offsets");
+    // the pass changes the groups it answers for: a response that did not fit could not be produced again
+    if (resp_bytes_capacity < n * frame_max)
+        return fail(a, RAFTGPU_ERR_INVALID, std::string("response capacity below ") + bound_name + "(n)");
+    return RAFTGPU_OK;
+}
+
+// The `_device` form after its checks, on st: no frame gives zero totals and resp_offsets[0] = 0.  Otherwise the
+// pass's scratch (u64 words) is carved into one record per frame, the {responses, bytes} of every block and the fit
+// flag, its first-frame table (first_n u32) reset, and four passes run with kWireThreads frames per block:
+// passes(blocks, recs, first, blk) launches the pass's scan and apply kernels, hbf_scan_kernel<2> turns the block sums
+// into block starts, the totals and the last offset, reply_write_kernel<P> writes the responses.
+template <class P, typename Passes>
+int32_t reply_run(raftgpu_arena *a, cudaStream_t st, PassScratch &scratch, uint64_t n, const uint8_t *d_status,
+                  uint8_t *d_resp_bytes, uint64_t resp_bytes_capacity, uint32_t *d_resp_offsets, uint64_t *d_totals,
+                  size_t first_n, Passes &&passes) {
+    using Rec = typename P::Rec;
+    if (n == 0) {
+        CK(a, cudaMemsetAsync(d_totals, 0, 16, st));
+        CK(a, cudaMemsetAsync(d_resp_offsets, 0, 4, st));
+        return RAFTGPU_OK;
+    }
+    const uint32_t nb = div_up(n, kWireThreads);
+    const int32_t rc = pass_scratch(a, st, scratch, first_n, (sizeof(Rec) / 8) * n + nb + 1);
+    if (rc != RAFTGPU_OK) return rc;
+    Rec *recs = reinterpret_cast<Rec *>(scratch.buf);
+    uint32_t *blk = reinterpret_cast<uint32_t *>(scratch.buf + (sizeof(Rec) / 8) * n), *flag = blk + 2ull * nb;
+    passes(nb, recs, scratch.first, blk);
+    // (the capacities always hold: resp_bytes_capacity >= P::kFrameMax * n was checked, d_resp_offsets has n + 1 values)
+    hbf_scan_kernel<2><<<1, kHbfScanThreads, 0, st>>>(blk, nb, resp_bytes_capacity, n, d_totals, d_resp_offsets, flag);
+    reply_write_kernel<P><<<nb, kWireThreads, 0, st>>>(static_cast<uint32_t>(n), d_status, recs, blk, d_resp_bytes, d_resp_offsets);
+    CKL(a);
+    return RAFTGPU_OK;
+}
+
+// What reply_host hands the `_device` form: the staged batch and tables, the outputs' places in d_wire, the totals' in
+// the arena's scratch.
+struct ReplyStaged {
+    const uint8_t *bytes;
+    const uint32_t *offsets;
+    const void *table[2];
+    uint8_t *status;
+    uint64_t *out;  // nullptr when the caller passed none
+    uint8_t *resp_bytes;
+    uint32_t *resp_offsets;
+    uint64_t *totals;
+};
+struct ReplyTable {
+    const void *src;
+    uint64_t bytes;
+};
+
+// The host form after its checks (HostFrame): d_wire holds [bytes | offsets | the pass's tables | status | out, out_width
+// bytes per frame | response offsets | response bytes, `bound`], the totals go to the arena's scratch.  The totals,
+// status and out come back, then the responses the totals give.
+template <typename Device>
+int32_t reply_host(raftgpu_arena *a, const void *bytes, uint64_t n_bytes, const uint32_t *offsets, uint64_t n,
+                   const ReplyTable (&tables)[2], uint8_t *status, uint64_t *out, uint64_t out_width, uint64_t bound,
+                   uint8_t *resp_bytes, uint32_t *resp_offsets, uint64_t *totals, Device &&device) {
+    totals[0] = totals[1] = 0;
+    resp_offsets[0] = 0;
+    if (n == 0) return RAFTGPU_OK;
+    HostFrame f(a);
+    int32_t rc = f.open();
+    if (rc != RAFTGPU_OK) return rc;
+    const WireRegion bytes_at = f.in(bytes, n_bytes), off_at = f.in(offsets, 4 * (n + 1));
+    const WireRegion table_at[2] = {f.in(tables[0].src, tables[0].bytes), f.in(tables[1].src, tables[1].bytes)};
+    const WireRegion status_at = f.out(n), out_at = f.out(out_width * n), roff_at = f.out(4 * (n + 1)), rbytes_at = f.out(bound);
+    uint64_t *d_totals = scratch<uint64_t, 2>(a->d_scratch), *h_totals = scratch<uint64_t, 2>(a->h_scratch);
+    rc = f.run([&](const Staged &d) {
+        return device(ReplyStaged{d.at<const uint8_t>(bytes_at), d.at<const uint32_t>(off_at),
+                                  {d.at<const void>(table_at[0]), d.at<const void>(table_at[1])}, d.at<uint8_t>(status_at),
+                                  out ? d.at<uint64_t>(out_at) : nullptr, d.at<uint8_t>(rbytes_at), d.at<uint32_t>(roff_at),
+                                  d_totals});
+    });
+    if (rc == RAFTGPU_OK) rc = f.back(h_totals, d_totals, 16);
+    if (rc == RAFTGPU_OK) rc = f.back(status, status_at, n);
+    if (rc == RAFTGPU_OK) rc = f.back(out, out_at, out_width * n);
+    if (rc == RAFTGPU_OK) rc = f.wait();
+    if (rc != RAFTGPU_OK) return rc;
+    totals[0] = h_totals[0];
+    totals[1] = h_totals[1];
+    rc = f.back(resp_offsets, roff_at, 4 * (totals[0] + 1));
+    if (rc == RAFTGPU_OK) rc = f.back(resp_bytes, rbytes_at, totals[1]);
+    return rc == RAFTGPU_OK ? f.wait() : rc;
+}
 
 // ---- the step frame: every raftgpu_step_begin* form is step_admit -> the form's own function, which queues its H2D
 // copies on s_h2d and its apply kernels on s_compute and says what it queued (StepWork) -> step_finish -> step_book.

@@ -10,9 +10,8 @@
 // Four kernels and no waiting between blocks: hfw_scan_kernel stages and decodes every frame once, classifies it and
 // writes a 48-byte record per passing frame; hfw_apply_kernel marks the later frames of a group DUP, runs commit_to
 // on the first one and sums the responses per block; hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block
-// starts; hfw_write_kernel encodes the responses (wire_put_hb_frame<9>) and stores them through shared memory.
-
-constexpr uint32_t kHfwThreads = kWireThreads;  // frames per block of every kernel here: one block sum per scan block
+// starts; reply_write_kernel<HfwReply> (k_wire.cuh) encodes the responses (wire_put_hb_frame<9>) and stores them
+// through shared memory.  Every kernel takes kWireThreads frames per block: one block sum per scan block.
 
 // The caller's tables: select = bitmap from group 0 (required), self_ids = u64 [group slots].
 struct HfwSrc {
@@ -60,7 +59,7 @@ __device__ __forceinline__ uint32_t hfw_frame(const Columns &c, const WireSrc &w
 }
 
 // Pass 1: classify every frame; status[i] = wire status << 4; a passing frame's record, first_frame[group] = the
-// lowest passing frame of the group.  Launched with kHfwThreads threads per block; __maxnreg__ as hb_wire_scan_kernel,
+// lowest passing frame of the group.  Launched with kWireThreads threads per block; __maxnreg__ as hb_wire_scan_kernel,
 // because ptxas, left alone, settles on 32 registers and spills.
 __global__ void __maxnreg__(40) hfw_scan_kernel(Columns c, WireSrc w, HfwSrc f, uint8_t *__restrict__ status,
                                                                HfwRec *__restrict__ recs, uint32_t *__restrict__ first_frame) {
@@ -83,10 +82,10 @@ __global__ void __maxnreg__(40) hfw_scan_kernel(Columns c, WireSrc w, HfwSrc f, 
 // block's responses and their bytes.  Algorithmic bytes per frame: 1 read + 1 written (+ 8 from_out); per passing
 // frame 48 (record) + 4 (first_frame) read; per applied one 16-32 (committed, last_index) read, 8-16 (committed) + 8
 // (record) written.
-__global__ void __launch_bounds__(kHfwThreads) hfw_apply_kernel(Columns c, uint32_t n, uint8_t *__restrict__ status,
-                                                                HfwRec *__restrict__ recs, const uint32_t *__restrict__ first_frame,
-                                                                uint64_t *__restrict__ from_out, uint32_t *__restrict__ blk) {
-    const uint32_t i = blockIdx.x * kHfwThreads + threadIdx.x;
+__global__ void __launch_bounds__(kWireThreads) hfw_apply_kernel(Columns c, uint32_t n, uint8_t *__restrict__ status,
+                                                                 HfwRec *__restrict__ recs, const uint32_t *__restrict__ first_frame,
+                                                                 uint64_t *__restrict__ from_out, uint32_t *__restrict__ blk) {
+    const uint32_t i = blockIdx.x * kWireThreads + threadIdx.x;
     uint32_t resp = 0, bytes = 0;
     if (i < n) {
         uint64_t from = 0;
@@ -111,31 +110,16 @@ __global__ void __launch_bounds__(kHfwThreads) hfw_apply_kernel(Columns c, uint3
         }
         if (from_out) from_out[i] = from;
     }
-    block_sums<2, kHfwThreads>({resp, bytes}, blk);
+    block_sums<2, kWireThreads>({resp, bytes}, blk);
 }
 
-// Pass 4 (after hbf_scan_kernel<2>, k_wire.cuh, turned blk into block starts): every block encodes its responses, in frame order,
-// into shared memory at their offset from the 16-byte boundary below the block's start and stores them with
-// wire_store_block; offsets [blk start, + its responses).  Reads 1 per frame + 48 per response; writes the responses
-// and 4 per response.
-__global__ void __launch_bounds__(kHfwThreads) hfw_write_kernel(uint32_t n, const uint8_t *__restrict__ status,
-                                                                const HfwRec *__restrict__ recs, const uint32_t *__restrict__ blk,
-                                                                uint8_t *__restrict__ out, uint32_t *__restrict__ offsets) {
-    __shared__ __align__(16) uint8_t buf[kHfwThreads * kWireHbFrameMax + 16];
-    __shared__ uint32_t offs[kHfwThreads];
-    const uint32_t i = blockIdx.x * kHfwThreads + threadIdx.x;
-    const bool has = i < n && (status[i] & RAFTGPU_RES_OK);
-    HfwRec r{};
-    if (has) r = recs[i];
-    uint32_t lf = has, lb = has ? hfw_len(r) : 0u, nf, nbytes;
-    wire_block_scan<kHfwThreads / 32>(lf, lb, nf, nbytes);
-    const uint32_t f0 = blk[2 * blockIdx.x], b0 = blk[2 * blockIdx.x + 1], pad = b0 & 15u;
-    if (has) {
-        offs[lf] = b0 + lb;
-        wire_put_hb_frame<9>(buf + pad + lb, static_cast<uint32_t>(r.w0), r.to, r.from, r.term, r.commit, (r.w0 >> 32) & 1u,
-                        r.ctx);  // MsgHeartbeatResponse, raft.rs:2458-2463
+// Pass 4 is reply_write_kernel<HfwReply> (k_wire.cuh): the frames the apply pass marked RAFTGPU_RES_OK answer.
+struct HfwReply {
+    using Rec = HfwRec;
+    static constexpr uint32_t kFrameMax = kWireHbFrameMax;
+    __device__ __forceinline__ static bool answers(uint8_t status) { return status & RAFTGPU_RES_OK; }
+    __device__ __forceinline__ static uint32_t len(const HfwRec &r) { return hfw_len(r); }
+    __device__ __forceinline__ static uint8_t *put(uint8_t *p, const HfwRec &r) {  // MsgHeartbeatResponse, raft.rs:2458-2463
+        return wire_put_hb_frame<9>(p, static_cast<uint32_t>(r.w0), r.to, r.from, r.term, r.commit, (r.w0 >> 32) & 1u, r.ctx);
     }
-    __syncthreads();
-    for (uint32_t j = threadIdx.x; j < nf; j += kHfwThreads) offsets[f0 + j] = offs[j];
-    wire_store_block<kHfwThreads>(out, buf, b0, nbytes);
-}
+};

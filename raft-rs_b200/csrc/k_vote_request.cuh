@@ -10,10 +10,9 @@
 // Four kernels and no waiting between blocks: vrq_scan_kernel stages and decodes every frame once, classifies and
 // decides it and writes a 48-byte record per frame that reached the term rules; vrq_apply_kernel marks the later frames
 // of a group DUP, raises the term and resets the group where the first one bumps it, and sums the responses per block;
-// hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block starts; vrq_write_kernel encodes the responses
-// (wire_put_vote_frame) and stores them through shared memory.
-
-constexpr uint32_t kVrqThreads = kWireThreads;  // frames per block of every kernel here: one block sum per scan block
+// hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block starts; reply_write_kernel<VrqReply> (k_wire.cuh) encodes
+// the responses (wire_put_vote_frame) and stores them through shared memory.  Every kernel takes kWireThreads frames per
+// block: one block sum per scan block.
 
 // A decided frame's record: w0 = its header | the kVrq* bits; the response's to (= m.from), from (the table's id),
 // term, commit and commit_term.  A bumped frame's new term is its response's term (m.term: a bump is only decided at
@@ -95,10 +94,10 @@ __device__ __forceinline__ uint32_t vrq_frame(const Columns &c, const WireSrc &w
 }
 
 // Pass 1: classify every frame; status[i] = wire status << 4; the record of a frame that reached the term rules,
-// first_frame[group] = the lowest such frame of the group.  Launched with kVrqThreads threads per block.
-__global__ void __launch_bounds__(kVrqThreads) vrq_scan_kernel(Columns c, WireSrc w, const raftgpu_voter *__restrict__ voters,
-                                                               uint8_t *__restrict__ status, VrqRec *__restrict__ recs,
-                                                               uint32_t *__restrict__ first_frame) {
+// first_frame[group] = the lowest such frame of the group.  Launched with kWireThreads threads per block.
+__global__ void __launch_bounds__(kWireThreads) vrq_scan_kernel(Columns c, WireSrc w, const raftgpu_voter *__restrict__ voters,
+                                                                uint8_t *__restrict__ status, VrqRec *__restrict__ recs,
+                                                                uint32_t *__restrict__ first_frame) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
     WireStage s;
     const uint32_t i = wire_block_frame(w, stage, s);
@@ -118,11 +117,11 @@ __global__ void __launch_bounds__(kVrqThreads) vrq_scan_kernel(Columns c, WireSr
 // term after} of an applied frame, 0 otherwise.  blk[2 * block + {0, 1}] = the block's responses and their bytes.
 // Algorithmic bytes per frame: 1 read + 1 written (+ 16 out); per frame that reached the term rules 8 (w0) + 4
 // (first_frame) read; per applied one 40 (record) + 8 (term) read, and a bump's reset of its group.
-__global__ void __launch_bounds__(kVrqThreads) vrq_apply_kernel(Columns c, uint32_t n, const raftgpu_voter *__restrict__ voters,
-                                                                uint8_t *__restrict__ status, const VrqRec *__restrict__ recs,
-                                                                const uint32_t *__restrict__ first_frame,
-                                                                uint64_t *__restrict__ out, uint32_t *__restrict__ blk) {
-    const uint32_t i = blockIdx.x * kVrqThreads + threadIdx.x;
+__global__ void __launch_bounds__(kWireThreads) vrq_apply_kernel(Columns c, uint32_t n, const raftgpu_voter *__restrict__ voters,
+                                                                 uint8_t *__restrict__ status, const VrqRec *__restrict__ recs,
+                                                                 const uint32_t *__restrict__ first_frame,
+                                                                 uint64_t *__restrict__ out, uint32_t *__restrict__ blk) {
+    const uint32_t i = blockIdx.x * kWireThreads + threadIdx.x;
     uint32_t resp = 0, bytes = 0;
     if (i < n) {
         uint64_t from = 0, term = 0;
@@ -164,31 +163,18 @@ __global__ void __launch_bounds__(kVrqThreads) vrq_apply_kernel(Columns c, uint3
             out[2ull * i + 1] = term;
         }
     }
-    block_sums<2, kVrqThreads>({resp, bytes}, blk);
+    block_sums<2, kWireThreads>({resp, bytes}, blk);
 }
 
-// Pass 4 (after hbf_scan_kernel<2> turned blk into block starts): every block encodes its responses, in frame order,
-// into shared memory at their offset from the 16-byte boundary below the block's start and stores them with
-// wire_store_block; offsets [blk start, + its responses).  Reads 1 per frame + 48 per response; writes the responses
-// and 4 per response.
-__global__ void __launch_bounds__(kVrqThreads) vrq_write_kernel(uint32_t n, const uint8_t *__restrict__ status,
-                                                                const VrqRec *__restrict__ recs, const uint32_t *__restrict__ blk,
-                                                                uint8_t *__restrict__ out, uint32_t *__restrict__ offsets) {
-    __shared__ __align__(16) uint8_t buf[kVrqThreads * kWireVoteFrameMax + 16];
-    __shared__ uint32_t offs[kVrqThreads];
-    const uint32_t i = blockIdx.x * kVrqThreads + threadIdx.x;
-    const bool has = i < n && (status[i] >> 4) == RAFTGPU_WIRE_OK;
-    VrqRec r{};
-    if (has) r = recs[i];
-    uint32_t lf = has, lb = has ? vrq_len(r) : 0u, nf, nbytes;
-    wire_block_scan<kVrqThreads / 32>(lf, lb, nf, nbytes);
-    const uint32_t f0 = blk[2 * blockIdx.x], b0 = blk[2 * blockIdx.x + 1], pad = b0 & 15u;
-    if (has) {
-        offs[lf] = b0 + lb;
-        wire_put_vote_frame(buf + pad + lb, static_cast<uint32_t>(r.w0), (r.w0 & kVrqPre) ? 18u : 6u, r.to, r.from, r.term,
-                            r.commit, (r.w0 & kVrqReject) != 0, r.commit_term);  // vote_resp_msg_type, raft.rs:307-313
+// Pass 4 is reply_write_kernel<VrqReply> (k_wire.cuh): the frames that are still RAFTGPU_WIRE_OK after the apply pass
+// answer.
+struct VrqReply {
+    using Rec = VrqRec;
+    static constexpr uint32_t kFrameMax = kWireVoteFrameMax;
+    __device__ __forceinline__ static bool answers(uint8_t status) { return (status >> 4) == RAFTGPU_WIRE_OK; }
+    __device__ __forceinline__ static uint32_t len(const VrqRec &r) { return vrq_len(r); }
+    __device__ __forceinline__ static uint8_t *put(uint8_t *p, const VrqRec &r) {  // vote_resp_msg_type, raft.rs:307-313
+        return wire_put_vote_frame(p, static_cast<uint32_t>(r.w0), (r.w0 & kVrqPre) ? 18u : 6u, r.to, r.from, r.term, r.commit,
+                                   (r.w0 & kVrqReject) != 0, r.commit_term);
     }
-    __syncthreads();
-    for (uint32_t j = threadIdx.x; j < nf; j += kVrqThreads) offsets[f0 + j] = offs[j];
-    wire_store_block<kVrqThreads>(out, buf, b0, nbytes);
-}
+};

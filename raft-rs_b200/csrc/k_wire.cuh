@@ -485,3 +485,33 @@ __device__ __forceinline__ void wire_store_block(uint8_t *__restrict__ out, cons
         }
     }
 }
+
+// The last pass of a pass that answers frames with frames (k_hb_follow.cuh, k_vote_request.cuh), after hbf_scan_kernel<2>
+// turned blk into block starts: every block encodes its responses, in frame order, into shared memory at their offset
+// from the 16-byte boundary below the block's start and stores them with wire_store_block; offsets [blk start, + its
+// responses).  P holds what the pass knows at compile time: Rec (its record per frame), kFrameMax (bytes of its
+// largest response), answers(status) (the frame has a response), len(rec) and put(p, rec) (the response's bytes and its
+// encoder).  Launched with kWireThreads threads per block, as the pass's scan and apply kernels.  Reads 1 per frame +
+// sizeof(Rec) per response; writes the responses and 4 per response.
+template <class P>
+__global__ void __launch_bounds__(kWireThreads) reply_write_kernel(uint32_t n, const uint8_t *__restrict__ status,
+                                                                   const typename P::Rec *__restrict__ recs,
+                                                                   const uint32_t *__restrict__ blk, uint8_t *__restrict__ out,
+                                                                   uint32_t *__restrict__ offsets) {
+    __shared__ __align__(16) uint8_t buf[kWireThreads * P::kFrameMax + 16];
+    __shared__ uint32_t offs[kWireThreads];
+    const uint32_t i = blockIdx.x * kWireThreads + threadIdx.x;
+    const bool has = i < n && P::answers(status[i]);
+    typename P::Rec r{};
+    if (has) r = recs[i];
+    uint32_t lf = has, lb = has ? P::len(r) : 0u, nf, nbytes;
+    wire_block_scan<kWireThreads / 32>(lf, lb, nf, nbytes);
+    const uint32_t f0 = blk[2 * blockIdx.x], b0 = blk[2 * blockIdx.x + 1], pad = b0 & 15u;
+    if (has) {
+        offs[lf] = b0 + lb;
+        P::put(buf + pad + lb, r);
+    }
+    __syncthreads();
+    for (uint32_t j = threadIdx.x; j < nf; j += kWireThreads) offsets[f0 + j] = offs[j];
+    wire_store_block<kWireThreads>(out, buf, b0, nbytes);
+}
