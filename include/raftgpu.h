@@ -907,6 +907,56 @@ int32_t raftgpu_heartbeat_frames(raftgpu_arena *arena, uint32_t first, uint32_t 
                                  const uint64_t *ids, uint8_t *bytes, uint64_t bytes_capacity, uint32_t *offsets,
                                  uint64_t frames_capacity, uint64_t *out_totals);
 
+/* ---- the commit broadcast to the wire -------------------------------------------- */
+
+/* Raft::maybe_commit -> bcast_append (raft.rs:1745-1748, 857-865) -> send_append -> maybe_send_append(to, allow_empty =
+ * true) (raft.rs:764-819) -> prepare_send_entries (raft.rs:714-730) -> send (raft.rs:602-661) for groups [first,
+ * first + n), split by what the leader's log has to add: the entry-less MsgAppend frames, ready for the transport, and
+ * a rest list of the sends that need the log.  A read-only pass: no update_state (the reference calls it only when
+ * entries were sent), nothing in the arena is written.
+ *
+ * Selection.  As raftgpu_heartbeat_frames: d_select in the layout of d_adv_bitmap (normally the step's advanced
+ * bitmap, raftgpu_step_results), NULL = every group of the range; a selected group takes part only when it is
+ * allocated and a leader (term_start != RAFTGPU_NO_TERM_START); a non-leader is skipped silently, a leader whose term
+ * (raftgpu_group_set_term) is 0 sends nothing and is counted in totals[3].
+ * Peers.  Every present peer (voter of either half, or learner) other than the group's own slot -- the peers
+ * raftgpu_send_list_device visits -- in this order:
+ *   Progress::is_paused (progress.rs:210-216; with device Inflights RAFTGPU_PF_INS_FULL is the derived bit): nothing;
+ *   pending_request_snapshot != RAFTGPU_INVALID_INDEX: a rest entry with RAFTGPU_SEND_SNAPSHOT;
+ *   next_idx <= last_index (entries to send) or next_idx - 1 < term_start (its term needs the log): a rest entry;
+ *   otherwise one MsgAppend frame: msg_type 3, to, from, term = Raft::term, log_term = the term when next_idx - 1 <=
+ *   last_index and 0 above it (raft_log.rs:122-127), index = next_idx - 1, commit = committed, no entries.  Canonical
+ *   proto3 encoding of eraftpb.Message, fields in number order, zero scalars omitted: at most 68 bytes.
+ * The ids are the caller's: d_ids u64 [RAFTGPU_SLOTS + 1][n] as in raftgpu_heartbeat_frames (row 8 = the `from`).
+ * Wide groups.  Peer 8 + s is cell (g + 1, s), its frame header (g + 1) << 4 | s.  Selection bit, term, term_start and
+ * the `from` are the low half's; committed and last_index the larger of both halves' values.  A range that splits a
+ * wide group is RAFTGPU_ERR_INVALID before any launch.
+ * Output.  In ascending (group, slot) order each, so the output is deterministic: the frames in the format of
+ * raftgpu_wire_batch (d_bytes 16-byte aligned, d_offsets [frames + 1], d_offsets[0] = 0), and d_rest, the rest list
+ * as raftgpu_send_entry {group, peer_slot, RAFTGPU_SEND_SNAPSHOT or 0, next_idx}: the send list of the same selection
+ * minus the peers that got a frame.  The host builds the rest list's messages from its log and then calls
+ * raftgpu_update_state for those that carried entries, as it does with the send list.  d_totals (u64[4]) = {frames,
+ * bytes, rest entries, leaders without a term}, always the full need.  When frames > frames_capacity, bytes >
+ * bytes_capacity or rest entries > rest_capacity, NOTHING is written to d_bytes, d_offsets or d_rest; the pass only
+ * reads state, so calling again with larger buffers is always safe.  raftgpu_append_frames_bound(n) bytes are enough
+ * for any n groups and 8 n is enough frames or rest entries; a range whose bound exceeds what u32 offsets address is
+ * RAFTGPU_ERR_INVALID.
+ * Ordering.  The pass reads what steps write: order it against steps on the stream.  _device: asynchronous on
+ * `stream`, with its own scratch in the arena (run it on one stream at a time).  The host form copies select / ids,
+ * runs and waits, and sees the arena as if every submitted step had completed: RAFTGPU_ERR_FULL with *out_totals
+ * filled in when a capacity is short. */
+/* Worst-case bytes of raftgpu_append_frames* output for n group slots (8 frames x 72 bytes per slot). */
+uint64_t raftgpu_append_frames_bound(uint32_t n);
+int32_t raftgpu_append_frames_device(raftgpu_arena *arena, void *stream, uint32_t first, uint32_t n,
+                                     const uint32_t *d_select, const uint64_t *d_ids,
+                                     uint8_t *d_bytes, uint64_t bytes_capacity,
+                                     uint32_t *d_offsets, uint64_t frames_capacity,
+                                     raftgpu_send_entry *d_rest, uint64_t rest_capacity, uint64_t *d_totals);
+int32_t raftgpu_append_frames(raftgpu_arena *arena, uint32_t first, uint32_t n, const uint32_t *select,
+                              const uint64_t *ids, uint8_t *bytes, uint64_t bytes_capacity, uint32_t *offsets,
+                              uint64_t frames_capacity, raftgpu_send_entry *rest, uint64_t rest_capacity,
+                              uint64_t *out_totals);
+
 /* ---- heartbeats at the follower ------------------------------------------------ */
 
 /* RawNode::step -> Raft::step (raft.rs:1280-1411) -> step_follower (raft.rs:2276-2280) -> handle_heartbeat

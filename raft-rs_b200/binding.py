@@ -317,6 +317,9 @@ def lib() -> C.CDLL:
             "raftgpu_heartbeat_frames_bound": ([u32], u64),
             "raftgpu_heartbeat_frames_device": ([vp, vp, u32, u32, vp, vp, vp, u64, vp, u64, vp], i32),
             "raftgpu_heartbeat_frames": ([vp, u32, u32, vp, vp, vp, u64, vp, u64, vp], i32),
+            "raftgpu_append_frames_bound": ([u32], u64),
+            "raftgpu_append_frames_device": ([vp, vp, u32, u32, vp, vp, vp, u64, vp, u64, vp, u64, vp], i32),
+            "raftgpu_append_frames": ([vp, u32, u32, vp, vp, vp, u64, vp, u64, vp, u64, vp], i32),
             "raftgpu_follower_heartbeat_bound": ([u64], u64),
             "raftgpu_follower_heartbeat_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_heartbeat": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
@@ -432,6 +435,11 @@ def follower_heartbeat_bound(n: int) -> int:
 def heartbeat_frames_bound(n: int) -> int:
     """raftgpu_heartbeat_frames_bound: bytes enough for the heartbeat frames of any n group slots."""
     return int(lib().raftgpu_heartbeat_frames_bound(n))
+
+
+def append_frames_bound(n: int) -> int:
+    """raftgpu_append_frames_bound: bytes enough for the MsgAppend frames of any n group slots."""
+    return int(lib().raftgpu_append_frames_bound(n))
 
 
 def tile_groups() -> int:
@@ -929,6 +937,44 @@ class Arena:
                                 d_totals, stream=None):
         self._ck(self._L.raftgpu_heartbeat_frames_device(self._h, stream, first, n, d_select, d_ids, d_bytes, bytes_capacity,
                                                          d_offsets, frames_capacity, d_totals), "heartbeat_frames_device")
+
+    def append_frames(self, first, n, ids, select=None, bytes_out=None, offsets_out=None, rest_out=None,
+                      bytes_capacity=None, frames_capacity=None, rest_capacity=None):
+        """raftgpu_append_frames: bcast_append for groups [first, first + n) as entry-less MsgAppend frames and a rest
+        list of the sends that need the log.  ids: u64 [9][n] (peer ids by slot, row 8 = the group's own id); select:
+        u32 bitmap words from group 0, or None for all.  The output goes to bytes_out / offsets_out / rest_out
+        (allocated at the bound when None) with the given capacities (default: the arrays' sizes) -> (status, blob,
+        offsets, rest, totals u64[4]): status OK with the outputs as views of the output arrays, or ERR_FULL with empty
+        views (the totals still say what is needed); any other status raises."""
+        ids = np.ascontiguousarray(ids, dtype=np.uint64)
+        assert ids.shape == (SLOTS + 1, n)
+        sel = None if select is None else np.ascontiguousarray(select, dtype=np.uint32)
+        if bytes_out is None:
+            bytes_out = np.zeros(max(16, append_frames_bound(n)), dtype=np.uint8)
+        if offsets_out is None:
+            offsets_out = np.zeros(SLOTS * n + 1, dtype=np.uint32)
+        if rest_out is None:
+            rest_out = np.zeros(max(1, SLOTS * n), dtype=SEND_ENTRY_DTYPE)
+        assert bytes_out.dtype == np.uint8 and offsets_out.dtype == np.uint32 and len(offsets_out) >= 1
+        assert rest_out.dtype == SEND_ENTRY_DTYPE
+        bcap = len(bytes_out) if bytes_capacity is None else bytes_capacity
+        fcap = len(offsets_out) - 1 if frames_capacity is None else frames_capacity
+        rcap = len(rest_out) if rest_capacity is None else rest_capacity
+        assert bcap <= len(bytes_out) and fcap < len(offsets_out) and rcap <= len(rest_out)
+        totals = np.zeros(4, dtype=np.uint64)
+        rc = self._L.raftgpu_append_frames(self._h, first, n, None if sel is None else sel.ctypes.data, ids.ctypes.data,
+                                           bytes_out.ctypes.data, bcap, offsets_out.ctypes.data, fcap,
+                                           rest_out.ctypes.data, rcap, totals.ctypes.data)
+        if rc == ERR_FULL:
+            return rc, bytes_out[:0], offsets_out[:0], rest_out[:0], totals
+        self._ck(rc, "append_frames")
+        return rc, bytes_out[: int(totals[1])], offsets_out[: int(totals[0]) + 1], rest_out[: int(totals[2])], totals
+
+    def append_frames_device(self, first, n, d_select, d_ids, d_bytes, bytes_capacity, d_offsets, frames_capacity,
+                             d_rest, rest_capacity, d_totals, stream=None):
+        self._ck(self._L.raftgpu_append_frames_device(self._h, stream, first, n, d_select, d_ids, d_bytes, bytes_capacity,
+                                                      d_offsets, frames_capacity, d_rest, rest_capacity, d_totals),
+                 "append_frames_device")
 
     def follower_heartbeat(self, frames, self_ids, select):
         """raftgpu_follower_heartbeat: handle_heartbeat at this arena's followers for the MsgHeartbeat frames of a wire

@@ -223,7 +223,16 @@ struct PassScratch {
     uint64_t *buf = nullptr;
     uint64_t cap = 0;
 };
-enum Pass { kPassWireStep, kPassHbWire, kPassHbFrames, kPassHbFollow, kPassVoteWire, kPassVoteRequest, kPassCount };
+enum Pass {
+    kPassWireStep,
+    kPassHbWire,
+    kPassHbFrames,
+    kPassHbFollow,
+    kPassVoteWire,
+    kPassVoteRequest,
+    kPassAppFrames,
+    kPassCount
+};
 
 }  // namespace
 
@@ -718,6 +727,7 @@ int32_t create(int32_t device, uint32_t max_groups, uint32_t slots, uint32_t n_r
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
     TRYC(cudaFuncSetAttribute(hbf_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kHbfSmem)));
+    TRYC(cudaFuncSetAttribute(apf_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kApfSmem)));
     {
         const char *f = getenv("RAFTGPU_FORCE_GENERAL");
         a->force_general = f && f[0] == '1';
@@ -910,7 +920,7 @@ int32_t host_batch_admit(raftgpu_arena *a, StagingSet **out) {
 
 // ---- the host frame: every host form of a batch pass (raftgpu_heartbeat_resp, raftgpu_update_state, the three
 // raftgpu_read_index_* passes, raftgpu_heartbeat_wire, raftgpu_heartbeat_frames, raftgpu_follower_heartbeat,
-// raftgpu_vote_wire, raftgpu_vote_request_wire) stages its host buffers in the fill set, idle between steps, runs its `_device` form on s_compute
+// raftgpu_vote_wire, raftgpu_vote_request_wire, raftgpu_append_frames) stages its host buffers in the fill set, idle between steps, runs its `_device` form on s_compute
 // and copies the outputs back through one HostFrame:
 //   open   admission (host_batch_admit), and the record batch if the form has one: the batch goes to d_recs and one
 //          result byte per item to d_results, so it is refused with ERR_FULL past their room;
@@ -1246,6 +1256,7 @@ extern "C" {
 #include "abi_read.inc"
 #include "abi_hb_wire.inc"
 #include "abi_hb_frames.inc"
+#include "abi_app_frames.inc"
 #include "abi_hb_follow.inc"
 #include "abi_vote_wire.inc"
 #include "abi_vote_request.inc"

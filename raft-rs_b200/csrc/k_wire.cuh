@@ -376,6 +376,42 @@ __device__ __forceinline__ uint8_t *wire_put_vote_frame(uint8_t *p, uint32_t hdr
     return p;
 }
 
+// An entry-less MsgAppend (msg_type 3; k_app_frames.cuh): u32 LE header, then eraftpb.Message in field-number order
+// with zero scalars omitted: 1 msg_type, 2 to, 3 from, 4 term, 5 log_term, 6 index, 8 commit.  At most 4 + 2 + 6 * 11 =
+// 72 bytes.
+constexpr uint32_t kWireAppFrameMax = 72;
+
+// bytes of the frame, header included
+__device__ __forceinline__ uint32_t wire_app_len(uint64_t to, uint64_t from, uint64_t term, uint64_t log_term, uint64_t index,
+                                                 uint64_t commit) {
+    const uint64_t vals[6] = {to, from, term, log_term, index, commit};
+    uint32_t len = 6u;
+#pragma unroll
+    for (int k = 0; k < 6; k++) len += vals[k] ? 1u + wire_varint_len(vals[k]) : 0u;
+    return len;
+}
+
+__device__ __forceinline__ uint8_t *wire_put_append_frame(uint8_t *p, uint32_t hdr, uint64_t to, uint64_t from, uint64_t term,
+                                                          uint64_t log_term, uint64_t index, uint64_t commit) {
+    p[0] = static_cast<uint8_t>(hdr);
+    p[1] = static_cast<uint8_t>(hdr >> 8);
+    p[2] = static_cast<uint8_t>(hdr >> 16);
+    p[3] = static_cast<uint8_t>(hdr >> 24);
+    p[4] = 0x08;  // field 1, varint
+    p[5] = 3;     // MsgAppend, eraftpb.proto:53
+    p += 6;
+    const uint8_t tags[6] = {0x10, 0x18, 0x20, 0x28, 0x30, 0x40};  // fields 2, 3, 4, 5, 6, 8
+    const uint64_t vals[6] = {to, from, term, log_term, index, commit};
+#pragma unroll
+    for (int k = 0; k < 6; k++) {
+        if (vals[k]) {
+            *p++ = tags[k];
+            p = wire_put_varint(p, vals[k]);
+        }
+    }
+    return p;
+}
+
 // Exclusive scan of two u32 counts over a block of W warps; *tot_a / *tot_b = the block's sums (every thread).
 template <uint32_t W>
 __device__ __forceinline__ void wire_block_scan(uint32_t &a, uint32_t &b, uint32_t &tot_a, uint32_t &tot_b) {

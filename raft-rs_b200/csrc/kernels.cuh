@@ -25,6 +25,7 @@ namespace raftgpu {
 #include "k_wire.cuh"
 #include "k_hb_wire.cuh"
 #include "k_hb_frames.cuh"
+#include "k_app_frames.cuh"
 #include "k_hb_follow.cuh"
 #include "k_vote_wire.cuh"
 #include "k_vote_request.cuh"
