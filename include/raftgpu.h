@@ -649,18 +649,21 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
 #define RAFTGPU_WIRE_SKIP_TYPE 1u  /* any other MessageType: Raft::step on the host */
 #define RAFTGPU_WIRE_TERM 2u       /* m.term != the group's term (raftgpu_group_set_term; 0 = not checked): Raft::step's term rules */
 #define RAFTGPU_WIRE_NEEDS_LOG 3u  /* reject with log_term > 0: next_probe_index = find_conflict_by_term(..) needs the leader's
-                                      log (raft.rs:1562-1661); the host computes it and submits the 24-byte REJECT + EXT records */
+                                      log (raft.rs:1562-1661); the host computes it and submits the 24-byte REJECT + EXT records.
+                                      At raftgpu_follower_append: a MsgAppend with entries, or whose answer needs a term of
+                                      the follower's log outside the caller's run: RawNode::step on the host */
 #define RAFTGPU_WIRE_MALFORMED 4u  /* not a protobuf message, a bad frame, or a group that is not allocated */
 #define RAFTGPU_WIRE_DUP 5u        /* a later frame of a (group, peer) cell that already has one in this batch: cells are
                                       applied in arrival order, one message per step -- resubmit it with the next batch */
 #define RAFTGPU_WIRE_CONTEXT 6u    /* (raftgpu_heartbeat_wire only) a context that is not an 8-byte read id, or any context
                                       on an arena without read queues: the host's own ReadOnly handles the frame */
-#define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat, raftgpu_vote_wire, raftgpu_vote_request_wire) the group
-                                      is not selected for the role the pass serves, or is a leader; at raftgpu_vote_wire
-                                      also a response type that is not the candidate's own (step_candidate ignores it):
-                                      Raft::step on the host */
-#define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat only) m.commit beyond max(committed, last_index):
-                                        commit_to would be fatal! (raft_log.rs:291-298) */
+#define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat, raftgpu_follower_append, raftgpu_vote_wire,
+                                      raftgpu_vote_request_wire) the group is not selected for the role the pass serves,
+                                      or is a leader; at raftgpu_vote_wire also a response type that is not the
+                                      candidate's own (step_candidate ignores it): Raft::step on the host */
+#define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat, raftgpu_follower_append) the commit_to the frame asks
+                                        for -- m.commit, or min(m.commit, m.index) of a matching MsgAppend -- beyond
+                                        max(committed, last_index): commit_to would be fatal! (raft_log.rs:291-298) */
 #define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire, raftgpu_vote_request_wire) m.commit != 0, m.commit_term != 0
                                         and m.commit beyond committed -- at raftgpu_vote_request_wire for a rejected
                                         request: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
@@ -1121,6 +1124,80 @@ int32_t raftgpu_vote_request_wire(raftgpu_arena *arena, const void *bytes, uint6
                                   uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
                                   uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
                                   uint64_t *totals);
+
+/* ---- MsgAppend at the follower ------------------------------------------------ */
+
+/* RawNode::step -> Raft::step (raft.rs:1280-1411) -> step_follower (raft.rs:2271-2275) -> handle_append_entries
+ * (raft.rs:2389-2448, with maybe_append and find_conflict_by_term, raft_log.rs:209-279) for the entry-less MsgAppend
+ * frames (msg_type 3) of a wire batch -- the commit broadcast raftgpu_append_frames writes: commit_to and one
+ * MsgAppendResponse per decided frame.  No entry is ever written and last_index is never changed: a frame that carries
+ * entries, or whose answer needs a term of the log the pass does not know, goes back to the host whole.
+ * Input.  The frames of raftgpu_wire_batch, but the header is u32 LE (group << 4 | x) with `group` the follower's own
+ * group slot in this arena (the transport rewrites the header on the way in); x is not read and is copied into the
+ * response's header.  d_bytes 16-byte aligned, n and n_bytes below 4 GiB.  d_log (16-byte aligned, read only) has one
+ * raftgpu_follower_log per group slot below the highest allocated one.  term, term_start, committed and last_index come
+ * from the arena (the caller keeps last_index current with RAFTGPU_CTL_SET_LOG_BOUNDS, term start
+ * RAFTGPU_NO_TERM_START); for a wide pair (addressed by its low half) committed and last_index are the larger of both
+ * halves'.
+ * The run.  run_start / run_term state the last term run of the caller's log: raft_log.term(i) == run_term for every i
+ * in [run_start, last_index] (run_start > last_index: no run).  term(i) is known to the pass there and above last_index
+ * (0, raft_log.rs:125), nowhere else; a shorter run is always correct and only hands back more frames.
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4 | RAFTGPU_RES_OK [| RAFTGPU_FAPP_*] for an applied frame; the first failing
+ * check decides:
+ *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot (on an arena with read queues:
+ *                any unallocated group), or the high half of a wide pair;
+ *   SKIP_TYPE    any type but 3;
+ *   ROLE         RAFTGPU_FOLLOWER_SELECT is clear, or the group is a leader (term_start != RAFTGPU_NO_TERM_START);
+ *   TERM         the group's term (raftgpu_group_set_term) is 0 or m.term differs: a higher term is
+ *                become_follower(m.term, m.from), a lower one may need a MsgAppendResponse (raft.rs:1349-1376);
+ * then the first frame of each group in frame order that got this far is decided:
+ *   NEEDS_LOG    the frame carries entries (any field 7, an empty Entry included), or the decision reads a term
+ *                outside the run: run RawNode::step on it;
+ *   COMMIT_RANGE the log matches and min(m.commit, m.index) > max(committed, last_index): commit_to would be fatal!
+ *                (raft_log.rs:291-298);
+ *   OK           decided and applied:
+ *                - m.index < committed: the response is {index = committed, commit = committed} (RAFTGPU_FAPP_STALE);
+ *                - term(m.index) == m.log_term: commit_to(min(m.commit, m.index)) on both halves of a pair, as
+ *                  RAFTGPU_CTL_COMMIT_TO; the response is {index = m.index, commit = committed after};
+ *                - otherwise, with h = min(m.index, last_index) in the run and run_term <= m.log_term: the response is
+ *                  {reject, index = m.index, reject_hint = h, log_term = run_term, commit = committed}
+ *                  (RAFTGPU_FAPP_REJECT); every other rejection walks below the run and is NEEDS_LOG;
+ *   DUP          every later frame of a group whose first frame reached the decision in this batch: resubmit DUP
+ *                frames, in order, with the next batch.
+ * A frame that is not OK changes nothing.  d_from (nullable, u64[n]) = m.from of every applied frame (0 for the
+ * others), for step_follower's leader_id = m.from and election_elapsed = 0.  This pass and
+ * raftgpu_follower_heartbeat take disjoint types, so one received buffer can go through both; a group's heartbeats
+ * and appends are then not answered in the batch's own order (Raft allows it; split the buffer to keep that order).
+ * Output.  One MsgAppendResponse per applied frame, in frame order: the input header, then eraftpb.Message with
+ * msg_type 4, to = m.from, from = the table's id, term, log_term, index, commit, reject and reject_hint; canonical
+ * proto3 as raftgpu_synth_wire_encode writes (at most 85 bytes with the header).  d_resp_bytes (16-byte aligned) holds
+ * them back to back, d_resp_offsets (n + 1 values) their starts and the end, d_totals (u64[2]) = {responses, bytes}.  A
+ * response cannot be produced again once committed has moved: resp_bytes_capacity must be at least
+ * raftgpu_follower_append_bound(n), and that bound addressable by u32 offsets: RAFTGPU_ERR_INVALID before any launch
+ * otherwise, as are a missing d_log, d_status, d_bytes or d_offsets with n > 0 and misaligned buffers.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  The
+ * host form copies (log covers the groups below the highest allocated one), runs and waits; status, from,
+ * resp_bytes / resp_offsets as above, totals u64[2]. */
+#define RAFTGPU_FOLLOWER_SELECT 0x1u /* a Follower without pending_request_snapshot: the pass decides this group */
+#define RAFTGPU_FAPP_REJECT 0x2u     /* the response rejects (reject_hint, log_term = run_term) */
+#define RAFTGPU_FAPP_STALE 0x4u      /* m.index < committed: the response names committed, nothing changed */
+typedef struct raftgpu_follower_log {
+    uint64_t id;        /* Raft::id: the response's from */
+    uint64_t run_start; /* every index i in [run_start, last_index] has raft_log.term(i) == run_term */
+    uint64_t run_term;  /* (run_start > last_index: no run; only indexes above last_index are known, term 0) */
+    uint32_t flags;     /* RAFTGPU_FOLLOWER_* */
+    uint32_t reserved;  /* 0 */
+} raftgpu_follower_log;
+/* 85 bytes per frame: enough for the responses to any n frames. */
+uint64_t raftgpu_follower_append_bound(uint64_t n);
+int32_t raftgpu_follower_append_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                       const uint32_t *d_offsets, uint64_t n, const raftgpu_follower_log *d_log,
+                                       uint8_t *d_status, uint64_t *d_from, uint8_t *d_resp_bytes,
+                                       uint64_t resp_bytes_capacity, uint32_t *d_resp_offsets, uint64_t *d_totals);
+int32_t raftgpu_follower_append(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets,
+                                uint64_t n, const raftgpu_follower_log *log, uint8_t *status, uint64_t *from,
+                                uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
+                                uint64_t *totals);
 
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 

@@ -54,6 +54,12 @@ VOTER_DTYPE = np.dtype([("id", "<u8"), ("vote", "<u8"), ("last_term", "<u8"), ("
                         ("persisted", "<u8"), ("priority", "<u8"), ("flags", "<u4"), ("reserved", "<u4"),
                         ("reserved2", "<u8")])
 assert VOTER_DTYPE.itemsize == 64
+# raftgpu_follower_append: the caller's log table (raftgpu_follower_log), its flag, and the low nibble's extra bits
+FOLLOWER_SELECT = 0x1
+FAPP_REJECT, FAPP_STALE = 0x2, 0x4
+FOLLOWER_LOG_DTYPE = np.dtype([("id", "<u8"), ("run_start", "<u8"), ("run_term", "<u8"), ("flags", "<u4"),
+                               ("reserved", "<u4")])
+assert FOLLOWER_LOG_DTYPE.itemsize == 32
 # raftgpu_vote_wire's outcome: the group (a pair's low half) and its tally word (VoteResult | granted << 8 | rejected << 16)
 VOTE_OUTCOME_DTYPE = np.dtype([("group", "<u4"), ("result", "<u4")])
 assert VOTE_OUTCOME_DTYPE.itemsize == 8
@@ -328,6 +334,9 @@ def lib() -> C.CDLL:
             "raftgpu_vote_request_wire_bound": ([u64], u64),
             "raftgpu_vote_request_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_vote_request_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_follower_append_bound": ([u64], u64),
+            "raftgpu_follower_append_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_follower_append": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -425,6 +434,11 @@ def synth_encode_vote_requests(reqs: np.ndarray):
 def vote_request_wire_bound(n: int) -> int:
     """raftgpu_vote_request_wire_bound: response bytes enough for any n vote-request frames."""
     return int(lib().raftgpu_vote_request_wire_bound(n))
+
+
+def follower_append_bound(n: int) -> int:
+    """raftgpu_follower_append_bound: response bytes enough for any n MsgAppend frames."""
+    return int(lib().raftgpu_follower_append_bound(n))
 
 
 def follower_heartbeat_bound(n: int) -> int:
@@ -1047,6 +1061,28 @@ class Arena:
         self._ck(self._L.raftgpu_vote_request_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters, d_status,
                                                           d_out, d_resp_bytes, resp_bytes_capacity, d_resp_offsets, d_totals),
                  "vote_request_wire_device")
+
+    def follower_append(self, frames, log):
+        """raftgpu_follower_append: handle_append_entries at this arena's followers for the entry-less MsgAppend frames
+        of a wire batch (.bytes, .n_bytes, .offsets, .n; headers name the follower's group slot).  log:
+        FOLLOWER_LOG_DTYPE rows covering the groups below the highest allocated one -> (status u8[n], from u64[n],
+        response blob, response offsets u32[responses + 1], totals u64[2])."""
+        lt = np.ascontiguousarray(log, dtype=FOLLOWER_LOG_DTYPE)
+        assert len(lt) >= self.get_info().hi
+        n = frames.n
+        status, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
+        resp = np.zeros(max(16, follower_append_bound(n)), np.uint8)
+        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        self._ck(self._L.raftgpu_follower_append(self._h, frames.bytes.ctypes.data, frames.n_bytes, frames.offsets.ctypes.data,
+                                                 n, lt.ctypes.data, status.ctypes.data, frm.ctypes.data, resp.ctypes.data,
+                                                 len(resp), roff.ctypes.data, totals.ctypes.data), "follower_append")
+        return status, frm, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+
+    def follower_append_device(self, d_bytes, n_bytes, d_offsets, n, d_log, d_status, d_from, d_resp_bytes,
+                               resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
+        self._ck(self._L.raftgpu_follower_append_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_log, d_status,
+                                                        d_from, d_resp_bytes, resp_bytes_capacity, d_resp_offsets, d_totals),
+                 "follower_append_device")
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

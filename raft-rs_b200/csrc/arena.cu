@@ -231,6 +231,7 @@ enum Pass {
     kPassVoteWire,
     kPassVoteRequest,
     kPassAppFrames,
+    kPassAppFollow,
     kPassCount
 };
 
@@ -1260,5 +1261,6 @@ extern "C" {
 #include "abi_hb_follow.inc"
 #include "abi_vote_wire.inc"
 #include "abi_vote_request.inc"
+#include "abi_app_follow.inc"
 
 }  // extern "C"

@@ -1,0 +1,158 @@
+// k_app_follow.cuh -- entry-less MsgAppend frames at the follower (DESIGN 3.16): Raft::step's term rules as statuses,
+// then handle_append_entries (raft.rs:2389-2448) with maybe_append / find_conflict_by_term (raft_log.rs:209-279) and no
+// entries -- commit_to(min(m.commit, m.index)) or a rejection with its hint -- and one MsgAppendResponse back through
+// send (raft.rs:602-661) for the first frame of every group that reaches the decision.
+// Part of kernels.cuh (included there, inside namespace raftgpu; not a standalone header).
+//
+// The log stays with the caller: its table (raftgpu_follower_log, one row per group slot) states the log's last term
+// run [run_start, last_index] with its term, and the pass reads term(i) only for i in that run (run_term) and above
+// last_index (0, raft_log.rs:125).  A frame whose decision needs any other term, or that carries entries, goes back to
+// the host whole.  Nothing but committed is ever written.  The frame's header is the follower's own (group << 4 | x);
+// x is not read and goes back unchanged in the response's header.
+//
+// Four kernels and no waiting between blocks: afw_scan_kernel stages and decodes every frame once, classifies and
+// decides it and writes a 64-byte record per frame that reached the decision; afw_apply_kernel marks the later frames
+// of a group DUP, runs commit_to on the first one where it matched and sums the responses per block;
+// hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block starts; reply_write_kernel<AfwReply> (k_wire.cuh) encodes
+// the responses (wire_put_app_resp_frame) and stores them through shared memory.  Every kernel takes kWireThreads
+// frames per block: one block sum per scan block.
+
+// A decided frame's record: w0 = its header | the kAfw* bits; the response's fields.  A matching frame's commit is
+// min(m.commit, m.index) until the apply pass replaces it with the committed after commit_to.
+constexpr uint64_t kAfwReject = 1ull << 32, kAfwStale = 1ull << 33, kAfwCommit = 1ull << 34;
+struct __align__(16) AfwRec {
+    uint64_t w0, to, from, term, log_term, index, commit, reject_hint;
+};
+
+__device__ __forceinline__ uint32_t afw_len(const AfwRec &r) {
+    return wire_app_resp_len(r.to, r.from, r.term, r.log_term, r.index, r.commit, (r.w0 & kAfwReject) != 0, r.reject_hint);
+}
+
+// Frame i: its status before the duplicate rule (checks in the order of raftgpu.h) and, for the frames that reach the
+// decision (OK, NEEDS_LOG, COMMIT_RANGE), its record (w0 alone for the last two).
+__device__ __forceinline__ uint32_t afw_frame(const Columns &c, const WireSrc &w, const raftgpu_follower_log *__restrict__ logs,
+                                              const WireStage &s, const uint8_t *stage, uint32_t i, AfwRec &r) {
+    uint32_t hdr;
+    const uint8_t *msg;
+    WireMsg m;
+    if (wire_open<false, true, false, false, true>(w, s, stage, i, hdr, msg, m) != RAFTGPU_WIRE_OK) return RAFTGPU_WIRE_MALFORMED;
+    const uint32_t g = hdr >> 4, meta = c.meta[g];
+    if ((meta & RAFTGPU_META_WIDE_HI) || (c.rq_cap && !(c.rq_hc[g] & kRqAlloc))) return RAFTGPU_WIRE_MALFORMED;
+    if (m.msg_type != 3u) return RAFTGPU_WIRE_SKIP_TYPE;  // MsgAppend, eraftpb.proto:53
+    const raftgpu_follower_log &l = logs[g];
+    // a Follower (the caller's bit) and not a leader here: step_follower (raft.rs:2271-2275) is the only path taken
+    if (!(l.flags & RAFTGPU_FOLLOWER_SELECT) || c.term_start[g] != RAFTGPU_NO_TERM_START) return RAFTGPU_WIRE_ROLE;
+    const uint64_t term = c.term[g];
+    if (term == 0 || m.term != term) return RAFTGPU_WIRE_TERM;  // raft.rs:1280-1411 decide those on the host
+    r.w0 = hdr;
+    if (m.entries) return RAFTGPU_WIRE_NEEDS_LOG;
+    uint64_t last = c.last_index[g], committed = c.committed[g];
+    if (meta & RAFTGPU_META_WIDE_LO) {
+        last = umax64(last, c.last_index[g + 1]);
+        committed = umax64(committed, c.committed[g + 1]);
+    }
+    r.to = m.from;    // to_send.to = m.from (raft.rs:2400, 2407)
+    r.from = l.id;    // send: from = self.id (raft.rs:610-612)
+    r.term = term;    // send: term = self.term (raft.rs:650)
+    r.log_term = r.reject_hint = 0;
+    if (m.index < committed) {  // raft.rs:2394-2404
+        r.w0 |= kAfwStale;
+        r.index = r.commit = committed;
+        return RAFTGPU_WIRE_OK;
+    }
+    const uint64_t run_start = l.run_start, run_term = l.run_term;
+    if (m.index > last || m.index >= run_start) {  // term(m.index) is known: 0 above last_index, run_term in the run
+        if ((m.index > last ? 0ull : run_term) == m.log_term) {  // maybe_append matches (raft_log.rs:243)
+            const uint64_t to_commit = umin64(m.commit, m.index);
+            if (to_commit > umax64(committed, last)) return RAFTGPU_WIRE_COMMIT_RANGE;  // raft_log.rs:291-298 fatal!
+            r.w0 |= kAfwCommit;
+            r.index = m.index;  // last_new_index = idx + 0
+            r.commit = to_commit;
+            return RAFTGPU_WIRE_OK;
+        }
+    } else {
+        return RAFTGPU_WIRE_NEEDS_LOG;
+    }
+    // the rejection: find_conflict_by_term(min(m.index, last_index), m.log_term) stops at once inside the run
+    const uint64_t h = umin64(m.index, last);
+    if (h < run_start || run_term > m.log_term) return RAFTGPU_WIRE_NEEDS_LOG;
+    r.w0 |= kAfwReject;
+    r.index = m.index;
+    r.reject_hint = h;
+    r.log_term = run_term;
+    r.commit = committed;
+    return RAFTGPU_WIRE_OK;
+}
+
+// Pass 1: classify and decide every frame; status[i] = wire status << 4; the record of a frame that reached the
+// decision, first_frame[group] = the lowest such frame of the group.  Launched with kWireThreads threads per block.
+__global__ void __launch_bounds__(kWireThreads) afw_scan_kernel(Columns c, WireSrc w, const raftgpu_follower_log *__restrict__ logs,
+                                                                uint8_t *__restrict__ status, AfwRec *__restrict__ recs,
+                                                                uint32_t *__restrict__ first_frame) {
+    __shared__ __align__(16) uint8_t stage[kWireStage + 16];
+    WireStage s;
+    const uint32_t i = wire_block_frame(w, stage, s);
+    if (i == kNoFrame) return;
+    AfwRec r;
+    const uint32_t st = afw_frame(c, w, logs, s, stage, i, r);
+    status[i] = static_cast<uint8_t>(st << 4);
+    if (st == RAFTGPU_WIRE_OK) recs[i] = r;
+    else if (st == RAFTGPU_WIRE_NEEDS_LOG || st == RAFTGPU_WIRE_COMMIT_RANGE) recs[i].w0 = r.w0;
+    else return;
+    atomicMin(&first_frame[static_cast<uint32_t>(r.w0) >> 4], i);
+}
+
+// Pass 2: a later frame of a group is RAFTGPU_WIRE_DUP.  The first one, when OK and matching, runs commit_to -- on both
+// halves of a wide pair, after wide_sync, as RAFTGPU_CTL_COMMIT_TO does -- and keeps the new committed in its record.
+// from_out[i] (nullable) = m.from of an applied frame, 0 otherwise.  blk[2 * block + {0, 1}] = the block's responses
+// and their bytes.  Algorithmic bytes per frame: 1 read + 1 written (+ 8 from_out); per frame that reached the decision
+// 8 (w0) + 4 (first_frame) read; per applied one 56 (record) read, and for a match 16-32 (committed, last_index) read,
+// 8-16 (committed) + 8 (record) written.
+__global__ void __launch_bounds__(kWireThreads) afw_apply_kernel(Columns c, uint32_t n, uint8_t *__restrict__ status,
+                                                                 AfwRec *__restrict__ recs, const uint32_t *__restrict__ first_frame,
+                                                                 uint64_t *__restrict__ from_out, uint32_t *__restrict__ blk) {
+    const uint32_t i = blockIdx.x * kWireThreads + threadIdx.x;
+    uint32_t resp = 0, bytes = 0;
+    if (i < n) {
+        uint64_t from = 0;
+        const uint32_t st = status[i] >> 4;
+        if (st == RAFTGPU_WIRE_OK || st == RAFTGPU_WIRE_NEEDS_LOG || st == RAFTGPU_WIRE_COMMIT_RANGE) {
+            const uint64_t w0 = recs[i].w0;
+            const uint32_t g = static_cast<uint32_t>(w0) >> 4;
+            if (first_frame[g] != i) {
+                status[i] = static_cast<uint8_t>(RAFTGPU_WIRE_DUP << 4);
+            } else if (st == RAFTGPU_WIRE_OK) {
+                AfwRec r = recs[i];
+                if (w0 & kAfwCommit) {
+                    if (c.meta[g] & RAFTGPU_META_WIDE_LO) {
+                        wide_sync(c, g);
+                        commit_to_group(c, g + 1, r.commit);
+                    }
+                    commit_to_group(c, g, r.commit);  // (in range: the scan checked it)
+                    r.commit = c.committed[g];        // raft.rs:2446 to_send.commit = raft_log.committed
+                    recs[i].commit = r.commit;
+                }
+                status[i] = static_cast<uint8_t>((RAFTGPU_WIRE_OK << 4) | RAFTGPU_RES_OK |
+                                                 ((w0 & kAfwReject) ? RAFTGPU_FAPP_REJECT : 0u) |
+                                                 ((w0 & kAfwStale) ? RAFTGPU_FAPP_STALE : 0u));
+                from = r.to;
+                resp = 1;
+                bytes = afw_len(r);
+            }
+        }
+        if (from_out) from_out[i] = from;
+    }
+    block_sums<2, kWireThreads>({resp, bytes}, blk);
+}
+
+// Pass 4 is reply_write_kernel<AfwReply> (k_wire.cuh): the frames the apply pass marked RAFTGPU_RES_OK answer.
+struct AfwReply {
+    using Rec = AfwRec;
+    static constexpr uint32_t kFrameMax = kWireAppRespFrameMax;
+    __device__ __forceinline__ static bool answers(uint8_t status) { return status & RAFTGPU_RES_OK; }
+    __device__ __forceinline__ static uint32_t len(const AfwRec &r) { return afw_len(r); }
+    __device__ __forceinline__ static uint8_t *put(uint8_t *p, const AfwRec &r) {  // MsgAppendResponse, raft.rs:2406-2447
+        return wire_put_app_resp_frame(p, static_cast<uint32_t>(r.w0), r.to, r.from, r.term, r.log_term, r.index, r.commit,
+                                       (r.w0 & kAfwReject) != 0, r.reject_hint);
+    }
+};

@@ -42,6 +42,7 @@ struct WireMsg {  // the scalar fields this path looks at
     uint64_t from;              // wire_decode<true, true> only: field 3
     uint64_t commit_term;       // wire_decode<.., .., true> only: field 15
     uint64_t priority;          // wire_decode<.., .., .., true> only: field 14
+    bool entries;               // wire_decode<.., .., .., .., true> only: a field 7 (entries) is present
 };
 
 constexpr uint32_t kWireThreads = 256;
@@ -64,8 +65,9 @@ __device__ __forceinline__ bool wire_varint(const uint8_t *p, uint32_t &pos, uin
 // One serialized Message -> WireMsg.  false = not a well-formed protobuf message.  kContext: also the context's
 // position (the heartbeat-response path, k_hb_wire.cuh); the AppendResponse kernels instantiate it without.  kFrom:
 // also `from` (the follower's heartbeat path, k_hb_follow.cuh).  kCommitTerm: also commit_term (the vote responses,
-// k_vote_wire.cuh).  kPriority: also priority (the vote requests, k_vote_request.cuh).
-template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false, bool kPriority = false>
+// k_vote_wire.cuh).  kPriority: also priority (the vote requests, k_vote_request.cuh).  kEntries: also whether any
+// field 7 occurs, in any wire type (the follower's MsgAppend path, k_app_follow.cuh).
+template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false, bool kPriority = false, bool kEntries = false>
 __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, WireMsg &m) {
     m.msg_type = 0;
     m.reject = false;
@@ -74,12 +76,16 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
     if constexpr (kFrom) m.from = 0;
     if constexpr (kCommitTerm) m.commit_term = 0;
     if constexpr (kPriority) m.priority = 0;
+    if constexpr (kEntries) m.entries = false;
     uint32_t pos = 0;
     while (pos < len) {
         uint64_t tag;
         if (!wire_varint(p, pos, len, 5, tag) || tag > 0xffffffffull) return false;
         const uint32_t field = static_cast<uint32_t>(tag >> 3), wt = static_cast<uint32_t>(tag & 7u);
         if (field == 0) return false;
+        if constexpr (kEntries) {
+            if (field == 7) m.entries = true;  // repeated Entry entries = 7, an empty Entry included
+        }
         if (wt == 0) {
             uint64_t v;
             if (!wire_varint(p, pos, len, 10, v)) return false;
@@ -177,7 +183,7 @@ __device__ __forceinline__ uint32_t wire_block_frame(const WireSrc &w, uint8_t *
 // RAFTGPU_WIRE_MALFORMED when it is not a frame (offsets out of order or past the batch, shorter than the header),
 // names a group >= n_groups or is not a well-formed protobuf message; RAFTGPU_WIRE_OK otherwise.  The flags are
 // wire_decode's.
-template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false, bool kPriority = false>
+template <bool kContext = false, bool kFrom = false, bool kCommitTerm = false, bool kPriority = false, bool kEntries = false>
 __device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage &s, const uint8_t *stage, uint32_t i,
                                               uint32_t &hdr, const uint8_t *&msg, WireMsg &m) {
     const uint32_t a = w.offsets[i], b = w.offsets[i + 1];
@@ -185,7 +191,7 @@ __device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage 
     const uint8_t *p = (s.staged && a >= s.lo && b <= s.hi) ? stage + (a - s.base) : w.bytes + a;
     hdr = p[0] | (static_cast<uint32_t>(p[1]) << 8) | (static_cast<uint32_t>(p[2]) << 16) | (static_cast<uint32_t>(p[3]) << 24);
     msg = p + 4;
-    if ((hdr >> 4) >= w.n_groups || !wire_decode<kContext, kFrom, kCommitTerm, kPriority>(msg, b - a - 4u, m))
+    if ((hdr >> 4) >= w.n_groups || !wire_decode<kContext, kFrom, kCommitTerm, kPriority, kEntries>(msg, b - a - 4u, m))
         return RAFTGPU_WIRE_MALFORMED;
     return RAFTGPU_WIRE_OK;
 }
@@ -408,6 +414,49 @@ __device__ __forceinline__ uint8_t *wire_put_append_frame(uint8_t *p, uint32_t h
             *p++ = tags[k];
             p = wire_put_varint(p, vals[k]);
         }
+    }
+    return p;
+}
+
+// A MsgAppendResponse (msg_type 4; k_app_follow.cuh): u32 LE header, then eraftpb.Message in field-number order with
+// zero scalars omitted, as raftgpu_synth_wire_encode writes it: 1 msg_type, 2 to, 3 from, 4 term, 5 log_term, 6 index,
+// 8 commit, 10 reject, 11 reject_hint.  At most 4 + 2 + 6 * 11 + 2 + 11 = 85 bytes.
+constexpr uint32_t kWireAppRespFrameMax = 85;
+
+// bytes of the frame, header included
+__device__ __forceinline__ uint32_t wire_app_resp_len(uint64_t to, uint64_t from, uint64_t term, uint64_t log_term,
+                                                      uint64_t index, uint64_t commit, bool reject, uint64_t reject_hint) {
+    return wire_app_len(to, from, term, log_term, index, commit) + (reject ? 2u : 0u) +
+           (reject_hint ? 1u + wire_varint_len(reject_hint) : 0u);
+}
+
+__device__ __forceinline__ uint8_t *wire_put_app_resp_frame(uint8_t *p, uint32_t hdr, uint64_t to, uint64_t from,
+                                                            uint64_t term, uint64_t log_term, uint64_t index,
+                                                            uint64_t commit, bool reject, uint64_t reject_hint) {
+    p[0] = static_cast<uint8_t>(hdr);
+    p[1] = static_cast<uint8_t>(hdr >> 8);
+    p[2] = static_cast<uint8_t>(hdr >> 16);
+    p[3] = static_cast<uint8_t>(hdr >> 24);
+    p[4] = 0x08;  // field 1, varint
+    p[5] = 4;     // MsgAppendResponse, eraftpb.proto:54
+    p += 6;
+    const uint8_t tags[6] = {0x10, 0x18, 0x20, 0x28, 0x30, 0x40};  // fields 2, 3, 4, 5, 6, 8
+    const uint64_t vals[6] = {to, from, term, log_term, index, commit};
+#pragma unroll
+    for (int k = 0; k < 6; k++) {
+        if (vals[k]) {
+            *p++ = tags[k];
+            p = wire_put_varint(p, vals[k]);
+        }
+    }
+    if (reject) {
+        p[0] = 0x50;  // field 10
+        p[1] = 1;
+        p += 2;
+    }
+    if (reject_hint) {
+        *p++ = 0x58;  // field 11
+        p = wire_put_varint(p, reject_hint);
     }
     return p;
 }

@@ -29,5 +29,6 @@ namespace raftgpu {
 #include "k_hb_follow.cuh"
 #include "k_vote_wire.cuh"
 #include "k_vote_request.cuh"
+#include "k_app_follow.cuh"
 
 }  // namespace raftgpu
