@@ -1199,6 +1199,56 @@ int32_t raftgpu_follower_append(raftgpu_arena *arena, const void *bytes, uint64_
                                 uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
                                 uint64_t *totals);
 
+/* ---- MsgAppend with entries at the follower ------------------------------------ */
+
+/* raftgpu_follower_append, and for a frame that carries entries maybe_append (raft_log.rs:249-279) at the log's tail:
+ * find_conflict (raft_log.rs:182-198) from the run, the new last_index, commit_to and the MsgAppendResponse.  The log
+ * stays with the caller: the pass says which bytes of the frame the log takes (the appended records' span) and keeps
+ * the table's run current.
+ * The input, the header, MALFORMED, SKIP_TYPE, ROLE, TERM, the claim and DUP rule, the stale rule (m.index < committed
+ * is answered whatever entries the frame carries), the rejections (the entries are ignored), the responses, the bound
+ * (raftgpu_follower_append_bound), the refusals and the ordering are raftgpu_follower_append's.  What differs:
+ * Entries.  Each field 7 of a frame past TERM is decoded as an eraftpb.Entry (term = 2, index = 3; other fields
+ * skipped, a repeated scalar keeps its last value): an Entry whose bytes are not a well-formed protobuf message makes
+ * the frame MALFORMED (it does not claim its group).  A claiming frame whose log matches at m.index then runs
+ * maybe_append, in this order:
+ *   NEEDS_LOG    a field 7 that is not length-delimited; indexes that are not m.index + 1, m.index + 2, ...; an entry
+ *                of term 0; m.index > last_index (a gap: truncate_and_append panics); appended entries that are not
+ *                back to back in the frame (another field between them);
+ *   COMMIT_RANGE find_conflict's index is at or below committed (raft_log.rs:259-265 fatal!), or commit_to would be;
+ *   OK           find_conflict's index is the first entry whose index is <= last_index and whose term is not run_term,
+ *                or the first above last_index.  When there is one (`conflict`), last_index = m.index + entries (both
+ *                halves of a pair, as RAFTGPU_CTL_SET_LOG_BOUNDS) and the low nibble is RAFTGPU_RES_OK |
+ *                RAFTGPU_FAPP_APPENDED; when every entry matched nothing is appended and it is RAFTGPU_RES_OK.  Then
+ *                commit_to(min(m.commit, m.index + entries)); the response is {index = m.index + entries, commit =
+ *                committed after}.
+ * The run.  For an appended frame, let t be the last entry's term and k the first index of the trailing block of
+ * appended entries with term t.  When every appended entry has term t, t == run_term and conflict - 1 >= run_start,
+ * the run stays; otherwise it becomes [k, last_index] with term t.  The device form writes d_log's row (the table is
+ * read-write); the host form writes the caller's `log` rows of the appended frames from their records.
+ * Appended.  d_appended (u64-aligned, n records) = raftgpu_follower_appended of every RAFTGPU_FAPP_APPENDED frame, all
+ * zero for every other frame.  The span points into the caller's batch: the host hands those bytes to its log engine
+ * (or decodes only them for RaftLog::unstable), lowers persisted to first_index - 1 (raft_log.rs:269-272) and sends the
+ * response once the entries are durable.  The host form's `appended` has n records. */
+#define RAFTGPU_FAPP_APPENDED 0x8u /* the log took entries from this frame: see raftgpu_follower_appended */
+typedef struct raftgpu_follower_appended {
+    uint64_t first_index; /* find_conflict's index: the first entry the log took from this frame */
+    uint64_t last_index;  /* the log's last index after the append (m.index + number of entries) */
+    uint64_t run_start;   /* the log's last term run after the append (also written into the table) */
+    uint64_t run_term;
+    uint32_t span_off;    /* byte offset in the batch of that entry's field-7 tag */
+    uint32_t span_len;    /* the appended Entry records (tag, length, Entry), back to back */
+} raftgpu_follower_appended; /* all zero for every frame without RAFTGPU_FAPP_APPENDED */
+int32_t raftgpu_follower_append_entries_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                               const uint32_t *d_offsets, uint64_t n, raftgpu_follower_log *d_log,
+                                               uint8_t *d_status, uint64_t *d_from, raftgpu_follower_appended *d_appended,
+                                               uint8_t *d_resp_bytes, uint64_t resp_bytes_capacity,
+                                               uint32_t *d_resp_offsets, uint64_t *d_totals);
+int32_t raftgpu_follower_append_entries(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets,
+                                        uint64_t n, raftgpu_follower_log *log, uint8_t *status, uint64_t *from,
+                                        raftgpu_follower_appended *appended, uint8_t *resp_bytes,
+                                        uint64_t resp_bytes_capacity, uint32_t *resp_offsets, uint64_t *totals);
+
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 
 /* ProgressTracker::reset_votes / record_vote (tracker.rs:301-310). */

@@ -60,6 +60,11 @@ FAPP_REJECT, FAPP_STALE = 0x2, 0x4
 FOLLOWER_LOG_DTYPE = np.dtype([("id", "<u8"), ("run_start", "<u8"), ("run_term", "<u8"), ("flags", "<u4"),
                                ("reserved", "<u4")])
 assert FOLLOWER_LOG_DTYPE.itemsize == 32
+# raftgpu_follower_append_entries: an applied frame's extra bit and its record (raftgpu_follower_appended)
+FAPP_APPENDED = 0x8
+FOLLOWER_APPENDED_DTYPE = np.dtype([("first_index", "<u8"), ("last_index", "<u8"), ("run_start", "<u8"),
+                                    ("run_term", "<u8"), ("span_off", "<u4"), ("span_len", "<u4")])
+assert FOLLOWER_APPENDED_DTYPE.itemsize == 40
 # raftgpu_vote_wire's outcome: the group (a pair's low half) and its tally word (VoteResult | granted << 8 | rejected << 16)
 VOTE_OUTCOME_DTYPE = np.dtype([("group", "<u4"), ("result", "<u4")])
 assert VOTE_OUTCOME_DTYPE.itemsize == 8
@@ -337,6 +342,8 @@ def lib() -> C.CDLL:
             "raftgpu_follower_append_bound": ([u64], u64),
             "raftgpu_follower_append_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_append": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_follower_append_entries_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_follower_append_entries": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_update_state_device": ([vp, vp, vp, u64, vp], i32),
             "raftgpu_update_state": ([vp, vp, u64, vp], i32),
             "raftgpu_wire_apply_device": ([vp, vp, vp, u64, vp, u64, vp], i32),
@@ -1083,6 +1090,31 @@ class Arena:
         self._ck(self._L.raftgpu_follower_append_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_log, d_status,
                                                         d_from, d_resp_bytes, resp_bytes_capacity, d_resp_offsets, d_totals),
                  "follower_append_device")
+
+    def follower_append_entries(self, frames, log):
+        """raftgpu_follower_append_entries: handle_append_entries at this arena's followers for the MsgAppend frames of
+        a wire batch, entries appended at the log's tail.  log: FOLLOWER_LOG_DTYPE rows covering the groups below the
+        highest allocated one, a C-contiguous array whose appended rows' runs are updated in place -> (status u8[n],
+        from u64[n], appended FOLLOWER_APPENDED_DTYPE[n], response blob, response offsets u32[responses + 1], totals
+        u64[2])."""
+        assert log.dtype == FOLLOWER_LOG_DTYPE and log.flags.c_contiguous and len(log) >= self.get_info().hi
+        n = frames.n
+        status, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
+        app = np.zeros(n, FOLLOWER_APPENDED_DTYPE)
+        resp = np.zeros(max(16, follower_append_bound(n)), np.uint8)
+        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        self._ck(self._L.raftgpu_follower_append_entries(self._h, frames.bytes.ctypes.data, frames.n_bytes,
+                                                         frames.offsets.ctypes.data, n, log.ctypes.data, status.ctypes.data,
+                                                         frm.ctypes.data, app.ctypes.data, resp.ctypes.data, len(resp),
+                                                         roff.ctypes.data, totals.ctypes.data), "follower_append_entries")
+        return status, frm, app, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+
+    def follower_append_entries_device(self, d_bytes, n_bytes, d_offsets, n, d_log, d_status, d_from, d_appended,
+                                       d_resp_bytes, resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
+        self._ck(self._L.raftgpu_follower_append_entries_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_log,
+                                                                d_status, d_from, d_appended, d_resp_bytes,
+                                                                resp_bytes_capacity, d_resp_offsets, d_totals),
+                 "follower_append_entries_device")
 
     def update_state(self, entries: np.ndarray) -> np.ndarray:
         """raftgpu_update_state: send entries with next_idx = last -> result bytes."""

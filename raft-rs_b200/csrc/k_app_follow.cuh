@@ -10,6 +10,10 @@
 // the host whole.  Nothing but committed is ever written.  The frame's header is the follower's own (group << 4 | x);
 // x is not read and goes back unchanged in the response's header.
 //
+// kAppend = true is raftgpu_follower_append_entries (DESIGN 3.17): a matching frame's entries are walked once
+// (wire_entries, k_wire.cuh), find_conflict is decided from the run, and the apply pass moves last_index, keeps the
+// table's run current and reports the appended span; the log's bytes stay with the caller.
+//
 // Four kernels and no waiting between blocks: afw_scan_kernel stages and decodes every frame once, classifies and
 // decides it and writes a 64-byte record per frame that reached the decision; afw_apply_kernel marks the later frames
 // of a group DUP, runs commit_to on the first one where it matched and sums the responses per block;
@@ -19,7 +23,7 @@
 
 // A decided frame's record: w0 = its header | the kAfw* bits; the response's fields.  A matching frame's commit is
 // min(m.commit, m.index) until the apply pass replaces it with the committed after commit_to.
-constexpr uint64_t kAfwReject = 1ull << 32, kAfwStale = 1ull << 33, kAfwCommit = 1ull << 34;
+constexpr uint64_t kAfwReject = 1ull << 32, kAfwStale = 1ull << 33, kAfwCommit = 1ull << 34, kAfwAppend = 1ull << 35;
 struct __align__(16) AfwRec {
     uint64_t w0, to, from, term, log_term, index, commit, reject_hint;
 };
@@ -28,10 +32,46 @@ __device__ __forceinline__ uint32_t afw_len(const AfwRec &r) {
     return wire_app_resp_len(r.to, r.from, r.term, r.log_term, r.index, r.commit, (r.w0 & kAfwReject) != 0, r.reject_hint);
 }
 
+// A matching frame with entries (afw_frame<true>), its walk (ents, e) done: maybe_append from the run.  m.index is at or
+// above run_start here (the match is known and m.index <= last_index, or the frame is a gap and goes back to the host).
+__device__ __forceinline__ uint32_t afw_append(const WireSrc &w, AfwRec &r, raftgpu_follower_appended &ap, uint32_t i,
+                                               const WireMsg &m, uint32_t ents, const WireEntries &e, uint64_t last,
+                                               uint64_t committed, uint64_t run_start, uint64_t run_term) {
+    if (ents == kEntsNeedsLog || m.index > last) return RAFTGPU_WIRE_NEEDS_LOG;  // (m.index > last_index: a gap)
+    // Both COMMIT_RANGE checks below restate the reference's fatal!s and cannot fire here: past the stale rule
+    // m.index >= committed, so conflict >= m.index + 1 > committed; and to_commit <= last_new <= new_last.
+    const uint64_t conflict = e.conflict ? m.index + e.conflict : 0;
+    if (conflict && conflict <= committed) return RAFTGPU_WIRE_COMMIT_RANGE;  // raft_log.rs:259-265 fatal!
+    const uint64_t last_new = m.index + e.count, new_last = conflict ? last_new : last;
+    const uint64_t to_commit = umin64(m.commit, last_new);
+    if (to_commit > umax64(committed, new_last)) return RAFTGPU_WIRE_COMMIT_RANGE;  // raft_log.rs:291-298 fatal!
+    r.w0 |= kAfwCommit;
+    r.index = last_new;  // raft.rs:2441 to_send.index = last_idx
+    r.commit = to_commit;
+    if (conflict) {
+        r.w0 |= kAfwAppend;
+        const bool keep = e.uniform && e.tail_term == run_term && conflict - 1 >= run_start;
+        r.reject_hint = keep ? run_start : m.index + e.tail;
+        r.log_term = keep ? run_term : e.tail_term;
+        ap.first_index = conflict;
+        ap.last_index = last_new;
+        ap.run_start = r.reject_hint;
+        ap.run_term = r.log_term;
+        ap.span_off = w.offsets[i] + 4u + e.span_off;
+        ap.span_len = e.span_end - e.span_off;
+    }
+    return RAFTGPU_WIRE_OK;
+}
+
 // Frame i: its status before the duplicate rule (checks in the order of raftgpu.h) and, for the frames that reach the
-// decision (OK, NEEDS_LOG, COMMIT_RANGE), its record (w0 alone for the last two).
+// decision (OK, NEEDS_LOG, COMMIT_RANGE), its record (w0 alone for the last two).  kAppend (raftgpu_follower_append_entries):
+// a matching frame's entries are appended (maybe_append, raft_log.rs:249-279); an appended frame's record carries the
+// new run in log_term (its term) and reject_hint (its start) to the apply pass, and ap = its raftgpu_follower_appended
+// (untouched for every other frame).
+template <bool kAppend>
 __device__ __forceinline__ uint32_t afw_frame(const Columns &c, const WireSrc &w, const raftgpu_follower_log *__restrict__ logs,
-                                              const WireStage &s, const uint8_t *stage, uint32_t i, AfwRec &r) {
+                                              const WireStage &s, const uint8_t *stage, uint32_t i, AfwRec &r,
+                                              raftgpu_follower_appended &ap) {
     uint32_t hdr;
     const uint8_t *msg;
     WireMsg m;
@@ -45,11 +85,21 @@ __device__ __forceinline__ uint32_t afw_frame(const Columns &c, const WireSrc &w
     const uint64_t term = c.term[g];
     if (term == 0 || m.term != term) return RAFTGPU_WIRE_TERM;  // raft.rs:1280-1411 decide those on the host
     r.w0 = hdr;
-    if (m.entries) return RAFTGPU_WIRE_NEEDS_LOG;
+    if constexpr (!kAppend) {
+        if (m.entries) return RAFTGPU_WIRE_NEEDS_LOG;
+    }
     uint64_t last = c.last_index[g], committed = c.committed[g];
     if (meta & RAFTGPU_META_WIDE_LO) {
         last = umax64(last, c.last_index[g + 1]);
         committed = umax64(committed, c.committed[g + 1]);
+    }
+    uint32_t ents = kEntsOk;
+    WireEntries e;
+    if constexpr (kAppend) {  // every entry of every frame that got this far: an Entry that is not well formed is MALFORMED
+        if (m.entries) {
+            ents = wire_entries(msg, w.offsets[i + 1] - w.offsets[i] - 4u, m.index, last, l.run_term, e);
+            if (ents == kEntsMalformed) return RAFTGPU_WIRE_MALFORMED;
+        }
     }
     r.to = m.from;    // to_send.to = m.from (raft.rs:2400, 2407)
     r.from = l.id;    // send: from = self.id (raft.rs:610-612)
@@ -63,6 +113,9 @@ __device__ __forceinline__ uint32_t afw_frame(const Columns &c, const WireSrc &w
     const uint64_t run_start = l.run_start, run_term = l.run_term;
     if (m.index > last || m.index >= run_start) {  // term(m.index) is known: 0 above last_index, run_term in the run
         if ((m.index > last ? 0ull : run_term) == m.log_term) {  // maybe_append matches (raft_log.rs:243)
+            if constexpr (kAppend) {
+                if (m.entries) return afw_append(w, r, ap, i, m, ents, e, last, committed, run_start, run_term);
+            }
             const uint64_t to_commit = umin64(m.commit, m.index);
             if (to_commit > umax64(committed, last)) return RAFTGPU_WIRE_COMMIT_RANGE;  // raft_log.rs:291-298 fatal!
             r.w0 |= kAfwCommit;
@@ -85,17 +138,23 @@ __device__ __forceinline__ uint32_t afw_frame(const Columns &c, const WireSrc &w
 }
 
 // Pass 1: classify and decide every frame; status[i] = wire status << 4; the record of a frame that reached the
-// decision, first_frame[group] = the lowest such frame of the group.  Launched with kWireThreads threads per block.
+// decision, first_frame[group] = the lowest such frame of the group.  kAppend: appended[i] = the frame's
+// raftgpu_follower_appended (zero unless it appends; the apply pass zeroes a DUP one).  Launched with kWireThreads
+// threads per block.
+template <bool kAppend>
 __global__ void __launch_bounds__(kWireThreads) afw_scan_kernel(Columns c, WireSrc w, const raftgpu_follower_log *__restrict__ logs,
                                                                 uint8_t *__restrict__ status, AfwRec *__restrict__ recs,
-                                                                uint32_t *__restrict__ first_frame) {
+                                                                uint32_t *__restrict__ first_frame,
+                                                                raftgpu_follower_appended *__restrict__ appended) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
     WireStage s;
     const uint32_t i = wire_block_frame(w, stage, s);
     if (i == kNoFrame) return;
     AfwRec r;
-    const uint32_t st = afw_frame(c, w, logs, s, stage, i, r);
+    raftgpu_follower_appended ap{};
+    const uint32_t st = afw_frame<kAppend>(c, w, logs, s, stage, i, r, ap);
     status[i] = static_cast<uint8_t>(st << 4);
+    if constexpr (kAppend) appended[i] = ap;
     if (st == RAFTGPU_WIRE_OK) recs[i] = r;
     else if (st == RAFTGPU_WIRE_NEEDS_LOG || st == RAFTGPU_WIRE_COMMIT_RANGE) recs[i].w0 = r.w0;
     else return;
@@ -104,13 +163,18 @@ __global__ void __launch_bounds__(kWireThreads) afw_scan_kernel(Columns c, WireS
 
 // Pass 2: a later frame of a group is RAFTGPU_WIRE_DUP.  The first one, when OK and matching, runs commit_to -- on both
 // halves of a wide pair, after wide_sync, as RAFTGPU_CTL_COMMIT_TO does -- and keeps the new committed in its record.
+// kAppend: an appended frame first sets last_index (both halves of a pair, as RAFTGPU_CTL_SET_LOG_BOUNDS) and the
+// table's run, and clears the run from its record; a DUP frame's appended record is zeroed.
 // from_out[i] (nullable) = m.from of an applied frame, 0 otherwise.  blk[2 * block + {0, 1}] = the block's responses
 // and their bytes.  Algorithmic bytes per frame: 1 read + 1 written (+ 8 from_out); per frame that reached the decision
 // 8 (w0) + 4 (first_frame) read; per applied one 56 (record) read, and for a match 16-32 (committed, last_index) read,
-// 8-16 (committed) + 8 (record) written.
+// 8-16 (committed) + 8 (record) written; per appended one 8-16 (last_index) + 16 (run) + 16 (record) written.
+template <bool kAppend>
 __global__ void __launch_bounds__(kWireThreads) afw_apply_kernel(Columns c, uint32_t n, uint8_t *__restrict__ status,
                                                                  AfwRec *__restrict__ recs, const uint32_t *__restrict__ first_frame,
-                                                                 uint64_t *__restrict__ from_out, uint32_t *__restrict__ blk) {
+                                                                 uint64_t *__restrict__ from_out, uint32_t *__restrict__ blk,
+                                                                 raftgpu_follower_log *__restrict__ logs,
+                                                                 raftgpu_follower_appended *__restrict__ appended) {
     const uint32_t i = blockIdx.x * kWireThreads + threadIdx.x;
     uint32_t resp = 0, bytes = 0;
     if (i < n) {
@@ -121,8 +185,25 @@ __global__ void __launch_bounds__(kWireThreads) afw_apply_kernel(Columns c, uint
             const uint32_t g = static_cast<uint32_t>(w0) >> 4;
             if (first_frame[g] != i) {
                 status[i] = static_cast<uint8_t>(RAFTGPU_WIRE_DUP << 4);
+                if constexpr (kAppend) {
+                    if (st == RAFTGPU_WIRE_OK && (w0 & kAfwAppend)) appended[i] = raftgpu_follower_appended{};
+                }
             } else if (st == RAFTGPU_WIRE_OK) {
                 AfwRec r = recs[i];
+                if constexpr (kAppend) {
+                    if (w0 & kAfwAppend) {  // truncate_and_append: last_index = m.index + entries
+                        if (c.meta[g] & RAFTGPU_META_WIDE_LO) {
+                            wide_sync(c, g);
+                            c.last_index[g + 1] = r.index;
+                        }
+                        c.last_index[g] = r.index;
+                        logs[g].run_start = r.reject_hint;
+                        logs[g].run_term = r.log_term;
+                        r.log_term = r.reject_hint = 0;  // the response carries neither
+                        recs[i].log_term = 0;
+                        recs[i].reject_hint = 0;
+                    }
+                }
                 if (w0 & kAfwCommit) {
                     if (c.meta[g] & RAFTGPU_META_WIDE_LO) {
                         wide_sync(c, g);
@@ -132,9 +213,10 @@ __global__ void __launch_bounds__(kWireThreads) afw_apply_kernel(Columns c, uint
                     r.commit = c.committed[g];        // raft.rs:2446 to_send.commit = raft_log.committed
                     recs[i].commit = r.commit;
                 }
-                status[i] = static_cast<uint8_t>((RAFTGPU_WIRE_OK << 4) | RAFTGPU_RES_OK |
-                                                 ((w0 & kAfwReject) ? RAFTGPU_FAPP_REJECT : 0u) |
-                                                 ((w0 & kAfwStale) ? RAFTGPU_FAPP_STALE : 0u));
+                uint32_t low = RAFTGPU_RES_OK | ((w0 & kAfwReject) ? RAFTGPU_FAPP_REJECT : 0u) |
+                               ((w0 & kAfwStale) ? RAFTGPU_FAPP_STALE : 0u);
+                if constexpr (kAppend) low |= (w0 & kAfwAppend) ? RAFTGPU_FAPP_APPENDED : 0u;
+                status[i] = static_cast<uint8_t>((RAFTGPU_WIRE_OK << 4) | low);
                 from = r.to;
                 resp = 1;
                 bytes = afw_len(r);

@@ -130,6 +130,90 @@ __device__ __forceinline__ bool wire_decode(const uint8_t *p, uint32_t len, Wire
     return true;
 }
 
+// The entries of a MsgAppend whose log matches at idx (k_app_follow.cuh, raftgpu_follower_append_entries): every field 7
+// of the Message p[0, len) (already well formed: wire_decode) walked once, each length-delimited one decoded as an
+// eraftpb.Entry (term = 2, index = 3, eraftpb.proto:16-21; other fields skipped by their length, a repeated scalar
+// keeps its last value).  term(j) for j > idx is the follower's: run_term up to last, 0 above (raft_log.rs:125).
+struct WireEntries {
+    uint32_t count;               // field-7 records
+    uint32_t conflict;            // find_conflict (raft_log.rs:182-198): 1 + the position of the first entry whose term
+                                  // is not term(index) (index idx + conflict), 0 when every entry matches
+    uint32_t tail;                // 1 + the position of the trailing block of appended entries with the last one's term
+    uint32_t span_off, span_end;  // from p: the first appended entry's tag, the end of the last appended one
+    uint64_t tail_term;           // the last appended entry's term
+    bool uniform;                 // every appended entry has term tail_term
+};
+constexpr uint32_t kEntsOk = 0, kEntsMalformed = 1, kEntsNeedsLog = 2;
+
+// kEntsMalformed: an Entry is not a well-formed protobuf message.  kEntsNeedsLog: a field 7 that is not length-
+// delimited, an index other than idx + 1, idx + 2, ..., a term 0, or appended entries with another field between them.
+__device__ __noinline__ uint32_t wire_entries(const uint8_t *p, uint32_t len, uint64_t idx, uint64_t last,
+                                                 uint64_t run_term, WireEntries &e) {
+    e.count = e.conflict = e.tail = e.span_off = e.span_end = 0;
+    e.tail_term = 0;
+    e.uniform = true;
+    bool needs_log = false;
+    uint32_t pos = 0;
+    while (pos < len) {
+        const uint32_t at = pos;
+        uint64_t tag, l;
+        if (!wire_varint(p, pos, len, 5, tag)) return kEntsMalformed;
+        const uint32_t field = static_cast<uint32_t>(tag >> 3), wt = static_cast<uint32_t>(tag & 7u);
+        if (wt != 2) {  // a scalar: skipped (the Message is well formed)
+            if (field == 7) needs_log = true;
+            if (wt == 0) wire_varint(p, pos, len, 10, l);
+            else pos += wt == 1 ? 8u : 4u;
+            continue;
+        }
+        if (!wire_varint(p, pos, len, 10, l)) return kEntsMalformed;
+        const uint32_t end = pos + static_cast<uint32_t>(l);
+        if (field != 7) {
+            pos = end;
+            continue;
+        }
+        uint64_t term = 0, index = 0;
+        while (pos < end) {  // the Entry
+            uint64_t t, v;
+            if (!wire_varint(p, pos, end, 5, t) || t > 0xffffffffull || (t >> 3) == 0) return kEntsMalformed;
+            const uint32_t f = static_cast<uint32_t>(t >> 3), w = static_cast<uint32_t>(t & 7u);
+            if (w == 0) {
+                if (!wire_varint(p, pos, end, 10, v)) return kEntsMalformed;
+                if (f == 2) term = v;
+                else if (f == 3) index = v;
+            } else if (w == 1 || w == 5) {
+                const uint32_t k = w == 1 ? 8u : 4u;
+                if (end - pos < k) return kEntsMalformed;
+                pos += k;
+            } else if (w == 2) {
+                if (!wire_varint(p, pos, end, 10, v) || v > end - pos) return kEntsMalformed;
+                pos += static_cast<uint32_t>(v);
+            } else {
+                return kEntsMalformed;
+            }
+        }
+        const uint32_t k = ++e.count;  // this entry is index idx + k
+        if (index != idx + k || term == 0) {
+            needs_log = true;
+        } else if (!e.conflict) {
+            if (idx + k > last || term != run_term) {  // the first entry the log takes
+                e.conflict = e.tail = k;
+                e.tail_term = term;
+                e.span_off = at;
+                e.span_end = end;
+            }
+        } else {
+            if (at != e.span_end) needs_log = true;
+            e.span_end = end;
+            if (term != e.tail_term) {
+                e.tail = k;
+                e.tail_term = term;
+                e.uniform = false;
+            }
+        }
+    }
+    return needs_log ? kEntsNeedsLog : kEntsOk;
+}
+
 // The context convention of the heartbeat paths (DESIGN 3.10): a read id travels as the 8 bytes of the context,
 // little-endian.  q = the context's first byte (WireMsg::ctx_off from the Message's start).
 __device__ __forceinline__ uint64_t wire_ctx_u64(const uint8_t *q) {

@@ -4,7 +4,16 @@ frame's term, its log ending at m.index in a run of m.log_term.  Times the devic
 CUDA events around the call) over the same frames each run -- after the first run commit_to moves nothing, which costs
 the pass the same bytes -- median and range, then the host form end to end (copies in, the pass, copies back) and the C
 batch oracle on one core over the same batch.  Prints the GPU's name and power limit read in the same run.  Without a
-GPU it fails with RAFTGPU_ERR_NO_DEVICE."""
+GPU it fails with RAFTGPU_ERR_NO_DEVICE.
+
+--entries K [--payload B]: raftgpu_follower_append_entries instead, one MsgAppend per group with K entries of B data
+bytes each at the log's tail (index = last_index, log_term = run_term = the term), so every frame appends.  The table
+and last_index are restored before every pass (outside the CUDA events), so every timed pass appends.
+
+    python scripts/micro_follower_append.py                                  # 1M groups, entry-less
+    python scripts/micro_follower_append.py --entries 1 --payload 128        # 1M groups
+    N=100000 python scripts/micro_follower_append.py --entries 8 --payload 1024"""
+import argparse
 import importlib
 import os
 import subprocess
@@ -27,6 +36,14 @@ B = pkg.binding
 n = int(os.environ.get("N", 1_000_000))
 runs = int(os.environ.get("RUNS", 20))
 rng = np.random.default_rng(0xAF60)
+ap = argparse.ArgumentParser()
+ap.add_argument("--entries", type=int, default=0)
+ap.add_argument("--payload", type=int, default=0)
+args = ap.parse_args()
+if args.entries:
+    import micro_follower_append_entries as ME
+    ME.main(B, n, runs, args.entries, args.payload, rng)
+    sys.exit(0)
 
 # the frames: raftgpu_append_frames of n leaders with one caught-up peer each (slot 1)
 lc = O.new_columns(n, n)
