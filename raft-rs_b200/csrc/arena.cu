@@ -727,8 +727,10 @@ int32_t create(int32_t device, uint32_t max_groups, uint32_t slots, uint32_t n_r
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
     TRYC(cudaFuncSetAttribute(step_tile_compact_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tile_smem));
-    TRYC(cudaFuncSetAttribute(hbf_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kHbfSmem)));
-    TRYC(cudaFuncSetAttribute(apf_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kApfSmem)));
+    TRYC(cudaFuncSetAttribute(bcast_write_kernel<HbBcast>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              static_cast<int>(kBcastSmem<HbBcast>)));
+    TRYC(cudaFuncSetAttribute(bcast_write_kernel<AppBcast>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              static_cast<int>(kBcastSmem<AppBcast>)));
     {
         const char *f = getenv("RAFTGPU_FORCE_GENERAL");
         a->force_general = f && f[0] == '1';
@@ -1053,14 +1055,13 @@ int32_t reply_check(raftgpu_arena *a, uint64_t n_bytes, uint64_t n, uint64_t fra
 }
 
 // The `_device` form after its checks, on st: no frame gives zero totals and resp_offsets[0] = 0.  Otherwise the
-// pass's scratch (u64 words) is carved into one record per frame, the {responses, bytes} of every block and the fit
-// flag, its first-frame table (first_n u32) reset, and four passes run with kWireThreads frames per block:
-// passes(blocks, recs, first, blk) launches the pass's scan and apply kernels, hbf_scan_kernel<2> turns the block sums
-// into block starts, the totals and the last offset, reply_write_kernel<P> writes the responses.
+// pass's scratch (u64 words) is carved into one record per frame and the {responses, bytes} of every block, its
+// first-frame table (first_n u32) reset, and four passes run with kWireThreads frames per block: passes(blocks, recs,
+// first, blk) launches the pass's scan and apply kernels, block_starts_kernel<2> turns the block sums into block starts,
+// the totals and the last offset, reply_write_kernel<P> writes the responses.
 template <class P, typename Passes>
 int32_t reply_run(raftgpu_arena *a, cudaStream_t st, PassScratch &scratch, uint64_t n, const uint8_t *d_status,
-                  uint8_t *d_resp_bytes, uint64_t resp_bytes_capacity, uint32_t *d_resp_offsets, uint64_t *d_totals,
-                  size_t first_n, Passes &&passes) {
+                  uint8_t *d_resp_bytes, uint32_t *d_resp_offsets, uint64_t *d_totals, size_t first_n, Passes &&passes) {
     using Rec = typename P::Rec;
     if (n == 0) {
         CK(a, cudaMemsetAsync(d_totals, 0, 16, st));
@@ -1068,13 +1069,13 @@ int32_t reply_run(raftgpu_arena *a, cudaStream_t st, PassScratch &scratch, uint6
         return RAFTGPU_OK;
     }
     const uint32_t nb = div_up(n, kWireThreads);
-    const int32_t rc = pass_scratch(a, st, scratch, first_n, (sizeof(Rec) / 8) * n + nb + 1);
+    const int32_t rc = pass_scratch(a, st, scratch, first_n, (sizeof(Rec) / 8) * n + nb);
     if (rc != RAFTGPU_OK) return rc;
     Rec *recs = reinterpret_cast<Rec *>(scratch.buf);
-    uint32_t *blk = reinterpret_cast<uint32_t *>(scratch.buf + (sizeof(Rec) / 8) * n), *flag = blk + 2ull * nb;
+    uint32_t *blk = reinterpret_cast<uint32_t *>(scratch.buf + (sizeof(Rec) / 8) * n);
     passes(nb, recs, scratch.first, blk);
     // (the capacities always hold: resp_bytes_capacity >= P::kFrameMax * n was checked, d_resp_offsets has n + 1 values)
-    hbf_scan_kernel<2><<<1, kHbfScanThreads, 0, st>>>(blk, nb, resp_bytes_capacity, n, d_totals, d_resp_offsets, flag);
+    block_starts_kernel<2><<<1, kScanThreads, 0, st>>>(blk, nb, d_totals, d_resp_offsets);
     reply_write_kernel<P><<<nb, kWireThreads, 0, st>>>(static_cast<uint32_t>(n), d_status, recs, blk, d_resp_bytes, d_resp_offsets);
     CKL(a);
     return RAFTGPU_OK;
@@ -1129,6 +1130,110 @@ int32_t reply_host(raftgpu_arena *a, const void *bytes, uint64_t n_bytes, const 
     totals[1] = h_totals[1];
     rc = f.back(resp_offsets, roff_at, 4 * (totals[0] + 1));
     if (rc == RAFTGPU_OK) rc = f.back(resp_bytes, rbytes_at, totals[1]);
+    return rc == RAFTGPU_OK ? f.wait() : rc;
+}
+
+// ---- the broadcast pipeline (DESIGN 3.11): a pass that writes a leader's frames from the arena
+// (raftgpu_heartbeat_frames, raftgpu_append_frames) is a broadcast policy P (k_bcast.cuh) and shares the rest:
+// bcast_check, bcast_device<P> for the `_device` form, bcast_host<P> for the host form.  `pass` is its PassScratch slot,
+// `name` the word its messages start with.
+
+// The refusals both forms make before any copy or launch.
+int32_t bcast_check(raftgpu_arena *a, uint32_t first, uint32_t n, uint32_t frame_max, const char *name) {
+    if (static_cast<uint64_t>(first) + n > a->cap) return RAFTGPU_ERR_RANGE;
+    if (static_cast<uint64_t>(n) * kSlots * frame_max > 0xffffffffull)  // the pass's public bound
+        return fail(a, RAFTGPU_ERR_INVALID, std::string(name) + " frames of this range may not be addressable by u32 offsets");
+    if (n && ((a->h_meta[first] & RAFTGPU_META_WIDE_HI) || (a->h_meta[first + n - 1] & RAFTGPU_META_WIDE_LO)))
+        return fail(a, RAFTGPU_ERR_INVALID, "the range splits a wide group");
+    return RAFTGPU_OK;
+}
+
+// The `_device` form after its null checks, o on the device.  No group gives zero totals and offsets[0] = 0.
+template <class P>
+int32_t bcast_device(raftgpu_arena *a, void *stream, int pass, const char *name, uint32_t first, uint32_t n,
+                     const uint32_t *d_select, const uint64_t *d_ids, const BcastOut &o) {
+    int32_t rc = bcast_check(a, first, n, P::kFrameMax, name);
+    if (rc != RAFTGPU_OK) return rc;
+    if (reinterpret_cast<uintptr_t>(o.bytes) & 15u) return fail(a, RAFTGPU_ERR_INVALID, "frame bytes must be 16-byte aligned");
+    CK(a, cudaSetDevice(a->device));
+    cudaStream_t st = pick_stream(a, stream);
+    constexpr uint32_t kTotals = kBcastTotals<P>;
+    if (n == 0) {
+        CK(a, cudaMemsetAsync(o.totals, 0, 8 * kTotals, st));
+        if (o.offsets) CK(a, cudaMemsetAsync(o.offsets, 0, 4, st));
+        return RAFTGPU_OK;
+    }
+    // scratch in u64 words: {frames | rest << 16, bytes} per slot, the totals of the block starts, then u32: 3 per block
+    // (frames, bytes, leaders without a term) and, with a rest list, 1 per block (rest entries)
+    const uint32_t nb = div_up(n, kBcastThreads);
+    PassScratch &ps = a->pass[pass];
+    rc = pass_scratch(a, st, ps, 0, n + kTotals + div_up((P::kRest ? 4ull : 3ull) * nb, 2));
+    if (rc != RAFTGPU_OK) return rc;
+    uint2 *cnt = reinterpret_cast<uint2 *>(ps.buf);
+    uint64_t *tot = ps.buf + n;
+    uint32_t *blk = reinterpret_cast<uint32_t *>(tot + kTotals), *blk_rest = blk + 3ull * nb;
+    const BcastSrc s{first, n, a->hi, d_select, d_ids};
+    bcast_size_kernel<P><<<nb, kBcastThreads, 0, st>>>(a->cols, s, cnt, blk, blk_rest);
+    block_starts_kernel<3><<<1, kScanThreads, 0, st>>>(blk, nb, tot, nullptr);
+    if constexpr (P::kRest) block_starts_kernel<1><<<1, kScanThreads, 0, st>>>(blk_rest, nb, tot + 3, nullptr);
+    bcast_write_kernel<P><<<nb, kBcastThreads, kBcastSmem<P>, st>>>(a->cols, s, cnt, blk, blk_rest, tot, o);
+    CKL(a);
+    return RAFTGPU_OK;
+}
+
+// The host form after its null checks, o on the host (HostFrame): d_wire holds [ids | select | offsets | rest entries,
+// none without a rest list | bytes], the totals go to the arena's scratch.  The bytes are the rest region, what d_wire
+// already has room for; when the frames need more (and fit the caller's buffer) the region is enlarged to exactly that
+// and the pass runs again, so a caller with a steady load runs it once per call.
+template <class P>
+int32_t bcast_host(raftgpu_arena *a, int pass, const char *name, uint32_t first, uint32_t n, const uint32_t *select,
+                   const uint64_t *ids, const BcastOut &o) {
+    std::lock_guard<std::mutex> ctl_lock(a->ctl_mu);
+    int32_t rc = bcast_check(a, first, n, P::kFrameMax, name);
+    if (rc != RAFTGPU_OK) return rc;
+    constexpr uint32_t kTotals = kBcastTotals<P>;
+    for (uint32_t k = 0; k < kTotals; k++) o.totals[k] = 0;
+    if (n == 0) {
+        if (!o.offsets) return fail(a, RAFTGPU_ERR_FULL, "no offsets buffer");
+        o.offsets[0] = 0;
+        return RAFTGPU_OK;
+    }
+    HostFrame f(a);
+    rc = f.open();
+    if (rc != RAFTGPU_OK) return rc;
+    const uint64_t words = select ? (static_cast<uint64_t>(first) + n + 31) / 32 : 0;
+    const uint64_t frames_room = std::min<uint64_t>(o.frames_cap, static_cast<uint64_t>(kSlots) * n);
+    const uint64_t rest_room = std::min<uint64_t>(o.rest_cap, static_cast<uint64_t>(kSlots) * n);
+    const WireRegion ids_at = f.in(ids, 8ull * (kSlots + 1) * n), sel_at = f.in(select, 4 * words);
+    const WireRegion off_at = f.out(4 * (frames_room + 1)), rest_at = f.out(sizeof(raftgpu_send_entry) * rest_room);
+    const WireRegion bytes_at = f.rest(16);
+    uint64_t *d_totals = scratch<uint64_t, kTotals>(a->d_scratch), *h_totals = scratch<uint64_t, kTotals>(a->h_scratch);
+    uint64_t room = 0;
+    auto run = [&]() {
+        int32_t r = f.run([&](const Staged &d) {
+            room = std::min(o.bytes_cap, d.rest);
+            return bcast_device<P>(a, a->s_compute, pass, name, first, n, words ? d.at<const uint32_t>(sel_at) : nullptr,
+                                   d.at<const uint64_t>(ids_at),
+                                   {d.at<uint8_t>(bytes_at), d.at<uint32_t>(off_at), d.at<raftgpu_send_entry>(rest_at),
+                                    room, frames_room, rest_room, d_totals});
+        });
+        if (r == RAFTGPU_OK) r = f.back(h_totals, d_totals, 8 * kTotals);
+        return r == RAFTGPU_OK ? f.wait() : r;
+    };
+    rc = run();
+    if (rc != RAFTGPU_OK) return rc;
+    const uint64_t rest = P::kRest ? h_totals[2] : 0;
+    const bool fits = o.offsets && h_totals[0] <= o.frames_cap && h_totals[1] <= o.bytes_cap && (!P::kRest || rest <= o.rest_cap);
+    if (fits && h_totals[1] > room) {  // the caller's buffer is large enough, d_wire was not
+        f.enlarge(h_totals[1]);
+        rc = run();
+        if (rc != RAFTGPU_OK) return rc;
+    }
+    for (uint32_t k = 0; k < kTotals; k++) o.totals[k] = h_totals[k];
+    if (!fits) return fail(a, RAFTGPU_ERR_FULL, std::string(name) + " frames exceed the output buffers");
+    rc = f.back(o.offsets, off_at, 4 * (h_totals[0] + 1));
+    if (rc == RAFTGPU_OK) rc = f.back(o.rest, rest_at, sizeof(raftgpu_send_entry) * rest);
+    if (rc == RAFTGPU_OK) rc = f.back(o.bytes, bytes_at, h_totals[1]);
     return rc == RAFTGPU_OK ? f.wait() : rc;
 }
 

@@ -17,7 +17,7 @@
 // Four kernels and no waiting between blocks: afw_scan_kernel stages and decodes every frame once, classifies and
 // decides it and writes a 64-byte record per frame that reached the decision; afw_apply_kernel marks the later frames
 // of a group DUP, runs commit_to on the first one where it matched and sums the responses per block;
-// hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block starts; reply_write_kernel<AfwReply> (k_wire.cuh) encodes
+// block_starts_kernel<2> (k_wire.cuh) turns the sums into block starts; reply_write_kernel<AfwReply> (k_wire.cuh) encodes
 // the responses (wire_put_app_resp_frame) and stores them through shared memory.  Every kernel takes kWireThreads
 // frames per block: one block sum per scan block.
 

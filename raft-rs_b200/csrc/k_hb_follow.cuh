@@ -9,7 +9,7 @@
 //
 // Four kernels and no waiting between blocks: hfw_scan_kernel stages and decodes every frame once, classifies it and
 // writes a 48-byte record per passing frame; hfw_apply_kernel marks the later frames of a group DUP, runs commit_to
-// on the first one and sums the responses per block; hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block
+// on the first one and sums the responses per block; block_starts_kernel<2> (k_wire.cuh) turns the sums into block
 // starts; reply_write_kernel<HfwReply> (k_wire.cuh) encodes the responses (wire_put_hb_frame<9>) and stores them
 // through shared memory.  Every kernel takes kWireThreads frames per block: one block sum per scan block.
 

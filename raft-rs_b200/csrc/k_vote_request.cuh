@@ -10,7 +10,7 @@
 // Four kernels and no waiting between blocks: vrq_scan_kernel stages and decodes every frame once, classifies and
 // decides it and writes a 48-byte record per frame that reached the term rules; vrq_apply_kernel marks the later frames
 // of a group DUP, raises the term and resets the group where the first one bumps it, and sums the responses per block;
-// hbf_scan_kernel<2> (k_wire.cuh) turns the sums into block starts; reply_write_kernel<VrqReply> (k_wire.cuh) encodes
+// block_starts_kernel<2> (k_wire.cuh) turns the sums into block starts; reply_write_kernel<VrqReply> (k_wire.cuh) encodes
 // the responses (wire_put_vote_frame) and stores them through shared memory.  Every kernel takes kWireThreads frames per
 // block: one block sum per scan block.
 

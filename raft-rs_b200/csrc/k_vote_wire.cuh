@@ -11,7 +11,7 @@
 // Five kernels and no waiting between blocks: vw_scan_kernel stages and decodes every frame once, classifies it and
 // writes an 8-byte record per passing frame; vw_apply_kernel marks the later frames of a cell DUP, writes the first
 // one's vote and marks its group (pair) touched; vw_count_kernel tallies every touched group and sums the decided ones
-// per block; hbf_scan_kernel<1> (k_wire.cuh) turns the sums into block starts; vw_write_kernel lists the decided groups
+// per block; block_starts_kernel<1> (k_wire.cuh) turns the sums into block starts; vw_write_kernel lists the decided groups
 // in ascending order.
 
 constexpr uint32_t kVwThreads = 256;  // frames (scan, apply) or group slots (count, write) per block
@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(kVwThreads) vw_count_kernel(Columns c, uint32_
     block_flush_counts<1>(local, which, counters, nullptr);
 }
 
-// Pass 5 (after hbf_scan_kernel<1> turned blk into block starts): every decided group's outcome, in ascending group order;
+// Pass 5 (after block_starts_kernel<1> turned blk into block starts): every decided group's outcome, in ascending group order;
 // an outcome at or past `capacity` is not written (the count, *d_count, stays the true one).
 __global__ void __launch_bounds__(kVwThreads) vw_write_kernel(uint32_t n, const uint32_t *__restrict__ touched,
                                                               const uint32_t *__restrict__ words,

@@ -355,10 +355,10 @@ __global__ void __launch_bounds__(kWireThreads) wire_apply_kernel(Columns c, Wir
 // ---------------------------------------------------------------------------
 // The encoder: heartbeat-kind frames (MsgHeartbeat at the leader, MsgHeartbeatResponse at the follower), and the
 // block-output code of the passes that write them -- a block scan of {frames, bytes}, the one-block scan of the block
-// sums (hbf_scan_kernel) and the 16-byte store of a block's contiguous output.
+// sums (block_starts_kernel) and the 16-byte store of a block's contiguous output.
 
 constexpr uint32_t kWireHbFrameMax = 60;  // 4-byte header + at most 56 bytes of Message
-constexpr uint32_t kHbfScanThreads = 1024;
+constexpr uint32_t kScanThreads = 1024;  // block_starts_kernel
 
 // bytes of v as a base-128 varint
 __device__ __forceinline__ uint32_t wire_varint_len(uint64_t v) {
@@ -386,19 +386,24 @@ __device__ __forceinline__ uint8_t *wire_put_varint(uint8_t *p, uint64_t v) {
     return p;
 }
 
+// What every frame starts with: the u32 LE header, then the Message's field 1, msg_type (never 0 on these paths).
+__device__ __forceinline__ uint8_t *wire_put_head(uint8_t *p, uint32_t hdr, uint8_t type) {
+    p[0] = static_cast<uint8_t>(hdr);
+    p[1] = static_cast<uint8_t>(hdr >> 8);
+    p[2] = static_cast<uint8_t>(hdr >> 16);
+    p[3] = static_cast<uint8_t>(hdr >> 24);
+    p[4] = 0x08;  // field 1, varint
+    p[5] = type;
+    return p + 6;
+}
+
 // One heartbeat-kind frame: u32 LE header, then eraftpb.Message (eraftpb.proto:71-92) in field-number order with zero
 // scalars omitted: 1 msg_type = kType (MsgHeartbeat 8, MsgHeartbeatResponse 9, eraftpb.proto:58-59), 2 to, 3 from,
 // 4 term (never 0 on these paths), 8 commit, 12 context (the 8 little-endian bytes of ctx when has_ctx).
 template <uint8_t kType>
 __device__ __forceinline__ uint8_t *wire_put_hb_frame(uint8_t *p, uint32_t hdr, uint64_t to, uint64_t from, uint64_t term,
                                                  uint64_t commit, bool has_ctx, uint64_t ctx) {
-    p[0] = static_cast<uint8_t>(hdr);
-    p[1] = static_cast<uint8_t>(hdr >> 8);
-    p[2] = static_cast<uint8_t>(hdr >> 16);
-    p[3] = static_cast<uint8_t>(hdr >> 24);
-    p[4] = 0x08;  // field 1, varint
-    p[5] = kType;
-    p += 6;
+    p = wire_put_head(p, hdr, kType);
     if (to) {
         *p++ = 0x10;
         p = wire_put_varint(p, to);
@@ -438,13 +443,7 @@ __device__ __forceinline__ uint32_t wire_vote_len(uint64_t to, uint64_t from, ui
 
 __device__ __forceinline__ uint8_t *wire_put_vote_frame(uint8_t *p, uint32_t hdr, uint8_t type, uint64_t to, uint64_t from,
                                                         uint64_t term, uint64_t commit, bool reject, uint64_t commit_term) {
-    p[0] = static_cast<uint8_t>(hdr);
-    p[1] = static_cast<uint8_t>(hdr >> 8);
-    p[2] = static_cast<uint8_t>(hdr >> 16);
-    p[3] = static_cast<uint8_t>(hdr >> 24);
-    p[4] = 0x08;  // field 1, varint
-    p[5] = type;
-    p += 6;
+    p = wire_put_head(p, hdr, type);
     const uint8_t tags[4] = {0x10, 0x18, 0x20, 0x40};  // fields 2, 3, 4, 8
     const uint64_t vals[4] = {to, from, term, commit};
 #pragma unroll
@@ -481,15 +480,11 @@ __device__ __forceinline__ uint32_t wire_app_len(uint64_t to, uint64_t from, uin
     return len;
 }
 
+// kType: MsgAppend 3 here; MsgAppendResponse 4 (eraftpb.proto:53-54) writes these fields before its own.
+template <uint8_t kType>
 __device__ __forceinline__ uint8_t *wire_put_append_frame(uint8_t *p, uint32_t hdr, uint64_t to, uint64_t from, uint64_t term,
                                                           uint64_t log_term, uint64_t index, uint64_t commit) {
-    p[0] = static_cast<uint8_t>(hdr);
-    p[1] = static_cast<uint8_t>(hdr >> 8);
-    p[2] = static_cast<uint8_t>(hdr >> 16);
-    p[3] = static_cast<uint8_t>(hdr >> 24);
-    p[4] = 0x08;  // field 1, varint
-    p[5] = 3;     // MsgAppend, eraftpb.proto:53
-    p += 6;
+    p = wire_put_head(p, hdr, kType);
     const uint8_t tags[6] = {0x10, 0x18, 0x20, 0x28, 0x30, 0x40};  // fields 2, 3, 4, 5, 6, 8
     const uint64_t vals[6] = {to, from, term, log_term, index, commit};
 #pragma unroll
@@ -517,22 +512,7 @@ __device__ __forceinline__ uint32_t wire_app_resp_len(uint64_t to, uint64_t from
 __device__ __forceinline__ uint8_t *wire_put_app_resp_frame(uint8_t *p, uint32_t hdr, uint64_t to, uint64_t from,
                                                             uint64_t term, uint64_t log_term, uint64_t index,
                                                             uint64_t commit, bool reject, uint64_t reject_hint) {
-    p[0] = static_cast<uint8_t>(hdr);
-    p[1] = static_cast<uint8_t>(hdr >> 8);
-    p[2] = static_cast<uint8_t>(hdr >> 16);
-    p[3] = static_cast<uint8_t>(hdr >> 24);
-    p[4] = 0x08;  // field 1, varint
-    p[5] = 4;     // MsgAppendResponse, eraftpb.proto:54
-    p += 6;
-    const uint8_t tags[6] = {0x10, 0x18, 0x20, 0x28, 0x30, 0x40};  // fields 2, 3, 4, 5, 6, 8
-    const uint64_t vals[6] = {to, from, term, log_term, index, commit};
-#pragma unroll
-    for (int k = 0; k < 6; k++) {
-        if (vals[k]) {
-            *p++ = tags[k];
-            p = wire_put_varint(p, vals[k]);
-        }
-    }
+    p = wire_put_append_frame<4>(p, hdr, to, from, term, log_term, index, commit);
     if (reject) {
         p[0] = 0x50;  // field 10
         p[1] = 1;
@@ -588,18 +568,17 @@ __device__ __forceinline__ void wire_block_scan(uint32_t &a, uint32_t &b, uint32
     __syncthreads();  // wa / wb may be reused by the caller's next scan
 }
 
-// Pass 2, one block: blk's frames and bytes become each block's exclusive starts.  K = u32 per block in blk: {frames,
-// bytes} (K = 2, k_hb_follow.cuh) or {frames, bytes, leaders without a term} (K = 3); totals = the K sums.  flag[0] =
-// the output fits (d_offsets given, frames <= frames_cap, bytes <= bytes_cap); then offsets[frames] = bytes, the end of
-// the last frame.  K = 1 (k_vote_wire.cuh): blk holds one count per block, totals[0] = their sum; the capacities,
-// offsets and flag are not used.
+// One block: blk's counts become each block's exclusive starts.  K = u32 per block in blk: {count} (K = 1), {frames,
+// bytes} (K = 2) or {frames, bytes, leaders without a term} (K = 3); totals = the K sums.  offsets (K >= 2, nullable):
+// offsets[frames] = bytes, the end of the last frame, for a caller whose outputs always fit; a pass that may not fit
+// writes it where it decides the fit.
 template <uint32_t K>
-__global__ void __launch_bounds__(kHbfScanThreads) hbf_scan_kernel(uint32_t *__restrict__ blk, uint32_t nb, uint64_t bytes_cap,
-                                                                   uint64_t frames_cap, uint64_t *__restrict__ totals,
-                                                                   uint32_t *__restrict__ offsets, uint32_t *__restrict__ flag) {
+__global__ void __launch_bounds__(kScanThreads) block_starts_kernel(uint32_t *__restrict__ blk, uint32_t nb,
+                                                                    uint64_t *__restrict__ totals,
+                                                                    uint32_t *__restrict__ offsets) {
     static_assert(K >= 1 && K <= 3, "blk holds {count} or {frames, bytes[, leaders without a term]} per block");
     uint32_t carry_f = 0, carry_b = 0, no_term = 0;
-    for (uint32_t j0 = 0; j0 < nb; j0 += kHbfScanThreads) {  // (uniform trip count: every thread reaches the scan)
+    for (uint32_t j0 = 0; j0 < nb; j0 += kScanThreads) {  // (uniform trip count: every thread reaches the scan)
         const uint32_t j = j0 + threadIdx.x;
         uint32_t f = 0, b = 0;
         if (j < nb) {
@@ -608,7 +587,7 @@ __global__ void __launch_bounds__(kHbfScanThreads) hbf_scan_kernel(uint32_t *__r
             if constexpr (K == 3) no_term += blk[K * j + 2];
         }
         uint32_t tf, tb;
-        wire_block_scan<kHbfScanThreads / 32>(f, b, tf, tb);
+        wire_block_scan<kScanThreads / 32>(f, b, tf, tb);
         if (j < nb) {
             blk[K * j] = carry_f + f;
             if constexpr (K >= 2) blk[K * j + 1] = carry_b + b;
@@ -623,19 +602,17 @@ __global__ void __launch_bounds__(kHbfScanThreads) hbf_scan_kernel(uint32_t *__r
     uint64_t t = 0;
     if constexpr (K == 3) {
         no_term = __reduce_add_sync(0xffffffffu, no_term);
-        __shared__ uint32_t nt[kHbfScanThreads / 32];
+        __shared__ uint32_t nt[kScanThreads / 32];
         if ((threadIdx.x & 31u) == 0) nt[threadIdx.x >> 5] = no_term;
         __syncthreads();
         if (threadIdx.x == 0)
-            for (uint32_t w = 0; w < kHbfScanThreads / 32; w++) t += nt[w];
+            for (uint32_t w = 0; w < kScanThreads / 32; w++) t += nt[w];
     }
     if (threadIdx.x == 0) {
         totals[0] = carry_f;
         totals[1] = carry_b;
         if constexpr (K == 3) totals[2] = t;
-        const bool fits = offsets && carry_f <= frames_cap && carry_b <= bytes_cap;
-        flag[0] = fits;
-        if (fits) offsets[carry_f] = carry_b;
+        if (offsets) offsets[carry_f] = carry_b;
     }
 }
 
@@ -655,7 +632,7 @@ __device__ __forceinline__ void wire_store_block(uint8_t *__restrict__ out, cons
     }
 }
 
-// The last pass of a pass that answers frames with frames (k_hb_follow.cuh, k_vote_request.cuh), after hbf_scan_kernel<2>
+// The last pass of a pass that answers frames with frames (k_hb_follow.cuh, k_vote_request.cuh), after block_starts_kernel<2>
 // turned blk into block starts: every block encodes its responses, in frame order, into shared memory at their offset
 // from the 16-byte boundary below the block's start and stores them with wire_store_block; offsets [blk start, + its
 // responses).  P holds what the pass knows at compile time: Rec (its record per frame), kFrameMax (bytes of its

@@ -24,6 +24,7 @@ namespace raftgpu {
 #include "k_read.cuh"
 #include "k_wire.cuh"
 #include "k_hb_wire.cuh"
+#include "k_bcast.cuh"
 #include "k_hb_frames.cuh"
 #include "k_app_frames.cuh"
 #include "k_hb_follow.cuh"
