@@ -650,6 +650,8 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
 #define RAFTGPU_WIRE_TERM 2u       /* m.term != the group's term (raftgpu_group_set_term; 0 = not checked): Raft::step's term rules */
 #define RAFTGPU_WIRE_NEEDS_LOG 3u  /* reject with log_term > 0: next_probe_index = find_conflict_by_term(..) needs the leader's
                                       log (raft.rs:1562-1661); the host computes it and submits the 24-byte REJECT + EXT records.
+                                      On an arena with leader runs (raftgpu_arena_enable_leader_runs) only the rejections
+                                      the stated runs cannot decide come back so.
                                       At raftgpu_follower_append: a MsgAppend with entries, or whose answer needs a term of
                                       the follower's log outside the caller's run: RawNode::step on the host */
 #define RAFTGPU_WIRE_MALFORMED 4u  /* not a protobuf message, a bad frame, or a group that is not allocated */
@@ -677,7 +679,8 @@ typedef struct raftgpu_wire_batch {
     /* 24-byte records that travel with the batch and are applied BEFORE the frames: the leader's own
      * RAFTGPU_REC_LOCAL events (append_entry / on_persist_entries are calls, not messages) and REJECTs whose
      * next_probe_index the host has resolved (RAFTGPU_WIRE_NEEDS_LOG of an earlier step).  At most one
-     * record per (group, peer) cell, verified on the GPU like raftgpu_step_begin_packed.  May be NULL / 0. */
+     * record per (group, peer) cell, verified on the GPU like raftgpu_step_begin_packed.  May be NULL / 0.
+     * On an arena with leader runs, a rejection the runs decide is applied from its frame and needs no record. */
     const raftgpu_append_resp *records;
     uint64_t n_records;
 } raftgpu_wire_batch;
@@ -694,6 +697,49 @@ int32_t raftgpu_wire_apply_device(raftgpu_arena *arena, void *stream, const void
  * raftgpu_step_wait returns.  raftgpu_step_wire_status: the status bytes of the last completed wire step. */
 int32_t raftgpu_step_begin_wire(raftgpu_arena *arena, const raftgpu_wire_batch *batch, uint32_t flags);
 int32_t raftgpu_step_wire_status(raftgpu_arena *arena, const uint8_t **status, uint64_t *n);
+
+/* ---- the leader's term runs: rejections decided in the wire step ---------- */
+
+/* A rejected MsgAppendResponse with log_term > 0 needs find_conflict_by_term(m.reject_hint, m.log_term) on the leader's
+ * log (raft.rs:1562, raft_log.rs:209-235).  The arena already knows the leader's own term: term(i) = term on
+ * [term_start, last_index] and 0 above last_index.  A row per group states up to two earlier term runs below
+ * term_start; with it raftgpu_wire_apply_device and raftgpu_step_begin_wire decide such a frame on the device whenever
+ * the walk ends inside what is known, and apply it as RAFTGPU_WIRE_OK with the result as next_probe_index.  The others
+ * stay RAFTGPU_WIRE_NEEDS_LOG, handled by the host as before.  Accepts never read the rows.
+ *
+ * A row is used only while its group is a leader (term_start != RAFTGPU_NO_TERM_START) with a non-zero term and
+ * (term, term_start) equal the row's anchor; any call that changes either (reset, become_leader, set_log_bounds,
+ * set_term, a vote-request pass's become_follower, ...) leaves the row inert until it is stated again.  Group alloc and
+ * free clear the row.  A wide pair's row is stated on its low half and read with the pair's term_start and the larger
+ * last_index.
+ *
+ * Opt-in: call before groups are allocated.  Memory: 48 bytes per group slot (48 MB per million).  An arena that does
+ * not call it behaves exactly as without the feature. */
+int32_t raftgpu_arena_enable_leader_runs(raftgpu_arena *arena);
+
+/* One group's row: 56 bytes.  Run 1 is [run_start[0], term_start - 1] at run_term[0], run 2 is [run_start[1],
+ * run_start[0] - 1] at run_term[1]; a run_start of 0 states no run.  Every stated run must still be readable by the
+ * leader's RaftLog::term (at or above first_index - 1): on compaction, restate the row or drop runs.  Fewer runs are
+ * never wrong; they leave more frames to the host. */
+typedef struct raftgpu_leader_runs {
+    uint32_t group;        /* the group (the low half of a wide pair) */
+    uint32_t reserved;     /* ignored */
+    uint64_t term;         /* the anchor: Raft::term and term_start of the leadership the runs belong to */
+    uint64_t term_start;
+    uint64_t run_start[2];
+    uint64_t run_term[2];
+} raftgpu_leader_runs;
+
+/* State rows for many groups (a store-wide election: right after the raftgpu_control list that makes them leaders, in
+ * either order).  status[i] per row, and a refused row is not stored:
+ *   RAFTGPU_ERR_RANGE    the group is not allocated, or is the high half of a wide pair;
+ *   RAFTGPU_ERR_INVALID  term is 0, term_start is 0 or RAFTGPU_NO_TERM_START, run 2 without run 1, starts that do not
+ *                        satisfy 0 < run_start[1] < run_start[0] < term_start where stated, or run terms that do not
+ *                        satisfy 0 < run_term[1] < run_term[0] < term where stated.
+ * Returns RAFTGPU_OK when the list ran (n == 0 included), RAFTGPU_ERR_INVALID for an arena without leader runs or a
+ * NULL rows / status with n > 0.  The rows take effect at the call, in submission order with steps in flight (like
+ * the control calls); synchronous.  A later row of the same group wins. */
+int32_t raftgpu_leader_runs_set(raftgpu_arena *arena, const raftgpu_leader_runs *rows, uint64_t n, int32_t *status);
 
 /* ---- heartbeat responses (SURVEY 8(f) rank 3, response side) ---------------- */
 

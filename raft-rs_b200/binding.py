@@ -60,6 +60,10 @@ FAPP_REJECT, FAPP_STALE = 0x2, 0x4
 FOLLOWER_LOG_DTYPE = np.dtype([("id", "<u8"), ("run_start", "<u8"), ("run_term", "<u8"), ("flags", "<u4"),
                                ("reserved", "<u4")])
 assert FOLLOWER_LOG_DTYPE.itemsize == 32
+# raftgpu_leader_runs_set: one group's leader runs (raftgpu_leader_runs)
+LEADER_RUNS_DTYPE = np.dtype([("group", "<u4"), ("reserved", "<u4"), ("term", "<u8"), ("term_start", "<u8"),
+                              ("run_start", "<u8", (2,)), ("run_term", "<u8", (2,))])
+assert LEADER_RUNS_DTYPE.itemsize == 56
 # raftgpu_follower_append_entries: an applied frame's extra bit and its record (raftgpu_follower_appended)
 FAPP_APPENDED = 0x8
 FOLLOWER_APPENDED_DTYPE = np.dtype([("first_index", "<u8"), ("last_index", "<u8"), ("run_start", "<u8"),
@@ -311,6 +315,8 @@ def lib() -> C.CDLL:
             "raftgpu_group_set_term": ([vp, u32, u64], i32),
             "raftgpu_control": ([vp, vp, u64, vp], i32),
             "raftgpu_arena_enable_inflights": ([vp, u32], i32),
+            "raftgpu_arena_enable_leader_runs": ([vp], i32),
+            "raftgpu_leader_runs_set": ([vp, vp, u64, vp], i32),
             "raftgpu_inflights_get": ([vp, u32, u32, C.POINTER(u32), C.POINTER(u32), vp, u32], i32),
             "raftgpu_heartbeat_resp_device": ([vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_heartbeat_resp": ([vp, vp, u64, vp], i32),
@@ -852,6 +858,18 @@ class Arena:
         res = np.zeros(len(recs), dtype=np.uint8)
         self._ck(self._L.raftgpu_heartbeat_resp(self._h, recs.ctypes.data, len(recs), res.ctypes.data), "heartbeat_resp")
         return res
+
+    # -- the leader's term runs (include/raftgpu.h)
+    def enable_leader_runs(self):
+        self._ck(self._L.raftgpu_arena_enable_leader_runs(self._h), "arena_enable_leader_runs")
+
+    def leader_runs_set(self, rows: np.ndarray) -> np.ndarray:
+        """raftgpu_leader_runs_set: LEADER_RUNS_DTYPE rows -> the i32 status of each row (a refused row is not stored;
+        only the call's own failure raises)."""
+        rows = np.ascontiguousarray(rows, dtype=LEADER_RUNS_DTYPE)
+        st = np.zeros(len(rows), dtype=np.int32)
+        self._ck(self._L.raftgpu_leader_runs_set(self._h, rows.ctypes.data, len(rows), st.ctypes.data), "leader_runs_set")
+        return st
 
     # -- ReadIndex, ReadOnlyOption::Safe (include/raftgpu.h)
     def enable_read_index(self, max_pending: int = 8):

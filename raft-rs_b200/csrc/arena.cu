@@ -271,6 +271,12 @@ struct raftgpu_arena {
     // rq_flag[1] = the touched list's length
     unsigned long long *rq_hit = nullptr;
     uint32_t *rq_list = nullptr, *rq_flag = nullptr;
+    // leader runs (raftgpu_arena_enable_leader_runs): the rows [cap], nullptr = off; raftgpu_leader_runs_set's device copy
+    // of a list (lr_stage_n rows) and, per group, its position in the list being built (UINT32_MAX = none)
+    LeaderRuns *lr_rows = nullptr;
+    raftgpu_leader_runs *lr_stage = nullptr;
+    uint64_t lr_stage_n = 0;
+    std::vector<uint32_t> lr_pos;
     PassScratch pass[kPassCount];  // the wire passes' scratch, one each
     // group allocation
     std::mutex alloc_mu;
@@ -648,6 +654,8 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->rq_hit);
     cudaFree(a->rq_list);
     cudaFree(a->rq_flag);
+    cudaFree(a->lr_rows);
+    cudaFree(a->lr_stage);
     for (PassScratch &p : a->pass) {
         cudaFree(p.first);
         cudaFree(p.buf);
@@ -821,6 +829,16 @@ int32_t read_mark(raftgpu_arena *a, uint32_t first, uint32_t n, uint32_t value) 
     if (!a->cols.rq_cap || n == 0) return RAFTGPU_OK;
     const uint32_t blocks = std::min<uint32_t>(div_up(n, 256), 8u * static_cast<uint32_t>(a->sm_count));
     return sync_op(a, [&](cudaStream_t st) { read_mark_kernel<<<blocks, 256, 0, st>>>(a->cols.rq_hc, first, n, value); });
+}
+
+// Leader runs (arenas with raftgpu_arena_enable_leader_runs only): the rows of groups [first, first + n) are cleared, so
+// that a slot that is allocated or freed matches no anchor.
+int32_t runs_clear(raftgpu_arena *a, uint32_t first, uint32_t n) {
+    if (!a->lr_rows || n == 0) return RAFTGPU_OK;
+    CK(a, cudaSetDevice(a->device));
+    CK(a, cudaMemsetAsync(a->lr_rows + first, 0, sizeof(LeaderRuns) * n, a->s_compute));
+    CK(a, cudaStreamSynchronize(a->s_compute));
+    return RAFTGPU_OK;
 }
 
 struct ColumnDesc {
@@ -1367,5 +1385,6 @@ extern "C" {
 #include "abi_vote_wire.inc"
 #include "abi_vote_request.inc"
 #include "abi_app_follow.inc"
+#include "abi_leader_runs.inc"
 
 }  // extern "C"

@@ -16,7 +16,8 @@
 // (apply_one, raft.rs:1663-1743) and reports every later one as RAFTGPU_WIRE_DUP for the next batch.
 // What cannot be decided here goes back to the host as a status: other message types, a term that is not
 // the group's (Raft::step's term rules), a rejection with log_term > 0 (its next_probe_index needs the
-// leader's log, raft.rs:1562-1661), malformed bytes.
+// leader's log, raft.rs:1562-1661) unless the leader's term runs decide it (the <true> kernels, DESIGN 3.18),
+// malformed bytes.
 //
 // HBM-bound byte work: every block stages the contiguous byte range of its 256 frames into shared memory
 // with 16-byte loads (frames are ~26 bytes, unaligned) and the threads parse from there.
@@ -280,9 +281,64 @@ __device__ __forceinline__ uint32_t wire_open(const WireSrc &w, const WireStage 
     return RAFTGPU_WIRE_OK;
 }
 
-// Frame i: its status before the duplicate rule, the record, the REJECT's hint / request_snapshot.
-__device__ __forceinline__ uint32_t wire_frame(const Columns &c, const WireSrc &w, const WireStage &s, const uint8_t *stage,
-                                               uint32_t i, RecRegs &rec, uint64_t &hint, uint64_t &request_snapshot) {
+// The leader's term runs (raftgpu_arena_enable_leader_runs, DESIGN 3.18): one row per group slot, 48 bytes, read as three
+// 16-byte loads -- {term, term_start} (the anchor), {run_start[0], run_start[1]}, {run_term[0], run_term[1]}.  Run 1
+// is [run_start[0], term_start - 1] at run_term[0], run 2 [run_start[1], run_start[0] - 1] at run_term[1]; a start of 0
+// is not stated.  raftgpu_leader_runs_set stores only rows with 0 < run_start[1] < run_start[0] < term_start and
+// 0 < run_term[1] < run_term[0] < term where stated.  A pair's row lives on its low half.
+struct LeaderRuns {
+    ulonglong2 anchor, start, term;
+};
+
+// next_probe_index = find_conflict_by_term(h, lt) (raft.rs:1562, raft_log.rs:209-235) of group g's leader, from the
+// arena and its row: term(i) = term on [term_start, last_index] (DESIGN 1), run_term[k] on run k, 0 at 0.  A pair reads
+// its low half's term, term_start and row, and the larger last_index (as DESIGN 3.15).  false = undecided: the row is
+// not anchored to the group's leadership (a leader, a term, the row's (term, term_start)), or the walk leaves the stated
+// runs at an index whose bound -- the lowest stated run's term, terms being monotone -- is above lt.
+__device__ __forceinline__ bool wire_probe_by_runs(const Columns &c, const LeaderRuns *__restrict__ runs, uint32_t g,
+                                                   uint64_t h, uint64_t lt, uint64_t &out) {
+    const uint32_t meta = c.meta[g];
+    const uint32_t lo = (meta & RAFTGPU_META_WIDE_HI) ? g - 1 : g;
+    const uint64_t ts = c.term_start[lo], term = c.term[lo];
+    if (ts == RAFTGPU_NO_TERM_START || term == 0) return false;
+    const ulonglong2 anchor = runs[lo].anchor;
+    if (anchor.x != term || anchor.y != ts) return false;
+    uint64_t last = c.last_index[lo];
+    if (meta & (RAFTGPU_META_WIDE_LO | RAFTGPU_META_WIDE_HI)) last = umax64(last, c.last_index[lo + 1]);
+    out = h;
+    if (h > last) return true;  // raft_log.rs:213-221
+    // the segments from the top: [ts, last] at term, run 1, run 2; i walks down to the first one whose term is <= lt
+    uint64_t i = h;
+    if (term <= lt) return true;  // (i >= ts, or i below ts whose term is <= term)
+    i = umin64(i, ts - 1);
+    uint64_t bound = term;  // every index at or below i has a term <= bound
+    const ulonglong2 rs = runs[lo].start, rt = runs[lo].term;
+    if (rs.x) {
+        if (i >= rs.x && rt.x <= lt) {
+            out = i;
+            return true;
+        }
+        bound = rt.x;
+        if (rs.x <= i) i = rs.x - 1;
+        if (rs.y) {
+            if (i >= rs.y && rt.y <= lt) {
+                out = i;
+                return true;
+            }
+            bound = rt.y;
+            if (rs.y <= i) i = rs.y - 1;
+        }
+    }
+    out = i;
+    return i == 0 || bound <= lt;  // term(0) = 0 < lt
+}
+
+// Frame i: its status before the duplicate rule, the record, the REJECT's hint / request_snapshot.  kRuns: a rejection
+// with log_term > 0 is decided from the leader's runs (wire_probe_by_runs) where they say enough.
+template <bool kRuns>
+__device__ __forceinline__ uint32_t wire_frame(const Columns &c, const LeaderRuns *runs, const WireSrc &w, const WireStage &s,
+                                               const uint8_t *stage, uint32_t i, RecRegs &rec, uint64_t &hint,
+                                               uint64_t &request_snapshot) {
     uint32_t hdr;
     const uint8_t *msg;
     WireMsg m;
@@ -291,39 +347,56 @@ __device__ __forceinline__ uint32_t wire_frame(const Columns &c, const WireSrc &
     if (m.msg_type != 4u) return RAFTGPU_WIRE_SKIP_TYPE;  // MsgAppendResponse, eraftpb.proto:54
     const uint64_t gterm = c.term[group];
     if (gterm != 0 && m.term != gterm) return RAFTGPU_WIRE_TERM;
-    if (m.reject && m.log_term > 0) return RAFTGPU_WIRE_NEEDS_LOG;  // raft.rs:1562
+    uint64_t h = m.reject_hint;  // raft.rs:1560
+    if (m.reject && m.log_term > 0) {  // raft.rs:1562
+        if constexpr (!kRuns) return RAFTGPU_WIRE_NEEDS_LOG;
+        else if (!wire_probe_by_runs(c, runs, group, m.reject_hint, m.log_term, h)) return RAFTGPU_WIRE_NEEDS_LOG;
+    }
     rec.w0 = static_cast<uint64_t>(group) | (static_cast<uint64_t>(slot) << 32) |
              (static_cast<uint64_t>(m.reject ? RAFTGPU_REC_REJECT : 0u) << 40);
     rec.index = m.index;
     rec.commit = m.commit;
-    hint = m.reject_hint;                  // raft.rs:1560
+    hint = h;
     request_snapshot = m.request_snapshot;  // raft.rs:1709
     return RAFTGPU_WIRE_OK;
 }
 
-// Pass 1: classify every frame; first_frame[cell] = the lowest frame index that wants the cell.
-__global__ void __launch_bounds__(kWireThreads) wire_scan_kernel(Columns c, WireSrc w, uint8_t *__restrict__ status,
-                                                                 uint32_t *__restrict__ first_frame) {
+// Pass 1: classify every frame; first_frame[cell] = the lowest frame index that wants the cell.  runs: the arena's rows
+// (kRuns only; the last parameter, so that the others keep their offsets).
+template <bool kRuns>
+__device__ __forceinline__ void wire_scan(const Columns &c, const WireSrc &w, uint8_t *__restrict__ status,
+                                          uint32_t *__restrict__ first_frame, const LeaderRuns *__restrict__ runs) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
     WireStage s;
     const uint32_t i = wire_block_frame(w, stage, s);
     if (i == kNoFrame) return;
     RecRegs rec;
     uint64_t hint, snap;
-    const uint32_t st = wire_frame(c, w, s, stage, i, rec, hint, snap);
+    const uint32_t st = wire_frame<kRuns>(c, runs, w, s, stage, i, rec, hint, snap);
     status[i] = static_cast<uint8_t>(st << 4);
     if (st == RAFTGPU_WIRE_OK) {
         const uint32_t g = static_cast<uint32_t>(rec.w0), slot = static_cast<uint32_t>(rec.w0 >> 32) & 0xffu;
         if (slot < kSlots) atomicMin(&first_frame[static_cast<size_t>(slot) * c.cap + g], i);
     }
 }
+// With the runs, at least 6 blocks per SM, so ptxas works to a cap of 40 registers (it takes 35, allocated as 40: 6 blocks
+// of 256 threads per SM, where the 32-register <false> kernel fits 8).  At __launch_bounds__(kWireThreads) alone ptxas
+// settles on 32 registers and spills 24 bytes, as it does in hb_wire_scan_kernel.
+template <bool kRuns>
+__global__ void __launch_bounds__(kWireThreads, kRuns ? 6 : 0) wire_scan_kernel(Columns c, WireSrc w, uint8_t *__restrict__ status,
+                                                                 uint32_t *__restrict__ first_frame,
+                                                                 const LeaderRuns *__restrict__ runs) {
+    wire_scan<kRuns>(c, w, status, first_frame, runs);
+}
 
 // Pass 2: the first frame of every cell is applied (raft.rs:1663-1743), later ones are RAFTGPU_WIRE_DUP.
 // status[i] = wire status << 4 | RAFTGPU_RES_* of the applied message.
+template <bool kRuns>
 __global__ void __launch_bounds__(kWireThreads) wire_apply_kernel(Columns c, WireSrc w, uint8_t *__restrict__ status,
                                                                   const uint32_t *__restrict__ first_frame,
                                                                   unsigned long long *__restrict__ counters,
-                                                                  uint32_t *__restrict__ dup_count) {
+                                                                  uint32_t *__restrict__ dup_count,
+                                                                  const LeaderRuns *__restrict__ runs) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
     uint32_t local[5] = {0, 0, 0, 0, 0};  // records, updates, rejects, decrements, no_progress
     // the prologue of wire_block_frame written out: through the helper, ptxas spills in this kernel
@@ -335,7 +408,7 @@ __global__ void __launch_bounds__(kWireThreads) wire_apply_kernel(Columns c, Wir
         if (i < last && status[i] == (RAFTGPU_WIRE_OK << 4)) {
             RecRegs rec;
             uint64_t hint, snap;
-            wire_frame(c, w, s, stage, i, rec, hint, snap);  // same verdict as in the scan pass
+            wire_frame<kRuns>(c, runs, w, s, stage, i, rec, hint, snap);  // same verdict as in the scan pass
             const uint32_t g = static_cast<uint32_t>(rec.w0), slot = static_cast<uint32_t>(rec.w0 >> 32) & 0xffu;
             if (slot < kSlots && first_frame[static_cast<size_t>(slot) * c.cap + g] != i) {
                 status[i] = static_cast<uint8_t>(RAFTGPU_WIRE_DUP << 4);
@@ -350,6 +423,15 @@ __global__ void __launch_bounds__(kWireThreads) wire_apply_kernel(Columns c, Wir
     }
     const int which[5] = {kCntRecords, kCntUpdates, kCntRejects, kCntDecrements, kCntNoProgress};
     block_flush_counts<5>(local, which, counters, nullptr);
+}
+
+// Clears or states leader-run rows: rows[i] of the list go to row group[i] (raftgpu_leader_runs_set, after its checks).
+__global__ void leader_runs_set_kernel(LeaderRuns *__restrict__ dst, const raftgpu_leader_runs *__restrict__ rows, uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const raftgpu_leader_runs r = rows[i];
+    dst[r.group] = LeaderRuns{make_ulonglong2(r.term, r.term_start), make_ulonglong2(r.run_start[0], r.run_start[1]),
+                              make_ulonglong2(r.run_term[0], r.run_term[1])};
 }
 
 // ---------------------------------------------------------------------------
