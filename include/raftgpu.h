@@ -698,6 +698,33 @@ int32_t raftgpu_wire_apply_device(raftgpu_arena *arena, void *stream, const void
 int32_t raftgpu_step_begin_wire(raftgpu_arena *arena, const raftgpu_wire_batch *batch, uint32_t flags);
 int32_t raftgpu_step_wire_status(raftgpu_arena *arena, const uint8_t **status, uint64_t *n);
 
+/* ---- waves: pipelined frames of one cell or group in one call -------------- */
+
+/* A leader sends as many MsgAppend to a peer as its inflight window allows (raft.rs:1755-1761), so one received batch
+ * may hold several MsgAppend for one follower group, and several MsgAppendResponse for one leader cell.  At `waves` = k
+ * the passes below decide up to k of them per cell (the wire step: raftgpu_wire_apply_device, raftgpu_step_begin_wire)
+ * or per group (raftgpu_follower_append[_device], raftgpu_follower_append_entries[_device]) in one call, in arrival
+ * order.  Let F1 be every frame of the batch; run j is the pass as it is at one wave, over the frames Fj in their batch
+ * order; a call at k waves returns what up to k runs return:
+ *   - the wire step: Fj+1 = the frames run j returned RAFTGPU_WIRE_DUP (a frame that is not OK claims no cell: the
+ *     host's resubmission with no host work between);
+ *   - the follower's append passes: Fj+1 = the frames run j returned DUP, but for those of groups whose claiming frame in
+ *     run j was RAFTGPU_WIRE_NEEDS_LOG or RAFTGPU_WIRE_COMMIT_RANGE: they stay DUP, as the host handles the claimant
+ *     first.  A frame of a later run is decided against the group's state after the earlier runs: committed,
+ *     last_index and (the _device form with entries) the table's run.
+ * A frame's status byte is that of the last run that saw it (a frame still DUP after run k stays DUP); its `from` and
+ * appended record come from the run that decided it, zero for a frame left DUP.  The responses of every run go to one
+ * output in frame order, the totals summed: a frame is answered at most once, so raftgpu_follower_append_bound(n)
+ * still bounds them.  The wire step runs one Raft::maybe_commit pass after the last run; its counters count every run.
+ *
+ * 1 (the default) is the passes as they are.  Each wave costs two kernel launches whether or not it finds frames, so
+ * k bounds the cost of a call; a cell or group with more frames than k gets DUP for the rest.  The heartbeat and vote
+ * passes keep one frame per cell or group: they bring at most one message per peer per tick or election.
+ * raftgpu_arena_set_wire_waves takes effect for the calls queued after it (a step already begun keeps its value);
+ * RAFTGPU_ERR_INVALID for a NULL arena, 0 or more than RAFTGPU_WIRE_WAVES_MAX. */
+#define RAFTGPU_WIRE_WAVES_MAX 64u
+int32_t raftgpu_arena_set_wire_waves(raftgpu_arena *arena, uint32_t waves);
+
 /* ---- the leader's term runs: rejections decided in the wire step ---------- */
 
 /* A rejected MsgAppendResponse with log_term > 0 needs find_conflict_by_term(m.reject_hint, m.log_term) on the leader's

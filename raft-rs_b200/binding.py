@@ -47,6 +47,7 @@ WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WI
 WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat (ROLE also raftgpu_vote_wire)
 WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire, raftgpu_vote_request_wire
 WIRE_IGNORED = 10  # raftgpu_vote_request_wire only
+WIRE_WAVES_MAX = 64  # raftgpu_arena_set_wire_waves
 # raftgpu_vote_request_wire: the caller's table (raftgpu_voter), its flags, and the low nibble of an applied frame
 VOTER_SELECT, VOTER_LEADER, VOTER_LEASE = 0x1, 0x2, 0x4
 VREQ_GRANTED, VREQ_VOTED, VREQ_BUMPED = 0x1, 0x2, 0x4
@@ -317,6 +318,7 @@ def lib() -> C.CDLL:
             "raftgpu_arena_enable_inflights": ([vp, u32], i32),
             "raftgpu_arena_enable_leader_runs": ([vp], i32),
             "raftgpu_leader_runs_set": ([vp, vp, u64, vp], i32),
+            "raftgpu_arena_set_wire_waves": ([vp, u32], i32),
             "raftgpu_inflights_get": ([vp, u32, u32, C.POINTER(u32), C.POINTER(u32), vp, u32], i32),
             "raftgpu_heartbeat_resp_device": ([vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_heartbeat_resp": ([vp, vp, u64, vp], i32),
@@ -862,6 +864,11 @@ class Arena:
     # -- the leader's term runs (include/raftgpu.h)
     def enable_leader_runs(self):
         self._ck(self._L.raftgpu_arena_enable_leader_runs(self._h), "arena_enable_leader_runs")
+
+    def set_wire_waves(self, waves: int) -> int:
+        """raftgpu_arena_set_wire_waves: frames of a cell (the wire step) or group (the follower's append passes)
+        decided per call.  Returns the status (RAFTGPU_ERR_INVALID for 0 or more than WIRE_WAVES_MAX)."""
+        return int(self._L.raftgpu_arena_set_wire_waves(self._h, waves))
 
     def leader_runs_set(self, rows: np.ndarray) -> np.ndarray:
         """raftgpu_leader_runs_set: LEADER_RUNS_DTYPE rows -> the i32 status of each row (a refused row is not stored;

@@ -277,6 +277,9 @@ struct raftgpu_arena {
     raftgpu_leader_runs *lr_stage = nullptr;
     uint64_t lr_stage_n = 0;
     std::vector<uint32_t> lr_pos;
+    // raftgpu_arena_set_wire_waves: frames of a cell (the wire step) or group (the follower's append passes) decided per
+    // call, read by each call as it is queued
+    uint32_t wire_waves = 1;
     PassScratch pass[kPassCount];  // the wire passes' scratch, one each
     // group allocation
     std::mutex alloc_mu;
@@ -1076,10 +1079,13 @@ int32_t reply_check(raftgpu_arena *a, uint64_t n_bytes, uint64_t n, uint64_t fra
 // pass's scratch (u64 words) is carved into one record per frame and the {responses, bytes} of every block, its
 // first-frame table (first_n u32) reset, and four passes run with kWireThreads frames per block: passes(blocks, recs,
 // first, blk) launches the pass's scan and apply kernels, block_starts_kernel<2> turns the block sums into block starts,
-// the totals and the last offset, reply_write_kernel<P> writes the responses.
+// the totals and the last offset, reply_write_kernel<P> writes the responses.  extra_words: u64 words behind blk that
+// the pass uses as it likes (the follower's wave lists); the passes' launch errors, and those of anything else they
+// queue, are reported after the last launch.
 template <class P, typename Passes>
 int32_t reply_run(raftgpu_arena *a, cudaStream_t st, PassScratch &scratch, uint64_t n, const uint8_t *d_status,
-                  uint8_t *d_resp_bytes, uint32_t *d_resp_offsets, uint64_t *d_totals, size_t first_n, Passes &&passes) {
+                  uint8_t *d_resp_bytes, uint32_t *d_resp_offsets, uint64_t *d_totals, size_t first_n, Passes &&passes,
+                  uint64_t extra_words = 0) {
     using Rec = typename P::Rec;
     if (n == 0) {
         CK(a, cudaMemsetAsync(d_totals, 0, 16, st));
@@ -1087,7 +1093,7 @@ int32_t reply_run(raftgpu_arena *a, cudaStream_t st, PassScratch &scratch, uint6
         return RAFTGPU_OK;
     }
     const uint32_t nb = div_up(n, kWireThreads);
-    const int32_t rc = pass_scratch(a, st, scratch, first_n, (sizeof(Rec) / 8) * n + nb);
+    const int32_t rc = pass_scratch(a, st, scratch, first_n, (sizeof(Rec) / 8) * n + nb + extra_words);
     if (rc != RAFTGPU_OK) return rc;
     Rec *recs = reinterpret_cast<Rec *>(scratch.buf);
     uint32_t *blk = reinterpret_cast<uint32_t *>(scratch.buf + (sizeof(Rec) / 8) * n);
@@ -1149,6 +1155,56 @@ int32_t reply_host(raftgpu_arena *a, const void *bytes, uint64_t n_bytes, const 
     rc = f.back(resp_offsets, roff_at, 4 * (totals[0] + 1));
     if (rc == RAFTGPU_OK) rc = f.back(resp_bytes, rbytes_at, totals[1]);
     return rc == RAFTGPU_OK ? f.wait() : rc;
+}
+
+// ---- waves (DESIGN 3.19): a pass at raftgpu_arena_set_wire_waves > 1 repeats its decision over the frames it left DUP.
+// Its scratch holds two lists of n frames, used in turn, and one count per wave, zeroed on st before wave 1; a pass at
+// one wave keeps none.  Wave j >= 2 reads the list wave j - 1 wrote, on a grid of grid_apply blocks at most: its
+// kernels loop over whatever the list holds, and return at once when it is empty.
+uint64_t wave_list_words(uint64_t n, uint32_t waves) { return waves > 1 ? (2 * n + waves + 1) / 2 : 0; }
+
+// Wave j's lists (0-based; wave 0 reads the whole batch).
+WaveIo wave_io(uint32_t *lists, uint64_t n, uint32_t j) {
+    uint32_t *cnt = lists + 2 * n;
+    return WaveIo{j ? lists + ((j - 1) & 1u) * n : nullptr, j ? cnt + j - 1 : nullptr, lists + (j & 1u) * n, cnt + j};
+}
+
+// The wire step (abi_wire.inc): wave 1 is wire_scan_kernel and wire_wave_apply_kernel over the batch, each later wave
+// wire_wave_claim_kernel<false> and wire_wave_apply_kernel over its list.
+template <bool kRuns>
+int32_t launch_wire_waves(raftgpu_arena *a, cudaStream_t st, const WireSrc &w, uint8_t *d_status, uint32_t *first,
+                          uint32_t *lists, uint32_t waves) {
+    const LeaderRuns *runs = kRuns ? a->lr_rows : nullptr;
+    const uint32_t blocks = div_up(w.n, kWireThreads), grid = std::min<uint32_t>(blocks, a->grid_apply);
+    CK(a, cudaMemsetAsync(lists + 2ull * w.n, 0, 4ull * waves, st));
+    wire_scan_kernel<kRuns><<<blocks, kWireThreads, 0, st>>>(a->cols, w, d_status, first, runs);
+    for (uint32_t j = 0; j < waves; j++) {
+        const WaveIo io = wave_io(lists, w.n, j);
+        if (j) wire_wave_claim_kernel<false><<<grid, kWireThreads, 0, st>>>(w, a->cap, first, io.in, io.in_n);
+        wire_wave_apply_kernel<kRuns><<<j ? grid : blocks, kWireThreads, 0, st>>>(a->cols, w, d_status, first, a->d_counters,
+                                                                                 runs, io);
+    }
+    CKL(a);
+    return RAFTGPU_OK;
+}
+
+// The follower's append passes (abi_app_follow.inc), after afw_scan_kernel<kAppend>: afw_wave_apply_kernel over the
+// batch, then wire_wave_claim_kernel<true> and afw_wave_apply_kernel over each later wave's list.  Called from
+// reply_run's passes, which reports the launch errors.
+template <bool kAppend>
+void launch_afw_waves(raftgpu_arena *a, cudaStream_t st, const WireSrc &w, const raftgpu_follower_log *d_log, uint8_t *d_status,
+                      AfwRec *recs, uint32_t *first, uint64_t *d_from, uint32_t *blk, raftgpu_follower_appended *d_appended,
+                      uint32_t *lists, uint32_t waves) {
+    // (only the <true> kernel writes the table: raftgpu_follower_append_entries_device's, which is not const)
+    raftgpu_follower_log *logs = const_cast<raftgpu_follower_log *>(d_log);
+    const uint32_t blocks = div_up(w.n, kWireThreads), grid = std::min<uint32_t>(blocks, a->grid_apply);
+    cudaMemsetAsync(lists + 2ull * w.n, 0, 4ull * waves, st);
+    for (uint32_t j = 0; j < waves; j++) {
+        const WaveIo io = wave_io(lists, w.n, j);
+        if (j) wire_wave_claim_kernel<true><<<grid, kWireThreads, 0, st>>>(w, a->cap, first, io.in, io.in_n);
+        afw_wave_apply_kernel<kAppend><<<j ? grid : blocks, kWireThreads, 0, st>>>(a->cols, w, d_status, recs, first, d_from,
+                                                                                  blk, logs, d_appended, io);
+    }
 }
 
 // ---- the broadcast pipeline (DESIGN 3.11): a pass that writes a leader's frames from the arena

@@ -227,6 +227,124 @@ __global__ void __launch_bounds__(kWireThreads) afw_apply_kernel(Columns c, uint
     block_sums<2, kWireThreads>({resp, bytes}, blk);
 }
 
+// Waves (raftgpu_arena_set_wire_waves, DESIGN 3.19): the decision repeated over the frames it left DUP, each wave against
+// the state the waves before it left (committed, last_index, the table's run).  Wave 1 is afw_scan_kernel and
+// afw_wave_apply_kernel over the batch; a later wave is wire_wave_claim_kernel<true> (k_wire.cuh) and
+// afw_wave_apply_kernel over the list (WaveIo) the wave before it wrote, which decides the claimant only.  A group's claimant leaves the group's first_frame entry kNoFrame
+// when it was applied, kWaveStop when it was not (NEEDS_LOG, COMMIT_RANGE): the group's later frames then stay DUP, as
+// the host resubmits them only after it has handled the claimant.  block_starts_kernel<2> and reply_write_kernel run
+// once after the last wave.
+
+// Frame i after its wave's scan, as afw_apply_kernel decides it, with the claimant's mark on the group's entry.  true =
+// DUP and on the next wave's list; *resp_bytes = the bytes of its response (0: none), *from = m.from when applied.
+template <bool kAppend>
+__device__ __forceinline__ bool afw_wave_frame(const Columns &c, uint32_t i, uint8_t *__restrict__ status, AfwRec *__restrict__ recs,
+                                               uint32_t *__restrict__ first_frame, raftgpu_follower_log *__restrict__ logs,
+                                               raftgpu_follower_appended *__restrict__ appended, uint64_t &from,
+                                               uint32_t &resp_bytes) {
+    const uint32_t st = status[i] >> 4;
+    if (st != RAFTGPU_WIRE_OK && st != RAFTGPU_WIRE_NEEDS_LOG && st != RAFTGPU_WIRE_COMMIT_RANGE) return false;
+    const uint64_t w0 = recs[i].w0;
+    const uint32_t g = static_cast<uint32_t>(w0) >> 4;
+    if (first_frame[g] != i) {  // (reads i, kNoFrame or kWaveStop: the claimant writes its mark during this pass)
+        status[i] = static_cast<uint8_t>(RAFTGPU_WIRE_DUP << 4);
+        if constexpr (kAppend) {
+            if (st == RAFTGPU_WIRE_OK && (w0 & kAfwAppend)) appended[i] = raftgpu_follower_appended{};
+        }
+        return true;
+    }
+    first_frame[g] = st == RAFTGPU_WIRE_OK ? kNoFrame : kWaveStop;
+    if (st != RAFTGPU_WIRE_OK) return false;
+    AfwRec r = recs[i];
+    if constexpr (kAppend) {
+        if (w0 & kAfwAppend) {  // truncate_and_append: last_index = m.index + entries
+            if (c.meta[g] & RAFTGPU_META_WIDE_LO) {
+                wide_sync(c, g);
+                c.last_index[g + 1] = r.index;
+            }
+            c.last_index[g] = r.index;
+            logs[g].run_start = r.reject_hint;
+            logs[g].run_term = r.log_term;
+            r.log_term = r.reject_hint = 0;  // the response carries neither
+            recs[i].log_term = 0;
+            recs[i].reject_hint = 0;
+        }
+    }
+    if (w0 & kAfwCommit) {
+        if (c.meta[g] & RAFTGPU_META_WIDE_LO) {
+            wide_sync(c, g);
+            commit_to_group(c, g + 1, r.commit);
+        }
+        commit_to_group(c, g, r.commit);
+        r.commit = c.committed[g];  // raft.rs:2446 to_send.commit = raft_log.committed
+        recs[i].commit = r.commit;
+    }
+    uint32_t low = RAFTGPU_RES_OK | ((w0 & kAfwReject) ? RAFTGPU_FAPP_REJECT : 0u) | ((w0 & kAfwStale) ? RAFTGPU_FAPP_STALE : 0u);
+    if constexpr (kAppend) low |= (w0 & kAfwAppend) ? RAFTGPU_FAPP_APPENDED : 0u;
+    status[i] = static_cast<uint8_t>((RAFTGPU_WIRE_OK << 4) | low);
+    from = r.to;
+    resp_bytes = afw_len(r);
+    return false;
+}
+
+// The apply pass of a wave.  io.in == nullptr (wave 1): every frame of the batch after afw_scan_kernel, one per thread,
+// and blk written as afw_apply_kernel writes it; else the frames of io.in over a grid-stride loop, the claimant of each
+// group decided and applied, each response added to its frame's block in blk (a wave that finds no frame returns at
+// once).  Every DUP frame goes on io.out.  logs: the table, written by the <true> kernel only.
+template <bool kAppend>
+__global__ void __launch_bounds__(kWireThreads) afw_wave_apply_kernel(Columns c, WireSrc w, uint8_t *__restrict__ status,
+                                                                      AfwRec *__restrict__ recs, uint32_t *__restrict__ first_frame,
+                                                                      uint64_t *__restrict__ from_out, uint32_t *__restrict__ blk,
+                                                                      raftgpu_follower_log *__restrict__ logs,
+                                                                      raftgpu_follower_appended *__restrict__ appended,
+                                                                      WaveIo io) {
+    if (!io.in) {
+        const uint32_t i = blockIdx.x * kWireThreads + threadIdx.x;
+        uint32_t bytes = 0;
+        bool dup = false;
+        if (i < w.n) {
+            uint64_t from = 0;
+            dup = afw_wave_frame<kAppend>(c, i, status, recs, first_frame, logs, appended, from, bytes);
+            if (from_out) from_out[i] = from;
+        }
+        wave_enlist(io, dup, i);
+        block_sums<2, kWireThreads>({bytes ? 1u : 0u, bytes}, blk);
+        return;
+    }
+    const uint32_t m = *io.in_n;
+    const WireStage s{0, 0, 0, false};
+    for (uint32_t k0 = blockIdx.x * kWireThreads; k0 < m; k0 += gridDim.x * kWireThreads) {  // (uniform per warp)
+        const uint32_t k = k0 + threadIdx.x, i = k < m ? io.in[k] : kNoFrame;
+        uint32_t bytes = 0;
+        bool dup = false;
+        bool claim = false;
+        if (i != kNoFrame) {
+            // A listed frame is DUP with a zero appended record and from.  One that does not claim stays so, and leaves
+            // the lists once its group is stopped (kWaveStop, written before or during this pass).
+            const uint32_t f = first_frame[wire_header(w, i) >> 4];
+            claim = f == i;
+            dup = !claim && f != kWaveStop;
+        }
+        if (claim) {  // afw_scan_kernel's decision, then afw_apply_kernel's
+            AfwRec r;
+            raftgpu_follower_appended ap{};
+            const uint32_t st = afw_frame<kAppend>(c, w, logs, s, nullptr, i, r, ap);
+            status[i] = static_cast<uint8_t>(st << 4);
+            if constexpr (kAppend) appended[i] = ap;
+            if (st == RAFTGPU_WIRE_OK) recs[i] = r;
+            else recs[i].w0 = r.w0;  // (NEEDS_LOG, COMMIT_RANGE: a listed frame reaches the decision)
+            uint64_t from = 0;
+            afw_wave_frame<kAppend>(c, i, status, recs, first_frame, logs, appended, from, bytes);
+            if (from_out) from_out[i] = from;
+            if (bytes) {
+                atomicAdd(&blk[2 * (i / kWireThreads)], 1u);
+                atomicAdd(&blk[2 * (i / kWireThreads) + 1], bytes);
+            }
+        }
+        wave_enlist(io, dup, i);
+    }
+}
+
 // Pass 4 is reply_write_kernel<AfwReply> (k_wire.cuh): the frames the apply pass marked RAFTGPU_RES_OK answer.
 struct AfwReply {
     using Rec = AfwRec;

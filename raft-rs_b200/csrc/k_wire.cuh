@@ -425,6 +425,102 @@ __global__ void __launch_bounds__(kWireThreads) wire_apply_kernel(Columns c, Wir
     block_flush_counts<5>(local, which, counters, nullptr);
 }
 
+// ---------------------------------------------------------------------------
+// Waves (raftgpu_arena_set_wire_waves, DESIGN 3.19): the pass above repeated over the frames it left DUP, in their batch
+// order, until `waves` runs are done or no frame is left.  Wave 1 is the scan kernel above and wire_wave_apply_kernel
+// over the whole batch; every later wave is wire_wave_claim_kernel<false> and wire_wave_apply_kernel over the list the wave
+// before it wrote, so its cost follows its frames, not the batch or the arena.  The first-frame table is filled with
+// 0xff once per call: the frame that takes a cell clears the cell's entry again, so the next wave finds it free.
+// kNoFrame = free; kWaveStop (k_app_follow.cuh's waves only) = the group's claimant was not applied.
+constexpr uint32_t kWaveStop = 0xfffffffeu;
+
+// A wave's frames: its list (nullptr = the whole batch, wave 1) and count, and the list and count of the frames it
+// leaves DUP for the next wave.
+struct WaveIo {
+    const uint32_t *in, *in_n;
+    uint32_t *out, *out_n;
+};
+
+// Every lane of a full warp: frame i goes on the next wave's list when dup.
+__device__ __forceinline__ void wave_enlist(const WaveIo &io, bool dup, uint32_t i) {
+    const uint32_t at = warp_reserve(io.out_n, dup ? 1u : 0u);
+    if (dup) io.out[at] = i;
+}
+
+// The u32 LE header of frame i, read from the batch (a frame on a wave list was opened by wave 1).
+__device__ __forceinline__ uint32_t wire_header(const WireSrc &w, uint32_t i) {
+    const uint8_t *p = w.bytes + w.offsets[i];
+    return p[0] | (static_cast<uint32_t>(p[1]) << 8) | (static_cast<uint32_t>(p[2]) << 16) | (static_cast<uint32_t>(p[3]) << 24);
+}
+
+// Wave j >= 2, pass 1: every frame on the list claims its cell (kGroup: its group, k_app_follow.cuh's waves, unless the
+// group is stopped).  A listed frame reached the decision in every wave before -- what it is decided on beyond that
+// (committed, last_index, the run, matched) does not move it out -- so the lowest listed frame of a cell is the one that
+// takes it, and the header alone names the cell.
+template <bool kGroup>
+__global__ void __launch_bounds__(kWireThreads) wire_wave_claim_kernel(WireSrc w, uint32_t cap, uint32_t *__restrict__ first_frame,
+                                                                       const uint32_t *__restrict__ list,
+                                                                       const uint32_t *__restrict__ list_n) {
+    const uint32_t n = *list_n;
+    for (uint32_t k = blockIdx.x * kWireThreads + threadIdx.x; k < n; k += gridDim.x * kWireThreads) {
+        const uint32_t i = list[k], hdr = wire_header(w, i);
+        if constexpr (kGroup) {
+            if (first_frame[hdr >> 4] != kWaveStop) atomicMin(&first_frame[hdr >> 4], i);  // (a stopped entry never moves)
+        } else {
+            atomicMin(&first_frame[static_cast<size_t>(hdr & 15u) * cap + (hdr >> 4)], i);  // (slot < kSlots: it was DUP)
+        }
+    }
+}
+
+// The apply pass of a wave: wire_apply_kernel's rule, the cell's entry cleared by the frame that takes it, and every DUP
+// frame put on io.out.  io.in == nullptr (wave 1): every frame of the batch the scan left OK, staged as there; else the
+// frames of io.in, read from global memory, over a grid-stride loop (a wave that finds no frame returns at once), where
+// a frame that does not take its cell stays DUP untouched.
+template <bool kRuns>
+__global__ void __launch_bounds__(kWireThreads) wire_wave_apply_kernel(Columns c, WireSrc w, uint8_t *__restrict__ status,
+                                                                       uint32_t *__restrict__ first_frame,
+                                                                       unsigned long long *__restrict__ counters,
+                                                                       const LeaderRuns *__restrict__ runs, WaveIo io) {
+    __shared__ __align__(16) uint8_t stage[kWireStage + 16];
+    uint32_t local[5] = {0, 0, 0, 0, 0};  // records, updates, rejects, decrements, no_progress
+    const uint32_t n = io.in ? *io.in_n : w.n;
+    if (n == 0) return;
+    const uint32_t stride = io.in ? gridDim.x * kWireThreads : w.n;  // (wave 1: one tile per block, the stage used once)
+    for (uint32_t k0 = blockIdx.x * kWireThreads; k0 < n; k0 += stride) {  // (uniform per block)
+        const uint32_t last = min(k0 + kWireThreads, n), k = k0 + threadIdx.x;
+        WireStage s{0, 0, 0, false};
+        if (!io.in) s = wire_stage_block(w, k0, last, stage);
+        const uint32_t i = k < last ? (io.in ? io.in[k] : k) : kNoFrame;
+        bool dup = false;
+        uint32_t *cell = nullptr;
+        if (i != kNoFrame && io.in) {  // a listed frame is DUP already: only the one that takes its cell is decoded
+            const uint32_t hdr = wire_header(w, i);
+            cell = &first_frame[static_cast<size_t>(hdr & 15u) * c.cap + (hdr >> 4)];
+            dup = *cell != i;
+        }
+        if (i != kNoFrame && !dup && (io.in || status[i] == (RAFTGPU_WIRE_OK << 4))) {
+            RecRegs rec;
+            uint64_t hint, snap;
+            wire_frame<kRuns>(c, runs, w, s, stage, i, rec, hint, snap);  // same verdict as in wave 1's scan
+            const uint32_t g = static_cast<uint32_t>(rec.w0), slot = static_cast<uint32_t>(rec.w0 >> 32) & 0xffu;
+            if (!io.in) cell = slot < kSlots ? &first_frame[static_cast<size_t>(slot) * c.cap + g] : nullptr;
+            if (cell && *cell != i) {
+                status[i] = static_cast<uint8_t>(RAFTGPU_WIRE_DUP << 4);
+                dup = true;
+            } else {
+                if (cell) *cell = kNoFrame;  // (the cell's other frames read i or kNoFrame: DUP either way)
+                const CellRegs cr = load_cell(c, rec);
+                const CellPtrs gp = global_cell_ptrs(c, rec);
+                const uint32_t res = apply_one<2>(c, nullptr, hint, snap, rec, cr, gp, local);
+                status[i] = static_cast<uint8_t>((RAFTGPU_WIRE_OK << 4) | (res & 0xfu));
+            }
+        }
+        wave_enlist(io, dup, i);
+    }
+    const int which[5] = {kCntRecords, kCntUpdates, kCntRejects, kCntDecrements, kCntNoProgress};
+    block_flush_counts<5>(local, which, counters, nullptr);
+}
+
 // Clears or states leader-run rows: rows[i] of the list go to row group[i] (raftgpu_leader_runs_set, after its checks).
 __global__ void leader_runs_set_kernel(LeaderRuns *__restrict__ dst, const raftgpu_leader_runs *__restrict__ rows, uint32_t n) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
