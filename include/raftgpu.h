@@ -660,7 +660,7 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
 #define RAFTGPU_WIRE_CONTEXT 6u    /* (raftgpu_heartbeat_wire only) a context that is not an 8-byte read id, or any context
                                       on an arena without read queues: the host's own ReadOnly handles the frame */
 #define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat, raftgpu_follower_append, raftgpu_vote_wire,
-                                      raftgpu_vote_request_wire) the group is not selected for the role the pass serves,
+                                      raftgpu_vote_request_wire, raftgpu_follower_term_wire) the group is not selected for the role the pass serves,
                                       or is a leader; at raftgpu_vote_wire also a response type that is not the
                                       candidate's own (step_candidate ignores it): Raft::step on the host */
 #define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat, raftgpu_follower_append) the commit_to the frame asks
@@ -671,6 +671,8 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
                                         request: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
 #define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire only) the reference drops the frame: a vote request
                                         in lease (raft.rs:1288-1316) or a MsgRequestVote at a lower term (:1399-1409) */
+#define RAFTGPU_WIRE_STALE 11u       /* (raftgpu_follower_term_wire only) m.term below the group's (new) term: settled by the
+                                        pass, which answered it when the low nibble is RAFTGPU_RES_OK; drop the frame */
 typedef struct raftgpu_wire_batch {
     const uint8_t *bytes;    /* the frames, back to back */
     uint64_t n_bytes;
@@ -1173,6 +1175,8 @@ int32_t raftgpu_vote_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_by
 #define RAFTGPU_VOTER_SELECT 0x1u /* the pass decides this group: a Follower, PreCandidate or Candidate */
 #define RAFTGPU_VOTER_LEADER 0x2u /* leader_id != INVALID_ID */
 #define RAFTGPU_VOTER_LEASE 0x4u  /* check_quorum && leader_id != INVALID_ID && election_elapsed < election_timeout */
+#define RAFTGPU_VOTER_STALE_REPLY 0x8u /* check_quorum || pre_vote (raft.rs:1350): raftgpu_follower_term_wire answers a
+                                          lower-term frame; raftgpu_vote_request_wire does not read it */
 #define RAFTGPU_VREQ_GRANTED 0x1u /* the response has reject = false */
 #define RAFTGPU_VREQ_VOTED 0x2u   /* a granted MsgRequestVote: the caller sets vote = m.from, election_elapsed = 0 */
 #define RAFTGPU_VREQ_BUMPED 0x4u  /* the term was raised: the caller runs become_follower(m.term, INVALID_ID)'s host side */
@@ -1197,6 +1201,72 @@ int32_t raftgpu_vote_request_wire(raftgpu_arena *arena, const void *bytes, uint6
                                   uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
                                   uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
                                   uint64_t *totals);
+
+/* ---- the term prefix of MsgAppend and MsgHeartbeat at a follower --------------- */
+
+/* RawNode::step -> Raft::step's term rules (raft.rs:1280-1376) for the MsgAppend (3) and MsgHeartbeat (8) frames of a
+ * wire batch at a Follower, PreCandidate or Candidate: become_follower(m.term, m.from)'s arena part for a higher term,
+ * the empty MsgAppendResponse check_quorum or pre_vote asks for at a lower one.  Nothing past the term prefix: the
+ * frames this pass lets through meet raftgpu_follower_heartbeat and raftgpu_follower_append[_entries] at the group's
+ * (new) term.
+ * Input.  The frames of those passes: u32 LE header (group << 4 | x) with `group` the follower's own group slot; x is
+ * not read and is copied into the response's header.  d_bytes 16-byte aligned, n and n_bytes below 4 GiB.  d_voters
+ * (16-byte aligned, read only) is raftgpu_vote_request_wire's table: the pass reads id, persisted and the flags
+ * (RAFTGPU_VOTER_SELECT: a Follower, PreCandidate or Candidate, the roles whose term rule is the same;
+ * RAFTGPU_VOTER_STALE_REPLY: check_quorum || pre_vote).
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4 | a low nibble; the first failing check decides:
+ *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot, or a wide pair's high half;
+ *   SKIP_TYPE    any type but 3 and 8 (MsgSnapshot and MsgTimeoutNow stay with the host);
+ *   ROLE         RAFTGPU_VOTER_SELECT is clear, or the group is a leader (term_start != RAFTGPU_NO_TERM_START): a leader
+ *                that steps down has host-side consequences;
+ *   TERM         the group's term (raftgpu_group_set_term) is 0, or m.term is 0 (a local message);
+ * then every passing frame is decided per group.  Let T be the larger of the group's term and the largest m.term
+ * among its passing frames:
+ *   OK           m.term == T: the frame is left for the follower passes, nothing is written for it.  When T is above
+ *                the group's term the lowest such frame is the group's claimant, with the low nibble
+ *                RAFTGPU_FTERM_BUMPED: it runs become_follower(T, m.from)'s arena part (term = T, and RAFTGPU_CTL_RESET's
+ *                reset on both halves of a pair with term_start RAFTGPU_NO_TERM_START, last_index, committed -- the
+ *                larger of the halves' -- and the table's persisted), exactly RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET;
+ *   STALE        m.term < T: settled here; drop the frame.  With RAFTGPU_VOTER_STALE_REPLY the pass answers it with one
+ *                MsgAppendResponse {to = m.from, from = the table's id, term = T}, every other field zero
+ *                (raft.rs:1375-1376), and the low nibble is RAFTGPU_RES_OK; without it the reference ignores the frame.
+ * There is no DUP: every frame gets its verdict in one call.  d_out (nullable, u64[2 n]) = {m.from, T} for each
+ * claimant, zero for every other frame.
+ * What the result equals.  For a group whose frames at T carry one `from`, as a real leader's do, the reference reaches
+ * the same state when its frames are delivered in this order: the heartbeats at T in batch order, the appends at T in
+ * batch order, then the stale frames -- the order in which this pass, raftgpu_follower_heartbeat and
+ * raftgpu_follower_append[_entries] apply them.  The first frame delivered at T does the bump, and the bump does not
+ * depend on which frame it is.  When the frames at T carry different `from`s, leader_id is the claimant's m.from.
+ * Output.  The replies in frame order: the input header, then eraftpb.Message with msg_type 4, to, from and term;
+ * canonical proto3 as raftgpu_synth_wire_encode writes (zero fields omitted, at most 39 bytes with the header).
+ * d_resp_bytes (16-byte aligned) holds them back to back, d_resp_offsets (n + 1 values) their starts and the end,
+ * d_totals (u64[2]) = {responses, bytes}.  The pass writes terms and resets groups, so its responses cannot be
+ * produced again: resp_bytes_capacity must be at least raftgpu_follower_term_wire_bound(n), and that bound addressable
+ * by u32 offsets: RAFTGPU_ERR_INVALID before any launch otherwise, as are a missing d_voters, d_status, d_bytes or
+ * d_offsets with n > 0 and misaligned buffers.  The caller sends the replies only after it has made the changed
+ * HardState (term) durable.
+ * Host side.  For every RAFTGPU_FTERM_BUMPED frame the caller runs become_follower's host side -- role Follower,
+ * leader_id = m.from, vote = 0, election_elapsed = 0 -- and updates its select bitmap, log table and voter row before
+ * the next call that reads them: a voter row left stale could grant a vote the reference, now following m.from,
+ * refuses.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  When
+ * one received buffer goes through several passes: raftgpu_vote_request_wire first, then this pass, then the follower
+ * passes (their types are disjoint).  A candidate this pass bumps is a Follower only once the caller says so: the
+ * follower passes of the same sequence return ROLE for it until then, and the host steps those frames.  The host form
+ * copies (voters covers the groups below the highest allocated one), runs and waits; status, out, resp_bytes /
+ * resp_offsets as above, totals u64[2]. */
+#define RAFTGPU_FTERM_BUMPED 0x4u /* the claimant: the term was raised, the caller runs become_follower(T, m.from)'s
+                                     host side */
+/* 39 bytes per frame: enough for the responses to any n frames. */
+uint64_t raftgpu_follower_term_wire_bound(uint64_t n);
+int32_t raftgpu_follower_term_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                          const uint32_t *d_offsets, uint64_t n, const raftgpu_voter *d_voters,
+                                          uint8_t *d_status, uint64_t *d_out, uint8_t *d_resp_bytes,
+                                          uint64_t resp_bytes_capacity, uint32_t *d_resp_offsets, uint64_t *d_totals);
+int32_t raftgpu_follower_term_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets,
+                                   uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
+                                   uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
+                                   uint64_t *totals);
 
 /* ---- MsgAppend at the follower ------------------------------------------------ */
 

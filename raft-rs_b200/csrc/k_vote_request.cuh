@@ -111,6 +111,27 @@ __global__ void __launch_bounds__(kWireThreads) vrq_scan_kernel(Columns c, WireS
     atomicMin(&first_frame[static_cast<uint32_t>(r.w0) >> 4], i);
 }
 
+// become_follower(term, ..)'s arena part (raft.rs:1087-1096) for group g, a wide pair by its low half: the term, then
+// reset_group on both halves with RAFTGPU_CTL_RESET's arguments -- no term_start, last_index and committed (the larger
+// of the halves'), the table's persisted -- exactly as RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET.  Shared by the two
+// passes that raise a follower's term: vrq_apply_kernel here and ftm_apply_kernel (k_follow_term.cuh).
+__device__ __forceinline__ void become_follower_arena(const Columns &c, uint32_t g, uint64_t term,
+                                                      const raftgpu_voter *__restrict__ voters) {
+    const bool wide = c.meta[g] & RAFTGPU_META_WIDE_LO;
+    uint64_t last = c.last_index[g], committed = c.committed[g];
+    if (wide) {
+        last = umax64(last, c.last_index[g + 1]);
+        committed = umax64(committed, c.committed[g + 1]);
+    }
+    const uint64_t persisted = voters[g].persisted;
+    c.term[g] = term;
+    reset_group(c, g, RAFTGPU_NO_TERM_START, last, committed, persisted);
+    if (wide) {
+        c.term[g + 1] = term;
+        reset_group(c, g + 1, RAFTGPU_NO_TERM_START, last, committed, persisted);
+    }
+}
+
 // Pass 2: a later frame of a group is RAFTGPU_WIRE_DUP.  The first one, when OK, is applied: a bump sets the term and
 // resets both halves of a pair (reset_group with RAFTGPU_CTL_RESET's arguments: no term_start, last_index, committed,
 // the table's persisted), exactly as RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET.  out[2 i..] (nullable) = {m.from, the
@@ -135,20 +156,8 @@ __global__ void __launch_bounds__(kWireThreads) vrq_apply_kernel(Columns c, uint
                 const VrqRec r = recs[i];
                 term = c.term[g];
                 if (w0 & kVrqBumped) {
-                    const bool wide = c.meta[g] & RAFTGPU_META_WIDE_LO;
-                    uint64_t last = c.last_index[g], committed = c.committed[g];
-                    if (wide) {
-                        last = umax64(last, c.last_index[g + 1]);
-                        committed = umax64(committed, c.committed[g + 1]);
-                    }
                     term = r.term;
-                    const uint64_t persisted = voters[g].persisted;
-                    c.term[g] = term;
-                    reset_group(c, g, RAFTGPU_NO_TERM_START, last, committed, persisted);
-                    if (wide) {
-                        c.term[g + 1] = term;
-                        reset_group(c, g + 1, RAFTGPU_NO_TERM_START, last, committed, persisted);
-                    }
+                    become_follower_arena(c, g, term, voters);
                 }
                 const uint32_t f = ((w0 & kVrqReject) ? 0u : RAFTGPU_VREQ_GRANTED) | ((w0 & kVrqVoted) ? RAFTGPU_VREQ_VOTED : 0u) |
                                    ((w0 & kVrqBumped) ? RAFTGPU_VREQ_BUMPED : 0u);

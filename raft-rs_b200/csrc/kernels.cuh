@@ -31,5 +31,6 @@ namespace raftgpu {
 #include "k_vote_wire.cuh"
 #include "k_vote_request.cuh"
 #include "k_app_follow.cuh"
+#include "k_follow_term.cuh"
 
 }  // namespace raftgpu
