@@ -662,17 +662,20 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
 #define RAFTGPU_WIRE_ROLE 7u       /* (raftgpu_follower_heartbeat, raftgpu_follower_append, raftgpu_vote_wire,
                                       raftgpu_vote_request_wire, raftgpu_follower_term_wire) the group is not selected for the role the pass serves,
                                       or is a leader; at raftgpu_vote_wire also a response type that is not the
-                                      candidate's own (step_candidate ignores it): Raft::step on the host */
+                                      candidate's own (step_candidate ignores it); at raftgpu_leader_term_wire the group
+                                      is not a leader: Raft::step on the host */
 #define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat, raftgpu_follower_append) the commit_to the frame asks
                                         for -- m.commit, or min(m.commit, m.index) of a matching MsgAppend -- beyond
                                         max(committed, last_index): commit_to would be fatal! (raft_log.rs:291-298) */
 #define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire, raftgpu_vote_request_wire) m.commit != 0, m.commit_term != 0
                                         and m.commit beyond committed -- at raftgpu_vote_request_wire for a rejected
                                         request: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
-#define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire only) the reference drops the frame: a vote request
-                                        in lease (raft.rs:1288-1316) or a MsgRequestVote at a lower term (:1399-1409) */
-#define RAFTGPU_WIRE_STALE 11u       /* (raftgpu_follower_term_wire only) m.term below the group's (new) term: settled by the
-                                        pass, which answered it when the low nibble is RAFTGPU_RES_OK; drop the frame */
+#define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire, raftgpu_leader_term_wire) the reference drops the frame:
+                                        a vote request in lease (raft.rs:1288-1316) or a MsgRequestVote at a lower term
+                                        (:1399-1409); at a leader a frame step_leader or step_follower has no arm for */
+#define RAFTGPU_WIRE_STALE 11u       /* (raftgpu_follower_term_wire, raftgpu_leader_term_wire) m.term below the group's (new)
+                                        term: settled by the pass, which answered it when the low nibble is
+                                        RAFTGPU_RES_OK; drop the frame */
 typedef struct raftgpu_wire_batch {
     const uint8_t *bytes;    /* the frames, back to back */
     uint64_t n_bytes;
@@ -1267,6 +1270,73 @@ int32_t raftgpu_follower_term_wire(raftgpu_arena *arena, const void *bytes, uint
                                    uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
                                    uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
                                    uint64_t *totals);
+
+/* ---- the term prefix of the frames that reach a leader -------------------------- */
+
+/* RawNode::step -> Raft::step's term rules (raft.rs:1280-1411), step_leader's drop arm (:2111-2119) and, after a
+ * step-down, step_follower's, for the MsgAppend (3), MsgAppendResponse (4), MsgRequestVoteResponse (6), MsgHeartbeat
+ * (8), MsgHeartbeatResponse (9) and MsgRequestPreVoteResponse (18) frames of a wire batch at a leader:
+ * become_follower(T, ..)'s arena part for a higher term, the empty MsgAppendResponse check_quorum or pre_vote asks for
+ * at a lower-term MsgAppend / MsgHeartbeat, and a verdict for every frame the reference drops.  The frames at the
+ * leader's term of types 4 and 9 are their own passes' (the wire step, raftgpu_heartbeat_wire).
+ * Input.  Types 4, 6, 9 and 18 carry the leader's cell (group << 4 | slot), as the wire step and raftgpu_vote_wire take
+ * them: a wide pair's high half stands for its pair's low half.  Types 3 and 8 carry the group's own slot (group << 4 |
+ * x), as the follower passes take them; x is copied into the reply's header.  d_bytes 16-byte aligned, n and n_bytes
+ * below 4 GiB.  d_voters (16-byte aligned, read only) is raftgpu_vote_request_wire's table, one row per group slot below
+ * the highest allocated one (a pair's row is its low half's): the pass reads id, persisted and
+ * RAFTGPU_VOTER_STALE_REPLY.  Leadership is the arena's own: term_start != RAFTGPU_NO_TERM_START.
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4 | a low nibble; the first failing check decides:
+ *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot, or a wide pair's high half in
+ *                the header of type 3 or 8;
+ *   SKIP_TYPE    any type but 3, 4, 6, 8, 9 and 18;
+ *   ROLE         the group (a pair: its low half) is not a leader;
+ *   TERM         the group's term (raftgpu_group_set_term) is 0, or m.term is 0 (a local message);
+ * then every passing frame is decided per group.  A MsgRequestPreVoteResponse with reject = false never raises the term
+ * (raft.rs:1319-1320): it is STALE below the group's term and IGNORED at or above it.  Let T be the larger of the
+ * group's term and the largest m.term among its other passing frames:
+ *   OK | RAFTGPU_FTERM_BUMPED  T is above the term and this is the lowest frame at T: it runs become_follower(T, ..)'s
+ *                arena part, exactly RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET (as raftgpu_follower_term_wire's claimant).
+ *                A claimant of type 3 or 8 is left for the follower passes;
+ *   OK           a frame of type 4 or 9 at the leader's term (its own pass decided it), or another frame of type 3 or 8
+ *                at T above the term (left for the follower passes);
+ *   IGNORED      a frame of type 3, 6, 8 or 18 at the leader's term (step_leader drops it), or another frame of type 4,
+ *                6, 9 or 18 at T above the term (step_follower drops it);
+ *   STALE        any other frame, below T: settled here; drop it.  A MsgAppend or MsgHeartbeat of a group with
+ *                RAFTGPU_VOTER_STALE_REPLY is answered with one MsgAppendResponse {to = m.from, from = the table's id,
+ *                term = T}, every other field zero (raft.rs:1375-1376), and the low nibble is RAFTGPU_RES_OK.
+ * There is no DUP: every frame gets its verdict in one call.  d_out (nullable, u64[2 n]) = {leader_id, T} for each
+ * claimant -- leader_id = m.from for types 3 and 8, 0 for the others (raft.rs:1340-1347) -- zero for every other frame.
+ * What the result equals.  The reference reaches the same state when a group's frames are delivered in this order: the
+ * frames at the leader's term, the claimant, the other frames at T in batch order (types 3 and 8 through the follower
+ * passes), then the stale frames; the granting pre-vote responses anywhere.
+ * Output.  The replies in frame order, as raftgpu_follower_term_wire writes them (at most 39 bytes with the header):
+ * d_resp_bytes (16-byte aligned) holds them back to back, d_resp_offsets (n + 1 values) their starts and the end,
+ * d_totals (u64[2]) = {responses, bytes}.  resp_bytes_capacity must be at least raftgpu_follower_term_wire_bound(n), and
+ * that bound addressable by u32 offsets: RAFTGPU_ERR_INVALID before any launch otherwise, as are a missing d_voters,
+ * d_status, d_bytes or d_offsets with n > 0 and misaligned buffers.  The caller sends the replies only after it has
+ * made the changed HardState (term) durable.
+ * Host side.  For every RAFTGPU_FTERM_BUMPED frame the caller runs become_follower (raft.rs:1082-1093) and the host part
+ * of reset (:942-971) for the group: role Follower, leader_id as out gives it, vote = 0, election_elapsed = 0, no
+ * leadership transferee, no pending conf index, the read-index map emptied; and updates its voter row and select
+ * bitmaps before the next call that reads them.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  When
+ * one received buffer goes through several passes: raftgpu_vote_request_wire, raftgpu_follower_term_wire,
+ * raftgpu_vote_wire, the leader passes (the wire step and raftgpu_heartbeat_wire), then this pass, then the host side
+ * of every BUMPED of raftgpu_follower_term_wire and of this pass, then the follower passes.  This pass must come after
+ * the leader passes, which would apply the frames at T after a bump; after a step's begin is enough.  The follower
+ * term pass must come before it, or a group bumped here could be answered twice.  Merging statuses: this pass's
+ * STALE, IGNORED and the BUMPED of types 4, 6, 9 and 18 are settled; its OK leaves the frame to its own pass's status;
+ * a frame of a bumped group that a leader pass left DUP, NEEDS_LOG or CONTEXT is stale: drop it.  The host form copies
+ * (voters covers the groups below the highest allocated one), runs and waits; status, out, resp_bytes / resp_offsets
+ * as above, totals u64[2]. */
+int32_t raftgpu_leader_term_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                        const uint32_t *d_offsets, uint64_t n, const raftgpu_voter *d_voters,
+                                        uint8_t *d_status, uint64_t *d_out, uint8_t *d_resp_bytes,
+                                        uint64_t resp_bytes_capacity, uint32_t *d_resp_offsets, uint64_t *d_totals);
+int32_t raftgpu_leader_term_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets,
+                                 uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
+                                 uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
+                                 uint64_t *totals);
 
 /* ---- MsgAppend at the follower ------------------------------------------------ */
 

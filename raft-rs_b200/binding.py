@@ -46,8 +46,8 @@ BULK_SORTED = 0x1
 WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WIRE_CONTEXT = range(7)
 WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat (ROLE also raftgpu_vote_wire)
 WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire, raftgpu_vote_request_wire
-WIRE_IGNORED = 10  # raftgpu_vote_request_wire only
-WIRE_STALE = 11  # raftgpu_follower_term_wire only
+WIRE_IGNORED = 10  # raftgpu_vote_request_wire, raftgpu_leader_term_wire
+WIRE_STALE = 11  # raftgpu_follower_term_wire, raftgpu_leader_term_wire
 WIRE_WAVES_MAX = 64  # raftgpu_arena_set_wire_waves
 # raftgpu_vote_request_wire: the caller's table (raftgpu_voter), its flags, and the low nibble of an applied frame
 VOTER_SELECT, VOTER_LEADER, VOTER_LEASE = 0x1, 0x2, 0x4
@@ -354,6 +354,8 @@ def lib() -> C.CDLL:
             "raftgpu_follower_term_wire_bound": ([u64], u64),
             "raftgpu_follower_term_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_term_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_leader_term_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_leader_term_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_append_bound": ([u64], u64),
             "raftgpu_follower_append_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_append": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
@@ -1128,6 +1130,30 @@ class Arena:
         self._ck(self._L.raftgpu_follower_term_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters,
                                                            d_status, d_out, d_resp_bytes, resp_bytes_capacity,
                                                            d_resp_offsets, d_totals), "follower_term_wire_device")
+
+    def leader_term_wire(self, frames, voters):
+        """raftgpu_leader_term_wire: Raft::step's term rules and the leader's drop arms for the MsgAppend,
+        MsgAppendResponse, MsgRequestVoteResponse, MsgHeartbeat, MsgHeartbeatResponse and MsgRequestPreVoteResponse
+        frames of a wire batch at this arena's leaders (.bytes, .n_bytes, .offsets, .n).  voters: VOTER_DTYPE rows
+        covering the groups below the highest allocated one -> (status u8[n], out u64[n][2] = {leader_id, T} of the
+        claimants, response blob, response offsets u32[responses + 1], totals u64[2])."""
+        vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
+        assert len(vt) >= self.get_info().hi
+        n = frames.n
+        status, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
+        resp = np.zeros(max(16, follower_term_wire_bound(n)), np.uint8)
+        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        self._ck(self._L.raftgpu_leader_term_wire(self._h, frames.bytes.ctypes.data, frames.n_bytes,
+                                                  frames.offsets.ctypes.data, n, vt.ctypes.data, status.ctypes.data,
+                                                  out.ctypes.data, resp.ctypes.data, len(resp), roff.ctypes.data,
+                                                  totals.ctypes.data), "leader_term_wire")
+        return status, out, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+
+    def leader_term_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_voters, d_status, d_out, d_resp_bytes,
+                                resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
+        self._ck(self._L.raftgpu_leader_term_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters,
+                                                         d_status, d_out, d_resp_bytes, resp_bytes_capacity,
+                                                         d_resp_offsets, d_totals), "leader_term_wire_device")
 
     def follower_append(self, frames, log):
         """raftgpu_follower_append: handle_append_entries at this arena's followers for the entry-less MsgAppend frames

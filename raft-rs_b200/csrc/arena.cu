@@ -233,6 +233,7 @@ enum Pass {
     kPassAppFrames,
     kPassAppFollow,
     kPassFollowTerm,
+    kPassLeaderTerm,
     kPassCount
 };
 
@@ -1059,7 +1060,7 @@ class HostFrame {
 };
 
 // ---- the reply pipeline (DESIGN 3.12): a pass that answers every frame it applies with a frame of its own
-// (raftgpu_follower_heartbeat, raftgpu_vote_request_wire, raftgpu_follower_term_wire's stale replies) keeps its decision -- a scan and an apply kernel -- and
+// (raftgpu_follower_heartbeat, raftgpu_vote_request_wire, raftgpu_follower_term_wire's and raftgpu_leader_term_wire's stale replies) keeps its decision -- a scan and an apply kernel -- and
 // shares the rest: reply_check, reply_run<P> for the `_device` form, reply_host for the host form.  P is the pass's
 // reply policy (reply_write_kernel, k_wire.cuh).
 
@@ -1444,5 +1445,6 @@ extern "C" {
 #include "abi_app_follow.inc"
 #include "abi_leader_runs.inc"
 #include "abi_follow_term.inc"
+#include "abi_leader_term.inc"
 
 }  // extern "C"

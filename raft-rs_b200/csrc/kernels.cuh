@@ -32,5 +32,6 @@ namespace raftgpu {
 #include "k_vote_request.cuh"
 #include "k_app_follow.cuh"
 #include "k_follow_term.cuh"
+#include "k_leader_term.cuh"
 
 }  // namespace raftgpu
