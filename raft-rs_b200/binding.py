@@ -1036,6 +1036,20 @@ class Arena:
                                                       d_offsets, frames_capacity, d_rest, rest_capacity, d_totals),
                  "append_frames_device")
 
+    def _reply(self, name, frames, tables, out_shape, bound, extra=None):
+        """The host form of a reply pass: raftgpu_<name>(handle, the batch, tables, status u8[n], out u64[n][*out_shape],
+        extra[n] when given, response bytes and their capacity bound(n), response offsets, totals u64[2]) -> (status, out,
+        extra when given, response blob, response offsets u32[responses + 1], totals)."""
+        n = frames.n
+        outs = [np.zeros(n, np.uint8), np.zeros((n,) + out_shape, np.uint64)] + ([] if extra is None else [np.zeros(n, extra)])
+        resp = np.zeros(max(16, bound(n)), np.uint8)
+        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        self._ck(getattr(self._L, "raftgpu_" + name)(self._h, frames.bytes.ctypes.data, frames.n_bytes,
+                                                     frames.offsets.ctypes.data, n, *[t.ctypes.data for t in tables],
+                                                     *[o.ctypes.data for o in outs], resp.ctypes.data, len(resp),
+                                                     roff.ctypes.data, totals.ctypes.data), name)
+        return (*outs, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals)
+
     def follower_heartbeat(self, frames, self_ids, select):
         """raftgpu_follower_heartbeat: handle_heartbeat at this arena's followers for the MsgHeartbeat frames of a wire
         batch (.bytes, .n_bytes, .offsets, .n; headers name the follower's group slot).  self_ids: u64 per group slot
@@ -1045,15 +1059,7 @@ class Arena:
         ids = np.ascontiguousarray(self_ids, dtype=np.uint64)
         sel = np.ascontiguousarray(select, dtype=np.uint32)
         assert len(ids) >= self.cap and len(sel) * 32 >= self.cap
-        n = frames.n
-        status, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
-        resp = np.zeros(max(16, follower_heartbeat_bound(n)), np.uint8)
-        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-        self._ck(self._L.raftgpu_follower_heartbeat(self._h, frames.bytes.ctypes.data, frames.n_bytes,
-                                                    frames.offsets.ctypes.data, n, sel.ctypes.data, ids.ctypes.data,
-                                                    status.ctypes.data, frm.ctypes.data, resp.ctypes.data, len(resp),
-                                                    roff.ctypes.data, totals.ctypes.data), "follower_heartbeat")
-        return status, frm, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+        return self._reply("follower_heartbeat", frames, (sel, ids), (), follower_heartbeat_bound)
 
     def follower_heartbeat_device(self, d_bytes, n_bytes, d_offsets, n, d_select, d_self_ids, d_status, d_from, d_resp_bytes,
                                   resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
@@ -1092,15 +1098,7 @@ class Arena:
         {m.from, term after} of the applied frames, response blob, response offsets u32[responses + 1], totals u64[2])."""
         vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
         assert len(vt) >= self.get_info().hi
-        n = frames.n
-        status, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
-        resp = np.zeros(max(16, vote_request_wire_bound(n)), np.uint8)
-        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-        self._ck(self._L.raftgpu_vote_request_wire(self._h, frames.bytes.ctypes.data, frames.n_bytes,
-                                                   frames.offsets.ctypes.data, n, vt.ctypes.data, status.ctypes.data,
-                                                   out.ctypes.data, resp.ctypes.data, len(resp), roff.ctypes.data,
-                                                   totals.ctypes.data), "vote_request_wire")
-        return status, out, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+        return self._reply("vote_request_wire", frames, (vt,), (2,), vote_request_wire_bound)
 
     def vote_request_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_voters, d_status, d_out, d_resp_bytes,
                                  resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
@@ -1115,15 +1113,7 @@ class Arena:
         blob, response offsets u32[responses + 1], totals u64[2])."""
         vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
         assert len(vt) >= self.get_info().hi
-        n = frames.n
-        status, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
-        resp = np.zeros(max(16, follower_term_wire_bound(n)), np.uint8)
-        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-        self._ck(self._L.raftgpu_follower_term_wire(self._h, frames.bytes.ctypes.data, frames.n_bytes,
-                                                    frames.offsets.ctypes.data, n, vt.ctypes.data, status.ctypes.data,
-                                                    out.ctypes.data, resp.ctypes.data, len(resp), roff.ctypes.data,
-                                                    totals.ctypes.data), "follower_term_wire")
-        return status, out, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+        return self._reply("follower_term_wire", frames, (vt,), (2,), follower_term_wire_bound)
 
     def follower_term_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_voters, d_status, d_out, d_resp_bytes,
                                   resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
@@ -1139,15 +1129,7 @@ class Arena:
         claimants, response blob, response offsets u32[responses + 1], totals u64[2])."""
         vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
         assert len(vt) >= self.get_info().hi
-        n = frames.n
-        status, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
-        resp = np.zeros(max(16, follower_term_wire_bound(n)), np.uint8)
-        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-        self._ck(self._L.raftgpu_leader_term_wire(self._h, frames.bytes.ctypes.data, frames.n_bytes,
-                                                  frames.offsets.ctypes.data, n, vt.ctypes.data, status.ctypes.data,
-                                                  out.ctypes.data, resp.ctypes.data, len(resp), roff.ctypes.data,
-                                                  totals.ctypes.data), "leader_term_wire")
-        return status, out, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+        return self._reply("leader_term_wire", frames, (vt,), (2,), follower_term_wire_bound)
 
     def leader_term_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_voters, d_status, d_out, d_resp_bytes,
                                 resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
@@ -1162,14 +1144,7 @@ class Arena:
         response blob, response offsets u32[responses + 1], totals u64[2])."""
         lt = np.ascontiguousarray(log, dtype=FOLLOWER_LOG_DTYPE)
         assert len(lt) >= self.get_info().hi
-        n = frames.n
-        status, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
-        resp = np.zeros(max(16, follower_append_bound(n)), np.uint8)
-        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-        self._ck(self._L.raftgpu_follower_append(self._h, frames.bytes.ctypes.data, frames.n_bytes, frames.offsets.ctypes.data,
-                                                 n, lt.ctypes.data, status.ctypes.data, frm.ctypes.data, resp.ctypes.data,
-                                                 len(resp), roff.ctypes.data, totals.ctypes.data), "follower_append")
-        return status, frm, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+        return self._reply("follower_append", frames, (lt,), (), follower_append_bound)
 
     def follower_append_device(self, d_bytes, n_bytes, d_offsets, n, d_log, d_status, d_from, d_resp_bytes,
                                resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
@@ -1184,16 +1159,7 @@ class Arena:
         from u64[n], appended FOLLOWER_APPENDED_DTYPE[n], response blob, response offsets u32[responses + 1], totals
         u64[2])."""
         assert log.dtype == FOLLOWER_LOG_DTYPE and log.flags.c_contiguous and len(log) >= self.get_info().hi
-        n = frames.n
-        status, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
-        app = np.zeros(n, FOLLOWER_APPENDED_DTYPE)
-        resp = np.zeros(max(16, follower_append_bound(n)), np.uint8)
-        roff, totals = np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-        self._ck(self._L.raftgpu_follower_append_entries(self._h, frames.bytes.ctypes.data, frames.n_bytes,
-                                                         frames.offsets.ctypes.data, n, log.ctypes.data, status.ctypes.data,
-                                                         frm.ctypes.data, app.ctypes.data, resp.ctypes.data, len(resp),
-                                                         roff.ctypes.data, totals.ctypes.data), "follower_append_entries")
-        return status, frm, app, resp[: int(totals[1])], roff[: int(totals[0]) + 1], totals
+        return self._reply("follower_append_entries", frames, (log,), (), follower_append_bound, FOLLOWER_APPENDED_DTYPE)
 
     def follower_append_entries_device(self, d_bytes, n_bytes, d_offsets, n, d_log, d_status, d_from, d_appended,
                                        d_resp_bytes, resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):

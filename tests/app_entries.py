@@ -3,6 +3,8 @@ eraftpb.Entry records with every field, Messages built from them (hostile layout
 follower whose log, run and committed index are known."""
 import numpy as np
 
+from helpers import B
+from oracle import app_follow_oracle as AL
 import app_follow as A
 
 varint = A.varint
@@ -103,3 +105,34 @@ def random_frame(rng, last, run_start, run_term, term, committed, big=False, hos
             ents[j] = ents[j] + b"\x10"                                   # a tag without its value
     commit = int(rng.integers(0, index + n + 1)) if rng.random() < 0.95 else int(rng.integers(0, last + n + 5))
     return message(term, log_term, index, commit, int(rng.integers(1, 1 << 40)), [record(e) for e in ents], split_at=split)
+
+
+WIDE_LO = 0x20000000  # RAFTGPU_META_WIDE_LO
+
+
+NAMES = ("status", "from", "appended", "response bytes", "response offsets", "totals")
+
+
+def world(rng, n_narrow, n_wide, reads):
+    """A follower arena of n_narrow groups then n_wide pairs at random terms and logs, and its log table with random runs
+    -> (arena, host columns, read queues or None, table)."""
+    n = n_narrow + 2 * n_wide
+    terms = rng.integers(2, 1000, n).astype(np.uint64)
+    last = rng.integers(0, 1 << 20, n).astype(np.uint64)
+    committed = last - np.minimum(last, rng.integers(0, 40, n).astype(np.uint64))
+    hi = np.arange(n_narrow + 1, n, 2)
+    terms[hi] = terms[hi - 1]
+    term_start = np.where(rng.random(n) < 0.03, np.uint64(1), np.uint64(A.NO_TERM_START))
+    cols = {B.COL_TERM: terms, B.COL_LAST_INDEX: last, B.COL_COMMITTED: committed, B.COL_TERM_START: term_start}
+    a, c, q = A.follower_arena(n_narrow, n_wide, cols, reads)
+    table = np.zeros(a.get_info().hi, AL.LOG_DTYPE)
+    table["id"][:n] = rng.integers(1, 1 << 63, n, dtype=np.uint64)
+    table["flags"][:n] = np.where(rng.random(n) < 0.97, AL.SELECT, 0)
+    top = np.maximum(c.last_index[:n], np.concatenate([c.last_index[1:n], [0]]))
+    table["run_start"][:n] = np.where(rng.random(n) < 0.95, top - np.minimum(top, rng.integers(0, 50, n).astype(np.uint64)),
+                                      top + 1)
+    table["run_term"][:n] = terms - rng.integers(0, 2, n).astype(np.uint64)
+    return a, c, q, table
+
+
+N_NARROW, N_WIDE = 99_000, 500

@@ -5,6 +5,7 @@ reads."""
 import numpy as np
 
 from helpers import B, O
+import pass_forms as PF
 from oracle import app_follow_oracle as AL
 
 U64 = (1 << 64) - 1
@@ -158,3 +159,69 @@ def state(c, n):
 
 
 LOG_STATUS_OK = B.WIRE_OK << 4 | B.RES_OK
+
+
+NAMES = ("status", "from", "response bytes", "response offsets", "totals")
+
+
+def host_form(a, blob, off, table, n_bytes=None):
+    """raftgpu_follower_append's host form over the batch, with the table extended to the arena's highest group."""
+    return a.follower_append(PF.host_batch(blob, off, n_bytes), full_table(a, table))
+
+
+def full_table(a, table):
+    """table cut or zero-extended to the arena's highest group."""
+    t = np.zeros(a.get_info().hi, AL.LOG_DTYPE)
+    t[: min(len(t), len(table))] = table[: len(t)]
+    return t
+
+
+def follower_arena(n_narrow, n_wide, cols, reads=False, extra=64):
+    """An arena of n_narrow groups then n_wide pairs, its group columns written from cols (name -> u64[n]) -> (arena, host
+    columns with c.term, read queues or None)."""
+    n = n_narrow + 2 * n_wide
+    a = B.Arena(n + extra)
+    if reads:
+        a.enable_read_index(8)
+    assert a.group_alloc_range(n_narrow) == 0
+    for k in range(n_wide):
+        assert a.group_alloc_wide() == n_narrow + 2 * k
+    for col, arr in cols.items():
+        a.column_write(col, 0, 0, np.ascontiguousarray(arr[:n], np.uint64))
+    c = a.read_columns(n)
+    c.term = a.column_read(B.COL_TERM, 0, 0, n, np.uint64)
+    q = None
+    if reads:
+        from oracle import read_oracle as RO
+        q = RO.ReadQueues(c.cap, 8)
+        q.allocated[:n] = 1
+    return a, c, q
+
+
+def hostile(rng, terms, k):
+    """k frames that must not pass or that go back to the host: garbage, unknown groups, truncations, other types,
+    frames with entries, term 0, stale and future terms, a commit out of range."""
+    out, n_f = [], len(terms)
+    for j in range(k):
+        g, x = int(rng.integers(0, n_f)), int(rng.integers(16))
+        t = int(terms[g])
+        kind = j % 9
+        if kind == 0:
+            out.append(frame(g, x, rng.integers(0, 256, int(rng.integers(0, 24)), dtype=np.uint8).tobytes()))
+        elif kind == 1:
+            out.append(frame(n_f + int(rng.integers(0, 100)), x, message(3, term=t, index=1)))
+        elif kind == 2:
+            out.append(frame(g, x, message(3, term=t, index=5, commit=1 << 40, frm=3)[:-1]))
+        elif kind == 3:
+            out.append(frame(g, x, message(int(rng.choice([4, 8, 9, 17])), term=t, index=1)))
+        elif kind == 4:
+            out.append(frame(g, x, message(3, term=t, index=1, frm=2, entries=[(t, 2)] * int(rng.integers(1, 3)))))
+        elif kind == 5:
+            out.append(frame(g, x, message(3, term=0, index=1)))
+        elif kind == 6:
+            out.append(frame(g, x, message(3, term=max(1, t + int(rng.choice([-1, 1]))), index=1)))
+        elif kind == 7:                                                # matches above last_index, commit_to out of range
+            out.append(frame(g, x, message(3, term=t, log_term=0, index=U64 - 1, commit=U64 - 1, frm=2)))
+        else:
+            out.append(np.array([g << 4 | x], "<u4").tobytes()[: int(rng.integers(0, 4))])
+    return out

@@ -71,3 +71,77 @@ def oracle_step(ref, rows, blob, offsets, n_bytes=None):
     want = (status.astype(np.uint32) << 4).astype(np.uint8)
     want[ok] |= res[main] & 0xF
     return want
+
+
+def leader_arena(c, n, runs):
+    """An arena of n groups loaded from the oracle columns c (terms included), with leader runs when runs is set."""
+    a = B.Arena(n)
+    if runs:
+        a.enable_leader_runs()
+    assert a.group_alloc_range(n) == 0
+    a.load_columns(c)
+    a.column_write(B.COL_TERM, 0, 0, c.term[:n].copy())
+    return a
+
+
+def leader_frames(rng, c, groups, peers, per_cell, needs_log=0.0, stale=0.2):
+    """1..per_cell MsgAppendResponse frames per (group, peer) cell, the cells interleaved in a random arrival order (a
+    cell's frames keep theirs): accepts at increasing indexes (a fraction `stale` at an index already matched),
+    rejections with log_term 0 at the probe's index, and a fraction needs_log of rejections with log_term > 0."""
+    cells = []
+    for g in groups:
+        last = int(c.last_index[g])
+        for s in peers:
+            k = int(rng.integers(1, per_cell + 1))
+            idx = sorted(rng.integers(0, last + 1, k).tolist())
+            fr = []
+            for j in range(k):
+                if rng.random() < 0.25:
+                    lt = int(rng.integers(1, 40)) if rng.random() < needs_log else 0
+                    body = response(int(c.term[g]), index=int(rng.integers(0, last + 1)), reject=True,
+                                      hint=int(rng.integers(0, last + 2)), log_term=lt)
+                else:
+                    i = idx[j] if rng.random() >= stale else int(rng.integers(0, idx[j] + 1))
+                    body = response(int(c.term[g]), index=i, commit=int(rng.integers(0, last + 1)))
+                fr.append(A.frame(g, s, body))
+            cells.append(fr)
+    order = rng.permutation(sum(len(f) for f in cells))
+    owner = np.repeat(np.arange(len(cells)), [len(f) for f in cells])[order]
+    pos = [0] * len(cells)
+    out = []
+    for cell in owner.tolist():       # each cell's frames in their order, cells interleaved
+        out.append(cells[cell][pos[cell]])
+        pos[cell] += 1
+    return out
+
+
+def pipelined_appends(rng, last, run_term, term, committed, k, entries=True):
+    """k pipelined MsgAppend bodies to a follower whose log ends at `last` with term run_term: frame j's entries (1-3
+    at `term`) start at frame j-1's last index + 1; without entries, k heartbeat-like appends at `last` with rising
+    commits.  -> [(body, last index after it)]."""
+    out, idx, lt = [], last, run_term
+    for _ in range(k):
+        if entries:
+            cnt = int(rng.integers(1, 4))
+            ents = [(term, idx + j + 1) for j in range(cnt)]
+        else:
+            cnt, ents = 0, None
+        top = idx + cnt
+        commit = int(rng.integers(min(committed, top), top + 1))
+        out.append((A.message(3, term=term, log_term=lt, index=idx, commit=commit, frm=int(rng.integers(1, 1 << 40)),
+                              entries=ents), top))
+        if entries:
+            idx, lt = top, term
+    return out
+
+
+def interleave(rng, per_group):
+    """[(group, [frames])] -> one batch order: every group's frames in their order, the groups interleaved."""
+    owner = np.repeat(np.arange(len(per_group)), [len(f) for _, f in per_group])
+    owner = owner[rng.permutation(len(owner))]
+    pos = [0] * len(per_group)
+    out = []
+    for k in owner.tolist():
+        out.append(per_group[k][1][pos[k]])
+        pos[k] += 1
+    return out

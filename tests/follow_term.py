@@ -5,6 +5,7 @@ raftgpu_follower_append" run on the batch oracles, with its DUP frames resubmitt
 import numpy as np
 
 from helpers import B
+from control_cmds import cmds
 from oracle import app_follow_oracle as AL
 from oracle import follow_term_oracle as FT
 from oracle import hb_follow_oracle as HF
@@ -104,3 +105,73 @@ def follower_passes(c, s, role, table, frames_, idx):
                     nxt.append(i)
             pend = nxt
     return final, resps
+
+
+def noise(rng, s, k):
+    """Frames the checks before the verdict settle: other types, garbage, truncated frames, high halves, m.term 0 and
+    groups past the arena's highest slot."""
+    out = []
+    for _ in range(k):
+        g = int(rng.choice(s.lows))
+        term = int(s.term[g])
+        kind = int(rng.integers(6))
+        if kind == 0:
+            out.append(F.frame(g, 0, F.message(int(rng.choice([4, 9, 5, 7, 10])), term + 1, frm=2)))
+        elif kind == 1:
+            out.append(F.frame(g, 0, rng.integers(0, 256, int(rng.integers(1, 12)), dtype=np.uint8).tobytes()))
+        elif kind == 2:
+            out.append(F.frame(g, 0, F.message(8, term + 1, 1 << 40, frm=2)[:-3]))
+        elif kind == 3:
+            out.append(F.frame(g + 1 if s.wide[g] else g, 0, F.message(8, term + 1 if s.wide[g] else 0, frm=2)))
+        elif kind == 4:
+            out.append(F.frame(g, 0, F.message(3, 0, frm=2)))
+        else:
+            out.append(F.frame(s.n + int(rng.integers(1, 100)), 0, F.message(8, term + 1, frm=2)))
+    return out
+
+
+def leaders(n, P, term, li):
+    """n narrow leader groups of P voters (self slot 0) at `term`: the empty entry at li + 1 = term_start, committed li,
+    every peer a Replicate peer matched at li that was sent the empty entry (next li + 2), and the earlier run [1, li]
+    at term - 1 stated."""
+    a = B.Arena(n + 64)
+    a.enable_leader_runs()
+    assert a.group_alloc_range(n) == 0
+    ops = []
+    for g in range(n):
+        ops += [(B.CTL_SET_CONF, g, 0, 0, ((1 << P) - 1, 0, 0, li + 1)), (B.CTL_RESET, g, 0, 0, (li + 1, li, li, li)),
+                (B.CTL_SET_TERM, g, 0, 0, (term,)), (B.CTL_BECOME_LEADER, g)]
+        for s in range(1, P):
+            ops += [(B.CTL_PROGRESS_OP, g, s, B.POP_MAYBE_UPDATE, (li,)), (B.CTL_PROGRESS_OP, g, s, B.POP_BECOME_REPLICATE),
+                    (B.CTL_PROGRESS_OP, g, s, B.POP_OPTIMISTIC_UPDATE, (li + 1,))]
+    assert np.all(a.control(cmds(*ops))["status"] == 0)
+    rows = np.zeros(n, B.LEADER_RUNS_DTYPE)
+    rows["group"], rows["term"], rows["term_start"] = np.arange(n), term, li + 1
+    rows["run_start"][:, 0], rows["run_term"][:, 0] = 1, term - 1
+    assert np.all(a.leader_runs_set(rows) == 0)
+    return a
+
+
+def to_followers(blob, off, P):
+    """The transport: leader cell (g, s) -> follower group g * (P - 1) + s - 1, x = s."""
+    h = HB.headers(blob, off)
+    return HB.with_headers(blob, off, (((h >> 4) * (P - 1) + (h & 15) - 1) << 4 | (h & 15)).astype(np.uint32))
+
+
+def to_leaders(blob, off, P):
+    h = HB.headers(blob, off)
+    return HB.with_headers(blob, off, (((h >> 4) // (P - 1)) << 4 | (h & 15)).astype(np.uint32))
+
+
+def followers(nf, term, li, P, rng):
+    fa = B.Arena(nf + 64)
+    assert fa.group_alloc_range(nf) == 0
+    fcom = (li - rng.integers(0, 4, nf)).astype(np.uint64)
+    for col, arr in ((B.COL_TERM, np.full(nf, term, np.uint64)), (B.COL_LAST_INDEX, np.full(nf, li, np.uint64)),
+                     (B.COL_COMMITTED, fcom), (B.COL_TERM_START, np.full(nf, B.NO_TERM_START, np.uint64))):
+        fa.column_write(col, 0, 0, arr)
+    table = Q.voters(nf)
+    table["id"] = np.arange(nf) % (P - 1) + 2
+    table["persisted"], table["last_term"] = li, term
+    table["flags"] = B.VOTER_SELECT | B.VOTER_STALE_REPLY
+    return fa, table

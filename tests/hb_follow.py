@@ -3,6 +3,8 @@
 write."""
 import numpy as np
 
+from helpers import B
+
 GROUP_STATE = ("committed", "last_index", "term", "term_start", "meta")
 
 
@@ -43,3 +45,20 @@ def state(c, n):
 
 def same_state(x, y) -> bool:
     return all(np.array_equal(x[k], y[k]) for k in GROUP_STATE)
+
+
+def self_ids(rng, n):
+    """Random Raft ids for n followers, a few of them 0, 128 and 2^64 - 1."""
+    ids = rng.integers(1, 1 << 63, n, dtype=np.uint64)
+    k = rng.random(n)
+    ids[k < 0.03] = 0
+    ids[(k > 0.03) & (k < 0.06)] = (1 << 64) - 1
+    ids[(k > 0.06) & (k < 0.09)] = 128
+    return ids
+
+
+def group_state(a, n):
+    """The group columns the follower passes write (and meta, which they leave alone) of groups [0, n)."""
+    c = a.read_columns(n)
+    return {"committed": c.committed, "last_index": c.last_index, "term_start": c.term_start,
+            "term": a.column_read(B.COL_TERM, 0, 0, n, np.uint64), "meta": c.meta}

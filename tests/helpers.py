@@ -5,6 +5,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from oracle import datadriven as dd
 from oracle import oracle as O
 
 B = importlib.import_module("raft-rs_b200").binding
@@ -531,3 +532,301 @@ def records_round(arena, n, recs, ref, what):
     adv = bitmap_to_bool(bm, n)
     assert np.array_equal(com[adv], ref.committed[:n][adv]), what
     assert_columns_equal(arena.read_columns(n), ref, n, f"records API, {what}")
+
+
+# --------------------------------------------------------------------------- arenas set up like a wire-pass scenario
+
+ARENA_COLUMNS = ("term_start", "committed", "last_index", "matched", "next_idx", "peer_committed", "pflags")
+
+
+def votes(a, n):
+    """The arena's votes of groups [0, n): u8 [SLOTS][n]."""
+    return np.stack([a.column_read(B.COL_VOTES, s, 0, n, np.uint8) for s in range(O.SLOTS)])
+
+
+def check_columns(a, c, vt, n, ins=False):
+    """The arena's ARENA_COLUMNS, terms and votes (and Inflights metas with ins) of groups [0, n) against the oracle's
+    columns c and votes vt."""
+    cols = a.read_columns(n)
+    for name in ARENA_COLUMNS:
+        assert np.array_equal(getattr(cols, name), getattr(c, name)[..., :n]), name
+    assert np.array_equal(a.column_read(B.COL_TERM, 0, 0, n, np.uint64), c.term[:n])
+    assert np.array_equal(votes(a, n), vt[:, :n])
+    if ins:
+        for s in range(O.SLOTS):
+            assert np.array_equal(a.column_read(B.COL_INS_META, s, 0, n, np.uint32), c.ins_meta[s, :n]), s
+
+
+def arena_of(s, read_index=False, inflights=0, leader_runs=False):
+    """An arena of s.n + 64 group slots set up like scenario s (vote_request_frames.Scenario, follow_term.scenario,
+    vote_frames.Election): s.n_narrow narrow groups from slot 0, then s.n_wide wide pairs, then the control list
+    s.setup and, where s has one, s.campaign."""
+    a = B.Arena(s.n + 64)
+    if read_index:
+        a.enable_read_index()
+    if inflights:
+        a.enable_inflights(inflights)
+    if leader_runs:
+        a.enable_leader_runs()
+    if s.n_narrow:
+        assert a.group_alloc_range(s.n_narrow) == 0
+    for k in range(s.n_wide):
+        assert a.group_alloc_wide() == s.n_narrow + 2 * k
+    assert np.all(a.control(s.setup)["status"] == 0)
+    if getattr(s, "campaign", None) is not None:
+        a.control(s.campaign)
+    return a
+
+
+def oracle_wire_step(ref, wb, n_groups, terms):
+    """What the step must do: local records first, then every frame the decoder accepts, in frame order (the first
+    frame of a cell; later ones are DUP), then Raft::maybe_commit for every group.  Returns (status bytes, adv bitmap)."""
+    res_local = O.arena_apply(ref, wb.records[: wb.n_records].copy(), mode=0) if wb.n_records else None
+    status, recs, hint, snap = O.wire_decode_batch(wb.bytes[: wb.n_bytes], wb.offsets[: wb.n + 1], n_groups, terms)
+    ok = np.nonzero(status == O.WIRE_OK)[0]
+    rows = []
+    for i in ok:
+        rows.append(tuple(recs[i]))
+        if recs["flags"][i] & B.REC_REJECT:
+            rows.append((recs["group"][i], recs["peer_slot"][i], B.REC_EXT, 0, hint[i], snap[i]))
+    seq = np.array(rows, dtype=B.APPEND_RESP_DTYPE) if rows else np.zeros(0, dtype=B.APPEND_RESP_DTYPE)
+    res = O.arena_apply(ref, seq, mode=0)
+    main = (seq["flags"] & B.REC_EXT) == 0
+    want = (status.astype(np.uint32) << 4).astype(np.uint8)
+    want[ok] |= res[main] & 0xF
+    adv, bm, _, _ = O.arena_recompute(ref)
+    return want, bm, adv, res_local
+
+
+def oracle_wire_apply(c, blob, offsets, n, terms, n_bytes=None):
+    """raftgpu_wire_apply_device: the AppendResponse frames, first of every cell, in frame order."""
+    status, recs, hint, snap = O.wire_decode_batch(blob, offsets, n, terms, n_bytes)
+    ok = np.nonzero(status == O.WIRE_OK)[0]
+    rows = []
+    for i in ok:
+        rows.append(tuple(recs[i]))
+        if recs["flags"][i] & B.REC_REJECT:
+            rows.append((recs["group"][i], recs["peer_slot"][i], B.REC_EXT, 0, hint[i], snap[i]))
+    seq = np.array(rows, dtype=B.APPEND_RESP_DTYPE) if rows else np.zeros(0, dtype=B.APPEND_RESP_DTYPE)
+    res = O.arena_apply(c, seq, mode=0)
+    want = (status.astype(np.uint32) << 4).astype(np.uint8)
+    want[ok] |= res[(seq["flags"] & B.REC_EXT) == 0] & 0xF
+    return want
+
+
+def full_state(arena, n, inflights=False):
+    """Every column of groups [0, n): the host-column set, votes, term and (with inflights) the Inflights meta."""
+    c = arena.read_columns(n)
+    votes = np.stack([arena.column_read(B.COL_VOTES, s, 0, n, np.uint8) for s in range(B.SLOTS)])
+    c.term[:] = arena.column_read(B.COL_TERM, 0, 0, n, np.uint64)
+    ins = None
+    if inflights:
+        ins = np.stack([arena.column_read(B.COL_INS_META, s, 0, n, np.uint32) for s in range(B.SLOTS)])
+    return c, votes, ins
+
+
+def assert_state_equal(a, b, n, what):
+    ca, va, ia = a
+    cb, vb, ib = b
+    assert_columns_equal(ca, cb, n, what)
+    assert np.array_equal(ca.term[:n], cb.term[:n]), f"{what}: term"
+    assert np.array_equal(va[:, :n], vb[:, :n]), f"{what}: votes"
+    if ia is not None or ib is not None:
+        assert np.array_equal(ia[:, :n], ib[:, :n]), f"{what}: ins_meta"
+
+
+def records_step(arena, n, recs, ref, what):
+    """raftgpu_step_begin_records (the library picks the kernel from its launch plan), checked against the oracle."""
+    arena.step_begin_records(recs, B.STEP_READ_COMMITTED)
+    r = arena.step_wait()
+    O.arena_apply(ref, recs, mode=0)
+    want_adv, want_bm, _, _ = O.arena_recompute(ref)
+    assert r.n_advanced == want_adv, what
+    bm, com = arena.step_results(n)
+    assert np.array_equal(bm, want_bm[: len(bm)]), what
+    adv = bitmap_to_bool(bm, n)
+    assert np.array_equal(com[adv], ref.committed[:n][adv]), what
+    assert_columns_equal(arena.read_columns(n), ref, n, what)
+
+
+def scatter_step(arena, n, recs, ref, what):
+    """Enqueued records and raftgpu_step, checked against the oracle."""
+    arena.enqueue(recs)
+    r = arena.step(B.STEP_READ_COMMITTED)
+    O.arena_apply(ref, recs, mode=0)
+    want_adv, _, _, _ = O.arena_recompute(ref)
+    assert r.n_advanced == want_adv, what
+    assert_columns_equal(arena.read_columns(n), ref, n, what)
+
+
+def several_tiles():
+    """Seven full tiles and a ragged eighth."""
+    return 7 * B.tile_groups() + 77
+
+
+def escape_tiles(n):
+    """Every ninth tile: each of its cells escaped."""
+    return (np.arange(n) // B.tile_groups()) % 9 == 4
+
+
+def storm(c, rng, n):
+    """The state right after an election at a last index past 2^31 (Raft::reset, then become_leader): every peer
+    cell but the leader's own has matched 0 and next_idx = last_index + 1, both escaped."""
+    last = np.array(RESET_LAST[1:])[rng.integers(0, len(RESET_LAST) - 1, n)]
+    meta = c.meta[:n].astype(np.int64)
+    own = ((meta & O.META_HAS_SELF) != 0)[None, :] & (((meta >> 24) & 7)[None, :] == np.arange(O.SLOTS)[:, None])
+    follower = ~own
+    c.last_index[:n] = last
+    c.term_start[:n] = last
+    c.committed[:n] = np.minimum(c.committed[:n], last - 1)
+    c.matched[:, :n] = np.where(follower, 0, last)                 # the leader: persisted = last_index
+    c.peer_committed[:, :n] = np.where(follower, c.peer_committed[:, :n], c.committed[:n])
+    c.next_idx[:, :n] = last + 1
+    c.pflags[:, :n] = np.where(follower, O.STATE_PROBE, c.pflags[:, :n])
+    c.pending_snapshot[:, :n] = np.where(follower, 0, c.pending_snapshot[:, :n])
+    c.pending_request_snapshot[:, :n] = np.where(follower, 0, c.pending_request_snapshot[:, :n])
+    assert not fits(c.next_idx[:, :n][follower], 0).any()
+    return c
+
+
+def as_set(e):
+    return sorted(zip(e["group"].tolist(), e["peer_slot"].tolist(), e["flags"].tolist(), e["next_idx"].tolist()))
+
+
+class GpuQuorum:
+    """Evaluates the quorum functions on the GPU: voter ids are mapped to peer slots of one
+    arena group, acked indexes become its matched / commit_group_id columns."""
+
+    def __init__(self, arena):
+        self.a = arena
+        self.g = arena.group_alloc()
+
+    def _setup(self, incoming, outgoing, lookup, gc):
+        ids = []
+        for i in list(incoming) + list(outgoing):
+            if i not in ids:
+                ids.append(i)
+        assert len(ids) <= B.SLOTS
+        slot = {i: s for s, i in enumerate(ids)}
+        m_in = sum(1 << slot[i] for i in set(incoming))
+        m_out = sum(1 << slot[i] for i in set(outgoing))
+        self.a.group_set_conf(self.g, 0, 0, 0, None, 1)            # drop every Progress
+        self.a.group_set_conf(self.g, m_in, m_out, 0, None, 1)
+        self.a.set_group_commit(self.g, gc)
+        for i, s in slot.items():
+            p = self.a.progress_get(self.g, s)
+            p.matched, p.commit_group_id = lookup.get(i, (0, 0))   # missing voter == (0, 0)
+            self.a.progress_set(self.g, s, p)
+        return slot
+
+    def joint(self, incoming, outgoing, lookup, gc):
+        self._setup(incoming, outgoing, lookup, gc)
+        return self.a.maximal_committed_index(self.g)
+
+    def majority(self, voters, lookup, gc):
+        return self.joint(voters, [], lookup, gc)
+
+    def joint_vote(self, incoming, outgoing, votes):
+        slot = self._setup(incoming, outgoing, {}, False)
+        self.a.reset_votes(self.g)
+        for i, v in votes.items():
+            if i in slot:
+                self.a.record_vote(self.g, slot[i], v)
+        return self.a.vote_result(self.g)[2]
+
+    def majority_vote(self, voters, votes):
+        return self.joint_vote(voters, [], votes)
+
+    def impl(self):
+        return dd.Impl(self.majority, self.joint, self.majority_vote, self.joint_vote)
+
+
+def random_config_state(n, rng):
+    """Arbitrary configurations (joint, learners, group commit, no self) and per-peer states."""
+    c = O.new_columns(n, n)
+    for g in range(n):
+        inc = int(rng.integers(1, 256))
+        out = int(rng.integers(0, 256)) if rng.random() < 0.3 else 0
+        learners = int(rng.integers(0, 256)) & ~(inc | out) if rng.random() < 0.4 else 0
+        voters = [s_ for s_ in range(8) if (inc | out) >> s_ & 1]
+        self_slot = int(rng.choice(voters)) if rng.random() < 0.9 else None
+        c.meta[g] = O.make_meta(inc, out, learners, self_slot, group_commit=bool(rng.random() < 0.15))
+        base = int(rng.integers(100, 1 << 40))
+        c.last_index[g] = base + int(rng.integers(0, 10))
+        c.term_start[g] = (1 << 64) - 1 if rng.random() < 0.05 else max(1, base - int(rng.integers(0, 30)))
+        c.committed[g] = base - int(rng.integers(0, 40))
+        c.term[g] = int(rng.integers(1, 1000))
+        for s_ in range(8):
+            m = base - int(rng.integers(0, 50))
+            c.matched[s_, g] = m
+            c.next_idx[s_, g] = m + 1 + int(rng.integers(0, 5))
+            c.peer_committed[s_, g] = m - int(rng.integers(0, 5))
+            state = int(rng.choice([O.STATE_PROBE, O.STATE_REPLICATE, O.STATE_REPLICATE, O.STATE_SNAPSHOT]))
+            c.pflags[s_, g] = state | (O.PF_PAUSED if rng.random() < 0.3 else 0) | (O.PF_INS_FULL if rng.random() < 0.2 else 0) | \
+                (O.PF_RECENT_ACTIVE if rng.random() < 0.5 else 0)
+            c.pending_snapshot[s_, g] = m + int(rng.integers(0, 6)) if state == O.STATE_SNAPSHOT else 0
+            c.pending_request_snapshot[s_, g] = int(rng.integers(1, 100)) if rng.random() < 0.05 else 0
+            c.commit_group_id[s_, g] = int(rng.integers(0, 4))
+    return c
+
+
+def random_cell_batch(ref, n, rng, per_cell):
+    """Group-ordered batch; `per_cell` > 1 lets a (group, peer) cell receive several records."""
+    rows = []
+    for g in range(n):
+        if rng.random() < 0.3:
+            continue
+        meta = int(ref.meta[g])
+        has_self, self_slot = bool(meta & O.META_HAS_SELF), (meta >> 24) & 7
+        slots = rng.permutation(8)[: int(rng.integers(1, 6))]
+        for s_ in slots:
+            s_ = int(s_)
+            for _ in range(int(rng.integers(1, per_cell + 1))):
+                m, nx = int(ref.matched[s_, g]), int(ref.next_idx[s_, g])
+                kind = rng.random()
+                if has_self and s_ == self_slot:
+                    idx = m + int(rng.integers(0, 8))
+                    rows.append((g, s_, B.REC_LOCAL, 0, idx, 0 if rng.random() < 0.2 else idx + int(rng.integers(0, 5))))
+                elif kind < 0.7:
+                    idx = max(0, m + int(rng.integers(-6, 12)))
+                    commit = idx + 3 if rng.random() < 0.03 else max(0, idx - int(rng.integers(0, 300 if rng.random() < 0.05 else 6)))
+                    rows.append((g, s_, 0, 0, idx, commit))
+                else:
+                    idx = int(rng.choice([nx - 1, m, m + 1, m + 3, max(0, m - 2)]))
+                    rows.append((g, s_, B.REC_REJECT, 0, idx, max(0, m - int(rng.integers(0, 4)))))
+                    if rng.random() < 0.85:
+                        rows.append((g, s_, B.REC_EXT, 0, max(0, idx + int(rng.integers(-5, 3))),
+                                     int(rng.integers(1, 1 << 30)) if rng.random() < 0.2 else 0))
+    return np.array(rows, dtype=B.APPEND_RESP_DTYPE) if rows else np.zeros(0, dtype=B.APPEND_RESP_DTYPE)
+
+
+# k_tile.cuh: tile geometry and shared memory of the fused tile kernels
+TILE, GROUPS, MAX_STAGES = 256, 3, 8
+
+
+ROW64, ROW8 = (TILE + 2) * 8, TILE + 16
+
+
+SMEM = 227 * 1024 - 5 * 1024
+
+
+UNIT_CAP = 1536
+
+
+KERNELS = {"packed": (0, 0), "compact": (4 * UNIT_CAP, GROUPS * TILE * 4)}   # (payload bytes, extra bytes)
+
+
+def stage_bytes(h, payload):
+    return 3 * h * ROW64 + 3 * ROW64 + TILE * 4 + h * ROW8 + payload
+
+
+def stages(h, kernel):
+    payload, extra = KERNELS[kernel]
+    return min(MAX_STAGES, (SMEM - extra) // stage_bytes(h, payload))
+
+
+def plan(meta, force_general, kernel):
+    """tile_plan (arena.cu): (simple5 instantiation, hint, stages) of an arena whose groups hold `meta`."""
+    simple5 = not force_general and bool(is_simple5(meta).all())
+    hint = 0x1f if simple5 else int(np.bitwise_or.reduce((meta & 0xff) | ((meta >> 8) & 0xff)))
+    return simple5, hint, stages(bin(hint).count("1"), kernel)

@@ -101,3 +101,26 @@ def delivery_order(s, meta):
     taken = set(grant) | set(at_term) | set(at_top)
     stale = [i for i in range(len(meta)) if i not in taken]
     return grant + at_term + claimants + rest + stale, at_top
+
+
+def noise(rng, s, k):
+    """Frames the checks before the verdict settle: other types, garbage, truncated frames, a pair's high half on types
+    3 and 8, m.term 0 and groups past the arena's highest slot."""
+    out = []
+    for _ in range(k):
+        g = int(rng.choice(s.lows))
+        term = int(s.term[g])
+        kind = int(rng.integers(6))
+        if kind == 0:
+            out.append(F.frame(g, 0, F.message(int(rng.choice([5, 7, 10, 17])), term + 1, frm=2)))
+        elif kind == 1:
+            out.append(F.frame(g, 0, rng.integers(0, 256, int(rng.integers(1, 12)), dtype=np.uint8).tobytes()))
+        elif kind == 2:
+            out.append(F.frame(g, 0, F.message(4, term + 1, 1 << 40, frm=2)[:-3]))
+        elif kind == 3:
+            out.append(F.frame(g + 1 if s.wide[g] else g, 0, F.message(8, term + 1 if s.wide[g] else 0, frm=2)))
+        elif kind == 4:
+            out.append(F.frame(g, 1, F.message(9, 0, frm=2)))
+        else:
+            out.append(F.frame(s.n + int(rng.integers(1, 100)), 0, F.message(4, term + 1, frm=2)))
+    return out

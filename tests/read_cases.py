@@ -6,6 +6,7 @@ import numpy as np
 from oracle import oracle as O
 from oracle import read_oracle as RO
 from helpers import B
+import hb_frames as F
 from control_cmds import NO_TERM_START, META_WIDE_LO, META_WIDE_HI, cmds
 
 HB_CTX = B.REC_HEARTBEAT | B.REC_READ_CTX
@@ -294,3 +295,53 @@ def oracle_queue_view(q, n):
     k = np.arange(q.max_pending)[None, :] < q.count[:n, None]
     return (q.count[:n].copy(), np.where(k, q.ctx[:n], 0).astype(np.uint64), np.where(k, q.index[:n], 0).astype(np.uint64),
             np.where(k, q.acks[:n], 0).astype(np.uint16))
+
+
+def queues_equal(a, q, n, what):
+    got, want = a.read_index_read(0, n), oracle_queue_view(q, n)
+    for name, x, y in zip(("count", "ctx", "index", "acks"), got, want):
+        if not np.array_equal(x, y):
+            g = int(np.argwhere(x != y)[0][0])
+            raise AssertionError(f"{what}: queue {name} of group {g}: got {x[g]} want {y[g]}")
+
+
+def mixed_batch(rng, d, n, terms, reads, k):
+    """k frames, shuffled: append responses (accepts near matched, rejects without log_term), heartbeat responses
+    (contexts of length 0, 8 and others; ids pending, released earlier or never queued), other message types;
+    stale terms; several frames per cell (a wide group's peers 8..15 are named through its high half)."""
+    gs = rng.integers(0, n, k)
+    hi_half = (d.c.meta[gs] & META_WIDE_HI) != 0
+    slots = rng.integers(0, 8, k)
+    kind = rng.random(k)
+    stale = rng.random(k) < 0.05
+    qg = np.where(hi_half, gs - 1, gs)
+    frames = []
+    for i in range(k):
+        g, s = int(gs[i]), int(slots[i])
+        t = int(terms[g]) + (1 if stale[i] else 0)
+        if kind[i] < 0.35:     # MsgAppendResponse
+            m = int(d.c.matched[s, g])
+            if rng.random() < 0.1:
+                body = F.message(4, term=t, index=m + 1, reject=True, reject_hint=max(0, m - 1))
+            else:
+                body = F.message(4, term=t, index=m + int(rng.integers(0, 4)), commit=m)
+        elif kind[i] < 0.93:   # MsgHeartbeatResponse
+            r = rng.random()
+            ctx = None
+            if r < 0.55:
+                cnt = int(d.q.count[qg[i]])
+                x = int(d.q.ctx[qg[i], int(rng.integers(0, cnt))]) if cnt else int(rng.integers(1, 60))
+                ctx = F.ctx_bytes(x)
+            elif r < 0.65:
+                ctx = F.ctx_bytes(int(rng.integers(1, 1 << 62)))                 # never queued
+            elif r < 0.72:
+                ctx = bytes(rng.integers(0, 256, int(rng.choice([1, 7, 9, 16]))).astype(np.uint8))
+            body = F.message(9, term=t, commit=int(rng.integers(0, 80)), context=ctx)
+        else:                  # other types, some with a context
+            body = F.message(int(rng.choice([3, 6, 8, 15, 16])), term=t, index=5,
+                             context=F.ctx_bytes(7) if rng.random() < 0.5 else None)
+        frames.append(F.frame(g, s, body))
+    dup = rng.random(k) < 0.1                       # more frames for cells already in the batch
+    frames += [frames[j] for j in rng.integers(0, k, int(dup.sum()))]
+    order = rng.permutation(len(frames))
+    return F.batch([frames[j] for j in order])

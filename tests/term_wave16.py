@@ -27,7 +27,7 @@ import append_reject as R
 import app_follow as A
 import follow_term as T
 import leader_term as L
-import test_oracle_vote_request as TV
+import vote_request_frames as Q
 
 INS_CAP = 4
 COMMIT16_D = (I16_MAX, I16_MAX + 1, I16_MIN + 1, I16_MIN, 0)   # committed - persisted: the self slot's new peer_committed
@@ -177,7 +177,7 @@ def bump_world(rng, name, n_narrow, n_wide):
     filled and read requests queued -> (scenario, columns, votes, queues, fill commands, read requests).  The arena
     takes s.setup, then the columns (load_columns), then the fill commands and the requests."""
     s = T.scenario(rng, n_narrow, n_wide, p_role=ROLES[name])
-    c, vt = TV.state_of(s)
+    c, vt = Q.state_of(s)
     fill, _ = bump_edges16(s, c, rng)
     O.enable_inflights(c, INS_CAP)
     assert np.all(CO.arena_control(c, vt, fill)["status"] == 0)

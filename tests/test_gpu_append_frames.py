@@ -10,40 +10,12 @@ from oracle import app_frames_oracle as AF
 from helpers import B
 import app_frames as A
 import hb_frames as F
+import pass_forms as PF
 import offset16 as E
 
 pytestmark = pytest.mark.gpu
 
 ENTRY = ["group", "peer_slot", "flags", "next_idx"]
-
-
-def _device(a, first, n, ids, select, bytes_capacity=None, frames_capacity=None, rest_capacity=None):
-    """The device form -> (blob, offsets, rest, totals); the output buffers are sized at the bound."""
-    bound = B.append_frames_bound(n)
-    bcap = bound if bytes_capacity is None else bytes_capacity
-    fcap = 8 * n if frames_capacity is None else frames_capacity
-    rcap = 8 * n if rest_capacity is None else rest_capacity
-    d_ids, d_bytes = a.device_alloc(max(8, ids.nbytes)), a.device_alloc(max(16, bound))
-    d_off, d_rest, d_tot = a.device_alloc(4 * (8 * n + 1)), a.device_alloc(max(16, 16 * 8 * n)), a.device_alloc(32)
-    d_sel = a.device_alloc(select.nbytes) if select is not None else None
-    a.h2d(d_ids, ids)
-    if select is not None:
-        a.h2d(d_sel, select)
-    a.append_frames_device(first, n, d_sel, d_ids, d_bytes, bcap, d_off, fcap, d_rest, rcap, d_tot)
-    a.synchronize()
-    tot = np.zeros(4, np.uint64)
-    a.d2h(tot, d_tot)
-    blob, off = np.zeros(int(tot[1]), np.uint8), np.zeros(int(tot[0]) + 1, np.uint32)
-    rest = np.zeros(int(tot[2]), B.SEND_ENTRY_DTYPE)
-    if len(blob):
-        a.d2h(blob, d_bytes)
-    if len(rest):
-        a.d2h(rest, d_rest)
-    a.d2h(off, d_off)
-    for p in (d_ids, d_bytes, d_off, d_rest, d_tot, d_sel):
-        if p is not None:
-            a.device_free(p)
-    return blob, off, rest, tot
 
 
 def _check(a, c, first, n, ids, select, what):
@@ -55,7 +27,7 @@ def _check(a, c, first, n, ids, select, what):
     assert np.array_equal(off, want[1]), what
     assert np.array_equal(blob, want[0]), (what, int(np.argmax(blob != want[0])) if len(blob) == len(want[0]) else None)
     assert np.array_equal(rest, want[2]), what
-    dblob, doff, drest, dtot = _device(a, first, n, ids, select)
+    dblob, doff, drest, dtot = PF.broadcast(a, "append_frames", first, n, ids, select)
     assert dtot.tolist() == tot.tolist() and np.array_equal(doff, off) and np.array_equal(dblob, blob), what
     assert np.array_equal(drest, rest), what
     return want

@@ -18,41 +18,12 @@ from oracle import app_follow_oracle as AL
 import app_entries as E
 import app_follow as A
 import append_reject as R
-import test_gpu_follower_append_entries as GFE
-import test_gpu_wire_batches as WBT
+import pass_forms as PF
 
 pytestmark = pytest.mark.gpu
 
 W = importlib.import_module("raft-rs_b200.wire")
 HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-def _arena(c, n, runs):
-    a = B.Arena(n)
-    if runs:
-        a.enable_leader_runs()
-    assert a.group_alloc_range(n) == 0
-    a.load_columns(c)
-    a.column_write(B.COL_TERM, 0, 0, c.term[:n].copy())
-    return a
-
-
-def _apply_device(a, blob, off):
-    """raftgpu_wire_apply_device on a device copy of the batch -> status bytes."""
-    n = len(off) - 1
-    nb = (len(blob) + 15) & ~15
-    d_bytes, d_off, d_st = a.device_alloc(nb + 16), a.device_alloc(4 * (n + 1)), a.device_alloc(max(n, 1))
-    buf = np.zeros(nb, np.uint8)
-    buf[: len(blob)] = blob
-    a.h2d(d_bytes, buf)
-    a.h2d(d_off, np.ascontiguousarray(off, np.uint32))
-    a.wire_apply_device(d_bytes, len(blob), d_off, n, d_st)
-    a.synchronize()
-    st = np.zeros(n, np.uint8)
-    a.d2h(st, d_st)
-    for p in (d_bytes, d_off, d_st):
-        a.device_free(p)
-    return st
 
 
 def _random_batch(rng, logs, c, n_frames, golden=True):
@@ -99,13 +70,13 @@ def test_random_leaders_host_and_device_forms_against_the_oracle():
     n = 100_000
     logs, c, rows = _leaders(rng, n)
     blob, off = _random_batch(rng, logs, c, 300_000)
-    with_runs, without = _arena(c, n, True), _arena(c, n, False)
+    with_runs, without = R.leader_arena(c, n, True), R.leader_arena(c, n, False)
     assert (with_runs.leader_runs_set(rows) == 0).all()
     ref, ref0 = O.copy_columns(c), O.copy_columns(c)
     want = R.oracle_step(ref, rows, blob, off)
     want0 = R.oracle_step(ref0, None, blob, off)
-    got = _apply_device(with_runs, blob, off)
-    got0 = _apply_device(without, blob, off)
+    got = PF.device(with_runs, "wire_apply", blob, off)[0]
+    got0 = PF.device(without, "wire_apply", blob, off)[0]
     assert np.array_equal(got0, want0)
     bad = np.nonzero(got != want)[0]
     assert len(bad) == 0, [(int(i), hex(got[i]), hex(want[i])) for i in bad[:5]]
@@ -136,7 +107,7 @@ def test_stale_anchors_and_refusals():
     n = 64
     logs = [[0, 1, 1, 3, 3, 3, 5, 5, 7, 7, 7] for _ in range(n)]
     c = R.leader_columns(logs, n)
-    a = _arena(c, n, True)
+    a = R.leader_arena(c, n, True)
     rows = R.rows_for(logs, np.ones(n), 2)
     assert (a.leader_runs_set(rows) == 0).all()
     a.group_reset(1, 9, 10, 0, 0)
@@ -158,7 +129,7 @@ def test_stale_anchors_and_refusals():
                                        log_term=4)) for g in range(n)]
     blob, off = A.batch(frames)
     want = R.oracle_step(ref, rows, blob, off)
-    got = _apply_device(a, blob, off)
+    got = PF.device(a, "wire_apply", blob, off)[0]
     assert np.array_equal(got, want), [(g, hex(got[g]), hex(want[g])) for g in range(n) if got[g] != want[g]]
     st = got >> 4
     assert (st[[1, 2, 3, 4, 5]] == B.WIRE_NEEDS_LOG).all() and st[0] == B.WIRE_OK and (st[6:] == B.WIRE_OK).all()
@@ -237,7 +208,7 @@ def test_wide_pairs():
                                                                       log_term=lt if reject else 0)))
     blob, off = A.batch(frames)
     want = R.oracle_step(c, rows, blob, off)
-    got = _apply_device(a, blob, off)
+    got = PF.device(a, "wire_apply", blob, off)[0]
     bad = np.nonzero(got != want)[0]
     assert len(bad) == 0, [(int(i), hex(got[i]), hex(want[i])) for i in bad[:5]]
     assert_columns_equal(a.read_columns(n), c, n, "wide pairs")
@@ -286,7 +257,7 @@ def test_next_idx_offset_window_edges():
     blob, off = A.batch(frames)
     want = R.oracle_step(c, rows, blob, off)
     assert ((want >> 4) == B.WIRE_OK).all()
-    got = _apply_device(a, blob, off)
+    got = PF.device(a, "wire_apply", blob, off)[0]
     assert np.array_equal(got, want)
     got_c = a.read_columns(n)
     assert_columns_equal(got_c, c, n, "offset window edges")
@@ -304,7 +275,7 @@ def test_setter_between_begin_and_wait():
     n = 20_000
     logs = [R.random_log(rng, int(rng.integers(2, 7))) for _ in range(n)]
     c = R.leader_columns(logs, n)
-    a = _arena(c, n, True)
+    a = R.leader_arena(c, n, True)
     rows = R.rows_for(logs, np.ones(n), 2)
     none = np.zeros(n, LR.ROW_DTYPE)
     ref = O.copy_columns(c)
@@ -382,7 +353,7 @@ def test_round_trip_after_an_election_100k_x5():
     c.meta[:n] = O.make_meta((1 << P) - 1, self_slot=0)
     c.next_idx[:, :n] = ts                                                   # reset(): last_index + 1 before the append
     c.matched[0, :n] = ts
-    la = _arena(c, n, True)
+    la = R.leader_arena(c, n, True)
     rows = R.rows_for(leaders, np.ones(n), 2)
     assert (la.leader_runs_set(rows) == 0).all()
     ids = rng.integers(1, 1 << 40, (P, n), dtype=np.uint64)
@@ -411,8 +382,8 @@ def test_round_trip_after_an_election_100k_x5():
             fa.column_write(col, 0, 0, getattr(fc, name)[:n].copy())
         want_table = table.copy()
         w = AE.batch(fc, None, want_table, fblob, foff)
-        got = GFE._device(fa, fblob, foff, table)
-        WBT._equal(w, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), GFE.NAMES, ("slot", sl))
+        got = PF.device(fa, "follower_append_entries", fblob, foff, table)
+        PF.equal(w, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), E.NAMES, ("slot", sl))
         fa.close()
         st = w[0] >> 4
         assert set(np.unique(st).tolist()) <= {B.WIRE_OK, B.WIRE_NEEDS_LOG}
@@ -439,7 +410,7 @@ def test_round_trip_after_an_election_100k_x5():
     ref = O.copy_columns(c)
     want = R.oracle_step(ref, rows, blob, off)
     O.arena_recompute(ref)
-    la.step_begin_wire(WBT._host_batch(blob, off, len(blob)), B.STEP_READ_COMMITTED)
+    la.step_begin_wire(PF.host_batch(blob, off, len(blob)), B.STEP_READ_COMMITTED)
     la.step_wait()
     got = la.wire_status().copy()
     assert np.array_equal(got, want)
@@ -452,7 +423,7 @@ def test_round_trip_after_an_election_100k_x5():
     for i in undecided.tolist():
         recs.append(tuple(lrecs[i]))
         recs.append((lrecs["group"][i], lrecs["peer_slot"][i], B.REC_EXT, 0, lhint[i], lsnap[i]))
-    rb = WBT._host_batch(np.zeros(0, np.uint8), np.zeros(1, np.uint32), 0)
+    rb = PF.host_batch(np.zeros(0, np.uint8), np.zeros(1, np.uint32), 0)
     rb.records = np.array(recs, B.APPEND_RESP_DTYPE)
     rb.n_records = len(rb.records)
     la.step_begin_wire(rb, B.STEP_READ_COMMITTED)

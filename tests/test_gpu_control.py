@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 from oracle import control_oracle as CO
-from helpers import B, O, Shape, assert_columns_equal, bitmap_to_bool, random_batch, random_state
+from helpers import (B, O, Shape, assert_columns_equal, assert_state_equal, full_state, random_batch,
+                     random_state, records_step, scatter_step)
 from control_cmds import NO_TERM_START, cmds, random_list
 
 pytestmark = pytest.mark.gpu
@@ -55,51 +56,6 @@ def single(arena, m):
         rc = L.raftgpu_progress_op(h, g, s, arg, a[0], a[1], a[2], C.byref(out))
         return rc, out.value if rc == B.OK else 0
     return B.ERR_INVALID, 0
-
-
-def full_state(arena, n, inflights=False):
-    """Every column of groups [0, n): the host-column set, votes, term and (with inflights) the Inflights meta."""
-    c = arena.read_columns(n)
-    votes = np.stack([arena.column_read(B.COL_VOTES, s, 0, n, np.uint8) for s in range(B.SLOTS)])
-    c.term[:] = arena.column_read(B.COL_TERM, 0, 0, n, np.uint64)
-    ins = None
-    if inflights:
-        ins = np.stack([arena.column_read(B.COL_INS_META, s, 0, n, np.uint32) for s in range(B.SLOTS)])
-    return c, votes, ins
-
-
-def assert_state_equal(a, b, n, what):
-    ca, va, ia = a
-    cb, vb, ib = b
-    assert_columns_equal(ca, cb, n, what)
-    assert np.array_equal(ca.term[:n], cb.term[:n]), f"{what}: term"
-    assert np.array_equal(va[:, :n], vb[:, :n]), f"{what}: votes"
-    if ia is not None or ib is not None:
-        assert np.array_equal(ia[:, :n], ib[:, :n]), f"{what}: ins_meta"
-
-
-def records_step(arena, n, recs, ref, what):
-    """raftgpu_step_begin_records (the library picks the kernel from its launch plan), checked against the oracle."""
-    arena.step_begin_records(recs, B.STEP_READ_COMMITTED)
-    r = arena.step_wait()
-    O.arena_apply(ref, recs, mode=0)
-    want_adv, want_bm, _, _ = O.arena_recompute(ref)
-    assert r.n_advanced == want_adv, what
-    bm, com = arena.step_results(n)
-    assert np.array_equal(bm, want_bm[: len(bm)]), what
-    adv = bitmap_to_bool(bm, n)
-    assert np.array_equal(com[adv], ref.committed[:n][adv]), what
-    assert_columns_equal(arena.read_columns(n), ref, n, what)
-
-
-def scatter_step(arena, n, recs, ref, what):
-    """Enqueued records and raftgpu_step, checked against the oracle."""
-    arena.enqueue(recs)
-    r = arena.step(B.STEP_READ_COMMITTED)
-    O.arena_apply(ref, recs, mode=0)
-    want_adv, _, _, _ = O.arena_recompute(ref)
-    assert r.n_advanced == want_adv, what
-    assert_columns_equal(arena.read_columns(n), ref, n, what)
 
 
 N_NARROW, N_WIDE = 4088, 4   # 4096 group slots: 4088 narrow groups, then 4 wide pairs

@@ -10,9 +10,9 @@ import numpy as np
 import pytest
 
 from oracle import control_oracle as CO
-from helpers import B, O, Shape, TILE_SHAPES, assert_columns_equal, is_simple5, random_batch, random_state
+from helpers import (B, O, Shape, TILE_SHAPES, assert_columns_equal, assert_state_equal, full_state, is_simple5,
+                     random_batch, random_state, records_step, scatter_step)
 from control_cmds import cmds
-from test_gpu_control import assert_state_equal, full_state, records_step, scatter_step
 
 pytestmark = pytest.mark.gpu
 

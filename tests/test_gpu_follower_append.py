@@ -11,90 +11,25 @@ from helpers import B, O
 import app_follow as A
 import hb_follow as FL
 import hb_frames as F
+import pass_forms as PF
 import wire_batches as WB
-import test_gpu_append_frames as GAF
-import test_gpu_wire_batches as WBT
 
 pytestmark = pytest.mark.gpu
 
 P = 8
 U64 = A.U64
 OK = A.LOG_STATUS_OK
-NAMES = ("status", "from", "response bytes", "response offsets", "totals")
-
-
-def _device(a, blob, off, table, n_bytes=None):
-    """The device form over buffers from raftgpu_device_alloc -> (status, from, response blob, offsets, totals)."""
-    n = len(off) - 1
-    bound = B.follower_append_bound(n)
-    bufs = [a.device_alloc(x) for x in (max(16, len(blob)), 4 * (n + 1), max(16, table.nbytes), max(1, n), 8 * max(1, n),
-                                         max(16, bound), 4 * (n + 1), 16)]
-    d_b, d_o, d_t, d_st, d_f, d_rb, d_ro, d_tot = bufs
-    for p, x in ((d_b, blob), (d_o, off), (d_t, table)):
-        if x.nbytes:
-            a.h2d(p, x)
-    a.follower_append_device(d_b, len(blob) if n_bytes is None else n_bytes, d_o, n, d_t, d_st, d_f, d_rb, bound, d_ro, d_tot)
-    a.synchronize()
-    tot = np.zeros(2, np.uint64)
-    a.d2h(tot, d_tot)
-    st, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
-    rb, ro = np.zeros(int(tot[1]), np.uint8), np.zeros(int(tot[0]) + 1, np.uint32)
-    if n:
-        a.d2h(st, d_st), a.d2h(frm, d_f)
-    a.d2h(ro, d_ro)
-    if len(rb):
-        a.d2h(rb, d_rb)
-    for p in bufs:
-        a.device_free(p)
-    return st, frm, rb, ro, tot
-
-
-def _host(a, blob, off, table, n_bytes=None):
-    return a.follower_append(WBT._host_batch(blob, off, len(blob) if n_bytes is None else n_bytes), _full(a, table))
-
-
-def _full(a, table):
-    t = np.zeros(a.get_info().hi, AL.LOG_DTYPE)
-    t[: min(len(t), len(table))] = table[: len(t)]
-    return t
-
-
-def _group_state(a, n):
-    c = a.read_columns(n)
-    return {"committed": c.committed, "last_index": c.last_index, "term_start": c.term_start,
-            "term": a.column_read(B.COL_TERM, 0, 0, n, np.uint64), "meta": c.meta}
 
 
 def _compare(a, c, q, blob, off, table, device, what, n_bytes=None):
     want = AL.batch(c, q, table, blob, off, n_bytes=n_bytes)
-    got = (_device if device else _host)(a, blob, off, table, n_bytes)
-    WBT._equal(want, got, NAMES, what)
-    s = _group_state(a, c.n_groups)
+    got = PF.device(a, "follower_append", blob, off, table, n_bytes=n_bytes) if device else \
+        A.host_form(a, blob, off, table, n_bytes)
+    PF.equal(want, got, A.NAMES, what)
+    s = FL.group_state(a, c.n_groups)
     for name, col in s.items():
         assert np.array_equal(col, getattr(c, name)[: c.n_groups]), (what, name)
     return want
-
-
-def _follower_arena(n_narrow, n_wide, cols, reads=False, extra=64):
-    """An arena of n_narrow groups then n_wide pairs, its group columns written from cols (name -> u64[n]) -> (arena, host
-    columns with c.term, read queues or None)."""
-    n = n_narrow + 2 * n_wide
-    a = B.Arena(n + extra)
-    if reads:
-        a.enable_read_index(P)
-    assert a.group_alloc_range(n_narrow) == 0
-    for k in range(n_wide):
-        assert a.group_alloc_wide() == n_narrow + 2 * k
-    for col, arr in cols.items():
-        a.column_write(col, 0, 0, np.ascontiguousarray(arr[:n], np.uint64))
-    c = a.read_columns(n)
-    c.term = a.column_read(B.COL_TERM, 0, 0, n, np.uint64)
-    q = None
-    if reads:
-        from oracle import read_oracle as RO
-        q = RO.ReadQueues(c.cap, P)
-        q.allocated[:n] = 1
-    return a, c, q
 
 
 # --------------------------------------------------------------------------- 1. random 100K-group follower arenas
@@ -116,42 +51,13 @@ def _leader_frames(seed, n_l):
     for k in range(B.SLOTS):
         la.column_write(B.COL_NEXT_IDX, k, 0, (c.last_index[:n_l] + 1).astype(np.uint64))
         la.column_write(B.COL_PFLAGS, k, 0, np.full(n_l, B.STATE_REPLICATE, np.uint8))
-    blob, off, rest, tot = GAF._device(la, 0, n_l, rng.integers(1, 1 << 63, (9, n_l), dtype=np.uint64), None)
+    blob, off, rest, tot = PF.broadcast(la, "append_frames", 0, n_l, rng.integers(1, 1 << 63, (9, n_l), dtype=np.uint64), None)
     la.close()
     assert int(tot[0]) > 3 * n_l
     out = []
     for _, body in FL.frames_of(blob, off):
         m = O.wire_decode_message(body)
         out.append((m["term"], m["index"], m["commit"], body))
-    return out
-
-
-def _hostile(rng, terms, k):
-    """k frames that must not pass or that go back to the host: garbage, unknown groups, truncations, other types,
-    frames with entries, term 0, stale and future terms, a commit out of range."""
-    out, n_f = [], len(terms)
-    for j in range(k):
-        g, x = int(rng.integers(0, n_f)), int(rng.integers(16))
-        t = int(terms[g])
-        kind = j % 9
-        if kind == 0:
-            out.append(A.frame(g, x, rng.integers(0, 256, int(rng.integers(0, 24)), dtype=np.uint8).tobytes()))
-        elif kind == 1:
-            out.append(A.frame(n_f + int(rng.integers(0, 100)), x, A.message(3, term=t, index=1)))
-        elif kind == 2:
-            out.append(A.frame(g, x, A.message(3, term=t, index=5, commit=1 << 40, frm=3)[:-1]))
-        elif kind == 3:
-            out.append(A.frame(g, x, A.message(int(rng.choice([4, 8, 9, 17])), term=t, index=1)))
-        elif kind == 4:
-            out.append(A.frame(g, x, A.message(3, term=t, index=1, frm=2, entries=[(t, 2)] * int(rng.integers(1, 3)))))
-        elif kind == 5:
-            out.append(A.frame(g, x, A.message(3, term=0, index=1)))
-        elif kind == 6:
-            out.append(A.frame(g, x, A.message(3, term=max(1, t + int(rng.choice([-1, 1]))), index=1)))
-        elif kind == 7:                                                # matches above last_index, commit_to out of range
-            out.append(A.frame(g, x, A.message(3, term=t, log_term=0, index=U64 - 1, commit=U64 - 1, frm=2)))
-        else:
-            out.append(np.array([g << 4 | x], "<u4").tobytes()[: int(rng.integers(0, 4))])
     return out
 
 
@@ -179,7 +85,7 @@ def test_random_arenas_vs_oracle(reads):
     terms[hi] = terms[hi - 1]
     term_start = np.where(rng.random(n) < 0.05, np.uint64(1), np.uint64(A.NO_TERM_START))
     cols = {B.COL_TERM: terms, B.COL_LAST_INDEX: last, B.COL_COMMITTED: committed, B.COL_TERM_START: term_start}
-    a, c, q = _follower_arena(N_NARROW, N_WIDE, cols, reads)
+    a, c, q = A.follower_arena(N_NARROW, N_WIDE, cols, reads)
     table = np.zeros(n, AL.LOG_DTYPE)
     table["id"] = rng.integers(1, 1 << 63, n, dtype=np.uint64)
     table["flags"] = np.where(rng.random(n) < 0.95, AL.SELECT, 0)
@@ -192,7 +98,7 @@ def test_random_arenas_vs_oracle(reads):
         order = rng.permutation(nl)
         order = np.concatenate([order, order[rng.random(nl) < 0.15]])   # repeated frames: DUP
         frames = [A.frame(int(fg[i]), int(rng.integers(16)), leader[i][3]) for i in order]
-        frames += _hostile(rng, terms, nl // 20)
+        frames += A.hostile(rng, terms, nl // 20)
         frames = [frames[i] for i in rng.permutation(len(frames))]
         blob, off = A.batch(frames)
         st = _compare(a, c, q, blob, off, table, device, ("round", rnd))[0]
@@ -220,7 +126,7 @@ def test_edges():
     committed = np.minimum(last, pick(n))
     cols = {B.COL_TERM: terms, B.COL_LAST_INDEX: last, B.COL_COMMITTED: committed,
             B.COL_TERM_START: np.full(n, A.NO_TERM_START, np.uint64)}
-    a, c, _ = _follower_arena(n, 0, cols)
+    a, c, _ = A.follower_arena(n, 0, cols)
     table = np.zeros(n, AL.LOG_DTYPE)
     table["id"], table["flags"] = pick(n), AL.SELECT
     kind = rng.integers(0, 3, n)                                       # empty, length one, from an edge value
@@ -265,17 +171,18 @@ class Followers:
         c = self.w.columns()
         cols = {B.COL_TERM: c.term, B.COL_LAST_INDEX: c.last_index, B.COL_COMMITTED: c.committed,
                 B.COL_TERM_START: c.term_start}
-        a, hc, _ = _follower_arena(self.n, 0, cols)
+        a, hc, _ = A.follower_arena(self.n, 0, cols)
         return a, hc
 
     def run(self, a, c, buf, n_bytes, off, device, what):
         want = AL.batch(c, None, self.table, buf, off, n_bytes=n_bytes)
-        got = (_device if device else _host)(a, buf, off, self.table, n_bytes)
-        WBT._equal(want, got, NAMES, what)
+        got = PF.device(a, "follower_append", buf, off, self.table, n_bytes=n_bytes) if device else \
+            A.host_form(a, buf, off, self.table, n_bytes)
+        PF.equal(want, got, A.NAMES, what)
         return got
 
     def check(self, a, c, what):
-        s = _group_state(a, self.n)
+        s = FL.group_state(a, self.n)
         for name, col in s.items():
             assert np.array_equal(col, getattr(c, name)[: self.n]), (what, name)
 
@@ -283,7 +190,7 @@ class Followers:
 @pytest.mark.parametrize("device", [False, True], ids=["host", "device"])
 def test_across_the_stage(device):
     sc = Followers(0xAF30, 20_000)
-    frames, ballast = WBT.stage_batch(sc, 0xAF31)
+    frames, ballast = WB.stage_batch(sc, 0xAF31)
     blob, off = F.batch(frames)
     assert WB.geometry(off, len(blob)) >= {WB.STAGED, WB.SPAN, "frame>16K", "frame>64K"}
     a, c = sc.fresh()
@@ -309,7 +216,7 @@ def test_hostile_offsets(device):
     if not device:
         blob, off = F.batch(sc.frames(np.random.default_rng(1)))
         sc.run(a, c, blob, len(blob), off, False, "valid")
-    for k, (buf, n_bytes, off) in enumerate(WBT.hostile_batches(sc, 0xAF33, device)):
+    for k, (buf, n_bytes, off) in enumerate(WB.hostile_batches(sc, 0xAF33, device)):
         got = sc.run(a, c, buf, n_bytes, off, device, k)[0]
         sc.check(a, c, k)
         seen += np.bincount(got >> 4, minlength=16)
@@ -323,8 +230,8 @@ def test_refusals_before_any_launch():
     n_g = 64
     cols = {B.COL_TERM: np.full(n_g, 3, np.uint64), B.COL_LAST_INDEX: np.full(n_g, 9, np.uint64),
             B.COL_TERM_START: np.full(n_g, A.NO_TERM_START, np.uint64)}
-    a, c, _ = _follower_arena(n_g, 0, cols)
-    before = _group_state(a, n_g)
+    a, c, _ = A.follower_arena(n_g, 0, cols)
+    before = FL.group_state(a, n_g)
     L, h = a._L, a._h
     n = 16
     blob, off = A.batch([A.frame(g, 0, A.message(3, term=3, log_term=3, index=9, commit=7, frm=2)) for g in range(n)])
@@ -332,36 +239,28 @@ def test_refusals_before_any_launch():
     assert bound == 85 * n
     table = np.zeros(a.get_info().hi, AL.LOG_DTYPE)
     table["id"], table["run_start"], table["run_term"], table["flags"] = 5, 1, 3, AL.SELECT
-    d_b, d_o, d_t = a.device_alloc(1024), a.device_alloc(4 * (n + 1)), a.device_alloc(table.nbytes + 16)
-    d_st, d_f, d_rb, d_ro, d_tot = a.device_alloc(n), a.device_alloc(8 * n), a.device_alloc(bound + 64), \
-        a.device_alloc(4 * (n + 1)), a.device_alloc(16)
-    for p, x in ((d_b, blob), (d_o, off), (d_t, table), (d_st, np.full(n, 0xEE, np.uint8)), (d_tot, np.full(2, 77, np.uint64)),
-                 (d_rb, np.full(bound + 64, 0xCD, np.uint8))):
-        a.h2d(p, x)
     nb = len(blob)
-    dev = lambda **k: L.raftgpu_follower_append_device(h, None, k.get("b", d_b), k.get("nb", nb), d_o, k.get("n", n),
-                                                       k.get("t", d_t), d_st, d_f, k.get("rb", d_rb), k.get("cap", bound),
-                                                       k.get("ro", d_ro), k.get("tot", d_tot))
-    big = (1 << 32) // 85 + 1                                   # the first n whose bound exceeds u32 offsets
-    assert B.follower_append_bound(big - 1) < (1 << 32) <= B.follower_append_bound(big)
-    refused = [dev(cap=bound - 1), dev(cap=0), dev(b=d_b + 4), dev(rb=d_rb + 8), dev(t=d_t + 8), dev(n=big, cap=85 * big),
-               dev(n=1 << 32, cap=U64), dev(nb=1 << 32), dev(t=None), dev(ro=None), dev(tot=None), dev(b=None)]
-    assert refused == [B.ERR_INVALID] * len(refused), refused
-    st, tot, rb = np.zeros(n, np.uint8), np.zeros(2, np.uint64), np.zeros(bound, np.uint8)
-    ro = np.zeros(n + 1, np.uint32)
-    host = lambda cap, t=table: L.raftgpu_follower_append(h, blob.ctypes.data, nb, off.ctypes.data, n,
-                                                          None if t is None else t.ctypes.data, st.ctypes.data, None,
-                                                          rb.ctypes.data, cap, ro.ctypes.data, tot.ctypes.data)
-    assert host(bound - 1) == B.ERR_INVALID and host(bound, None) == B.ERR_INVALID
-    a.synchronize()
-    gst, gt, grb = np.zeros(n, np.uint8), np.zeros(2, np.uint64), np.zeros(bound + 64, np.uint8)
-    a.d2h(gst, d_st), a.d2h(gt, d_tot), a.d2h(grb, d_rb)
-    assert np.all(gst == 0xEE) and gt.tolist() == [77, 77] and np.all(grb == 0xCD)   # nothing was launched
-    after = _group_state(a, n_g)
-    assert all(np.array_equal(before[k], after[k]) for k in before)
-    # the exact bound is accepted, and the host form equals the device form
-    assert host(bound) == B.OK and tot.tolist()[0] == n and np.all(st == OK)
-    assert np.all(a.read_columns(n_g).committed[:n] == 7)
+    with PF.refusals(a, "follower_append", blob, off, table) as r:
+        dev, d = r.call, r.args
+        a.h2d(d["rb"], np.full(bound + 64, 0xCD, np.uint8))
+        big = (1 << 32) // 85 + 1                                   # the first n whose bound exceeds u32 offsets
+        assert B.follower_append_bound(big - 1) < (1 << 32) <= B.follower_append_bound(big)
+        refused = [dev(cap=bound - 1), dev(cap=0), dev(b=d["b"] + 4), dev(rb=d["rb"] + 8), dev(l=d["l"] + 8), dev(n=big, cap=85 * big),
+                   dev(n=1 << 32, cap=U64), dev(nb=1 << 32), dev(l=None), dev(ro=None), dev(t=None), dev(b=None)]
+        assert refused == [B.ERR_INVALID] * len(refused), refused
+        st, tot, rb = np.zeros(n, np.uint8), np.zeros(2, np.uint64), np.zeros(bound, np.uint8)
+        ro = np.zeros(n + 1, np.uint32)
+        host = lambda cap, t=table: L.raftgpu_follower_append(h, blob.ctypes.data, nb, off.ctypes.data, n,
+                                                              None if t is None else t.ctypes.data, st.ctypes.data, None,
+                                                              rb.ctypes.data, cap, ro.ctypes.data, tot.ctypes.data)
+        assert host(bound - 1) == B.ERR_INVALID and host(bound, None) == B.ERR_INVALID
+        grb = r.read("rb", np.zeros(bound + 64, np.uint8))
+        assert r.untouched() and np.all(grb == 0xCD)   # nothing was launched
+        after = FL.group_state(a, n_g)
+        assert all(np.array_equal(before[k], after[k]) for k in before)
+        # the exact bound is accepted, and the host form equals the device form
+        assert host(bound) == B.OK and tot.tolist()[0] == n and np.all(st == OK)
+        assert np.all(a.read_columns(n_g).committed[:n] == 7)
     a.close()
 
 
@@ -398,7 +297,7 @@ def test_full_commit_loop_1m():
     sel = bm
     # the oracle chain
     want_blob, want_off, want_rest, want_tot = AF.bcast_append(c, None, 0, n, ids, sel)
-    blob, off, rest, tot = GAF._device(la, 0, n, ids, sel)
+    blob, off, rest, tot = PF.broadcast(la, "append_frames", 0, n, ids, sel)
     assert np.array_equal(blob, want_blob) and np.array_equal(off, want_off) and tot.tolist() == want_tot.tolist()
     frames = int(tot[0])
     assert frames > 10_000 and len(rest) < frames, tot
@@ -425,8 +324,8 @@ def test_full_commit_loop_1m():
             fa.column_write(col, 0, 0, getattr(fc, name)[:n].copy())
         w = AL.batch(fc, None, table, fblob, foff)
         assert np.all(w[0] == OK), np.bincount(w[0])
-        got = _device(fa, fblob, foff, table)
-        WBT._equal(w, got, NAMES, ("follower slot", s_))
+        got = PF.device(fa, "follower_append", fblob, foff, table)
+        PF.equal(w, got, A.NAMES, ("follower slot", s_))
         assert np.array_equal(fa.read_columns(n).committed, fc.committed[:n]), s_
         fas.append(fa)
         back_parts.append((w[2], w[3]))
@@ -508,13 +407,13 @@ def test_host_form_between_begin_and_wait():
         frames += [frames[i] for i in rng.integers(0, len(frames), len(frames) // 8)]   # repeated frames: DUP
         blob, off = A.batch(frames)
         want = AL.batch(c, None, table, blob, off)
-        WBT._equal(want, _device(twin, blob, off, table), NAMES, ("device form after the step", rnd))
+        PF.equal(want, PF.device(twin, "follower_append", blob, off, table), A.NAMES, ("device form after the step", rnd))
         a.step_begin_records(recs, B.STEP_READ_COMMITTED)
-        during = [x.copy() for x in _host(a, blob, off, table)]
+        during = [x.copy() for x in A.host_form(a, blob, off, table)]
         assert a.step_wait().n_advanced == 0
-        WBT._equal(want, during, NAMES, ("host form during the step", rnd))
+        PF.equal(want, during, A.NAMES, ("host form during the step", rnd))
         for x in (a, twin):
-            st = _group_state(x, n)
+            st = FL.group_state(x, n)
             for name in ("committed", "last_index", "term", "term_start"):
                 assert np.array_equal(st[name], getattr(c, name)[:n]), (rnd, name)
         kinds += np.bincount(want[0] >> 4, minlength=16)

@@ -15,47 +15,9 @@ from helpers import B, O
 import app_entries as E
 import app_follow as A
 import hb_follow as FL
-import test_gpu_follower_append as GFA
-import test_gpu_wire_batches as WBT
+import pass_forms as PF
 
 pytestmark = pytest.mark.gpu
-
-WIDE_LO = 0x20000000  # RAFTGPU_META_WIDE_LO
-NAMES = ("status", "from", "appended", "response bytes", "response offsets", "totals")
-
-
-def _device(a, blob, off, table, n_bytes=None):
-    """The device form over buffers from raftgpu_device_alloc -> (status, from, appended, response blob, offsets,
-    totals); table (the full table) is updated in place from the device's copy."""
-    n = len(off) - 1
-    bound = B.follower_append_bound(n)
-    bufs = [a.device_alloc(x) for x in (max(16, len(blob)), 4 * (n + 1), max(16, table.nbytes), max(1, n), 8 * max(1, n),
-                                         40 * max(1, n), max(16, bound), 4 * (n + 1), 16)]
-    d_b, d_o, d_t, d_st, d_f, d_ap, d_rb, d_ro, d_tot = bufs
-    for p, x in ((d_b, blob), (d_o, off), (d_t, table)):
-        if x.nbytes:
-            a.h2d(p, x)
-    a.follower_append_entries_device(d_b, len(blob) if n_bytes is None else n_bytes, d_o, n, d_t, d_st, d_f, d_ap, d_rb,
-                                     bound, d_ro, d_tot)
-    a.synchronize()
-    tot = np.zeros(2, np.uint64)
-    a.d2h(tot, d_tot)
-    st, frm, app = np.zeros(n, np.uint8), np.zeros(n, np.uint64), np.zeros(n, B.FOLLOWER_APPENDED_DTYPE)
-    rb, ro = np.zeros(int(tot[1]), np.uint8), np.zeros(int(tot[0]) + 1, np.uint32)
-    if n:
-        a.d2h(st, d_st), a.d2h(frm, d_f), a.d2h(app, d_ap)
-    a.d2h(ro, d_ro)
-    if len(rb):
-        a.d2h(rb, d_rb)
-    if table.nbytes:
-        a.d2h(table, d_t)
-    for p in bufs:
-        a.device_free(p)
-    return st, frm, app, rb, ro, tot
-
-
-def _host(a, blob, off, table, n_bytes=None):
-    return a.follower_append_entries(WBT._host_batch(blob, off, len(blob) if n_bytes is None else n_bytes), table)
 
 
 def _compare(a, c, q, blob, off, table, device, what, n_bytes=None):
@@ -63,32 +25,12 @@ def _compare(a, c, q, blob, off, table, device, what, n_bytes=None):
     the oracle's result; every output, the table and the group columns must agree."""
     want_table = table.copy()
     want = AE.batch(c, q, want_table, blob, off, n_bytes=n_bytes)
-    got = (_device if device else _host)(a, blob, off, table, n_bytes)
-    WBT._equal(want, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), NAMES, what)
+    got = PF.run(a, "follower_append_entries", blob, off, table, device=device, n_bytes=n_bytes)
+    PF.equal(want, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), E.NAMES, what)
     assert np.array_equal(table, want_table), (what, "table")
-    for name, col in GFA._group_state(a, c.n_groups).items():
+    for name, col in FL.group_state(a, c.n_groups).items():
         assert np.array_equal(col, getattr(c, name)[: c.n_groups]), (what, name)
     return want
-
-
-def _world(rng, n_narrow, n_wide, reads):
-    n = n_narrow + 2 * n_wide
-    terms = rng.integers(2, 1000, n).astype(np.uint64)
-    last = rng.integers(0, 1 << 20, n).astype(np.uint64)
-    committed = last - np.minimum(last, rng.integers(0, 40, n).astype(np.uint64))
-    hi = np.arange(n_narrow + 1, n, 2)
-    terms[hi] = terms[hi - 1]
-    term_start = np.where(rng.random(n) < 0.03, np.uint64(1), np.uint64(A.NO_TERM_START))
-    cols = {B.COL_TERM: terms, B.COL_LAST_INDEX: last, B.COL_COMMITTED: committed, B.COL_TERM_START: term_start}
-    a, c, q = GFA._follower_arena(n_narrow, n_wide, cols, reads)
-    table = np.zeros(a.get_info().hi, AL.LOG_DTYPE)
-    table["id"][:n] = rng.integers(1, 1 << 63, n, dtype=np.uint64)
-    table["flags"][:n] = np.where(rng.random(n) < 0.97, AL.SELECT, 0)
-    top = np.maximum(c.last_index[:n], np.concatenate([c.last_index[1:n], [0]]))
-    table["run_start"][:n] = np.where(rng.random(n) < 0.95, top - np.minimum(top, rng.integers(0, 50, n).astype(np.uint64)),
-                                      top + 1)
-    table["run_term"][:n] = terms - rng.integers(0, 2, n).astype(np.uint64)
-    return a, c, q, table
 
 
 def _frames(rng, c, table, groups, big, hostile):
@@ -96,15 +38,12 @@ def _frames(rng, c, table, groups, big, hostile):
     out = []
     for g in groups.tolist():
         lo = g
-        last = int(max(c.last_index[g], c.last_index[g + 1])) if c.meta[g] & WIDE_LO else int(c.last_index[g])
-        com = int(max(c.committed[g], c.committed[g + 1])) if c.meta[g] & WIDE_LO else int(c.committed[g])
+        last = int(max(c.last_index[g], c.last_index[g + 1])) if c.meta[g] & E.WIDE_LO else int(c.last_index[g])
+        com = int(max(c.committed[g], c.committed[g + 1])) if c.meta[g] & E.WIDE_LO else int(c.committed[g])
         body = E.random_frame(rng, last, int(table["run_start"][lo]), int(table["run_term"][lo]), int(c.term[g]), com,
                               big=big, hostile=hostile)
         out.append(A.frame(g, int(rng.integers(16)), body))
     return out
-
-
-N_NARROW, N_WIDE = 99_000, 500
 
 
 @pytest.mark.parametrize("reads", [False, True], ids=["no_read_queues", "read_queues"])
@@ -112,9 +51,9 @@ def test_random_arenas_vs_oracle(reads):
     """100K groups; each round: one frame per group for most groups (the first half with payloads up to 128 bytes, the
     second up to 20 000), repeated frames (DUP) and garbage."""
     rng = np.random.default_rng(0xAE10 + reads)
-    n = N_NARROW + 2 * N_WIDE
-    a, c, q, table = _world(rng, N_NARROW, N_WIDE, reads)
-    hi = set(range(N_NARROW + 1, n, 2))
+    n = E.N_NARROW + 2 * E.N_WIDE
+    a, c, q, table = E.world(rng, E.N_NARROW, E.N_WIDE, reads)
+    hi = set(range(E.N_NARROW + 1, n, 2))
     kinds = np.zeros(16, np.int64)
     appended = 0
     for rnd, device in enumerate((True, False, True)):
@@ -122,7 +61,7 @@ def test_random_arenas_vs_oracle(reads):
         half = len(gs) // 2
         frames = _frames(rng, c, table, gs[:half], False, 0.02) + _frames(rng, c, table, gs[half:], True, 0.02)
         frames += [frames[i] for i in rng.integers(0, len(frames), len(frames) // 20)]   # DUP
-        frames += GFA._hostile(rng, c.term[:n], 2000)
+        frames += A.hostile(rng, c.term[:n], 2000)
         blob, off = A.batch(frames)
         st, _, app, *_ = _compare(a, c, q, blob, off, table, device, ("round", rnd))
         kinds += np.bincount(st >> 4, minlength=16)
@@ -164,7 +103,7 @@ def test_stage_paths_with_appended_frames(device):
     frames of 1-2 empty entries, asserted to fit) and, in the same batch, blocks that do not (payloads up to 20 000
     bytes), each with many frames the pass appends."""
     rng = np.random.default_rng(0xAE20 + device)
-    a, c, q, table = _world(rng, 3000, 8, False)
+    a, c, q, table = E.world(rng, 3000, 8, False)
     gs = rng.permutation(3000)
     # (the world's runs may start past a narrow group's last_index; these groups' runs reach it)
     table["run_start"][gs[:2048]] = np.minimum(table["run_start"][gs[:2048]], c.last_index[gs[:2048]])
@@ -183,7 +122,7 @@ def test_stage_paths_with_appended_frames(device):
 def test_hostile_offsets(device):
     """Offsets out of order and past the batch, and n_bytes short of the last frame, among appending frames."""
     rng = np.random.default_rng(0xAE24 + device)
-    a, c, q, table = _world(rng, 3000, 8, False)
+    a, c, q, table = E.world(rng, 3000, 8, False)
     gs = np.arange(0, 3000)
     blob, off = A.batch(_small_appends(rng, c, table, gs[:1500]) + _frames(rng, c, table, gs[1500:], True, 0.1))
     off = off.copy()
@@ -211,7 +150,7 @@ def test_golden_vectors_through_the_walk(device):
     last = np.array([m["index"] for m in ms], np.uint64)
     cols = {B.COL_TERM: terms, B.COL_LAST_INDEX: last, B.COL_COMMITTED: np.zeros(n, np.uint64),
             B.COL_TERM_START: np.full(n, A.NO_TERM_START, np.uint64)}
-    a, c, q = GFA._follower_arena(n, 0, cols)
+    a, c, q = A.follower_arena(n, 0, cols)
     table = np.zeros(a.get_info().hi, AL.LOG_DTYPE)
     table["id"][:n], table["flags"][:n] = 7, AL.SELECT
     table["run_start"][:n], table["run_term"][:n] = last, [m["log_term"] for m in ms]
@@ -263,18 +202,18 @@ def test_host_against_device_on_twins():
     """Twin arenas take the same batches, one through the host form and one through the device form, and end equal:
     outputs, tables and group columns."""
     rng = np.random.default_rng(0xAE30)
-    a1, c1, _, t1 = _world(np.random.default_rng(7), 20_000, 64, False)
-    a2, _, _, t2 = _world(np.random.default_rng(7), 20_000, 64, False)
+    a1, c1, _, t1 = E.world(np.random.default_rng(7), 20_000, 64, False)
+    a2, _, _, t2 = E.world(np.random.default_rng(7), 20_000, 64, False)
     n = 20_000 + 128
     hi = set(range(20_001, n, 2))
     for rnd in range(3):
         gs = np.array([g for g in rng.permutation(n)[: n // 2] if int(g) not in hi], np.int64)
         blob, off = A.batch(_frames(rng, c1, t1, gs, rnd == 1, 0.05))
-        r1, r2 = _host(a1, blob, off, t1), _device(a2, blob, off, t2)
-        WBT._equal(tuple(r1), tuple(r2), NAMES, ("twins", rnd))
+        r1, r2 = PF.host(a1, "follower_append_entries", blob, off, t1), PF.device(a2, "follower_append_entries", blob, off, t2)
+        PF.equal(tuple(r1), tuple(r2), E.NAMES, ("twins", rnd))
         assert np.count_nonzero(r1[0] & B.FAPP_APPENDED) > 500
         assert np.array_equal(t1, t2)
-        s1, s2 = GFA._group_state(a1, n), GFA._group_state(a2, n)
+        s1, s2 = FL.group_state(a1, n), FL.group_state(a2, n)
         for name in s1:
             assert np.array_equal(s1[name], s2[name]), name
         c1 = _refresh(a1, n)
@@ -286,23 +225,23 @@ def test_entry_less_pass_unchanged():
     """The same batches through raftgpu_follower_append: every claiming frame with entries is NEEDS_LOG, nothing is
     appended and a narrow group's last_index never moves, as its own oracle says."""
     rng = np.random.default_rng(0xAE40)
-    a, c, q, table = _world(rng, 20_000, 64, False)
+    a, c, q, table = E.world(rng, 20_000, 64, False)
     n = 20_000 + 128
     hi = set(range(20_001, n, 2))
-    before = GFA._group_state(a, n)["last_index"]
+    before = FL.group_state(a, n)["last_index"]
     for rnd in range(2):
         gs = np.array([g for g in rng.permutation(n)[: n // 2] if int(g) not in hi], np.int64)
         frames = _frames(rng, c, table, gs, rnd == 1, 0.05)
         blob, off = A.batch(frames)
         want = AL.batch(c, q, table, blob, off)
-        got = a.follower_append(WBT._host_batch(blob, off, len(blob)), GFA._full(a, table))
-        WBT._equal(want, got, GFA.NAMES, ("entry-less", rnd))
+        got = a.follower_append(PF.host_batch(blob, off, len(blob)), A.full_table(a, table))
+        PF.equal(want, got, A.NAMES, ("entry-less", rnd))
         decoded = [AE.decode(bytes(f[4:])) for f in frames]
         has = np.array([d is not None and len(d[1]) > 0 for d in decoded])
         st = want[0]
         assert not np.any(has & (st >> 4 == B.WIRE_OK) & ((st & (AL.STALE | AL.REJECT)) == 0))
         assert np.count_nonzero(has & (st >> 4 == B.WIRE_NEEDS_LOG)) > 1000
-        for name, col in GFA._group_state(a, n).items():                # as its own oracle says
+        for name, col in FL.group_state(a, n).items():                # as its own oracle says
             assert np.array_equal(col, getattr(c, name)[:n]), (rnd, name)
         # (a pair's commit_to evens its halves' last_index, wide_sync; a narrow group's never moves)
         assert np.array_equal(c.last_index[:20_000], before[:20_000])
@@ -354,17 +293,17 @@ def test_host_form_between_begin_and_wait():
         want_table = table.copy()
         want = AE.batch(c, None, want_table, blob, off)
         t_twin, t_a = table.copy(), table.copy()
-        got = _device(twin, blob, off, t_twin)
-        WBT._equal(want, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), NAMES,
+        got = PF.device(twin, "follower_append_entries", blob, off, t_twin)
+        PF.equal(want, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), E.NAMES,
                    ("device form after the step", rnd))
         a.step_begin_records(recs, B.STEP_READ_COMMITTED)
-        during = [x.copy() for x in _host(a, blob, off, t_a)]
+        during = [x.copy() for x in PF.host(a, "follower_append_entries", blob, off, t_a)]
         a.step_wait()
-        WBT._equal(want, tuple(during[:2]) + (during[2].view(AE.APPENDED_DTYPE),) + tuple(during[3:]), NAMES,
+        PF.equal(want, tuple(during[:2]) + (during[2].view(AE.APPENDED_DTYPE),) + tuple(during[3:]), E.NAMES,
                    ("host form during the step", rnd))
         assert np.array_equal(t_twin, want_table) and np.array_equal(t_a, want_table), rnd
         for x in (a, twin):
-            st = GFA._group_state(x, n)
+            st = FL.group_state(x, n)
             for name in ("committed", "last_index", "term", "term_start"):
                 assert np.array_equal(st[name], getattr(c, name)[:n]), (rnd, name)
         kinds += np.bincount(want[0] >> 4, minlength=16)
@@ -453,8 +392,8 @@ def test_replication_round_trip_100k_x5():
         w = AE.batch(fc, None, want_table, fblob, foff)
         assert np.all(w[0] >> 4 == B.WIRE_OK), np.bincount(w[0])
         assert np.array_equal(w[0] & B.FAPP_APPENDED != 0, ks[idx] > 0)
-        got = _device(fa, fblob, foff, table)
-        WBT._equal(w, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), NAMES, ("follower slot", sl))
+        got = PF.device(fa, "follower_append_entries", fblob, foff, table)
+        PF.equal(w, tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:]), E.NAMES, ("follower slot", sl))
         assert np.array_equal(table, want_table)
         fcols = fa.read_columns(n)
         assert np.array_equal(fcols.last_index[g_of[idx]], last[g_of[idx]]), sl      # the follower holds the log
@@ -471,7 +410,7 @@ def test_replication_round_trip_100k_x5():
     assert np.all(wst == B.WIRE_OK)
     O.arena_apply(c, recs, mode=0)
     O.arena_recompute(c)
-    la.step_begin_wire(WBT._host_batch(rblob, roff, len(rblob)), B.STEP_READ_COMMITTED)
+    la.step_begin_wire(PF.host_batch(rblob, roff, len(rblob)), B.STEP_READ_COMMITTED)
     la.step_wait()
     assert np.all(la.wire_status() >> 4 == B.WIRE_OK)
     bm = la.step_results(n)[0].copy()
@@ -486,8 +425,8 @@ def test_replication_round_trip_100k_x5():
         idx = np.flatnonzero((hdr1 & 15) == sl)
         fblob, foff = A.batch([bytes(blob1[off1[i]:off1[i + 1]]) for i in idx.tolist()])
         w = AL.batch(fc, None, table, fblob, foff)
-        got = GFA._device(fa, fblob, foff, table)
-        WBT._equal(w, got, GFA.NAMES, ("commit back", sl))
+        got = PF.device(fa, "follower_append", fblob, foff, table)
+        PF.equal(w, got, A.NAMES, ("commit back", sl))
         assert np.all(w[0] == A.LOG_STATUS_OK)
         fcols = fa.read_columns(n)
         mine = g_of[s_of == sl]

@@ -13,6 +13,7 @@ from helpers import B
 from control_cmds import cmds
 import hb_follow as FL
 import hb_frames as F
+import pass_forms as PF
 import read_cases as R
 
 pytestmark = pytest.mark.gpu
@@ -22,50 +23,11 @@ U64 = (1 << 64) - 1
 OK_RESP = B.WIRE_OK << 4 | B.RES_OK
 
 
-def _self_ids(rng, n):
-    ids = rng.integers(1, 1 << 63, n, dtype=np.uint64)
-    k = rng.random(n)
-    ids[k < 0.03] = 0
-    ids[(k > 0.03) & (k < 0.06)] = U64
-    ids[(k > 0.06) & (k < 0.09)] = 128
-    return ids
-
-
-def _device(a, blob, off, sel, ids, n_bytes=None):
-    """The device form over buffers from raftgpu_device_alloc (n_bytes: of blob, all of it by default) -> (status, from,
-    response blob, offsets, totals)."""
-    n = len(off) - 1
-    bound = B.follower_heartbeat_bound(n)
-    bufs = [a.device_alloc(x) for x in (max(16, len(blob)), 4 * (n + 1), sel.nbytes, ids.nbytes, max(1, n), 8 * max(1, n),
-                                         max(16, bound), 4 * (n + 1), 16)]
-    d_b, d_o, d_s, d_i, d_st, d_f, d_rb, d_ro, d_t = bufs
-    for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_i, ids)):
-        a.h2d(p, x)
-    a.follower_heartbeat_device(d_b, len(blob) if n_bytes is None else n_bytes, d_o, n, d_s, d_i, d_st, d_f, d_rb, bound, d_ro, d_t)
-    a.synchronize()
-    tot = np.zeros(2, np.uint64)
-    a.d2h(tot, d_t)
-    st, frm = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
-    rb, ro = np.zeros(int(tot[1]), np.uint8), np.zeros(int(tot[0]) + 1, np.uint32)
-    a.d2h(st, d_st), a.d2h(frm, d_f), a.d2h(ro, d_ro)
-    if len(rb):
-        a.d2h(rb, d_rb)
-    for p in bufs:
-        a.device_free(p)
-    return st, frm, rb, ro, tot
-
-
-def _group_state(a, n):
-    c = a.read_columns(n)
-    return {"committed": c.committed, "last_index": c.last_index, "term_start": c.term_start,
-            "term": a.column_read(B.COL_TERM, 0, 0, n, np.uint64)}
-
-
 def _compare(a, c, q, blob, off, sel, ids, device, what):
     """One pass through the arena (host or device form) and through the oracle: every output and the group columns."""
     want = HL.follower_heartbeats(c, q, blob, off, sel, ids)
     if device:
-        got = _device(a, blob, off, sel, ids)
+        got = PF.device(a, "follower_heartbeat", blob, off, sel, ids)
     else:
         fb = F.Frames([])
         fb.bytes, fb.offsets, fb.n, fb.n_bytes = np.concatenate([blob, np.zeros(16, np.uint8)]), off, len(off) - 1, len(blob)
@@ -75,7 +37,7 @@ def _compare(a, c, q, blob, off, sel, ids, device, what):
     for k, name in enumerate(("status", "from", "response bytes", "response offsets", "totals")):
         assert np.array_equal(got[k], want[k]), (what, name, np.flatnonzero(got[k] != want[k])[:5]
                                                  if len(got[k]) == len(want[k]) else (len(got[k]), len(want[k])))
-    s = _group_state(a, c.n_groups)
+    s = FL.group_state(a, c.n_groups)
     for name, col in s.items():
         assert np.array_equal(col, getattr(c, name)[:c.n_groups]), (what, name)
     return want
@@ -169,7 +131,7 @@ def test_random_arenas_vs_oracle(reads):
     if reads:
         q = R.RO.ReadQueues(c.cap, P)
         q.allocated[:n] = 1
-    ids = _self_ids(rng, n)
+    ids = FL.self_ids(rng, n)
     kinds = np.zeros(16, np.int64)
     for rnd, device in enumerate((False, True)):
         order = rng.permutation(nl)
@@ -222,7 +184,7 @@ def test_1m_followers():
     c = a.read_columns(n)
     c.term = terms.copy()
     sel = FL.bitmap(np.ones(n, bool))
-    st = _compare(a, c, None, blob, hoff, sel, _self_ids(rng, n), True, "1M")[0]
+    st = _compare(a, c, None, blob, hoff, sel, FL.self_ids(rng, n), True, "1M")[0]
     assert (st == OK_RESP).sum() > 0.95 * n and (st == B.WIRE_COMMIT_RANGE << 4).sum() > 0.01 * n
     a.close()
 
@@ -234,40 +196,31 @@ def test_refusals_before_any_launch():
     a = d.a
     for g in range(16):
         a.group_set_term(g, 3)
-    before = _group_state(a, 64)
+    before = FL.group_state(a, 64)
     L, h = a._L, a._h
     blob, off = F.batch([F.frame(g, 0, F.message(8, term=3, commit=0)) for g in range(16)])
     n = 16
     bound = B.follower_heartbeat_bound(n)
     assert bound == 60 * n
     sel, ids = FL.bitmap(np.ones(a.cap, bool)), np.arange(a.cap, dtype=np.uint64)
-    d_b, d_o, d_s, d_i = a.device_alloc(1024), a.device_alloc(4 * (n + 1)), a.device_alloc(sel.nbytes), a.device_alloc(ids.nbytes)
-    d_st, d_f, d_rb, d_ro, d_t = a.device_alloc(n), a.device_alloc(8 * n), a.device_alloc(bound + 64), a.device_alloc(4 * (n + 1)), \
-        a.device_alloc(16)
-    for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_i, ids), (d_st, np.full(n, 0xEE, np.uint8)), (d_t, np.full(2, 77, np.uint64))):
-        a.h2d(p, x)
     nb = len(blob)
-    dev = lambda **k: L.raftgpu_follower_heartbeat_device(h, None, k.get("b", d_b), k.get("nb", nb), d_o, k.get("n", n), k.get("s", d_s),
-                                                          d_i, d_st, d_f, k.get("rb", d_rb), k.get("cap", bound), k.get("ro", d_ro),
-                                                          k.get("t", d_t))
-    big = (1 << 32) // 60 + 1                                 # the first n whose bound exceeds u32 offsets
-    assert B.follower_heartbeat_bound(big - 1) < (1 << 32) <= B.follower_heartbeat_bound(big)
-    refused = [dev(cap=bound - 1), dev(cap=0), dev(b=d_b + 4), dev(rb=d_rb + 8), dev(n=big, cap=60 * big),
-               dev(n=1 << 32, cap=U64), dev(nb=1 << 32), dev(s=None), dev(ro=None), dev(t=None)]
-    assert refused == [B.ERR_INVALID] * len(refused), refused
-    st, tot, rb = np.zeros(n, np.uint8), np.zeros(2, np.uint64), np.zeros(bound, np.uint8)
-    ro = np.zeros(n + 1, np.uint32)
-    host = lambda cap: L.raftgpu_follower_heartbeat(h, blob.ctypes.data, nb, off.ctypes.data, n, sel.ctypes.data, ids.ctypes.data,
-                                                    st.ctypes.data, None, rb.ctypes.data, cap, ro.ctypes.data, tot.ctypes.data)
-    assert host(bound - 1) == B.ERR_INVALID
-    a.synchronize()
-    gst, gt = np.zeros(n, np.uint8), np.zeros(2, np.uint64)
-    a.d2h(gst, d_st), a.d2h(gt, d_t)
-    assert np.all(gst == 0xEE) and gt.tolist() == [77, 77]   # nothing was launched
-    after = _group_state(a, 64)
-    assert all(np.array_equal(before[k], after[k]) for k in before)
-    # the exact bound is accepted
-    assert host(bound) == B.OK and tot.tolist()[0] == 16 and np.all(st == OK_RESP)
+    with PF.refusals(a, "follower_heartbeat", blob, off, sel, ids) as r:
+        dev, d = r.call, r.args
+        big = (1 << 32) // 60 + 1                                 # the first n whose bound exceeds u32 offsets
+        assert B.follower_heartbeat_bound(big - 1) < (1 << 32) <= B.follower_heartbeat_bound(big)
+        refused = [dev(cap=bound - 1), dev(cap=0), dev(b=d["b"] + 4), dev(rb=d["rb"] + 8), dev(n=big, cap=60 * big),
+                   dev(n=1 << 32, cap=U64), dev(nb=1 << 32), dev(s=None), dev(ro=None), dev(t=None)]
+        assert refused == [B.ERR_INVALID] * len(refused), refused
+        st, tot, rb = np.zeros(n, np.uint8), np.zeros(2, np.uint64), np.zeros(bound, np.uint8)
+        ro = np.zeros(n + 1, np.uint32)
+        host = lambda cap: L.raftgpu_follower_heartbeat(h, blob.ctypes.data, nb, off.ctypes.data, n, sel.ctypes.data, ids.ctypes.data,
+                                                        st.ctypes.data, None, rb.ctypes.data, cap, ro.ctypes.data, tot.ctypes.data)
+        assert host(bound - 1) == B.ERR_INVALID
+        assert r.untouched()   # nothing was launched
+        after = FL.group_state(a, 64)
+        assert all(np.array_equal(before[k], after[k]) for k in before)
+        # the exact bound is accepted
+        assert host(bound) == B.OK and tot.tolist()[0] == 16 and np.all(st == OK_RESP)
     a.close()
 
 

@@ -10,6 +10,7 @@ from oracle import hb_wire_oracle as H
 from helpers import B
 from control_cmds import cmds
 import hb_frames as F
+import pass_forms as PF
 import read_cases as R
 
 pytestmark = pytest.mark.gpu
@@ -32,31 +33,6 @@ def _select(rng, cap, density):
     return np.packbits(bits, bitorder="little").view(np.uint32).copy() if cap % 32 == 0 else None
 
 
-def _device(a, first, n, ids, select, bytes_capacity=None, frames_capacity=None):
-    """The device form -> (blob, offsets, totals); the output buffers are sized at the bound."""
-    bound = B.heartbeat_frames_bound(n)
-    bcap = bound if bytes_capacity is None else bytes_capacity
-    fcap = 8 * n if frames_capacity is None else frames_capacity
-    d_ids, d_bytes = a.device_alloc(max(8, ids.nbytes)), a.device_alloc(max(16, bound))
-    d_off, d_tot = a.device_alloc(4 * (8 * n + 1)), a.device_alloc(24)
-    d_sel = a.device_alloc(select.nbytes) if select is not None else None
-    a.h2d(d_ids, ids)
-    if select is not None:
-        a.h2d(d_sel, select)
-    a.heartbeat_frames_device(first, n, d_sel, d_ids, d_bytes, bcap, d_off, fcap, d_tot)
-    a.synchronize()
-    tot = np.zeros(3, np.uint64)
-    a.d2h(tot, d_tot)
-    blob, off = np.zeros(int(tot[1]), np.uint8), np.zeros(int(tot[0]) + 1, np.uint32)
-    if len(blob):
-        a.d2h(blob, d_bytes)
-    a.d2h(off, d_off)
-    for p in (d_ids, d_bytes, d_off, d_tot, d_sel):
-        if p is not None:
-            a.device_free(p)
-    return blob, off, tot
-
-
 def _check(a, c, q, first, n, ids, select, what):
     want = HF.bcast_heartbeats(c, q, first, n, ids, select)
     rc, blob, off, tot = a.heartbeat_frames(first, n, ids, select)
@@ -64,7 +40,7 @@ def _check(a, c, q, first, n, ids, select, what):
     assert tot.tolist() == want[2].tolist(), (what, tot, want[2])
     assert np.array_equal(off, want[1]), what
     assert np.array_equal(blob, want[0]), (what, int(np.argmax(blob != want[0])) if len(blob) == len(want[0]) else None)
-    dblob, doff, dtot = _device(a, first, n, ids, select)
+    dblob, doff, dtot = PF.broadcast(a, "heartbeat_frames", first, n, ids, select)
     assert dtot.tolist() == tot.tolist() and np.array_equal(doff, off) and np.array_equal(dblob, blob), what
     return want
 

@@ -12,7 +12,7 @@ import pytest
 
 from oracle import control_oracle as CO
 from oracle import hb_wire_oracle as H
-from helpers import B, O, assert_columns_equal, checksum
+from helpers import B, O, assert_columns_equal, checksum, oracle_wire_apply
 from control_cmds import NO_TERM_START, cmds
 import hb_frames as F
 import read_cases as R
@@ -22,14 +22,6 @@ pytestmark = pytest.mark.gpu
 W = importlib.import_module("raft-rs_b200.wire")
 HERE = os.path.dirname(os.path.abspath(__file__))
 P = 8
-
-
-def _queues_equal(a, q, n, what):
-    got, want = a.read_index_read(0, n), R.oracle_queue_view(q, n)
-    for name, x, y in zip(("count", "ctx", "index", "acks"), got, want):
-        if not np.array_equal(x, y):
-            g = int(np.argwhere(x != y)[0][0])
-            raise AssertionError(f"{what}: queue {name} of group {g}: got {x[g]} want {y[g]}")
 
 
 def _released_equal(got, want, what):
@@ -90,7 +82,7 @@ def test_golden_vectors_through_the_gpu(reads):
     if reads:
         assert len(want_rel) > 20
         _released_equal(rel, want_rel, "golden frames")
-        _queues_equal(a, q, n, "golden frames")
+        R.queues_equal(a, q, n, "golden frames")
     else:
         assert len(rel) == 0
     a.close()
@@ -134,64 +126,6 @@ def _control(a, d, reads, lst, what):
     assert np.array_equal(a.control(lst), want), what
 
 
-def _mixed_batch(rng, d, n, terms, reads, k):
-    """k frames, shuffled: append responses (accepts near matched, rejects without log_term), heartbeat responses
-    (contexts of length 0, 8 and others; ids pending, released earlier or never queued), other message types;
-    stale terms; several frames per cell (a wide group's peers 8..15 are named through its high half)."""
-    gs = rng.integers(0, n, k)
-    hi_half = (d.c.meta[gs] & R.META_WIDE_HI) != 0
-    slots = rng.integers(0, 8, k)
-    kind = rng.random(k)
-    stale = rng.random(k) < 0.05
-    qg = np.where(hi_half, gs - 1, gs)
-    frames = []
-    for i in range(k):
-        g, s = int(gs[i]), int(slots[i])
-        t = int(terms[g]) + (1 if stale[i] else 0)
-        if kind[i] < 0.35:     # MsgAppendResponse
-            m = int(d.c.matched[s, g])
-            if rng.random() < 0.1:
-                body = F.message(4, term=t, index=m + 1, reject=True, reject_hint=max(0, m - 1))
-            else:
-                body = F.message(4, term=t, index=m + int(rng.integers(0, 4)), commit=m)
-        elif kind[i] < 0.93:   # MsgHeartbeatResponse
-            r = rng.random()
-            ctx = None
-            if r < 0.55:
-                cnt = int(d.q.count[qg[i]])
-                x = int(d.q.ctx[qg[i], int(rng.integers(0, cnt))]) if cnt else int(rng.integers(1, 60))
-                ctx = F.ctx_bytes(x)
-            elif r < 0.65:
-                ctx = F.ctx_bytes(int(rng.integers(1, 1 << 62)))                 # never queued
-            elif r < 0.72:
-                ctx = bytes(rng.integers(0, 256, int(rng.choice([1, 7, 9, 16]))).astype(np.uint8))
-            body = F.message(9, term=t, commit=int(rng.integers(0, 80)), context=ctx)
-        else:                  # other types, some with a context
-            body = F.message(int(rng.choice([3, 6, 8, 15, 16])), term=t, index=5,
-                             context=F.ctx_bytes(7) if rng.random() < 0.5 else None)
-        frames.append(F.frame(g, s, body))
-    dup = rng.random(k) < 0.1                       # more frames for cells already in the batch
-    frames += [frames[j] for j in rng.integers(0, k, int(dup.sum()))]
-    order = rng.permutation(len(frames))
-    return F.batch([frames[j] for j in order])
-
-
-def _oracle_append(c, blob, offsets, n, terms, n_bytes=None):
-    """raftgpu_wire_apply_device: the AppendResponse frames, first of every cell, in frame order."""
-    status, recs, hint, snap = O.wire_decode_batch(blob, offsets, n, terms, n_bytes)
-    ok = np.nonzero(status == O.WIRE_OK)[0]
-    rows = []
-    for i in ok:
-        rows.append(tuple(recs[i]))
-        if recs["flags"][i] & B.REC_REJECT:
-            rows.append((recs["group"][i], recs["peer_slot"][i], B.REC_EXT, 0, hint[i], snap[i]))
-    seq = np.array(rows, dtype=B.APPEND_RESP_DTYPE) if rows else np.zeros(0, dtype=B.APPEND_RESP_DTYPE)
-    res = O.arena_apply(c, seq, mode=0)
-    want = (status.astype(np.uint32) << 4).astype(np.uint8)
-    want[ok] |= res[(seq["flags"] & B.REC_EXT) == 0] & 0xF
-    return want
-
-
 @pytest.mark.parametrize("inflights", [False, True], ids=["host_inflights", "device_inflights"])
 @pytest.mark.parametrize("reads", [True, False], ids=["read_queues", "no_read_queues"])
 def test_mixed_batches_vs_oracle(reads, inflights):
@@ -212,7 +146,7 @@ def test_mixed_batches_vs_oracle(reads, inflights):
             want_res, want_rel = d.q.request(d.c, reqs)
             assert np.array_equal(res, want_res), rnd
             _released_equal(rel, want_rel, f"round {rnd}: requests")
-        blob, offsets = _mixed_batch(rng, d, n, terms, reads, k)
+        blob, offsets = R.mixed_batch(rng, d, n, terms, reads, k)
         m = len(offsets) - 1
         a.h2d(d_bytes, blob)
         a.h2d(d_off, offsets)
@@ -224,7 +158,7 @@ def test_mixed_batches_vs_oracle(reads, inflights):
         a.synchronize()
         st1, st2 = np.zeros(m, np.uint8), np.zeros(m, np.uint8)
         a.d2h(st1, d_st1), a.d2h(st2, d_st2)
-        want1 = _oracle_append(d.c, blob, offsets, n, terms)
+        want1 = oracle_wire_apply(d.c, blob, offsets, n, terms)
         want2, want_rel = H.apply(d.c, d.q if reads else None, blob, offsets, terms)
         assert np.array_equal(st1, want1), f"round {rnd}: append statuses"
         bad = np.nonzero(st2 != want2)[0]
@@ -241,7 +175,7 @@ def test_mixed_batches_vs_oracle(reads, inflights):
                 a.d2h(rel, d_rel)
             _released_equal(rel, want_rel, f"round {rnd}: released")
             n_rel += len(rel)
-            _queues_equal(a, d.q, n, f"round {rnd}")
+            R.queues_equal(a, d.q, n, f"round {rnd}")
         if inflights:           # sends fill the two-entry windows, so heartbeats free their first entries
             cells = rng.choice(8 * n, n // 2, replace=False)
             e = np.zeros(len(cells), B.SEND_ENTRY_DTYPE)

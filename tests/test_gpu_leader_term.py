@@ -9,74 +9,20 @@ from oracle import oracle as O
 from oracle import control_oracle as CO
 from oracle import leader_term_oracle as LT
 from oracle import read_oracle as RO
-from helpers import B
+from helpers import B, arena_of, check_columns, ARENA_COLUMNS
 from control_cmds import cmds
 import app_follow as A
 import follow_term as T
 import hb_follow as HB
 import hb_frames as F
 import leader_term as L
-import test_gpu_follower_term as GT
-import test_oracle_vote_request as TV
+import pass_forms as PF
 import vote_request_frames as Q
 
 pytestmark = pytest.mark.gpu
 
 
-def _device(a, blob, off, voters, n_bytes=None):
-    """The device form over buffers from raftgpu_device_alloc -> (status, out, response blob, offsets, totals)."""
-    n = len(off) - 1
-    n_bytes = len(blob) if n_bytes is None else n_bytes
-    blob = np.concatenate([blob, np.zeros(16, np.uint8)])
-    bound = B.follower_term_wire_bound(n)
-    vt = np.ascontiguousarray(voters, B.VOTER_DTYPE)
-    sizes = (len(blob), 4 * (n + 1), max(64, vt.nbytes), max(1, n), max(16, 16 * n), max(16, bound), 4 * (n + 1), 16)
-    bufs = [a.device_alloc(x) for x in sizes]
-    d_b, d_o, d_v, d_st, d_out, d_rb, d_ro, d_t = bufs
-    for p, x in ((d_b, blob), (d_o, off), (d_v, vt)):
-        a.h2d(p, x)
-    a.leader_term_wire_device(d_b, n_bytes, d_o, n, d_v, d_st, d_out, d_rb, bound, d_ro, d_t)
-    a.synchronize()
-    tot = np.zeros(2, np.uint64)
-    a.d2h(tot, d_t)
-    st, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
-    rb, ro = np.zeros(int(tot[1]), np.uint8), np.zeros(int(tot[0]) + 1, np.uint32)
-    for arr, p in ((st, d_st), (out, d_out), (ro, d_ro), (rb, d_rb)):
-        if arr.size:
-            a.d2h(arr, p)
-    for p in bufs:
-        a.device_free(p)
-    return st, out, rb, ro, tot
-
-
-def _run(a, frames_, voters, device):
-    if device:
-        blob, off = F.batch(frames_)
-        return _device(a, blob, off, voters)
-    return a.leader_term_wire(F.Frames(frames_), voters)
-
-
-def _noise(rng, s, k):
-    """Frames the checks before the verdict settle: other types, garbage, truncated frames, a pair's high half on types
-    3 and 8, m.term 0 and groups past the arena's highest slot."""
-    out = []
-    for _ in range(k):
-        g = int(rng.choice(s.lows))
-        term = int(s.term[g])
-        kind = int(rng.integers(6))
-        if kind == 0:
-            out.append(F.frame(g, 0, F.message(int(rng.choice([5, 7, 10, 17])), term + 1, frm=2)))
-        elif kind == 1:
-            out.append(F.frame(g, 0, rng.integers(0, 256, int(rng.integers(1, 12)), dtype=np.uint8).tobytes()))
-        elif kind == 2:
-            out.append(F.frame(g, 0, F.message(4, term + 1, 1 << 40, frm=2)[:-3]))
-        elif kind == 3:
-            out.append(F.frame(g + 1 if s.wide[g] else g, 0, F.message(8, term + 1 if s.wide[g] else 0, frm=2)))
-        elif kind == 4:
-            out.append(F.frame(g, 1, F.message(9, 0, frm=2)))
-        else:
-            out.append(F.frame(s.n + int(rng.integers(1, 100)), 0, F.message(4, term + 1, frm=2)))
-    return out
+NAMES = ("status", "out", "bytes", "offsets", "totals")
 
 
 # --------------------------------------------------------------------------- 1. random 100K-group batches
@@ -89,18 +35,8 @@ def _noise(rng, s, k):
 def test_random_batches_vs_oracle(device, read_index, inflights, runs):
     rng = np.random.default_rng(0x7500 + 8 * runs + 4 * device + 2 * read_index + (inflights > 0))
     s = T.scenario(rng, 96_000, 2_000, p_role=(0.1, 0.0, 0.0, 0.9))
-    a = B.Arena(s.n + 64)
-    if read_index:
-        a.enable_read_index()
-    if inflights:
-        a.enable_inflights(inflights)
-    if runs:
-        a.enable_leader_runs()
-    assert a.group_alloc_range(s.n_narrow) == 0
-    for k in range(s.n_wide):
-        assert a.group_alloc_wide() == s.n_narrow + 2 * k
-    assert np.all(a.control(s.setup)["status"] == 0)
-    c, vt = TV.state_of(s)
+    a = arena_of(s, read_index, inflights, runs)
+    c, vt = Q.state_of(s)
     q = None
     if read_index:
         q = RO.ReadQueues(c.cap, 8)
@@ -111,7 +47,7 @@ def test_random_batches_vs_oracle(device, read_index, inflights, runs):
                       for g in rng.choice(s.lows, 20_000) for sl in (1, 2) for k in (1, 2)])
         got = a.control(adds)
         assert np.array_equal(got, CO.arena_control(c, vt, adds))
-        GT._check_columns(a, c, vt, s.n, ins=True)
+        check_columns(a, c, vt, s.n, ins=True)
     leaders = np.array([g for g in s.lows if s.role[g] == Q.LEADER])
     if runs:
         rows = np.zeros(len(leaders), B.LEADER_RUNS_DTYPE)
@@ -122,13 +58,13 @@ def test_random_batches_vs_oracle(device, read_index, inflights, runs):
     kinds = np.zeros(16, np.int64)
     for rnd in range(2):
         frames_, meta = L.frames(rng, s, per_group=(1, 3))
-        frames_ += _noise(rng, s, 3000)
+        frames_ += L.noise(rng, s, 3000)
         frames_ = [frames_[i] for i in rng.permutation(len(frames_))]
         blob, off = F.batch(frames_)
         want = LT.batch(c, q, vt, blob, off, table)
-        got = _run(a, frames_, table, device)
-        GT._equal(want, got, rnd)
-        GT._check_columns(a, c, vt, s.n, ins=bool(inflights))
+        got = PF.run(a, "leader_term_wire", *F.batch(frames_), table, device=device)
+        PF.equal(want, got, NAMES, rnd)
+        check_columns(a, c, vt, s.n, ins=bool(inflights))
         if read_index:
             assert all(len(a.read_index_get(g)[0]) == q.count[g] for g in range(0, s.n, 997))
         s.term[:] = c.term[: s.n]
@@ -181,9 +117,9 @@ def test_hostile_terms(device):
                F.frame(3, 0, F.message(3, 5, frm=7)), F.frame(3, 1, F.message(4, 5, frm=7))]
     blob, off = F.batch(frames_)
     want = LT.batch(c, None, vt, blob, off, t)
-    got = _run(a, frames_, t, device)
-    GT._equal(want, got, "hostile")
-    GT._check_columns(a, c, vt, 4)
+    got = PF.run(a, "leader_term_wire", *F.batch(frames_), t, device=device)
+    PF.equal(want, got, NAMES, "hostile")
+    check_columns(a, c, vt, 4)
     assert c.term[:4].tolist() == [top, 1 << 32, top - 1, 5]
     assert int(got[4][0]) == 4   # frames 1, 2 (group 0), 3 and 5 (group 1) are MsgAppend / MsgHeartbeat below T
     a.close()
@@ -200,9 +136,9 @@ def test_ten_thousand_frames_of_one_group(device):
                for k, (x, y) in enumerate(zip(terms.tolist(), typs.tolist()))]
     blob, off = F.batch(frames_)
     want = LT.batch(c, None, vt, blob, off, t)
-    got = _run(a, frames_, t, device)
-    GT._equal(want, got, "one group")
-    GT._check_columns(a, c, vt, 2)
+    got = PF.run(a, "leader_term_wire", *F.batch(frames_), t, device=device)
+    PF.equal(want, got, NAMES, "one group")
+    check_columns(a, c, vt, 2)
     st = got[0]
     assert c.term[1] == terms.max() and np.count_nonzero(st & B.FTERM_BUMPED) == 1
     assert np.flatnonzero(st & B.FTERM_BUMPED)[0] == np.flatnonzero(terms == terms.max())[0]
@@ -212,11 +148,11 @@ def test_ten_thousand_frames_of_one_group(device):
 
 def test_no_frames():
     a, c, vt, t = _small(2)
-    st, out, rb, ro, tot = _device(a, np.zeros(0, np.uint8), np.zeros(1, np.uint32), t)
+    st, out, rb, ro, tot = PF.device(a, "leader_term_wire", np.zeros(0, np.uint8), np.zeros(1, np.uint32), t)
     assert st.size == 0 and tot.tolist() == [0, 0] and ro.tolist() == [0]
     st, out, rb, ro, tot = a.leader_term_wire(F.Frames([]), t)
     assert st.size == 0 and tot.tolist() == [0, 0] and ro.tolist() == [0]
-    GT._check_columns(a, c, vt, 2)
+    check_columns(a, c, vt, 2)
     a.close()
 
 
@@ -228,33 +164,24 @@ def test_refusals_before_any_launch():
     blob = np.concatenate([blob, np.zeros(16, np.uint8)])
     t = Q.voters(64)
     bound = B.follower_term_wire_bound(n)
-    d_b, d_o, d_v = a.device_alloc(len(blob)), a.device_alloc(4 * (n + 1)), a.device_alloc(t.nbytes + 64)
-    d_st, d_out, d_rb, d_ro, d_t = (a.device_alloc(x) for x in (n, 16 * n, bound + 16, 4 * (n + 1), 16))
-    for p, x in ((d_b, blob), (d_o, off), (d_v, t), (d_st, np.full(n, 0xEE, np.uint8)), (d_t, np.full(2, 77, np.uint64))):
-        a.h2d(p, x)
     nb = off[-1]
-    dev = lambda **k: Lb.raftgpu_leader_term_wire_device(
-        h, None, k.get("b", d_b), k.get("nb", nb), k.get("o", d_o), k.get("n", n), k.get("v", d_v), k.get("st", d_st),
-        k.get("out", d_out), k.get("rb", d_rb), k.get("cap", bound), k.get("ro", d_ro), k.get("t", d_t))
-    refused = [dev(cap=bound - 1), dev(b=d_b + 4), dev(v=d_v + 8), dev(rb=d_rb + 4), dev(nb=1 << 32),
-               dev(n=1 << 32, cap=1 << 40), dev(n=(1 << 32) // 39 + 1, cap=1 << 40), dev(v=None), dev(st=None),
-               dev(b=None), dev(o=None), dev(rb=None), dev(t=None), dev(ro=None)]
-    assert refused == [B.ERR_INVALID] * len(refused), refused
-    a.synchronize()
-    gst, gt = np.zeros(n, np.uint8), np.zeros(2, np.uint64)
-    a.d2h(gst, d_st), a.d2h(gt, d_t)
-    assert np.all(gst == 0xEE) and gt.tolist() == [77, 77]                    # nothing was launched
-    assert np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 3)
-    st, out, rb, ro, tot = np.zeros(n, np.uint8), np.zeros(2 * n, np.uint64), np.zeros(bound, np.uint8), \
-        np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-    assert Lb.raftgpu_leader_term_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, t.ctypes.data, st.ctypes.data,
-                                       out.ctypes.data, rb.ctypes.data, bound - 1, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
-    assert Lb.raftgpu_leader_term_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, None, st.ctypes.data,
-                                       out.ctypes.data, rb.ctypes.data, bound, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
-    assert dev() == B.OK                                                      # the same call with every rule kept
-    a.synchronize()
-    a.d2h(gst, d_st)
-    assert np.all(gst == (B.WIRE_OK << 4 | B.FTERM_BUMPED)) and np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 4)
+    with PF.refusals(a, "leader_term_wire", blob, off, t, n_bytes=nb) as r:
+        dev, d = r.call, r.args
+        refused = [dev(cap=bound - 1), dev(b=d["b"] + 4), dev(v=d["v"] + 8), dev(rb=d["rb"] + 4), dev(nb=1 << 32),
+                   dev(n=1 << 32, cap=1 << 40), dev(n=(1 << 32) // 39 + 1, cap=1 << 40), dev(v=None), dev(st=None),
+                   dev(b=None), dev(o=None), dev(rb=None), dev(t=None), dev(ro=None)]
+        assert refused == [B.ERR_INVALID] * len(refused), refused
+        assert r.untouched()                                                  # nothing was launched
+        assert np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 3)
+        st, out, rb, ro, tot = np.zeros(n, np.uint8), np.zeros(2 * n, np.uint64), np.zeros(bound, np.uint8), \
+            np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        assert Lb.raftgpu_leader_term_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, t.ctypes.data, st.ctypes.data,
+                                           out.ctypes.data, rb.ctypes.data, bound - 1, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
+        assert Lb.raftgpu_leader_term_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, None, st.ctypes.data,
+                                           out.ctypes.data, rb.ctypes.data, bound, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
+        assert dev() == B.OK                                                      # the same call with every rule kept
+        gst = r.read("st", np.zeros(n, np.uint8))
+        assert np.all(gst == (B.WIRE_OK << 4 | B.FTERM_BUMPED)) and np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 4)
     a.close()
 
 
@@ -263,12 +190,8 @@ def test_host_form_between_a_wire_steps_begin_and_its_wait():
     the term are applied first, then this pass deposes the groups that hear a higher term."""
     rng = np.random.default_rng(0x7502)
     s = T.scenario(rng, 20_000, 500, p_role=(0.0, 0.0, 0.0, 1.0))
-    a = B.Arena(s.n + 64)
-    assert a.group_alloc_range(s.n_narrow) == 0
-    for k in range(s.n_wide):
-        assert a.group_alloc_wide() == s.n_narrow + 2 * k
-    assert np.all(a.control(s.setup)["status"] == 0)
-    c, vt = TV.state_of(s)
+    a = arena_of(s)
+    c, vt = Q.state_of(s)
     step = [F.frame(g, 1, F.message(4, int(s.term[g]), index=int(s.last[g]), frm=2)) for g in s.lows]
     frames_, _ = L.frames(rng, s, per_group=(1, 3))
     L.leader_passes(c, step)
@@ -278,8 +201,8 @@ def test_host_form_between_a_wire_steps_begin_and_its_wait():
     got = a.leader_term_wire(F.Frames(frames_), s.table)
     a.step_wait()
     assert np.all(a.wire_status() >> 4 == B.WIRE_OK)
-    GT._equal(want, got, "overlap")
-    GT._check_columns(a, c, vt, s.n)
+    PF.equal(want, got, NAMES, "overlap")
+    check_columns(a, c, vt, s.n)
     a.close()
 
 
@@ -292,18 +215,18 @@ def test_disruptive_follower_round_trip():
     t + 1; the leaders' wire step returns them TERM, and this pass deposes every leader: term t + 1, no leader."""
     rng = np.random.default_rng(0x7503)
     n, P, t, li = 5_000, 5, 7, 1000
-    old = GT._leaders(n, P, t, li)
+    old = T.leaders(n, P, t, li)
     ids = np.zeros((B.SLOTS + 1, n), np.uint64)
     ids[:B.SLOTS] = (np.arange(B.SLOTS) + 1)[:, None]
     ids[B.SLOTS] = 1
     _, hb, hoff, _ = old.heartbeat_frames(0, n, ids)
     nf = n * (P - 1)
-    fa, ftable = GT._followers(nf, t + 1, li, P, rng)
-    to_f = GT._to_followers(hb, hoff, P)
-    fst, _, rb, ro, tot = GT._device(fa, to_f, hoff, ftable)
+    fa, ftable = T.followers(nf, t + 1, li, P, rng)
+    to_f = T.to_followers(hb, hoff, P)
+    fst, _, rb, ro, tot = PF.device(fa, "follower_term_wire", to_f, hoff, ftable)
     assert np.all(fst == B.WIRE_STALE << 4 | B.RES_OK) and int(tot[0]) == nf
     fa.close()
-    back = GT._to_leaders(rb, ro, P)
+    back = T.to_leaders(rb, ro, P)
     frames_ = [bytes(back[a0:b0]) for a0, b0 in zip(ro[:-1].tolist(), ro[1:].tolist())]
     old.step_begin_wire(F.Frames(frames_), B.STEP_READ_COMMITTED)
     old.step_wait()
@@ -353,7 +276,7 @@ def test_election_round_trip():
     st, out, _, _, tot = a.leader_term_wire(F.Frames(late), table)
     assert np.all(st == B.WIRE_IGNORED << 4) and not out.any() and tot.tolist() == [0, 0]
     after = a.read_columns(n)
-    for name in GT.ARENA_COLUMNS:
+    for name in ARENA_COLUMNS:
         assert np.array_equal(getattr(before, name), getattr(after, name)), name
     st, out, _, _, _ = a.leader_term_wire(F.Frames([F.frame(5, 4, F.message(6, t + 2, reject=True, frm=5))]), table)
     assert st.tolist() == [B.WIRE_OK << 4 | B.FTERM_BUMPED] and out.tolist() == [[0, t + 2]]

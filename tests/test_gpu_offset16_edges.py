@@ -14,13 +14,11 @@ import numpy as np
 import pytest
 
 from oracle import control_oracle as CO
-from helpers import (B, O, TILE_SHAPES, Paths, Shape, assert_columns_equal, bitmap_to_bool, offset_of, random_state,
-                     ring_wrapping_groups)
+from helpers import (B, O, Paths, Shape, TILE_SHAPES, as_set, assert_columns_equal, bitmap_to_bool, escape_tiles,
+                     offset_of, oracle_wire_step, random_state, records_step, ring_wrapping_groups, several_tiles,
+                     storm)
 from offset16 import (EDGE16_D, I16_MAX, I16_MIN, edge_batch, edge_state16, escaped16, fits16, self_behind16)
 from control_cmds import cmds
-from test_gpu_control import records_step
-from test_gpu_offset_edges import as_set, escape_tiles, several_tiles, storm
-from test_gpu_wire import oracle_wire_step
 
 pytestmark = pytest.mark.gpu
 

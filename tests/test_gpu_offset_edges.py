@@ -12,47 +12,16 @@ import numpy as np
 import pytest
 
 from oracle import control_oracle as CO
-from helpers import (B, EDGE_ESCAPES, EDGE_FITS, I32_MAX, I32_MIN, O, RESET_LAST, TILE_SHAPES, Paths, Shape,
-                     assert_columns_equal, bitmap_to_bool, edge_state, escaped_cells, fits, offset_of,
-                     random_batch, random_state, ring_wrapping_groups)
+from helpers import (B, EDGE_ESCAPES, EDGE_FITS, I32_MAX, I32_MIN, O, Paths, Shape, TILE_SHAPES, as_set,
+                     assert_columns_equal, bitmap_to_bool, edge_state, escape_tiles, escaped_cells, fits, offset_of,
+                     oracle_wire_step, random_batch, random_state, records_step, ring_wrapping_groups, several_tiles,
+                     storm)
 from control_cmds import cmds
-from test_gpu_control import records_step
-from test_gpu_wire import oracle_wire_step
 
 pytestmark = pytest.mark.gpu
 
 W = importlib.import_module("raft-rs_b200.wire")
 EDGE_D = np.array(EDGE_FITS + EDGE_ESCAPES)
-
-
-def several_tiles():
-    """Seven full tiles and a ragged eighth."""
-    return 7 * B.tile_groups() + 77
-
-
-def escape_tiles(n):
-    """Every ninth tile: each of its cells escaped."""
-    return (np.arange(n) // B.tile_groups()) % 9 == 4
-
-
-def storm(c, rng, n):
-    """The state right after an election at a last index past 2^31 (Raft::reset, then become_leader): every peer
-    cell but the leader's own has matched 0 and next_idx = last_index + 1, both escaped."""
-    last = np.array(RESET_LAST[1:])[rng.integers(0, len(RESET_LAST) - 1, n)]
-    meta = c.meta[:n].astype(np.int64)
-    own = ((meta & O.META_HAS_SELF) != 0)[None, :] & (((meta >> 24) & 7)[None, :] == np.arange(O.SLOTS)[:, None])
-    follower = ~own
-    c.last_index[:n] = last
-    c.term_start[:n] = last
-    c.committed[:n] = np.minimum(c.committed[:n], last - 1)
-    c.matched[:, :n] = np.where(follower, 0, last)                 # the leader: persisted = last_index
-    c.peer_committed[:, :n] = np.where(follower, c.peer_committed[:, :n], c.committed[:n])
-    c.next_idx[:, :n] = last + 1
-    c.pflags[:, :n] = np.where(follower, O.STATE_PROBE, c.pflags[:, :n])
-    c.pending_snapshot[:, :n] = np.where(follower, 0, c.pending_snapshot[:, :n])
-    c.pending_request_snapshot[:, :n] = np.where(follower, 0, c.pending_request_snapshot[:, :n])
-    assert not fits(c.next_idx[:, :n][follower], 0).any()
-    return c
 
 
 # --------------------------------------------------------------------------- the fused kernels
@@ -302,9 +271,6 @@ def test_heartbeat_responses_at_the_offset_edges():
 
 
 # --------------------------------------------------------------------------- update_state and the send lists
-
-def as_set(e):
-    return sorted(zip(e["group"].tolist(), e["peer_slot"].tolist(), e["flags"].tolist(), e["next_idx"].tolist()))
 
 
 def test_update_state_and_send_lists_at_the_offset_edges():

@@ -12,8 +12,8 @@ import random
 import numpy as np
 import pytest
 
-from helpers import (B, O, assert_columns_equal, bitmap_to_bool, checksum, compact_bufs, compact_round, edge_state, fused_round,
-                     random_batch)
+from helpers import (B, GpuQuorum, O, assert_columns_equal, bitmap_to_bool, checksum, compact_bufs, compact_round,
+                     edge_state, fused_round, random_batch, random_cell_batch, random_config_state)
 from oracle import datadriven as dd
 
 pytestmark = pytest.mark.gpu
@@ -27,53 +27,6 @@ def small():
 
 
 # --------------------------------------------------------------------------- goldens via GPU
-
-class GpuQuorum:
-    """Evaluates the quorum functions on the GPU: voter ids are mapped to peer slots of one
-    arena group, acked indexes become its matched / commit_group_id columns."""
-
-    def __init__(self, arena):
-        self.a = arena
-        self.g = arena.group_alloc()
-
-    def _setup(self, incoming, outgoing, lookup, gc):
-        ids = []
-        for i in list(incoming) + list(outgoing):
-            if i not in ids:
-                ids.append(i)
-        assert len(ids) <= B.SLOTS
-        slot = {i: s for s, i in enumerate(ids)}
-        m_in = sum(1 << slot[i] for i in set(incoming))
-        m_out = sum(1 << slot[i] for i in set(outgoing))
-        self.a.group_set_conf(self.g, 0, 0, 0, None, 1)            # drop every Progress
-        self.a.group_set_conf(self.g, m_in, m_out, 0, None, 1)
-        self.a.set_group_commit(self.g, gc)
-        for i, s in slot.items():
-            p = self.a.progress_get(self.g, s)
-            p.matched, p.commit_group_id = lookup.get(i, (0, 0))   # missing voter == (0, 0)
-            self.a.progress_set(self.g, s, p)
-        return slot
-
-    def joint(self, incoming, outgoing, lookup, gc):
-        self._setup(incoming, outgoing, lookup, gc)
-        return self.a.maximal_committed_index(self.g)
-
-    def majority(self, voters, lookup, gc):
-        return self.joint(voters, [], lookup, gc)
-
-    def joint_vote(self, incoming, outgoing, votes):
-        slot = self._setup(incoming, outgoing, {}, False)
-        self.a.reset_votes(self.g)
-        for i, v in votes.items():
-            if i in slot:
-                self.a.record_vote(self.g, slot[i], v)
-        return self.a.vote_result(self.g)[2]
-
-    def majority_vote(self, voters, votes):
-        return self.joint_vote(voters, [], votes)
-
-    def impl(self):
-        return dd.Impl(self.majority, self.joint, self.majority_vote, self.joint_vote)
 
 
 @pytest.mark.parametrize("name,count", [("majority_commit.txt", 16), ("joint_commit.txt", 50),
@@ -853,65 +806,6 @@ def test_fused_compact_step_corner_cases():
     arena.close()
 
 
-def _random_state(n, rng):
-    """Arbitrary configurations (joint, learners, group commit, no self) and per-peer states."""
-    c = O.new_columns(n, n)
-    for g in range(n):
-        inc = int(rng.integers(1, 256))
-        out = int(rng.integers(0, 256)) if rng.random() < 0.3 else 0
-        learners = int(rng.integers(0, 256)) & ~(inc | out) if rng.random() < 0.4 else 0
-        voters = [s_ for s_ in range(8) if (inc | out) >> s_ & 1]
-        self_slot = int(rng.choice(voters)) if rng.random() < 0.9 else None
-        c.meta[g] = O.make_meta(inc, out, learners, self_slot, group_commit=bool(rng.random() < 0.15))
-        base = int(rng.integers(100, 1 << 40))
-        c.last_index[g] = base + int(rng.integers(0, 10))
-        c.term_start[g] = (1 << 64) - 1 if rng.random() < 0.05 else max(1, base - int(rng.integers(0, 30)))
-        c.committed[g] = base - int(rng.integers(0, 40))
-        c.term[g] = int(rng.integers(1, 1000))
-        for s_ in range(8):
-            m = base - int(rng.integers(0, 50))
-            c.matched[s_, g] = m
-            c.next_idx[s_, g] = m + 1 + int(rng.integers(0, 5))
-            c.peer_committed[s_, g] = m - int(rng.integers(0, 5))
-            state = int(rng.choice([O.STATE_PROBE, O.STATE_REPLICATE, O.STATE_REPLICATE, O.STATE_SNAPSHOT]))
-            c.pflags[s_, g] = state | (O.PF_PAUSED if rng.random() < 0.3 else 0) | (O.PF_INS_FULL if rng.random() < 0.2 else 0) | \
-                (O.PF_RECENT_ACTIVE if rng.random() < 0.5 else 0)
-            c.pending_snapshot[s_, g] = m + int(rng.integers(0, 6)) if state == O.STATE_SNAPSHOT else 0
-            c.pending_request_snapshot[s_, g] = int(rng.integers(1, 100)) if rng.random() < 0.05 else 0
-            c.commit_group_id[s_, g] = int(rng.integers(0, 4))
-    return c
-
-
-def _random_batch(ref, n, rng, per_cell):
-    """Group-ordered batch; `per_cell` > 1 lets a (group, peer) cell receive several records."""
-    rows = []
-    for g in range(n):
-        if rng.random() < 0.3:
-            continue
-        meta = int(ref.meta[g])
-        has_self, self_slot = bool(meta & O.META_HAS_SELF), (meta >> 24) & 7
-        slots = rng.permutation(8)[: int(rng.integers(1, 6))]
-        for s_ in slots:
-            s_ = int(s_)
-            for _ in range(int(rng.integers(1, per_cell + 1))):
-                m, nx = int(ref.matched[s_, g]), int(ref.next_idx[s_, g])
-                kind = rng.random()
-                if has_self and s_ == self_slot:
-                    idx = m + int(rng.integers(0, 8))
-                    rows.append((g, s_, B.REC_LOCAL, 0, idx, 0 if rng.random() < 0.2 else idx + int(rng.integers(0, 5))))
-                elif kind < 0.7:
-                    idx = max(0, m + int(rng.integers(-6, 12)))
-                    commit = idx + 3 if rng.random() < 0.03 else max(0, idx - int(rng.integers(0, 300 if rng.random() < 0.05 else 6)))
-                    rows.append((g, s_, 0, 0, idx, commit))
-                else:
-                    idx = int(rng.choice([nx - 1, m, m + 1, m + 3, max(0, m - 2)]))
-                    rows.append((g, s_, B.REC_REJECT, 0, idx, max(0, m - int(rng.integers(0, 4)))))
-                    if rng.random() < 0.85:
-                        rows.append((g, s_, B.REC_EXT, 0, max(0, idx + int(rng.integers(-5, 3))),
-                                     int(rng.integers(1, 1 << 30)) if rng.random() < 0.2 else 0))
-    return np.array(rows, dtype=B.APPEND_RESP_DTYPE) if rows else np.zeros(0, dtype=B.APPEND_RESP_DTYPE)
-
-
 @pytest.mark.parametrize("seed", [1, 2, 3, "edges"])
 def test_every_ingest_path_agrees_with_the_oracle_on_random_states(seed):
     """Differential test: arbitrary configurations / peer states, random group-ordered batches (accepts,
@@ -924,7 +818,7 @@ def test_every_ingest_path_agrees_with_the_oracle_on_random_states(seed):
     edges = seed == "edges"
     rng = np.random.default_rng(4 if edges else seed)
     n = 2500
-    init = _random_state(n, rng)
+    init = random_config_state(n, rng)
     if edges:
         edge_state(init, rng)
     ref = O.copy_columns(init)
@@ -945,7 +839,7 @@ def test_every_ingest_path_agrees_with_the_oracle_on_random_states(seed):
     blob, dc = compact_bufs(arenas["fusedc"], n, 40)
     for rnd in range(5):
         per_cell = 3 if rnd >= 3 else 1          # the last rounds: several records per (group, peer)
-        recs = random_batch(ref, rng, per_cell, edge=True) if edges else _random_batch(ref, n, rng, per_cell)
+        recs = random_batch(ref, rng, per_cell, edge=True) if edges else random_cell_batch(ref, n, rng, per_cell)
         O.arena_apply(ref, recs, mode=0)
         want_adv, want_bm, _, _ = O.arena_recompute(ref)
         words = (n + 31) // 32
@@ -1128,7 +1022,7 @@ def test_heartbeat_commits_vs_oracle():
     (raft.rs:838-840, 875-889) as one dense pass, on arbitrary configurations."""
     rng = np.random.default_rng(21)
     n = 5000
-    init = _random_state(n, rng)
+    init = random_config_state(n, rng)
     arena = B.Arena(n)
     arena.group_alloc_range(n)
     arena.load_columns(init)

@@ -16,23 +16,21 @@ CPU by test_term_wave_edges.py.  Run with -m gpu."""
 import numpy as np
 import pytest
 
-from helpers import B, O, assert_columns_equal
+from helpers import B, O, assert_columns_equal, check_columns
 from oracle import control_oracle as CO
 from oracle import wire_waves_oracle as WW
+import follow_term as T
 import hb_frames as F
+import leader_term as L
+import pass_forms as PF
 import term_wave16 as W
-import test_gpu_append_reject as GAR
-import test_gpu_follower_term as GT
-import test_gpu_leader_term as GL
-import test_gpu_vote_request_wire as GV
-import test_gpu_wire_batches as WBT
 
 pytestmark = pytest.mark.gpu
 
 # sizes that keep every transition's count well above W.FLOOR (test_term_wave_edges.py checks the generators at
 # smaller ones) and the file's wall time near a minute
 N_NARROW, N_WIDE, N_LEADERS = 6_000, 200, 6_000
-RUN = {"vote_request": GV._run, "follower_term": GT._run, "leader_term": GL._run}
+RUN = {"vote_request": "vote_request_wire", "follower_term": "follower_term_wire", "leader_term": "leader_term_wire"}
 
 
 def _check_windows(a, c, n, rng, k=400):
@@ -69,16 +67,16 @@ def test_bumps_reset_onto_the_16bit_edges(name, device):
     assert np.all(a.control(fill)["status"] == 0)
     res, _ = a.read_index_request(reqs)
     assert (res == B.READ_QUEUED).sum() > 100
-    GT._check_columns(a, c, vt, s.n, ins=True)
+    check_columns(a, c, vt, s.n, ins=True)
     _check_reads(a, q, s.lows)
     before, q0 = O.copy_columns(c), q.copy()
     frames_ = W.bump_frames(rng, s, name)
-    frames_ += (GL._noise if name == "leader_term" else GT._noise)(rng, s, 250)
+    frames_ += (L.noise if name == "leader_term" else T.noise)(rng, s, 250)
     blob, off = F.batch(frames_)
     want = W.BATCH[name](c, q, vt, blob, off, s.table)
-    got = RUN[name](a, frames_, s.table, device)
-    GT._equal(want, got, name)
-    GT._check_columns(a, c, vt, s.n, ins=True)
+    got = PF.run(a, RUN[name], blob, off, s.table, device=device)
+    PF.equal(want, got, ("status", "out", "bytes", "offsets", "totals"), name)
+    check_columns(a, c, vt, s.n, ins=True)
     assert_columns_equal(a.read_columns(s.n), c, s.n, name)
     _check_windows(a, c, s.n, rng)
     _check_reads(a, q, s.lows)
@@ -112,9 +110,9 @@ def test_wave_kernels_at_the_16bit_edges_with_inflights(runs):
         assert a.set_wire_waves(waves) == 0
         want = WW.leader(c, r, blob, off, waves)
         if form == "device":
-            got = GAR._apply_device(a, blob, off)
+            got = PF.device(a, "wire_apply", blob, off)[0]
         else:
-            a.step_begin_wire(WBT._host_batch(blob, off, len(blob)), B.STEP_READ_COMMITTED)
+            a.step_begin_wire(PF.host_batch(blob, off, len(blob)), B.STEP_READ_COMMITTED)
             a.step_wait()
             got = a.wire_status().copy()
             O.arena_recompute(c)

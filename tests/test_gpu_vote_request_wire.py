@@ -8,74 +8,21 @@ import pytest
 from oracle import oracle as O
 from oracle import read_oracle as RO
 from oracle import vote_request_oracle as VR
-from helpers import B
+from helpers import B, arena_of, votes, ARENA_COLUMNS
 from control_cmds import cmds
 import hb_frames as F
+import pass_forms as PF
 import vote_request_frames as Q
-import test_oracle_vote_request as T
 
 pytestmark = pytest.mark.gpu
-
-ARENA_COLUMNS = ("term_start", "committed", "last_index", "matched", "next_idx", "peer_committed", "pflags")
-
-
-def _device(a, blob, off, voters, n_bytes=None):
-    """The device form over buffers from raftgpu_device_alloc (n_bytes: of blob, all of it by default) -> (status, out,
-    response blob, offsets, totals)."""
-    n = len(off) - 1
-    n_bytes = len(blob) if n_bytes is None else n_bytes
-    blob = np.concatenate([blob, np.zeros(16, np.uint8)])
-    bound = B.vote_request_wire_bound(n)
-    vt = np.ascontiguousarray(voters, B.VOTER_DTYPE)
-    sizes = (len(blob), 4 * (n + 1), max(64, vt.nbytes), max(1, n), max(16, 16 * n), max(16, bound), 4 * (n + 1), 16)
-    bufs = [a.device_alloc(x) for x in sizes]
-    d_b, d_o, d_v, d_st, d_out, d_rb, d_ro, d_t = bufs
-    for p, x in ((d_b, blob), (d_o, off), (d_v, vt)):
-        a.h2d(p, x)
-    a.vote_request_wire_device(d_b, n_bytes, d_o, n, d_v, d_st, d_out, d_rb, bound, d_ro, d_t)
-    a.synchronize()
-    tot = np.zeros(2, np.uint64)
-    a.d2h(tot, d_t)
-    st, out = np.zeros(n, np.uint8), np.zeros((n, 2), np.uint64)
-    rb, ro = np.zeros(int(tot[1]), np.uint8), np.zeros(int(tot[0]) + 1, np.uint32)
-    for arr, p in ((st, d_st), (out, d_out), (ro, d_ro), (rb, d_rb)):
-        if arr.size:
-            a.d2h(arr, p)
-    for p in bufs:
-        a.device_free(p)
-    return st, out, rb, ro, tot
-
-
-def _run(a, frames, voters, device):
-    if device:
-        blob, off = F.batch(frames)
-        return _device(a, blob, off, voters)
-    return a.vote_request_wire(F.Frames(frames), voters)
-
 
 def _columns(a, n):
     c = a.read_columns(n)
     return {k: getattr(c, k) for k in ARENA_COLUMNS} | {"term": a.column_read(B.COL_TERM, 0, 0, n, np.uint64)}
 
 
-def _votes(a, n):
-    return np.stack([a.column_read(B.COL_VOTES, s, 0, n, np.uint8) for s in range(O.SLOTS)])
-
-
-def _arena_of(s, read_index=False):
-    a = B.Arena(s.n + 64)
-    if read_index:
-        a.enable_read_index()
-    if s.n_narrow:
-        assert a.group_alloc_range(s.n_narrow) == 0
-    for k in range(s.n_wide):
-        assert a.group_alloc_wide() == s.n_narrow + 2 * k
-    assert np.all(a.control(s.setup)["status"] == 0)
-    return a
-
-
 def _single(state):
-    """An arena holding T._one's group 0."""
+    """An arena holding Q.one's group 0."""
     c, _, _, _ = state
     a = B.Arena(64)
     assert a.group_alloc_range(1) == 0
@@ -91,16 +38,16 @@ def _single(state):
 
 
 def _table_rows():
-    rows = [("recv", k) for k in range(len(T.RECV_VOTE))] + [("voter", k) for k in range(len(T.VOTER))]
+    rows = [("recv", k) for k in range(len(Q.RECV_VOTE))] + [("voter", k) for k in range(len(Q.VOTER))]
     return rows + [("any", (r, t)) for r in (Q.FOLLOWER, Q.CANDIDATE, Q.PRE_CANDIDATE, Q.LEADER) for t in (Q.VOTE, Q.PRE_VOTE)]
 
 
 def _table_case(kind, k):
     if kind == "recv":
-        return T.recv_vote_case(T.RECV_VOTE[k])
+        return Q.recv_vote_case(Q.RECV_VOTE[k])
     if kind == "voter":
-        return T.voter_case(T.VOTER[k])
-    return T.any_state_case(*k)
+        return Q.voter_case(Q.VOTER[k])
+    return Q.any_state_case(*k)
 
 
 @pytest.mark.parametrize("device", [False, True], ids=["host", "device"])
@@ -111,7 +58,7 @@ def test_reference_tables_match_the_oracle(device):
         c, vt, _, t = state
         blob, off = F.batch(frames)
         want = VR.batch(c, None, vt, blob, off, t)
-        got = _run(a, frames, t, device)
+        got = PF.run(a, "vote_request_wire", *F.batch(frames), t, device=device)
         for w, g, name in zip(want, got, ("status", "out", "bytes", "offsets", "totals")):
             assert np.array_equal(w, g), (kind, k, name, w, g)
         cols = _columns(a, 1)
@@ -142,7 +89,7 @@ def test_statuses_in_order_match_the_oracle():
                   F.frame(1, 0, Q.request(Q.PRE_VOTE, 4, 4, 10, frm=3))]
         blob, off = F.batch(frames)
         want = VR.batch(c, None, np.zeros((O.SLOTS, c.cap), np.uint8), blob, off, t)
-        got = _run(a, frames, t, device)
+        got = PF.run(a, "vote_request_wire", *F.batch(frames), t, device=device)
         assert all(np.array_equal(w, g) for w, g in zip(want, got)), (device, want[0], got[0])
         assert (got[0] >> 4).tolist() == [B.WIRE_MALFORMED, B.WIRE_MALFORMED, B.WIRE_SKIP_TYPE, B.WIRE_ROLE, B.WIRE_ROLE,
                                           B.WIRE_TERM, B.WIRE_TERM, B.WIRE_IGNORED, B.WIRE_DUP, B.WIRE_COMMIT_VOTE,
@@ -159,8 +106,8 @@ def test_statuses_in_order_match_the_oracle():
 def test_random_batches_vs_oracle(device, read_index):
     rng = np.random.default_rng(0x7200 + 2 * device + read_index)
     s = Q.Scenario(rng, 96_000, 2_000)
-    a = _arena_of(s, read_index)
-    c, vt = T.state_of(s)
+    a = arena_of(s, read_index)
+    c, vt = Q.state_of(s)
     q = None
     if read_index:
         q = RO.ReadQueues(c.cap, 8)
@@ -172,16 +119,16 @@ def test_random_batches_vs_oracle(device, read_index):
         frames = [frames[i] for i in rng.permutation(len(frames))]
         blob, off = F.batch(frames)
         want = VR.batch(c, q, vt, blob, off, table)
-        got = _run(a, frames, table, device)
+        got = PF.run(a, "vote_request_wire", *F.batch(frames), table, device=device)
         for w, g, name in zip(want, got, ("status", "out", "bytes", "offsets", "totals")):
             assert np.array_equal(w, g), (rnd, name, np.flatnonzero(w != g)[:5] if w.shape == g.shape else (w.shape, g.shape))
         cols = _columns(a, s.n)
         for name in ARENA_COLUMNS + ("term",):
             assert np.array_equal(cols[name], getattr(c, name)[..., : s.n]), (rnd, name)
-        assert np.array_equal(_votes(a, s.n), vt[:, : s.n])
+        assert np.array_equal(votes(a, s.n), vt[:, : s.n])
         if read_index:
             assert all(len(a.read_index_get(g)[0]) == q.count[g] for g in range(0, s.n, 997))
-        T.caller_update(table, s.role, got[0], got[1], frames)
+        Q.caller_update(table, s.role, got[0], got[1], frames)
         kinds += np.bincount(got[0] >> 4, minlength=16)
     for k in (B.WIRE_OK, B.WIRE_DUP, B.WIRE_ROLE, B.WIRE_TERM, B.WIRE_SKIP_TYPE, B.WIRE_MALFORMED, B.WIRE_COMMIT_VOTE,
               B.WIRE_IGNORED):
@@ -228,7 +175,7 @@ def test_1m_storm_pre_vote_then_vote_round():
         pending_blob, pending_off, rounds = blob, off, 0
         while len(pending_off) > 1:
             want = VR.batch(c, None, vt, pending_blob, pending_off, table)
-            got = _device(a, pending_blob[: pending_off[-1]], pending_off, table)
+            got = PF.device(a, "vote_request_wire", pending_blob[: pending_off[-1]], pending_off, table)
             for w, gg, name in zip(want, got, ("status", "out", "bytes", "offsets", "totals")):
                 assert np.array_equal(w, gg), (typ, rounds, name)
             st, out = got[0], got[1]
@@ -263,33 +210,24 @@ def test_refusals_before_any_launch():
     t = Q.voters(64)
     t["flags"] = B.VOTER_SELECT
     bound = B.vote_request_wire_bound(n)
-    d_b, d_o, d_v = a.device_alloc(len(blob)), a.device_alloc(4 * (n + 1)), a.device_alloc(t.nbytes + 64)
-    d_st, d_out, d_rb, d_ro, d_t = (a.device_alloc(x) for x in (n, 16 * n, bound + 16, 4 * (n + 1), 16))
-    for p, x in ((d_b, blob), (d_o, off), (d_v, t), (d_st, np.full(n, 0xEE, np.uint8)), (d_t, np.full(2, 77, np.uint64))):
-        a.h2d(p, x)
     nb = off[-1]
-    dev = lambda **k: L.raftgpu_vote_request_wire_device(
-        h, None, k.get("b", d_b), k.get("nb", nb), k.get("o", d_o), k.get("n", n), k.get("v", d_v), k.get("st", d_st),
-        k.get("out", d_out), k.get("rb", d_rb), k.get("cap", bound), k.get("ro", d_ro), k.get("t", d_t))
-    refused = [dev(cap=bound - 1), dev(b=d_b + 4), dev(v=d_v + 8), dev(rb=d_rb + 4), dev(nb=1 << 32),
-               dev(n=1 << 32, cap=1 << 40), dev(n=(1 << 26) + 1, cap=1 << 40), dev(v=None), dev(st=None), dev(b=None),
-               dev(o=None), dev(rb=None), dev(t=None), dev(ro=None)]
-    assert refused == [B.ERR_INVALID] * len(refused), refused
-    a.synchronize()
-    gst, gt = np.zeros(n, np.uint8), np.zeros(2, np.uint64)
-    a.d2h(gst, d_st), a.d2h(gt, d_t)
-    assert np.all(gst == 0xEE) and gt.tolist() == [77, 77]                    # nothing was launched
-    assert np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 3)
-    st, out, rb, ro, tot = np.zeros(n, np.uint8), np.zeros(2 * n, np.uint64), np.zeros(bound, np.uint8), \
-        np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
-    assert L.raftgpu_vote_request_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, t.ctypes.data, st.ctypes.data,
-                                       out.ctypes.data, rb.ctypes.data, bound - 1, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
-    assert L.raftgpu_vote_request_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, None, st.ctypes.data,
-                                       out.ctypes.data, rb.ctypes.data, bound, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
-    assert dev() == B.OK                                                      # the same call with every rule kept
-    a.synchronize()
-    a.d2h(gt, d_t)
-    assert gt.tolist()[0] == n and np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 4)
+    with PF.refusals(a, "vote_request_wire", blob, off, t, n_bytes=nb) as r:
+        dev, d = r.call, r.args
+        refused = [dev(cap=bound - 1), dev(b=d["b"] + 4), dev(v=d["v"] + 8), dev(rb=d["rb"] + 4), dev(nb=1 << 32),
+                   dev(n=1 << 32, cap=1 << 40), dev(n=(1 << 26) + 1, cap=1 << 40), dev(v=None), dev(st=None), dev(b=None),
+                   dev(o=None), dev(rb=None), dev(t=None), dev(ro=None)]
+        assert refused == [B.ERR_INVALID] * len(refused), refused
+        assert r.untouched()                                                  # nothing was launched
+        assert np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 3)
+        st, out, rb, ro, tot = np.zeros(n, np.uint8), np.zeros(2 * n, np.uint64), np.zeros(bound, np.uint8), \
+            np.zeros(n + 1, np.uint32), np.zeros(2, np.uint64)
+        assert L.raftgpu_vote_request_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, t.ctypes.data, st.ctypes.data,
+                                           out.ctypes.data, rb.ctypes.data, bound - 1, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
+        assert L.raftgpu_vote_request_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, None, st.ctypes.data,
+                                           out.ctypes.data, rb.ctypes.data, bound, ro.ctypes.data, tot.ctypes.data) == B.ERR_INVALID
+        assert dev() == B.OK                                                      # the same call with every rule kept
+        gt = r.read("t", np.zeros(2, np.uint64))
+        assert gt.tolist()[0] == n and np.all(a.column_read(B.COL_TERM, 0, 0, 16, np.uint64) == 4)
     a.close()
 
 

@@ -8,61 +8,22 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from oracle import oracle as O
-from oracle import control_oracle as CO
 from oracle import vote_wire_oracle as VW
-from helpers import B
+from helpers import B, arena_of, votes
 from control_cmds import cmds
 import hb_frames as F
+import pass_forms as PF
 import vote_frames as V
-import test_oracle_vote_wire as T
 
 pytestmark = pytest.mark.gpu
-
-
-def _arena(e):
-    a = B.Arena(e.n + 64)
-    if e.n_narrow:
-        assert a.group_alloc_range(e.n_narrow) == 0
-    for k in range(e.n_wide):
-        assert a.group_alloc_wide() == e.n_narrow + 2 * k
-    assert np.all(a.control(e.setup)["status"] == 0)
-    a.control(e.campaign)
-    return a
-
-
-def _votes(a, n):
-    return np.stack([a.column_read(B.COL_VOTES, s, 0, n, np.uint8) for s in range(O.SLOTS)])
-
-
-def _device(a, blob, off, sel, pre, cap=None, n_bytes=None):
-    """The device form over buffers from raftgpu_device_alloc (n_bytes: of blob, all of it by default) -> (status,
-    outcomes)."""
-    n = len(off) - 1
-    cap = min(n, a.get_info().n_alloc) if cap is None else cap
-    bufs = [a.device_alloc(x) for x in (max(16, len(blob)), 4 * (n + 1), sel.nbytes, pre.nbytes, max(1, n), 8 * max(1, cap), 8)]
-    d_b, d_o, d_s, d_p, d_st, d_out, d_cnt = bufs
-    for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_p, pre)):
-        a.h2d(p, x)
-    a.vote_wire_device(d_b, len(blob) if n_bytes is None else n_bytes, d_o, n, d_s, d_p, d_st, d_out, cap, d_cnt)
-    a.synchronize()
-    cnt = np.zeros(1, np.uint64)
-    a.d2h(cnt, d_cnt)
-    st, out = np.zeros(n, np.uint8), np.zeros(int(cnt[0]), B.VOTE_OUTCOME_DTYPE)
-    a.d2h(st, d_st)
-    if len(out):
-        a.d2h(out, d_out)
-    for p in bufs:
-        a.device_free(p)
-    return st, out
 
 
 # --------------------------------------------------------------------------- 1. the table and the statuses
 
 
-@pytest.mark.parametrize("case", range(len(T.ONE_ROUND)))
+@pytest.mark.parametrize("case", range(len(V.ONE_ROUND)))
 def test_leader_election_in_one_round_rpc(case):
-    size, votes, state = T.ONE_ROUND[case]
+    size, votes, state = V.ONE_ROUND[case]
     a = B.Arena(64)
     assert a.group_alloc_range(1) == 0
     a.control(cmds((B.CTL_SET_CONF, 0, 0, 0, ((1 << size) - 1, 0, 0, 11)), (B.CTL_RESET, 0, 0, 0, (B.NO_TERM_START, 10, 5, 10))))
@@ -72,7 +33,7 @@ def test_leader_election_in_one_round_rpc(case):
     frames = [F.frame(0, k - 1, V.message(6, 1, not v, to=1, frm=k)) for k, v in votes.items()]
     st, outs = a.vote_wire(F.Frames(frames), V.bitmap([True]))
     assert np.all(st == (B.WIRE_OK << 4 | B.RES_OK))
-    assert T.expected_state(first, outs) == state and len(outs) == (state != "Candidate" and bool(frames))
+    assert V.expected_state(first, outs) == state and len(outs) == (state != "Candidate" and bool(frames))
     a.close()
 
 
@@ -85,7 +46,7 @@ def test_statuses_match_the_oracle():
         a.control(cmds(*[(B.CTL_SET_CONF, g, 0, 0, (0x1F, 0, 0, 11)) for g in range(4)],
                        *[(B.CTL_RESET, g, 0, 0, (11 if g == 2 else B.NO_TERM_START, 10, 5, 10)) for g in range(4)],
                        *[(B.CTL_SET_TERM, g, 0, 0, (7,)) for g in range(4)]))
-        c, vt = T._arena([meta] * 4, [7] * 4)
+        c, vt = V.candidates([meta] * 4, [7] * 4)
         c.term_start[2] = 11
         frames = [F.frame(9, 1, V.message(6, 7)), F.frame(0, 1, b"\x08"), F.frame(0, 1, V.message(4, 7)),
                   F.frame(3, 1, V.message(6, 7)), F.frame(2, 1, V.message(6, 7)), F.frame(0, 1, V.message(18, 7)),
@@ -95,12 +56,13 @@ def test_statuses_match_the_oracle():
                   F.frame(0, 3, V.message(6, 7, True)), F.frame(0, 2, V.message(6, 7, True)), F.frame(1, 1, V.message(18, 8)),
                   F.frame(1, 9, V.message(18, 7)), F.frame(0, 4, V.message(6, 7))]
         sel, pre = V.bitmap([True, True, True, False]), V.bitmap([False, True, False, False])
-        want_st, want_out, _ = T._run(c, vt, frames, [True, True, True, False], [False, True, False, False])
+        want_st, want_out, _ = V.run_batch(c, vt, frames, [True, True, True, False], [False, True, False, False])
         blob, off = F.batch(frames)
-        got = _device(a, np.concatenate([blob, np.zeros(16, np.uint8)]), off, sel, pre) if device else \
+        got = PF.device(a, "vote_wire", np.concatenate([blob, np.zeros(16, np.uint8)]), off, sel, pre,
+                                           n_bytes=len(blob) + 16) if device else \
             a.vote_wire(F.Frames(frames), sel, pre)
         assert np.array_equal(got[0], want_st) and np.array_equal(got[1], want_out), (device, got, want_st, want_out)
-        assert np.array_equal(_votes(a, 4), vt[:, :4]) and np.count_nonzero(vt[:, :4]) == 4
+        assert np.array_equal(votes(a, 4), vt[:, :4]) and np.count_nonzero(vt[:, :4]) == 4
         a.close()
 
 
@@ -111,9 +73,9 @@ def test_statuses_match_the_oracle():
 def test_random_elections_vs_oracle(device):
     rng = np.random.default_rng(0x7077 + device)
     e = V.Election(rng, 96_000, 2_000)
-    a = _arena(e)
-    c, vt = T._state(e)
-    assert np.array_equal(_votes(a, e.n), vt[:, :e.n])
+    a = arena_of(e)
+    c, vt = V.state_of(e)
+    assert np.array_equal(votes(a, e.n), vt[:, :e.n])
     kinds = np.zeros(16, np.int64)
     for rnd in range(2):
         frames = e.frames(rng, commit_vote=True)
@@ -124,11 +86,12 @@ def test_random_elections_vs_oracle(device):
         pre = np.concatenate([e.pre(), np.zeros(4, np.uint32)])
         before = a.counters()["votes_tallied"]
         want_st, want_out, tallied = VW.batch(c, vt, blob, off, sel, pre)
-        got_st, got_out = _device(a, np.concatenate([blob, np.zeros(16, np.uint8)]), off, sel, pre) if device else \
+        got_st, got_out = PF.device(a, "vote_wire", np.concatenate([blob, np.zeros(16, np.uint8)]), off, sel, pre,
+                                           n_bytes=len(blob) + 16) if device else \
             a.vote_wire(F.Frames(frames), sel, pre)
         assert np.array_equal(got_st, want_st), (rnd, np.flatnonzero(got_st != want_st)[:5])
         assert np.array_equal(got_out, want_out), rnd
-        assert np.array_equal(_votes(a, e.n), vt[:, :e.n]), rnd
+        assert np.array_equal(votes(a, e.n), vt[:, :e.n]), rnd
         assert a.counters()["votes_tallied"] - before == tallied
         kinds += np.bincount(got_st >> 4, minlength=16)
         assert len(want_out) > 10_000
@@ -182,7 +145,7 @@ def test_1m_storm_against_the_control_list():
     e["hdr"], e["msg_type"], e["to"], e["from"] = gs << 4 | slots, 6, 1, slots + 1
     e["term"], e["reject"] = term[gs], 1 - granted
     blob, off = B.synth_encode_votes(e)
-    st, out = _device(arenas[0], blob, off, V.bitmap(np.ones(n, bool)), V.bitmap(np.zeros(n, bool)))
+    st, out = PF.device(arenas[0], "vote_wire", blob, off, V.bitmap(np.ones(n, bool)), V.bitmap(np.zeros(n, bool)))
     assert np.all(st == (B.WIRE_OK << 4 | B.RES_OK))
     res = arenas[1].control(_storm_list(gs, slots, granted))
     assert np.all(res["status"] == 0)
@@ -191,7 +154,7 @@ def test_1m_storm_against_the_control_list():
     decided = np.flatnonzero(last_word & 0xFF != B.VOTE_PENDING)
     assert np.array_equal(out["group"], decided) and np.array_equal(out["result"], last_word[decided])
     assert len(out) == n                                                     # 5 voters, every vote in: all decided
-    assert np.array_equal(_votes(arenas[0], n), _votes(arenas[1], n))
+    assert np.array_equal(votes(arenas[0], n), votes(arenas[1], n))
     won = out["group"][(out["result"] & 0xFF) == B.VOTE_WON]
     win = np.zeros(2 * len(won), B.CTL_CMD_DTYPE)                            # section 6 step 3 on both arenas
     win["group"] = np.repeat(won, 2)
@@ -202,7 +165,7 @@ def test_1m_storm_against_the_control_list():
     c0, c1 = arenas[0].read_columns(n), arenas[1].read_columns(n)
     for name in B.COLUMNS:
         assert np.array_equal(getattr(c0, name), getattr(c1, name)), name
-    assert np.array_equal(_votes(arenas[0], n), _votes(arenas[1], n))
+    assert np.array_equal(votes(arenas[0], n), votes(arenas[1], n))
     for a in arenas:
         a.close()
 
@@ -239,7 +202,7 @@ def test_freed_selected_groups_stay_within_capacity():
     a.d2h(st, d_st), a.d2h(out, d_out), a.d2h(cnt, d_c)
     assert st.tolist() == want and cnt.tolist() == [1]
     assert out[:8].view(B.VOTE_OUTCOME_DTYPE).tolist() == [(0, B.VOTE_WON | 2 << 8)] and np.all(out[8:] == 0xEE)
-    v = _votes(a, 100)
+    v = votes(a, 100)
     assert v[1, 0] == 2 and np.count_nonzero(v[:, 1:]) == 0
     for p in bufs:
         a.device_free(p)
@@ -260,28 +223,19 @@ def test_refusals_before_any_launch():
     n = 16
     blob, off = F.batch([F.frame(g, 1, V.message(6, 3)) for g in range(n)])
     sel = V.bitmap(np.ones(64, bool))
-    d_b, d_o, d_s = a.device_alloc(1024), a.device_alloc(4 * (n + 1)), a.device_alloc(sel.nbytes)
-    d_st, d_out, d_c = a.device_alloc(n), a.device_alloc(8 * n), a.device_alloc(8)
-    for p, x in ((d_b, blob), (d_o, off), (d_s, sel), (d_st, np.full(n, 0xEE, np.uint8)), (d_c, np.full(1, 77, np.uint64))):
-        a.h2d(p, x)
     nb = len(blob)
-    dev = lambda **k: L.raftgpu_vote_wire_device(h, None, k.get("b", d_b), k.get("nb", nb), k.get("o", d_o), k.get("n", n),
-                                                 k.get("s", d_s), None, k.get("st", d_st), k.get("out", d_out),
-                                                 k.get("cap", n), k.get("c", d_c))
-    refused = [dev(cap=n - 1), dev(cap=0, out=None), dev(b=d_b + 4), dev(nb=1 << 32), dev(n=1 << 32, cap=1 << 32),
-               dev(s=None), dev(c=None), dev(st=None), dev(o=None), dev(b=None), dev(out=None)]
-    assert refused == [B.ERR_INVALID] * len(refused), refused
-    a.synchronize()
-    gst, gc = np.zeros(n, np.uint8), np.zeros(1, np.uint64)
-    a.d2h(gst, d_st), a.d2h(gc, d_c)
-    assert np.all(gst == 0xEE) and gc.tolist() == [77]                       # nothing was launched
-    assert np.all(_votes(a, 16) == 0)
-    cnt, outs = C.c_uint64(), np.zeros(n, B.VOTE_OUTCOME_DTYPE)
-    assert L.raftgpu_vote_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, sel.ctypes.data, None, None, outs.ctypes.data,
-                               n - 1, C.byref(cnt)) == B.ERR_INVALID
-    # the capacity rule counts allocated groups: 16 of them, so 16 frames need 16
-    assert dev(cap=16) == B.OK
-    a.synchronize()
-    a.d2h(gc, d_c)
-    assert gc.tolist() == [0] and np.all(_votes(a, 16)[1] == 2)
+    with PF.refusals(a, "vote_wire", blob, off, sel, None, capacity=n) as r:
+        dev, d = r.call, r.args
+        refused = [dev(cap=n - 1), dev(cap=0, out=None), dev(b=d["b"] + 4), dev(nb=1 << 32), dev(n=1 << 32, cap=1 << 32),
+                   dev(s=None), dev(c=None), dev(st=None), dev(o=None), dev(b=None), dev(out=None)]
+        assert refused == [B.ERR_INVALID] * len(refused), refused
+        assert r.untouched()                                                     # nothing was launched
+        assert np.all(votes(a, 16) == 0)
+        cnt, outs = C.c_uint64(), np.zeros(n, B.VOTE_OUTCOME_DTYPE)
+        assert L.raftgpu_vote_wire(h, blob.ctypes.data, nb, off.ctypes.data, n, sel.ctypes.data, None, None, outs.ctypes.data,
+                                   n - 1, C.byref(cnt)) == B.ERR_INVALID
+        # the capacity rule counts allocated groups: 16 of them, so 16 frames need 16
+        assert dev(cap=16) == B.OK
+        gc = r.read("c", np.zeros(1, np.uint64))
+        assert gc.tolist() == [0] and np.all(votes(a, 16)[1] == 2)
     a.close()

@@ -16,8 +16,7 @@ import numpy as np
 import pytest
 
 from oracle import datadriven as dd
-from helpers import B, O, assert_columns_equal
-from test_gpu_parity import GpuQuorum, _random_batch, _random_state
+from helpers import B, O, assert_columns_equal, GpuQuorum, random_cell_batch, random_config_state
 
 pytestmark = pytest.mark.gpu
 
@@ -198,7 +197,7 @@ def test_steps_over_mixed_ordinary_and_wide_groups(seed):
     send list, the heartbeat commits and the vote tally of the result -- all against the oracle."""
     rng = np.random.default_rng(seed)
     n = 3000
-    init = _random_state(n, rng)
+    init = random_config_state(n, rng)
     wide = _widen(init, n, rng)
     assert 300 < wide.sum() < 700
     ref = O.copy_columns(init)
@@ -215,7 +214,7 @@ def test_steps_over_mixed_ordinary_and_wide_groups(seed):
     adv_wide = 0
     for rnd in range(5):
         per_cell = 3 if rnd >= 3 else 1
-        recs = _random_batch(ref, n, rng, per_cell)
+        recs = random_cell_batch(ref, n, rng, per_cell)
         O.arena_apply(ref, recs, mode=0)
         want_adv, want_bm, _, _ = O.arena_recompute(ref)
         lo_bits, hi_bits = np.nonzero(wide)[0], np.nonzero(wide)[0] + 1

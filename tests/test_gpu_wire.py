@@ -9,33 +9,13 @@ import os
 import numpy as np
 import pytest
 
-from helpers import B, O, assert_columns_equal, bitmap_to_bool, checksum
+from helpers import B, O, assert_columns_equal, bitmap_to_bool, checksum, oracle_wire_step
 
 pytestmark = pytest.mark.gpu
 
 W = importlib.import_module("raft-rs_b200.wire")
 HERE = os.path.dirname(os.path.abspath(__file__))
 FLAGS = B.STEP_READ_COMMITTED
-
-
-def oracle_wire_step(ref, wb, n_groups, terms):
-    """What the step must do: local records first, then every frame the decoder accepts, in frame order (the first
-    frame of a cell; later ones are DUP), then Raft::maybe_commit for every group.  Returns (status bytes, adv bitmap)."""
-    res_local = O.arena_apply(ref, wb.records[: wb.n_records].copy(), mode=0) if wb.n_records else None
-    status, recs, hint, snap = O.wire_decode_batch(wb.bytes[: wb.n_bytes], wb.offsets[: wb.n + 1], n_groups, terms)
-    ok = np.nonzero(status == O.WIRE_OK)[0]
-    rows = []
-    for i in ok:
-        rows.append(tuple(recs[i]))
-        if recs["flags"][i] & B.REC_REJECT:
-            rows.append((recs["group"][i], recs["peer_slot"][i], B.REC_EXT, 0, hint[i], snap[i]))
-    seq = np.array(rows, dtype=B.APPEND_RESP_DTYPE) if rows else np.zeros(0, dtype=B.APPEND_RESP_DTYPE)
-    res = O.arena_apply(ref, seq, mode=0)
-    main = (seq["flags"] & B.REC_EXT) == 0
-    want = (status.astype(np.uint32) << 4).astype(np.uint8)
-    want[ok] |= res[main] & 0xF
-    adv, bm, _, _ = O.arena_recompute(ref)
-    return want, bm, adv, res_local
 
 
 def test_golden_messages_through_the_gpu():

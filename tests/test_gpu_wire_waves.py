@@ -15,12 +15,10 @@ from oracle import app_follow_oracle as AL
 from oracle import leader_runs_oracle as LR
 from oracle import wire_waves_oracle as WW
 import app_follow as A
+import app_entries as E
 import append_reject as R
-import test_gpu_append_reject as GAR
-import test_gpu_follower_append as GFA
-import test_gpu_follower_append_entries as GFE
-import test_gpu_wire_batches as WBT
-import test_oracle_wire_waves as T
+import hb_follow as FL
+import pass_forms as PF
 
 pytestmark = pytest.mark.gpu
 
@@ -42,14 +40,14 @@ def _leaders(seed, n=N_LEADERS):
 
 
 def _leader_batch(rng, c, n):
-    frames = T.leader_frames(rng, c, range(n), PEERS, 6, needs_log=0.4)
+    frames = R.leader_frames(rng, c, range(n), PEERS, 6, needs_log=0.4)
     frames += [A.frame(5, 1, R.response(int(c.term[5]) + 1, index=1)), b"\x01\x02", A.frame(n + 7, 1, R.response(1)),
                A.frame(9, 2, b"\x08\x03")]                                      # TERM, hostile, another type
     return A.batch(frames)
 
 
 def _step_host(a, blob, off):
-    a.step_begin_wire(WBT._host_batch(blob, off, len(blob)), B.STEP_READ_COMMITTED)
+    a.step_begin_wire(PF.host_batch(blob, off, len(blob)), B.STEP_READ_COMMITTED)
     a.step_wait()
     return a.wire_status().copy()
 
@@ -61,7 +59,7 @@ def test_leader_waves_100k_x5(runs):
     then raftgpu_step_begin_wire at 4: statuses and columns against the wave oracle."""
     rng, logs, c, rows = _leaders(0x3A7E + runs)
     n = N_LEADERS
-    a = GAR._arena(c, n, runs)
+    a = R.leader_arena(c, n, runs)
     r = rows if runs else None
     if runs:
         assert (a.leader_runs_set(rows) == 0).all()
@@ -70,7 +68,7 @@ def test_leader_waves_100k_x5(runs):
         blob, off = _leader_batch(rng, ref, n)
         assert a.set_wire_waves(waves) == 0
         want = WW.leader(ref, r, blob, off, waves)
-        got = GAR._apply_device(a, blob, off)
+        got = PF.device(a, "wire_apply", blob, off)[0]
         bad = np.flatnonzero(got != want)
         assert len(bad) == 0, (waves, [(int(i), hex(got[i]), hex(want[i])) for i in bad[:5]])
         assert_columns_equal(a.read_columns(n), ref, n, f"device form, waves {waves}")
@@ -92,18 +90,18 @@ def test_one_wave_is_the_arena_without_the_setter():
     rng, logs, c, rows = _leaders(0x1A1, 20_000)
     n = 20_000
     blob, off = _leader_batch(rng, c, n)
-    a1, a0 = GAR._arena(c, n, False), GAR._arena(c, n, False)
+    a1, a0 = R.leader_arena(c, n, False), R.leader_arena(c, n, False)
     assert a1.set_wire_waves(5) == 0 and a1.set_wire_waves(1) == 0
-    assert np.array_equal(GAR._apply_device(a1, blob, off), GAR._apply_device(a0, blob, off))
+    assert np.array_equal(PF.device(a1, "wire_apply", blob, off)[0], PF.device(a0, "wire_apply", blob, off)[0])
     assert_columns_equal(a1.read_columns(n), a0.read_columns(n), n, "one wave")
     a1.close(), a0.close()
-    fa1, fc, _, table = GFE._world(rng, 20_000, 200, False)
-    fa0 = GFE._world(np.random.default_rng(0), 20_000, 200, False)[0]
+    fa1, fc, _, table = E.world(rng, 20_000, 200, False)
+    fa0 = E.world(np.random.default_rng(0), 20_000, 200, False)[0]
     _copy_state(fa1, fa0, fc.n_groups)
     fb, fo = _follower_batch(rng, fc, table, range(20_000), 4)
     assert fa1.set_wire_waves(1) == 0
     t1, t0 = table.copy(), table.copy()
-    g1, g0 = GFE._host(fa1, fb, fo, t1), GFE._host(fa0, fb, fo, t0)
+    g1, g0 = PF.host(fa1, "follower_append_entries", fb, fo, t1), PF.host(fa0, "follower_append_entries", fb, fo, t0)
     for x, y in zip(g1, g0):
         assert np.array_equal(x, y)
     assert np.array_equal(t1, t0)
@@ -121,13 +119,13 @@ def _follower_batch(rng, c, table, groups, per_group, entries=True, junk=True):
     groups' frames."""
     per = []
     for g in groups:
-        wide = bool(c.meta[g] & GFE.WIDE_LO)
+        wide = bool(c.meta[g] & E.WIDE_LO)
         last = int(max(c.last_index[g], c.last_index[g + 1])) if wide else int(c.last_index[g])
         com = int(max(c.committed[g], c.committed[g + 1])) if wide else int(c.committed[g])
         run_term, term = int(table["run_term"][g]), int(c.term[g])
         if int(table["run_start"][g]) > last or run_term > term:
             continue
-        bodies = [b for b, _ in T.pipelined_appends(rng, last, run_term, term, com, int(rng.integers(1, per_group + 1)),
+        bodies = [b for b, _ in R.pipelined_appends(rng, last, run_term, term, com, int(rng.integers(1, per_group + 1)),
                                                     entries)]
         if junk and len(bodies) > 1 and rng.random() < 0.2:
             k = int(rng.integers(1, len(bodies)))
@@ -141,7 +139,7 @@ def _follower_batch(rng, c, table, groups, per_group, entries=True, junk=True):
                 bad = A.message(3, term=term, log_term=0, index=last + 50, commit=last + 50, frm=3)
             bodies.insert(k, bad)
         per.append((g, [A.frame(g, int(rng.integers(16)), b) for b in bodies]))
-    return A.batch(T.interleave(rng, per))
+    return A.batch(R.interleave(rng, per))
 
 
 @pytest.mark.parametrize("entries", [False, True], ids=["entry_less", "entries"])
@@ -151,7 +149,7 @@ def test_follower_waves_100k(entries, device):
     COMMIT_RANGE frames among them, at waves 3 and RAFTGPU_WIRE_WAVES_MAX: every output, the table and the group columns
     against the wave oracle."""
     rng = np.random.default_rng(0xF0 + 2 * entries + device)
-    a, c, q, table = GFE._world(rng, GFE.N_NARROW, GFE.N_WIDE, False)
+    a, c, q, table = E.world(rng, E.N_NARROW, E.N_WIDE, False)
     n = c.n_groups
     lows = [g for g in range(n) if not (c.meta[g] & WIDE_HI)]
     for waves in (3, B.WIRE_WAVES_MAX):
@@ -160,14 +158,14 @@ def test_follower_waves_100k(entries, device):
         want_table = table.copy()
         want = WW.follower(c, q, want_table, blob, off, waves, entries)
         if entries:
-            got = (GFE._device if device else GFE._host)(a, blob, off, table)
+            got = PF.run(a, "follower_append_entries", blob, off, table, device=device)
             got = tuple(got[:2]) + (got[2].view(AE.APPENDED_DTYPE),) + tuple(got[3:])
-            WBT._equal(want, got, GFE.NAMES, ("waves", waves))
+            PF.equal(want, got, E.NAMES, ("waves", waves))
             assert np.array_equal(table, want_table)
         else:
-            got = (GFA._device if device else GFA._host)(a, blob, off, table)
-            WBT._equal(want[:2] + want[3:], got, GFA.NAMES, ("waves", waves))
-        for name, col in GFA._group_state(a, n).items():
+            got = PF.device(a, "follower_append", blob, off, table) if device else A.host_form(a, blob, off, table)
+            PF.equal(want[:2] + want[3:], got, A.NAMES, ("waves", waves))
+        for name, col in FL.group_state(a, n).items():
             assert np.array_equal(col, getattr(c, name)[:n]), (waves, name)
         st = want[0] >> 4
         assert (st == B.WIRE_COMMIT_RANGE).sum() > 100 and ((st == B.WIRE_NEEDS_LOG).sum() > 100) == entries
@@ -218,18 +216,18 @@ def test_round_trip_k_pipelined_appends():
         for col, name in ((B.COL_TERM, "term"), (B.COL_LAST_INDEX, "last_index"), (B.COL_COMMITTED, "committed"),
                           (B.COL_TERM_START, "term_start")):
             fa.column_write(col, 0, 0, getattr(fc, name)[:n].copy())
-        st, frm, app, rb, ro, tot = GFE._device(fa, blob, off, table)
+        st, frm, app, rb, ro, tot = PF.device(fa, "follower_append_entries", blob, off, table)
         fa.close()
         assert ((st >> 4) == B.WIRE_OK).all() and int(tot[0]) == n * k
         resp = [bytes(rb[x:y]) for x, y in zip(ro[:-1].tolist(), ro[1:].tolist())]
         for i, r in enumerate(resp):                                             # frame order: group g's j-th at g * k + j
             resp_by_round[i % k].append(r)
     # k rounds at one wave on a twin
-    twin = GAR._arena(lc, n, False)
+    twin = R.leader_arena(lc, n, False)
     for j in range(k):
         b1, o1 = A.batch(resp_by_round[j])
         assert ((_step_host(twin, b1, o1) >> 4) == B.WIRE_OK).all()
-    la = GAR._arena(lc, n, False)
+    la = R.leader_arena(lc, n, False)
     assert la.set_wire_waves(k) == 0
     allb, allo = A.batch([r for g in range(len(resp_by_round[0])) for r in (x[g] for x in resp_by_round)])
     assert ((_step_host(la, allb, allo) >> 4) == B.WIRE_OK).all()
@@ -247,10 +245,10 @@ def test_setter_between_begin_and_wait():
     the one begun after the setter runs at 4 waves."""
     rng, logs, c, rows = _leaders(0x5E7, 20_000)
     n = 20_000
-    a = GAR._arena(c, n, False)
+    a = R.leader_arena(c, n, False)
     ref = O.copy_columns(c)
     ba, bb = _leader_batch(rng, c, n), _leader_batch(rng, c, n)
-    wa, wb = WBT._host_batch(*ba, len(ba[0])), WBT._host_batch(*bb, len(bb[0]))
+    wa, wb = PF.host_batch(*ba, len(ba[0])), PF.host_batch(*bb, len(bb[0]))
     a.step_begin_wire(wa, B.STEP_READ_COMMITTED)
     assert a.set_wire_waves(4) == 0
     a.step_begin_wire(wb, B.STEP_READ_COMMITTED)
@@ -295,10 +293,10 @@ def test_wide_pairs():
             cells.append([A.frame(g, s, R.response(3, index=int(rng.integers(0, int(last[g]) + 1)), reject=rng.random() < 0.2,
                                                    hint=int(rng.integers(0, int(last[g])))))
                           for _ in range(int(rng.integers(1, 6)))])
-    blob, off = A.batch(T.interleave(rng, list(enumerate(cells))))
+    blob, off = A.batch(R.interleave(rng, list(enumerate(cells))))
     assert a.set_wire_waves(4) == 0
     want = WW.leader(c, None, blob, off, 4)
-    got = GAR._apply_device(a, blob, off)
+    got = PF.device(a, "wire_apply", blob, off)[0]
     assert np.array_equal(got, want)
     assert ((want >> 4) == B.WIRE_DUP).sum() > 100 and ((want >> 4) == B.WIRE_OK).sum() > 4 * n
     assert_columns_equal(a.read_columns(n), c, n, "wide pairs")
@@ -308,18 +306,18 @@ def test_wide_pairs():
 def test_edges():
     """One cell with 10 000 frames at 4 waves: exactly 4 applied, the rest DUP; n = 0; the setter's refusals."""
     rng, logs, c, rows = _leaders(0xED6E, 64)
-    a = GAR._arena(c, 64, False)
+    a = R.leader_arena(c, 64, False)
     assert a.set_wire_waves(4) == 0
     last = int(c.last_index[3])
     frames = [A.frame(3, 1, R.response(int(c.term[3]), index=min(i, last))) for i in range(10_000)]
     blob, off = A.batch(frames)
     ref = O.copy_columns(c)
     want = WW.leader(ref, None, blob, off, 4)
-    got = GAR._apply_device(a, blob, off)
+    got = PF.device(a, "wire_apply", blob, off)[0]
     assert np.array_equal(got, want)
     assert ((got[:4] >> 4) == B.WIRE_OK).all() and ((got[4:] >> 4) == B.WIRE_DUP).all()
     assert_columns_equal(a.read_columns(64), ref, 64, "one cell")
-    assert len(GAR._apply_device(a, np.zeros(16, np.uint8), np.zeros(1, np.uint32))) == 0
+    assert len(PF.device(a, "wire_apply", np.zeros(16, np.uint8), np.zeros(1, np.uint32))[0]) == 0
     for bad in (0, B.WIRE_WAVES_MAX + 1, 1 << 31):
         assert a.set_wire_waves(bad) == B.ERR_INVALID
     assert B.lib().raftgpu_arena_set_wire_waves(None, 2) == B.ERR_INVALID

@@ -15,7 +15,6 @@ from helpers import B
 import app_follow as A
 import follow_term as T
 import hb_frames as F
-import test_oracle_vote_request as TV
 import vote_request_frames as Q
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "wire", "follower_terms.json")
@@ -50,7 +49,7 @@ def test_frames_decode_as_python_protobuf_wrote_them():
 
 def _one(role, term, stale_reply=False, last_index=10, voters=0b111, pid=1):
     """One group (slot 0 = self, id pid) in `role` at `term` -> (columns, votes, role array, leader array, table)."""
-    c, vt, r, t = TV._one(role, term, pid if role != Q.FOLLOWER else 0, last_index, max(1, term - 1), voters=voters)
+    c, vt, r, t = Q.one(role, term, pid if role != Q.FOLLOWER else 0, last_index, max(1, term - 1), voters=voters)
     t["id"] = pid
     if stale_reply:
         t["flags"] |= FT.STALE_REPLY
@@ -161,7 +160,7 @@ def test_statuses_in_order():
 def _literal_sequence(s, frames_, order):
     """The literal form over frames_ in `order`, each frame it passes then through the follower passes' batch forms
     alone -> (columns, votes, role, leader, table, {frame: verdict}, sorted responses, stale replies)."""
-    c, vt = TV.state_of(s)
+    c, vt = Q.state_of(s)
     role, leader, table = s.role.copy(), s.leader.copy(), s.table.copy()
     verdict, resps, stale = {}, [], []
     for i in order:
@@ -184,7 +183,7 @@ def test_batch_then_follower_passes_equal_the_literal_form(seed):
     frames_ = T.frames(rng, s, per_group=(1, 5))
     frames_ = [frames_[i] for i in rng.permutation(len(frames_))]
     # the pass, the host side of its bumps, the follower passes
-    c, vt = TV.state_of(s)
+    c, vt = Q.state_of(s)
     role, leader, table = s.role.copy(), s.leader.copy(), s.table.copy()
     blob, off = F.batch(frames_)
     st, out, rb, ro, _ = FT.batch(c, None, vt, blob, off, table)
@@ -216,7 +215,7 @@ def test_leaders_and_unselected_groups_are_the_hosts():
     rng = np.random.default_rng(0x7310)
     s = T.scenario(rng, 300, 20, p_role=(0.4, 0.1, 0.1, 0.4), p_select=0.7)
     frames_ = T.frames(rng, s)
-    c, vt = TV.state_of(s)
+    c, vt = Q.state_of(s)
     c0 = O.copy_columns(c)
     blob, off = F.batch(frames_)
     st, _, _, _, _ = FT.batch(c, None, vt, blob, off, s.table)

@@ -18,7 +18,6 @@ import app_follow as A
 import follow_term as T
 import hb_frames as F
 import leader_term as L
-import test_oracle_vote_request as TV
 import vote_request_frames as Q
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "wire")
@@ -66,7 +65,7 @@ def test_golden_frames_of_the_six_types_decode():
 
 def _leader(term, stale_reply=False, last_index=10, voters=0b111, pid=1):
     """One Leader group (slot 0 = self, id pid) at `term` -> (columns, votes, role array, leader array, table)."""
-    c, vt, r, t = TV._one(Q.LEADER, term, pid, last_index, max(1, term - 1), voters=voters)
+    c, vt, r, t = Q.one(Q.LEADER, term, pid, last_index, max(1, term - 1), voters=voters)
     t["id"] = pid
     if stale_reply:
         t["flags"] |= FT.STALE_REPLY
@@ -204,7 +203,7 @@ def test_statuses_in_order():
 
 
 def _state(s):
-    c, vt = TV.state_of(s)
+    c, vt = Q.state_of(s)
     return c, vt, s.role.copy(), s.leader.copy(), s.table.copy()
 
 
@@ -267,7 +266,7 @@ def test_followers_are_the_hosts():
     rng = np.random.default_rng(0x7410)
     s = T.scenario(rng, 300, 20, p_role=(0.4, 0.1, 0.1, 0.4))
     frames_, meta = L.frames(rng, s)
-    c, vt = TV.state_of(s)
+    c, vt = Q.state_of(s)
     c0 = O.copy_columns(c)
     blob, off = F.batch(frames_)
     st, _, _, _, _ = LT.batch(c, None, vt, blob, off, s.table)

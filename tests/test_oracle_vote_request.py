@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 
 from oracle import oracle as O
-from oracle import control_oracle as CO
 from oracle import hb_wire_oracle as H
 from oracle import vote_request_oracle as VR
 from helpers import B
@@ -71,22 +70,6 @@ def test_response_encoder_is_the_vote_response_encoding():
 # --------------------------------------------------------------------------- 2. one group at a time
 
 
-def _one(role, term, vote, last_index, last_term, leader=False, lease=False, check_quorum=False, voters=0b1,
-         committed=None, commit_term=0, priority=0):
-    """One group (slot 0 = self, id 1) in `role` at `term` with the given log -> (columns, votes, role, table)."""
-    c = O.new_columns(8, 1)
-    c.meta[0] = B.make_meta(voters, 0, 0, 0)
-    c.term[0], c.last_index[0] = term, last_index
-    c.committed[0] = last_index if committed is None else committed
-    c.term_start[0] = last_index if role == Q.LEADER else B.NO_TERM_START
-    t = np.zeros(1, VR.VOTER_DTYPE)
-    t["id"], t["vote"], t["last_term"], t["commit_term"], t["persisted"], t["priority"] = \
-        1, vote, last_term, commit_term, last_index, priority
-    t["flags"] = (VR.SELECT if role != Q.LEADER else 0) | (VR.LEADER if leader else 0) | (VR.LEASE if lease else 0) | \
-        (VR.CHECK_QUORUM if check_quorum else 0)
-    return c, np.zeros((O.SLOTS, c.cap), np.uint8), np.array([role], np.uint8), t
-
-
 def _responses(blob, off):
     return [H.decode_message(blob[off[k] + 4:off[k + 1]].tobytes()) for k in range(len(off) - 1)]
 
@@ -105,74 +88,34 @@ def _batch(state, frames):
     return st, _responses(rb, ro)
 
 
-# test_raft.rs:1537-1605: (role, index, log_term, vote, want reject) against a log of two entries at term 2
-RECV_VOTE = [
-    (Q.FOLLOWER, 0, 0, 0, True), (Q.FOLLOWER, 0, 1, 0, True), (Q.FOLLOWER, 0, 2, 0, True), (Q.FOLLOWER, 0, 3, 0, False),
-    (Q.FOLLOWER, 1, 0, 0, True), (Q.FOLLOWER, 1, 1, 0, True), (Q.FOLLOWER, 1, 2, 0, True), (Q.FOLLOWER, 1, 3, 0, False),
-    (Q.FOLLOWER, 2, 0, 0, True), (Q.FOLLOWER, 2, 1, 0, True), (Q.FOLLOWER, 2, 2, 0, False), (Q.FOLLOWER, 2, 3, 0, False),
-    (Q.FOLLOWER, 3, 0, 0, True), (Q.FOLLOWER, 3, 1, 0, True), (Q.FOLLOWER, 3, 2, 0, False), (Q.FOLLOWER, 3, 3, 0, False),
-    (Q.FOLLOWER, 3, 2, 2, False), (Q.FOLLOWER, 3, 2, 1, True), (Q.LEADER, 3, 3, 1, True), (Q.PRE_CANDIDATE, 3, 3, 1, True),
-    (Q.CANDIDATE, 3, 3, 1, True),
-]
-
-
-def recv_vote_case(row):
-    role, index, log_term, vote, _ = row
-    term = max(2, log_term)
-    return _one(role, term, vote, 2, 2), [F.frame(0, 0, Q.request(Q.VOTE, term, log_term, index, frm=2))]
-
-
-@pytest.mark.parametrize("row", range(len(RECV_VOTE)))
+@pytest.mark.parametrize("row", range(len(Q.RECV_VOTE)))
 def test_recv_msg_request_vote(row):
-    state, frames = recv_vote_case(RECV_VOTE[row])
-    want = RECV_VOTE[row][4]
+    state, frames = Q.recv_vote_case(Q.RECV_VOTE[row])
+    want = Q.RECV_VOTE[row][4]
     r = _literal(state, frames)
     assert len(r) == 1 and r[0]["msg_type"] == 6 and bool(r[0]["reject"]) == want
-    state, _ = recv_vote_case(RECV_VOTE[row])
+    state, _ = Q.recv_vote_case(Q.RECV_VOTE[row])
     st, rb = _batch(state, frames)
-    if RECV_VOTE[row][0] == Q.LEADER:   # a leader is the host's
+    if Q.RECV_VOTE[row][0] == Q.LEADER:   # a leader is the host's
         assert st.tolist() == [VR.WIRE_ROLE << 4] and rb == []
     else:
         assert st.tolist() == [(0 if want else VR.GRANTED | VR.VOTED)] and bool(rb[0]["reject"]) == want
 
 
-# test_raft_paper.rs:962-1006: (log as (term, index) entries, m.log_term, m.index, want reject) at m.term 3
-VOTER = [([(1, 1)], 1, 1, False), ([(1, 1)], 1, 2, False), ([(1, 1), (1, 2)], 1, 1, True),
-         ([(1, 1)], 2, 1, False), ([(1, 1)], 2, 2, False), ([(1, 1), (1, 2)], 2, 1, False),
-         ([(2, 1)], 1, 1, True), ([(2, 1)], 1, 2, True), ([(2, 1), (1, 2)], 1, 1, True)]
-
-
-def voter_case(row):
-    ents, log_term, index, _ = row
-    # a new Raft at term 0 over that log (term 0 is the host's: the pass needs a known term, so the group sits at 1)
-    state = _one(Q.FOLLOWER, 1, 0, len(ents), ents[-1][0], voters=0b11)
-    return state, [F.frame(0, 0, Q.request(Q.VOTE, 3, log_term, index, frm=2))]
-
-
-@pytest.mark.parametrize("row", range(len(VOTER)))
+@pytest.mark.parametrize("row", range(len(Q.VOTER)))
 def test_voter(row):
-    want = VOTER[row][3]
+    want = Q.VOTER[row][3]
     for form in ("literal", "batch"):
-        state, frames = voter_case(VOTER[row])
+        state, frames = Q.voter_case(Q.VOTER[row])
         r = _literal(state, frames) if form == "literal" else _batch(state, frames)[1]
         assert len(r) == 1 and r[0]["msg_type"] == 6 and bool(r[0]["reject"]) == want and r[0]["term"] == 3, form
         assert state[0].term[0] == 3   # the higher term was taken either way
 
 
-def any_state_case(role, typ):
-    """test_raft.rs:655-760: three voters, term 1 (a Follower whose leader is 3, a PreCandidate), 2 (a Candidate or a
-    Leader, who voted for themselves; the leader appended its empty entry); a request from 2 at term + 1."""
-    term = 2 if role in (Q.CANDIDATE, Q.LEADER) else 1
-    vote = 1 if role in (Q.CANDIDATE, Q.LEADER) else 0
-    last = 1 if role == Q.LEADER else 0
-    state = _one(role, term, vote, last, term if last else 0, leader=role in (Q.FOLLOWER, Q.LEADER), voters=0b111)
-    return state, [F.frame(0, 0, Q.request(typ, term + 1, term + 1, 42, frm=2))]
-
-
 @pytest.mark.parametrize("typ", [Q.VOTE, Q.PRE_VOTE], ids=["vote", "prevote"])
 @pytest.mark.parametrize("role", [Q.FOLLOWER, Q.CANDIDATE, Q.PRE_CANDIDATE, Q.LEADER])
 def test_vote_from_any_state(role, typ):
-    state, frames = any_state_case(role, typ)
+    state, frames = Q.any_state_case(role, typ)
     c, _, r_role, t = state
     orig = int(c.term[0])
     r = _literal(state, frames)
@@ -182,7 +125,7 @@ def test_vote_from_any_state(role, typ):
         assert c.term_start[0] == B.NO_TERM_START
     else:
         assert (r_role[0], c.term[0]) == (role, orig) and t["vote"][0] in (0, 1)
-    state, frames = any_state_case(role, typ)
+    state, frames = Q.any_state_case(role, typ)
     st, rb = _batch(state, frames)
     if role == Q.LEADER:
         assert st.tolist() == [VR.WIRE_ROLE << 4]
@@ -198,7 +141,7 @@ def test_lease_and_priority_cases():
     for typ in (Q.VOTE, Q.PRE_VOTE):
         for ctx, dropped in ((b"", True), (Q.ELECTION, True), (Q.TRANSFER, False)):
             for form in ("literal", "batch"):
-                state = _one(Q.FOLLOWER, 1, 0, 1, 1, leader=True, lease=True, check_quorum=True, voters=0b111)
+                state = Q.one(Q.FOLLOWER, 1, 0, 1, 1, leader=True, lease=True, check_quorum=True, voters=0b111)
                 frames = [F.frame(0, 0, Q.request(typ, 2, 1, 1, context=ctx, frm=3))]
                 if form == "literal":
                     r = _literal(state, frames)
@@ -210,7 +153,7 @@ def test_lease_and_priority_cases():
                     assert not r[0]["reject"]
     for index, prio, want in ((1, 2, True), (1, 3, False), (1, 9, False), (2, 0, False)):
         for form in ("literal", "batch"):
-            state = _one(Q.FOLLOWER, 1, 0, 1, 1, priority=3, voters=0b111)
+            state = Q.one(Q.FOLLOWER, 1, 0, 1, 1, priority=3, voters=0b111)
             frames = [F.frame(0, 0, Q.request(Q.VOTE, 2, 1, index, priority=prio, frm=2))]
             r = _literal(state, frames) if form == "literal" else _batch(state, frames)[1]
             assert bool(r[0]["reject"]) == want, (index, prio, form)
@@ -254,29 +197,6 @@ def test_statuses_in_order():
 # --------------------------------------------------------------------------- 3. the resubmission loop is exact
 
 
-def state_of(s):
-    c = O.new_columns(s.n + 8, s.n)
-    c.term_start[:] = B.NO_TERM_START
-    c.meta[s.n_narrow:s.n:2], c.meta[s.n_narrow + 1:s.n:2] = Q.META_WIDE_LO, Q.META_WIDE_HI   # the allocated pairs
-    vt = np.zeros((O.SLOTS, c.cap), np.uint8)
-    assert np.all(CO.arena_control(c, vt, s.setup)["status"] == 0)
-    return c, vt
-
-
-def caller_update(table, role, status, out, frames):
-    """What the caller does with an applied frame's flags (INTEGRATION.md section 6)."""
-    for i in np.flatnonzero(status >> 4 == B.WIRE_OK):
-        g = int(np.frombuffer(frames[i][:4], "<u4")[0]) >> 4
-        if status[i] & B.VREQ_BUMPED:   # become_follower(m.term, INVALID_ID)'s host side
-            table["vote"][g] = 0
-            table["flags"][g] &= ~np.uint32(VR.LEADER | VR.LEASE)
-            role[g] = Q.FOLLOWER
-        if status[i] & B.VREQ_VOTED:    # vote = m.from, election_elapsed = 0
-            table["vote"][g] = out[i][0]
-            if table["flags"][g] & VR.LEADER and table["flags"][g] & VR.CHECK_QUORUM:
-                table["flags"][g] |= VR.LEASE
-
-
 @pytest.mark.parametrize("seed", range(8))
 def test_resubmission_loop_equals_the_literal_form(seed):
     rng = np.random.default_rng(0x7100 + seed)
@@ -287,7 +207,7 @@ def test_resubmission_loop_equals_the_literal_form(seed):
     frames = s.frames(rng, per_group=(1, 4), noise=False, only_decided=True)
     frames = [frames[i] for i in rng.permutation(len(frames))]
     # the literal form, every frame in order
-    c1, v1 = state_of(s)
+    c1, v1 = Q.state_of(s)
     t1, r1 = s.table.copy(), s.role.copy()
     blob, off = F.batch(frames)
     rb, ro, _ = VR.literal(c1, None, v1, r1, t1, blob, off)
@@ -296,7 +216,7 @@ def test_resubmission_loop_equals_the_literal_form(seed):
         fr = rb[ro[k]:ro[k + 1]].tobytes()
         lit.setdefault(int(np.frombuffer(fr[:4], "<u4")[0]) >> 4, []).append(fr)
     # the batch form, DUP frames resubmitted in order until none is left
-    c2, v2 = state_of(s)
+    c2, v2 = Q.state_of(s)
     t2, r2 = s.table.copy(), s.role.copy()
     pending, rounds, got = frames, 0, {}
     while pending:
@@ -306,7 +226,7 @@ def test_resubmission_loop_equals_the_literal_form(seed):
         for k in range(len(ro) - 1):
             fr = rb[ro[k]:ro[k + 1]].tobytes()
             got.setdefault(int(np.frombuffer(fr[:4], "<u4")[0]) >> 4, []).append(fr)
-        caller_update(t2, r2, st, out, pending)
+        Q.caller_update(t2, r2, st, out, pending)
         pending = [pending[i] for i in np.flatnonzero(st >> 4 == B.WIRE_DUP)]
         rounds += 1
     assert rounds > 1 and got == lit

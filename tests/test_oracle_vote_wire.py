@@ -57,18 +57,6 @@ def test_synth_encoder_matches_python_protobuf():
 # --------------------------------------------------------------------------- 2. one group at a time
 
 
-def _arena(metas, terms, committed=None):
-    """Oracle columns for the given group metas (one candidate each), last_index 10, committed 5 unless given."""
-    n = len(metas)
-    c = O.new_columns(n + 8, n)
-    c.term_start[:] = B.NO_TERM_START
-    c.meta[:n] = metas
-    c.term[:n] = terms
-    c.last_index[:n] = 10
-    c.committed[:n] = 5 if committed is None else committed
-    return c, np.zeros((O.SLOTS, c.cap), np.uint8)
-
-
 def same_decisions(outs, first):
     """The pass's outcomes against the literal form's first decided words: the same groups and VoteResults (the counts
     differ where votes came in after the decision: the pass tallies once, after the batch)."""
@@ -76,26 +64,10 @@ def same_decisions(outs, first):
     return np.array_equal(outs["group"], want["group"]) and np.array_equal(outs["result"] & 0xFF, want["result"] & 0xFF)
 
 
-def _run(c, votes, frames, select, pre=None):
-    blob, off = F.batch(frames)
-    return VW.batch(c, votes, blob, off, V.bitmap(select), None if pre is None else V.bitmap(pre))
-
-
-# test_raft_paper.rs:199-250: (size, {id: vote}, the state after) for a candidate at term 1 whose self vote is in
-ONE_ROUND = [
-    (1, {}, "Leader"), (3, {2: True, 3: True}, "Leader"), (3, {2: True}, "Leader"),
-    (5, {2: True, 3: True, 4: True, 5: True}, "Leader"), (5, {2: True, 3: True, 4: True}, "Leader"),
-    (5, {2: True, 3: True}, "Leader"),
-    (3, {2: False, 3: False}, "Follower"), (5, {2: False, 3: False, 4: False, 5: False}, "Follower"),
-    (5, {2: True, 3: False, 4: False, 5: False}, "Follower"),
-    (3, {}, "Candidate"), (5, {2: True}, "Candidate"), (5, {2: False, 3: False}, "Candidate"), (5, {}, "Candidate"),
-]
-
-
 def one_round_case(size, votes):
     """The case on a fresh arena: the campaign list of INTEGRATION.md section 6 (term 0 -> 1, self vote in slot 0),
     then the responses as frames (peer id k in slot k - 1) -> (campaign's VOTE_RESULT word, frames, columns, votes)."""
-    c, vt = _arena([B.make_meta((1 << size) - 1, 0, 0, 0)], [0])
+    c, vt = V.candidates([B.make_meta((1 << size) - 1, 0, 0, 0)], [0])
     camp = cmds((B.CTL_RESET, 0, 0, 0, (B.NO_TERM_START, 10, 5, 10)), (B.CTL_SET_TERM, 0, 0, 0, (1,)),
                 (B.CTL_RESET_VOTES, 0), (B.CTL_RECORD_VOTE, 0, 0, 1), (B.CTL_VOTE_RESULT, 0))
     first = int(CO.arena_control(c, vt, camp)["value"][-1])
@@ -103,20 +75,15 @@ def one_round_case(size, votes):
     return first, frames, c, vt
 
 
-def expected_state(first, outcomes):
-    w = first if first & 0xFF != B.VOTE_PENDING else (int(outcomes["result"][0]) if len(outcomes) else B.VOTE_PENDING)
-    return {B.VOTE_WON: "Leader", B.VOTE_LOST: "Follower", B.VOTE_PENDING: "Candidate"}[w & 0xFF]
-
-
-@pytest.mark.parametrize("case", range(len(ONE_ROUND)))
+@pytest.mark.parametrize("case", range(len(V.ONE_ROUND)))
 def test_leader_election_in_one_round_rpc(case):
-    size, votes, state = ONE_ROUND[case]
+    size, votes, state = V.ONE_ROUND[case]
     first, frames, c, vt = one_round_case(size, votes)
-    st, outs, tallied = _run(c, vt, frames, [True])
+    st, outs, tallied = V.run_batch(c, vt, frames, [True])
     assert np.all(st == (B.WIRE_OK << 4 | B.RES_OK))
     assert tallied == (1 if frames else 0)
     # a single voter wins on its own vote: the campaign list decides it, and there is no frame to pass
-    assert expected_state(first, outs) == state
+    assert V.expected_state(first, outs) == state
     assert len(outs) == (state != "Candidate" and bool(frames))
     assert int(c.term[0]) == 1
     # the literal form agrees
@@ -133,7 +100,7 @@ def test_statuses_in_order():
     """Each check of raftgpu.h on a candidate (group 0, term 7), a PreCandidate (group 1, term 7), a leader (2) and an
     unselected group (3); committed 5."""
     meta = B.make_meta(0x1F, 0, 0, 0)
-    c, vt = _arena([meta] * 4, [7, 7, 7, 7])
+    c, vt = V.candidates([meta] * 4, [7, 7, 7, 7])
     c.term_start[2] = 11
     sel, pre = [True, True, True, False], [False, True, False, False]
     rows = [
@@ -158,17 +125,17 @@ def test_statuses_in_order():
         (F.frame(1, 2, V.message(18, 7, True)), B.WIRE_OK),                       # pre-vote rejection at the term
         (F.frame(1, 9, V.message(18, 7)), B.WIRE_OK),                             # slot 9: no such peer
     ]
-    st, outs, tallied = _run(c, vt, [f for f, _ in rows], sel, pre)
+    st, outs, tallied = V.run_batch(c, vt, [f for f, _ in rows], sel, pre)
     assert (st >> 4).tolist() == [s for _, s in rows]
     assert st[-1] & 0xF == B.RES_NO_PROGRESS and st[-2] & 0xF == B.RES_OK and st[-6] & 0xF == B.RES_OK
     assert vt[:, 0].tolist()[:4] == [0, 0, 2, 2] and vt[:, 1].tolist()[:3] == [0, 2, 1]
     # group 0: slots 2 and 3 granted of 5 voters, pending; group 1: slot 1 granted, slot 2 rejected, pending
     assert tallied == 2 and outs.tolist() == []
     # the same frames, the rejected cell already voted before the batch: or_insert keeps the old vote, result 0
-    c, vt = _arena([meta] * 4, [7, 7, 7, 7])
+    c, vt = V.candidates([meta] * 4, [7, 7, 7, 7])
     c.term_start[2] = 11
     vt[2, 0] = 1
-    st, _, _ = _run(c, vt, [f for f, _ in rows], sel, pre)
+    st, _, _ = V.run_batch(c, vt, [f for f, _ in rows], sel, pre)
     assert st[14] == (B.WIRE_OK << 4) and vt[2, 0] == 1
 
 
@@ -176,10 +143,10 @@ def test_group_without_voters_is_role():
     """A selected group slot without voters -- freed (meta 0, its term left behind) or not configured yet -- is the
     host's: the pass neither records nor tallies it, so only allocated groups reach the outcome list."""
     meta = B.make_meta(0b11, 0, 0, 0)
-    c, vt = _arena([meta, 0, 0], [4, 4, 4])
+    c, vt = V.candidates([meta, 0, 0], [4, 4, 4])
     vt[0, 0] = 2                                               # group 0's self vote
     frames = [F.frame(g, 1, V.message(6, 4)) for g in (1, 0, 2)]
-    st, outs, tallied = _run(c, vt, frames, [True, True, True])
+    st, outs, tallied = V.run_batch(c, vt, frames, [True, True, True])
     assert (st >> 4).tolist() == [B.WIRE_ROLE, B.WIRE_OK, B.WIRE_ROLE]
     assert outs.tolist() == [(0, B.VOTE_WON | 2 << 8)] and tallied == 1
     assert np.count_nonzero(vt[:, 1:3]) == 0
@@ -190,27 +157,17 @@ def test_pre_vote_terms_and_commit_by_vote():
     at a higher term is the host's.  test_advance_commit_index_by_vote_response's shape (test_raft.rs:4646-4800): a
     response whose commit is beyond committed with a commit_term is COMMIT_VOTE and records nothing."""
     meta = B.make_meta(0b111, 0, 0, 0)
-    c, vt = _arena([meta, meta], [5, 5], committed=[3, 3])
+    c, vt = V.candidates([meta, meta], [5, 5], committed=[3, 3])
     vt[0, 0] = vt[0, 1] = 2                                    # both self votes
     frames = [F.frame(0, 1, V.message(18, 6)), F.frame(1, 1, V.message(18, 6, True)),
               F.frame(1, 2, V.message(18, 5, commit=4, commit_term=5)), F.frame(1, 2, V.message(18, 5, True, commit=3, commit_term=5))]
-    st, outs, _ = _run(c, vt, frames, [True, True], [True, True])
+    st, outs, _ = V.run_batch(c, vt, frames, [True, True], [True, True])
     assert (st >> 4).tolist() == [B.WIRE_OK, B.WIRE_TERM, B.WIRE_COMMIT_VOTE, B.WIRE_OK]
     assert outs.tolist() == [(0, B.VOTE_WON | 2 << 8)] and c.term[:2].tolist() == [5, 5]
     assert vt[2, 1] == 1
 
 
 # --------------------------------------------------------------------------- 3. batch form against the literal form
-
-
-def _state(e):
-    c = O.new_columns(e.n + 8, e.n)
-    c.term_start[:] = B.NO_TERM_START
-    c.meta[e.n_narrow:e.n:2], c.meta[e.n_narrow + 1:e.n:2] = V.META_WIDE_LO, V.META_WIDE_HI   # the allocated pairs
-    vt = np.zeros((O.SLOTS, c.cap), np.uint8)
-    assert np.all(CO.arena_control(c, vt, e.setup)["status"] == 0)
-    CO.arena_control(c, vt, e.campaign)
-    return c, vt
 
 
 @pytest.mark.parametrize("seed", range(6))
@@ -221,9 +178,9 @@ def test_batch_equals_literal_first_results_in_any_order(seed):
     for perm in range(8):
         order = rng.permutation(len(frames))
         blob, off = F.batch([frames[i] for i in order])
-        c, vt = _state(e)
+        c, vt = V.state_of(e)
         st, outs, tallied = VW.batch(c, vt, blob, off, e.select(), e.pre())
-        c2, vt2 = _state(e)
+        c2, vt2 = V.state_of(e)
         role = e.role.copy()
         first = VW.literal(c2, vt2, role, blob, off)
         assert same_decisions(outs, first), (seed, perm)
@@ -241,11 +198,11 @@ def test_caller_recipe_equals_literal_transitions(seed):
     e = V.Election(rng, 250, 30)
     frames = e.frames(rng)
     blob, off = F.batch([frames[i] for i in rng.permutation(len(frames))])
-    c, vt = _state(e)
+    c, vt = V.state_of(e)
     _, outs, _ = VW.batch(c, vt, blob, off, e.select(), e.pre())
     res = CO.arena_control(c, vt, e.transitions(outs, e.role))
     assert np.all(res["status"] == 0)
-    c2, vt2 = _state(e)
+    c2, vt2 = V.state_of(e)
     role = e.role.copy()
     VW.literal(c2, vt2, role, blob, off)
     for name in O.PEER_COLUMNS + ("pflags", "meta") + O.GROUP_COLUMNS:

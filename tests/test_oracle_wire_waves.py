@@ -18,36 +18,6 @@ DUP, NEEDS_LOG, COMMIT_RANGE = O.WIRE_DUP, O.WIRE_NEEDS_LOG, AL.WIRE_COMMIT_RANG
 
 # --------------------------------------------------------------------------- batch builders
 
-def leader_frames(rng, c, groups, peers, per_cell, needs_log=0.0, stale=0.2):
-    """1..per_cell MsgAppendResponse frames per (group, peer) cell, the cells interleaved in a random arrival order (a
-    cell's frames keep theirs): accepts at increasing indexes (a fraction `stale` at an index already matched),
-    rejections with log_term 0 at the probe's index, and a fraction needs_log of rejections with log_term > 0."""
-    cells = []
-    for g in groups:
-        last = int(c.last_index[g])
-        for s in peers:
-            k = int(rng.integers(1, per_cell + 1))
-            idx = sorted(rng.integers(0, last + 1, k).tolist())
-            fr = []
-            for j in range(k):
-                if rng.random() < 0.25:
-                    lt = int(rng.integers(1, 40)) if rng.random() < needs_log else 0
-                    body = R.response(int(c.term[g]), index=int(rng.integers(0, last + 1)), reject=True,
-                                      hint=int(rng.integers(0, last + 2)), log_term=lt)
-                else:
-                    i = idx[j] if rng.random() >= stale else int(rng.integers(0, idx[j] + 1))
-                    body = R.response(int(c.term[g]), index=i, commit=int(rng.integers(0, last + 1)))
-                fr.append(A.frame(g, s, body))
-            cells.append(fr)
-    order = rng.permutation(sum(len(f) for f in cells))
-    owner = np.repeat(np.arange(len(cells)), [len(f) for f in cells])[order]
-    pos = [0] * len(cells)
-    out = []
-    for cell in owner.tolist():       # each cell's frames in their order, cells interleaved
-        out.append(cells[cell][pos[cell]])
-        pos[cell] += 1
-    return out
-
 
 def literal_leader(c, blob, off):
     """The literal per-message application: every frame decoded, its record (and a REJECT's EXT) through
@@ -79,38 +49,6 @@ def _decode_all(c, blob, off):
     return st, recs, hint, snap
 
 
-def pipelined_appends(rng, last, run_term, term, committed, k, entries=True):
-    """k pipelined MsgAppend bodies to a follower whose log ends at `last` with term run_term: frame j's entries (1-3
-    at `term`) start at frame j-1's last index + 1; without entries, k heartbeat-like appends at `last` with rising
-    commits.  -> [(body, last index after it)]."""
-    out, idx, lt = [], last, run_term
-    for _ in range(k):
-        if entries:
-            cnt = int(rng.integers(1, 4))
-            ents = [(term, idx + j + 1) for j in range(cnt)]
-        else:
-            cnt, ents = 0, None
-        top = idx + cnt
-        commit = int(rng.integers(min(committed, top), top + 1))
-        out.append((A.message(3, term=term, log_term=lt, index=idx, commit=commit, frm=int(rng.integers(1, 1 << 40)),
-                              entries=ents), top))
-        if entries:
-            idx, lt = top, term
-    return out
-
-
-def interleave(rng, per_group):
-    """[(group, [frames])] -> one batch order: every group's frames in their order, the groups interleaved."""
-    owner = np.repeat(np.arange(len(per_group)), [len(f) for _, f in per_group])
-    owner = owner[rng.permutation(len(owner))]
-    pos = [0] * len(per_group)
-    out = []
-    for k in owner.tolist():
-        out.append(per_group[k][1][pos[k]])
-        pos[k] += 1
-    return out
-
-
 # --------------------------------------------------------------------------- the leader
 
 def _leaders(rng, n):
@@ -124,7 +62,7 @@ def test_leader_waves_equal_the_literal_application():
     rng = np.random.default_rng(0x3A7E)
     n = 400
     logs, c = _leaders(rng, n)
-    blob, off = A.batch(leader_frames(rng, c, range(n), range(1, 5), 6))
+    blob, off = A.batch(R.leader_frames(rng, c, range(n), range(1, 5), 6))
     lit = O.copy_columns(c)
     want = literal_leader(lit, blob, off)
     for waves in (6, 9, 64):
@@ -142,7 +80,7 @@ def test_leader_fewer_waves_leave_the_rest_dup():
     rng = np.random.default_rng(0x3A7F)
     n = 200
     _, c = _leaders(rng, n)
-    frames = leader_frames(rng, c, range(n), range(1, 4), 6)
+    frames = R.leader_frames(rng, c, range(n), range(1, 4), 6)
     blob, off = A.batch(frames)
     cell = np.array([int.from_bytes(f[:4], "little") for f in frames])
     rank = np.zeros(len(frames), int)
@@ -170,7 +108,7 @@ def test_leader_one_wave_is_the_batch_form():
     n = 300
     logs, c = _leaders(rng, n)
     rows = R.rows_for(logs, np.ones(n), 2)
-    frames = leader_frames(rng, c, range(n), range(1, 5), 4, needs_log=0.5)
+    frames = R.leader_frames(rng, c, range(n), range(1, 5), 4, needs_log=0.5)
     frames += [A.frame(3, 1, R.response(int(c.term[3]) + 1, index=1)), b"\x01\x02", A.frame(n + 7, 1, R.response(1))]
     blob, off = A.batch(frames)
     for r in (None, rows):
@@ -206,10 +144,10 @@ def test_follower_waves_equal_the_literal_form():
     per_group = []
     for g in range(n):
         last = int(w.groups["last_index"][g])
-        bodies = pipelined_appends(rng, last, int(w.terms[g, last]), int(w.groups["term"][g]),
+        bodies = R.pipelined_appends(rng, last, int(w.terms[g, last]), int(w.groups["term"][g]),
                                    int(w.groups["committed"][g]), int(rng.integers(1, 7)))
         per_group.append((g, [A.frame(g, 0, b) for b, _ in bodies]))
-    blob, off = A.batch(interleave(rng, per_group))
+    blob, off = A.batch(R.interleave(rng, per_group))
     lit, outcome, lrb, lro, ltot = _literal_follower(w, blob, off)
     assert (outcome == AL.ANSWERED).all()
     for waves in (6, 64):
@@ -233,10 +171,10 @@ def test_follower_entry_less_waves_equal_the_literal_form():
     per_group = []
     for g in range(n):
         last = int(w.groups["last_index"][g])
-        bodies = pipelined_appends(rng, last, int(w.terms[g, last]), int(w.groups["term"][g]),
+        bodies = R.pipelined_appends(rng, last, int(w.terms[g, last]), int(w.groups["term"][g]),
                                    int(w.groups["committed"][g]), int(rng.integers(1, 7)), entries=False)
         per_group.append((g, [A.frame(g, 0, b) for b, _ in bodies]))
-    blob, off = A.batch(interleave(rng, per_group))
+    blob, off = A.batch(R.interleave(rng, per_group))
     lit, outcome, lrb, lro, ltot = _literal_follower(w, blob, off)
     c, table = w.columns(), w.table(w.runs())
     st, frm, app, rb, ro, tot = WW.follower(c, None, table, blob, off, 6, entries=False)
@@ -277,7 +215,7 @@ def test_follower_stop_rule():
     for g, kind in enumerate(kinds):
         last = int(w.groups["last_index"][g])
         term = int(w.groups["term"][g])
-        b = pipelined_appends(rng, last, int(w.terms[g, last]), term, int(w.groups["committed"][g]), 3)
+        b = R.pipelined_appends(rng, last, int(w.terms[g, last]), term, int(w.groups["committed"][g]), 3)
         top = b[0][1]
         if kind == "needs_log":
             second = A.message(3, term=term, log_term=0, index=top + 5, commit=top, frm=9, entries=[(term, top + 6)])

@@ -4,8 +4,7 @@ test_gpu_tile_shapes.py reaching every stage count of that plan."""
 import numpy as np
 import pytest
 
-from helpers import B, TILE_SHAPES, random_state
-from test_tile_shapes import GROUPS, MAX_STAGES, ROW64, ROW8, SMEM, TILE, UNIT_CAP, plan
+from helpers import B, TILE_SHAPES, random_state, GROUPS, MAX_STAGES, ROW64, ROW8, SMEM, TILE, UNIT_CAP, plan
 
 ROW16 = (TILE + 8) * 2
 REC_CAP = 4 * TILE

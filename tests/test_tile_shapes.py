@@ -4,33 +4,12 @@ every apply path (through the oracle only, so the GPU tests cannot go vacuous un
 import numpy as np
 import pytest
 
-from helpers import B, O, TILE_SHAPES, is_simple5, random_batch, random_state
+from helpers import (B, GROUPS, KERNELS, O, TILE_SHAPES, UNIT_CAP, is_simple5, plan, random_batch, random_state,
+                     stage_bytes, stages)
 
-# k_tile.cuh: tile geometry and shared memory of the fused tile kernels
-TILE, GROUPS, MAX_STAGES = 256, 3, 8
-ROW64, ROW8 = (TILE + 2) * 8, TILE + 16
-SMEM = 227 * 1024 - 5 * 1024
-UNIT_CAP = 1536
-KERNELS = {"packed": (0, 0), "compact": (4 * UNIT_CAP, GROUPS * TILE * 4)}   # (payload bytes, extra bytes)
 
 # stage counts per number of hinted slots H = 1..8
 WANT_STAGES = {"packed": (8, 8, 8, 6, 5, 4, 4, 3), "compact": (8, 8, 6, 5, 4, 4, 3, 3)}
-
-
-def stage_bytes(h, payload):
-    return 3 * h * ROW64 + 3 * ROW64 + TILE * 4 + h * ROW8 + payload
-
-
-def stages(h, kernel):
-    payload, extra = KERNELS[kernel]
-    return min(MAX_STAGES, (SMEM - extra) // stage_bytes(h, payload))
-
-
-def plan(meta, force_general, kernel):
-    """tile_plan (arena.cu): (simple5 instantiation, hint, stages) of an arena whose groups hold `meta`."""
-    simple5 = not force_general and bool(is_simple5(meta).all())
-    hint = 0x1f if simple5 else int(np.bitwise_or.reduce((meta & 0xff) | ((meta >> 8) & 0xff)))
-    return simple5, hint, stages(bin(hint).count("1"), kernel)
 
 
 needs_256 = pytest.mark.skipif(B.tile_groups() != 256, reason="the stage table is for 256-group tiles")

@@ -15,7 +15,6 @@ import hb_frames as F
 import vote_frames as V
 import vote_request_frames as Q
 import wire_batches as WB
-import test_gpu_wire_batches as G
 
 NO_TERM_START = (1 << 64) - 1
 
@@ -121,27 +120,27 @@ def test_gpu_batches_reach_every_stage_geometry(name):
     """The batches of test_gpu_wire_batches.py -- the stage batch and the hostile batches of both forms -- reach every
     geometry of WB.WANT_GEOMETRY in this pass (staging cannot be seen in any output: this is what shows the unstaged path
     ran)."""
-    i = G.PASSES.index(name)
-    sc = G.scenario(name)
-    frames, ballast = G.stage_batch(sc, 0x5B00 + i)
+    i = WB.PASSES.index(name)
+    sc = WB.scenario(name)
+    frames, ballast = WB.stage_batch(sc, 0x5B00 + i)
     blob, off = F.batch(frames)
     got = WB.geometry(off, len(blob))
-    hostile = G.scenario(name, 2_000)
+    hostile = WB.scenario(name, 2_000)
     for device in (False, True):
-        for buf, n_bytes, off in G.hostile_batches(hostile, 0x5B10 + i, device):
+        for buf, n_bytes, off in WB.hostile_batches(hostile, 0x5B10 + i, device):
             assert n_bytes % 16 in range(16) and (len(buf) - n_bytes >= 4096 if device else len(buf) == n_bytes)
             assert int(off.max()) <= (len(buf) if device else n_bytes + 4 * len(off))
             got |= WB.geometry(off, n_bytes)
     assert got >= WB.WANT_GEOMETRY, WB.WANT_GEOMETRY - got
-    residues = {n_bytes % 16 for _, n_bytes, _ in G.hostile_batches(hostile, 0x5B10 + i, True)}
-    sizes = {len(off) - 1 for _, _, off in G.hostile_batches(hostile, 0x5B10 + i, True)}
+    residues = {n_bytes % 16 for _, n_bytes, _ in WB.hostile_batches(hostile, 0x5B10 + i, True)}
+    sizes = {len(off) - 1 for _, _, off in WB.hostile_batches(hostile, 0x5B10 + i, True)}
     assert residues == set(range(16)) and sizes == {1, 255, 256, 257}
 
 
 # --------------------------------------------------------------------------- 3. the golden vectors, retargeted
 
 
-@pytest.mark.parametrize("msg_type", sorted(set(G.GOLDEN_TYPE.values())))
+@pytest.mark.parametrize("msg_type", sorted(set(WB.GOLDEN_TYPE.values())))
 def test_retargeted_golden_vectors_keep_their_fields(msg_type):
     """Appending 0x08 <type> to an accepted messages.json vector changes its msg_type and nothing else (field 1 is a
     scalar: the last value wins), so python-protobuf's recorded fields stay the expected ones; a rejected vector stays

@@ -3,6 +3,9 @@
 of INTEGRATION.md section 6, and batches of frames -- that run the same on the device arena and on the oracle."""
 import numpy as np
 
+from oracle import oracle as O
+from oracle import control_oracle as CO
+from oracle import vote_wire_oracle as VW
 from helpers import B
 from control_cmds import cmds, META_WIDE_LO, META_WIDE_HI  # noqa: F401
 import hb_frames as F
@@ -150,3 +153,46 @@ class Election:
             else:
                 rows.append((B.CTL_RESET, g, 0, 0, (NO_TERM_START, li, com, li)))
         return cmds(*rows)
+
+
+def candidates(metas, terms, committed=None):
+    """Oracle columns for the given group metas (one candidate each), last_index 10, committed 5 unless given."""
+    n = len(metas)
+    c = O.new_columns(n + 8, n)
+    c.term_start[:] = B.NO_TERM_START
+    c.meta[:n] = metas
+    c.term[:n] = terms
+    c.last_index[:n] = 10
+    c.committed[:n] = 5 if committed is None else committed
+    return c, np.zeros((O.SLOTS, c.cap), np.uint8)
+
+
+def run_batch(c, votes, frames, select, pre=None):
+    blob, off = F.batch(frames)
+    return VW.batch(c, votes, blob, off, bitmap(select), None if pre is None else bitmap(pre))
+
+
+# test_raft_paper.rs:199-250: (size, {id: vote}, the state after) for a candidate at term 1 whose self vote is in
+ONE_ROUND = [
+    (1, {}, "Leader"), (3, {2: True, 3: True}, "Leader"), (3, {2: True}, "Leader"),
+    (5, {2: True, 3: True, 4: True, 5: True}, "Leader"), (5, {2: True, 3: True, 4: True}, "Leader"),
+    (5, {2: True, 3: True}, "Leader"),
+    (3, {2: False, 3: False}, "Follower"), (5, {2: False, 3: False, 4: False, 5: False}, "Follower"),
+    (5, {2: True, 3: False, 4: False, 5: False}, "Follower"),
+    (3, {}, "Candidate"), (5, {2: True}, "Candidate"), (5, {2: False, 3: False}, "Candidate"), (5, {}, "Candidate"),
+]
+
+
+def expected_state(first, outcomes):
+    w = first if first & 0xFF != B.VOTE_PENDING else (int(outcomes["result"][0]) if len(outcomes) else B.VOTE_PENDING)
+    return {B.VOTE_WON: "Leader", B.VOTE_LOST: "Follower", B.VOTE_PENDING: "Candidate"}[w & 0xFF]
+
+
+def state_of(e):
+    c = O.new_columns(e.n + 8, e.n)
+    c.term_start[:] = B.NO_TERM_START
+    c.meta[e.n_narrow:e.n:2], c.meta[e.n_narrow + 1:e.n:2] = META_WIDE_LO, META_WIDE_HI   # the allocated pairs
+    vt = np.zeros((O.SLOTS, c.cap), np.uint8)
+    assert np.all(CO.arena_control(c, vt, e.setup)["status"] == 0)
+    CO.arena_control(c, vt, e.campaign)
+    return c, vt

@@ -3,6 +3,9 @@ number order, zero scalars and an empty context not written), the caller's voter
 configurations, roles, tables and batches of frames -- that run the same on the device arena and on the oracle."""
 import numpy as np
 
+from oracle import oracle as O
+from oracle import control_oracle as CO
+from oracle import vote_request_oracle as VR
 from helpers import B
 from control_cmds import cmds, META_WIDE_LO, META_WIDE_HI
 import hb_frames as F
@@ -125,3 +128,82 @@ class Scenario:
             else:         # a group past the arena's highest slot
                 out.append(F.frame(self.n + int(rng.integers(1, 100)), 0, request(VOTE, term + 1)))
         return out
+
+
+def one(role, term, vote, last_index, last_term, leader=False, lease=False, check_quorum=False, voters=0b1,
+         committed=None, commit_term=0, priority=0):
+    """One group (slot 0 = self, id 1) in `role` at `term` with the given log -> (columns, votes, role, table)."""
+    c = O.new_columns(8, 1)
+    c.meta[0] = B.make_meta(voters, 0, 0, 0)
+    c.term[0], c.last_index[0] = term, last_index
+    c.committed[0] = last_index if committed is None else committed
+    c.term_start[0] = last_index if role == LEADER else B.NO_TERM_START
+    t = np.zeros(1, VR.VOTER_DTYPE)
+    t["id"], t["vote"], t["last_term"], t["commit_term"], t["persisted"], t["priority"] = \
+        1, vote, last_term, commit_term, last_index, priority
+    t["flags"] = (VR.SELECT if role != LEADER else 0) | (VR.LEADER if leader else 0) | (VR.LEASE if lease else 0) | \
+        (VR.CHECK_QUORUM if check_quorum else 0)
+    return c, np.zeros((O.SLOTS, c.cap), np.uint8), np.array([role], np.uint8), t
+
+
+# test_raft.rs:1537-1605: (role, index, log_term, vote, want reject) against a log of two entries at term 2
+RECV_VOTE = [
+    (FOLLOWER, 0, 0, 0, True), (FOLLOWER, 0, 1, 0, True), (FOLLOWER, 0, 2, 0, True), (FOLLOWER, 0, 3, 0, False),
+    (FOLLOWER, 1, 0, 0, True), (FOLLOWER, 1, 1, 0, True), (FOLLOWER, 1, 2, 0, True), (FOLLOWER, 1, 3, 0, False),
+    (FOLLOWER, 2, 0, 0, True), (FOLLOWER, 2, 1, 0, True), (FOLLOWER, 2, 2, 0, False), (FOLLOWER, 2, 3, 0, False),
+    (FOLLOWER, 3, 0, 0, True), (FOLLOWER, 3, 1, 0, True), (FOLLOWER, 3, 2, 0, False), (FOLLOWER, 3, 3, 0, False),
+    (FOLLOWER, 3, 2, 2, False), (FOLLOWER, 3, 2, 1, True), (LEADER, 3, 3, 1, True), (PRE_CANDIDATE, 3, 3, 1, True),
+    (CANDIDATE, 3, 3, 1, True),
+]
+
+
+def recv_vote_case(row):
+    role, index, log_term, vote, _ = row
+    term = max(2, log_term)
+    return one(role, term, vote, 2, 2), [F.frame(0, 0, request(VOTE, term, log_term, index, frm=2))]
+
+
+# test_raft_paper.rs:962-1006: (log as (term, index) entries, m.log_term, m.index, want reject) at m.term 3
+VOTER = [([(1, 1)], 1, 1, False), ([(1, 1)], 1, 2, False), ([(1, 1), (1, 2)], 1, 1, True),
+         ([(1, 1)], 2, 1, False), ([(1, 1)], 2, 2, False), ([(1, 1), (1, 2)], 2, 1, False),
+         ([(2, 1)], 1, 1, True), ([(2, 1)], 1, 2, True), ([(2, 1), (1, 2)], 1, 1, True)]
+
+
+def voter_case(row):
+    ents, log_term, index, _ = row
+    # a new Raft at term 0 over that log (term 0 is the host's: the pass needs a known term, so the group sits at 1)
+    state = one(FOLLOWER, 1, 0, len(ents), ents[-1][0], voters=0b11)
+    return state, [F.frame(0, 0, request(VOTE, 3, log_term, index, frm=2))]
+
+
+def any_state_case(role, typ):
+    """test_raft.rs:655-760: three voters, term 1 (a Follower whose leader is 3, a PreCandidate), 2 (a Candidate or a
+    Leader, who voted for themselves; the leader appended its empty entry); a request from 2 at term + 1."""
+    term = 2 if role in (CANDIDATE, LEADER) else 1
+    vote = 1 if role in (CANDIDATE, LEADER) else 0
+    last = 1 if role == LEADER else 0
+    state = one(role, term, vote, last, term if last else 0, leader=role in (FOLLOWER, LEADER), voters=0b111)
+    return state, [F.frame(0, 0, request(typ, term + 1, term + 1, 42, frm=2))]
+
+
+def state_of(s):
+    c = O.new_columns(s.n + 8, s.n)
+    c.term_start[:] = B.NO_TERM_START
+    c.meta[s.n_narrow:s.n:2], c.meta[s.n_narrow + 1:s.n:2] = META_WIDE_LO, META_WIDE_HI   # the allocated pairs
+    vt = np.zeros((O.SLOTS, c.cap), np.uint8)
+    assert np.all(CO.arena_control(c, vt, s.setup)["status"] == 0)
+    return c, vt
+
+
+def caller_update(table, role, status, out, frames):
+    """What the caller does with an applied frame's flags (INTEGRATION.md section 6)."""
+    for i in np.flatnonzero(status >> 4 == B.WIRE_OK):
+        g = int(np.frombuffer(frames[i][:4], "<u4")[0]) >> 4
+        if status[i] & B.VREQ_BUMPED:   # become_follower(m.term, INVALID_ID)'s host side
+            table["vote"][g] = 0
+            table["flags"][g] &= ~np.uint32(VR.LEADER | VR.LEASE)
+            role[g] = FOLLOWER
+        if status[i] & B.VREQ_VOTED:    # vote = m.from, election_elapsed = 0
+            table["vote"][g] = out[i][0]
+            if table["flags"][g] & VR.LEADER and table["flags"][g] & VR.CHECK_QUORUM:
+                table["flags"][g] |= VR.LEASE

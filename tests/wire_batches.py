@@ -1,13 +1,27 @@
 """Wire batches at the edges of the prologue every wire-frame pass shares (k_wire.cuh: wire_stage_block, wire_open,
 wire_decode): the stage rule restated, ballast frames that place a batch's blocks on both sides of the 16 KiB stage,
-hostile offset layouts, and the golden decoder vectors retargeted to another message type.  Pure numpy: the CPU tests
-check what these batches reach, the GPU tests (test_gpu_wire_batches.py) run them."""
+hostile offset layouts, the golden decoder vectors retargeted to another message type, and each pass's scenario --
+an arena and its oracle state in step, one batch through both and the comparison.  The CPU tests
+(test_wire_batches.py) check what these batches reach, the GPU tests (test_gpu_wire_batches.py) run them."""
 import json
 import os
+import types
 
 import numpy as np
 
+from oracle import hb_follow_oracle as HL
+from oracle import hb_frames_oracle as HF
+from oracle import hb_wire_oracle as H
+from oracle import vote_request_oracle as VR
+from oracle import vote_wire_oracle as VW
+from helpers import B, O, arena_of, assert_columns_equal, check_columns, oracle_wire_step, oracle_wire_apply, votes
+from control_cmds import cmds
+import hb_follow as FL
 import hb_frames as F
+import pass_forms as PF
+import read_cases as R
+import vote_frames as V
+import vote_request_frames as Q
 
 THREADS, STAGE = 256, 16 * 1024            # kWireThreads, kWireStage
 STAGED, SPAN, ORDER, PAST = "staged", "span", "order", "past"
@@ -184,3 +198,316 @@ def retarget(vector, msg_type):
     if not vector["ok"]:
         return raw, None
     return raw + bytes([0x08, msg_type]), dict(vector["fields"], msg_type=msg_type)
+
+
+# --------------------------------------------------------------------------- the five passes
+# Each pass: frames(rng) builds its scenario's frames on the CPU; fresh() an arena and the oracle's state in the same
+# state; run() one batch through the arena (host or device form) and the oracle, compares every output and returns the
+# outputs, the status bytes (WIRE_* << 4 | low nibble) first; PER_FRAME names the outputs with one row per frame;
+# check() compares the arena with the oracle's state.
+
+P = 8
+U64_MAX = (1 << 64) - 1
+
+
+class Leaders:
+    """Leaders set up by a control list, with group terms in the term column and read requests queued: the
+    AppendResponse step (kind "append") or the heartbeat-response pass with read queues (kind "heartbeat")."""
+
+    PER_FRAME = (0,)
+
+    def __init__(self, kind, n, setup, terms, reqs):
+        self.kind, self.n, self.setup, self.reqs = kind, n, setup, reqs
+        self.terms = np.zeros(n + 64, np.uint64)
+        self.terms[:n] = terms
+        self.d = self._driver()
+
+    def _driver(self):
+        d = R.OracleDriver(self.n, max_pending=P)
+        d.q.control(d.c, d.votes, self.setup)
+        d.c.term[: self.n] = self.terms[: self.n]
+        if len(self.reqs):
+            d.q.request(d.c, self.reqs)
+        return d
+
+    def frames(self, rng, k=None):
+        blob, off = R.mixed_batch(rng, self.d, self.n, self.terms, True, k or self.n)
+        return PF.split(blob, off)
+
+    def fresh(self):
+        a = B.Arena(self.n + 64)
+        a.enable_read_index(P)
+        assert a.group_alloc_range(self.n) == 0
+        a.control(self.setup)
+        a.column_write(B.COL_TERM, 0, 0, self.terms[: self.n].copy())
+        if len(self.reqs):
+            a.read_index_request(self.reqs)
+        return a, self._driver()
+
+    def run(self, a, d, buf, n_bytes, off, device, what):
+        if self.kind == "append":
+            if device:
+                got, = PF.device(a, "wire_apply", buf, off, n_bytes=n_bytes)
+                want = oracle_wire_apply(d.c, buf, off, self.n, self.terms, n_bytes=n_bytes)
+            else:
+                fb = PF.host_batch(buf, off, n_bytes)
+                fb.records = None
+                a.step_begin_wire(fb, B.STEP_READ_COMMITTED)
+                sr = a.step_wait()
+                got = a.wire_status().copy()
+                want, bm, adv, _ = oracle_wire_step(d.c, fb, self.n, self.terms)
+                gbm, _ = a.step_results(self.n)
+                assert np.array_equal(gbm, bm[: len(gbm)]) and sr.n_advanced == adv, what
+            PF.equal([want], [got], ["status"], what)
+            return (got,)
+        st, rel = PF.run(a, "heartbeat_wire", buf, off, device=device, n_bytes=n_bytes)
+        want, want_rel = H.apply(d.c, d.q, buf, off, self.terms, n_bytes=n_bytes)
+        got = (st, R.by_group(rel))
+        PF.equal([want, R.by_group(want_rel)], got, ["status", "released reads"], what)
+        return got
+
+    def check(self, a, d, what):
+        assert_columns_equal(a.read_columns(self.n), d.c, self.n, what)
+        R.queues_equal(a, d.q, self.n, what)
+
+
+def random_leaders(kind, seed, n):
+    """Leaders with random configurations (read_cases.random_setup), terms 1..3 (0 for a tenth: not checked) and
+    random read requests."""
+    rng = np.random.default_rng(seed)
+    setup = R.random_setup(rng, n, 0)
+    terms = rng.integers(1, 4, n).astype(np.uint64)
+    terms[rng.random(n) < 0.1] = 0
+    return Leaders(kind, n, setup, terms, R.random_requests(rng, n, 2.0, 12))
+
+
+class Followers:
+    """Followers whose group columns (term, last_index, term_start, committed) are written directly, with the
+    selection bitmap and self ids the caller passes: the follower pass.  frames: the random scenario's heartbeats."""
+
+    PER_FRAME = (0, 1)
+
+    def __init__(self, n, cols, sel, ids, frames=None):
+        self.n, self.cols, self.sel, self.ids, self._frames = n, cols, sel, ids, frames
+
+    def frames(self, rng):
+        return self._frames(rng)
+
+    def fresh(self):
+        a = B.Arena(self.n + 64)
+        assert a.group_alloc_range(self.n) == 0
+        for col, arr in self.cols.items():
+            a.column_write(col, 0, 0, arr)
+        c = a.read_columns(self.n)
+        c.term = self.cols[B.COL_TERM].copy()
+        return a, c
+
+    def run(self, a, c, buf, n_bytes, off, device, what):
+        want = HL.follower_heartbeats(c, None, buf, off, self.sel, self.ids, n_bytes=n_bytes)
+        if device:
+            got = PF.device(a, "follower_heartbeat", buf, off, self.sel, self.ids, n_bytes=n_bytes)
+        else:
+            ids, sel = np.zeros(a.cap, np.uint64), np.zeros((a.cap + 31) // 32, np.uint32)
+            ids[: self.n], sel[: len(self.sel)] = self.ids, self.sel
+            got = a.follower_heartbeat(PF.host_batch(buf, off, n_bytes), ids, sel)
+        PF.equal(want, got, ("status", "from", "response bytes", "response offsets", "totals"), what)
+        return got
+
+    def check(self, a, c, what):
+        s = FL.group_state(a, self.n)
+        for name, col in s.items():
+            assert np.array_equal(col, getattr(c, name)[: self.n]), (what, name)
+
+
+def random_followers(seed, n):
+    """Followers fed with the heartbeat-frames oracle's MsgHeartbeat frames, most at their term and below their log's
+    end, a few unselected."""
+    rng = np.random.default_rng(seed)
+    lc = O.new_columns(n, n)
+    lc.meta[:] = B.make_meta(0b11, 0, 0, 0)
+    lc.term_start[:] = 1
+    lc.term[:] = rng.integers(1, 1 << 33, n)
+    lc.committed[:] = rng.integers(0, 1 << 40, n)
+    lc.matched[1] = rng.integers(0, 1 << 40, n)
+    q = R.RO.ReadQueues(n, 1)
+    q.allocated[:] = 1
+    q.count[:] = rng.random(n) < 0.75
+    q.ctx[:, 0] = rng.integers(1, 1 << 63, n, dtype=np.uint64)
+    hb, hoff, _ = HF.bcast_heartbeats(lc, q, 0, n, rng.integers(1, 1 << 63, (9, n), dtype=np.uint64))
+    perm = rng.permutation(n).astype(np.uint32)
+    commit = np.minimum(lc.matched[1], lc.committed)
+    cols = {B.COL_TERM: np.zeros(n, np.uint64), B.COL_LAST_INDEX: np.zeros(n, np.uint64),
+            B.COL_TERM_START: np.where(rng.random(n) < 0.05, np.uint64(1), np.uint64(B.NO_TERM_START))}
+    cols[B.COL_TERM][perm] = lc.term + (rng.random(n) < 0.05).astype(np.uint64)
+    cols[B.COL_LAST_INDEX][perm] = commit + rng.integers(0, 1000, n).astype(np.uint64) - \
+        (rng.random(n) < 0.02).astype(np.uint64) * np.minimum(commit, np.uint64(1001))
+    last = cols[B.COL_LAST_INDEX]
+    cols[B.COL_COMMITTED] = last - np.minimum(last, rng.integers(0, 2000, n).astype(np.uint64))
+
+    def frames(rng):
+        hdr = perm << 4 | rng.integers(0, 16, n).astype(np.uint32)
+        out = PF.split(FL.with_headers(hb, hoff, hdr), hoff)
+        out += [out[i] for i in rng.integers(0, len(out), len(out) // 10)]         # repeated heartbeats: DUP
+        return [out[i] for i in rng.permutation(len(out))]
+
+    return Followers(n, cols, FL.bitmap(rng.random(n) < 0.95), FL.self_ids(rng, n), frames)
+
+
+class Candidates:
+    """Candidates polling, set up like a vote_frames.Election (setup and campaign control lists; e.frames the random
+    scenario's responses), with the select and pre bitmaps: the vote-response pass."""
+
+    PER_FRAME = (0,)
+
+    def __init__(self, e, sel, pre):
+        self.e, self.n = e, e.n
+        pad = np.zeros(4, np.uint32)
+        self.sel, self.pre = np.concatenate([sel, pad]), np.concatenate([pre, pad])
+
+    def frames(self, rng):
+        return self.e.frames(rng, commit_vote=True)
+
+    def fresh(self):
+        return arena_of(self.e), V.state_of(self.e)
+
+    def run(self, a, state, buf, n_bytes, off, device, what):
+        c, vt = state
+        want_st, want_out, _ = VW.batch(c, vt, buf, off, self.sel, self.pre, n_bytes=n_bytes)
+        got = PF.device(a, "vote_wire", buf, off, self.sel, self.pre, n_bytes=n_bytes) if device else \
+            a.vote_wire(PF.host_batch(buf, off, n_bytes), self.sel, self.pre)
+        PF.equal([want_st, want_out], got, ("status", "outcomes"), what)
+        return got
+
+    def check(self, a, state, what):
+        assert np.array_equal(votes(a, self.n), state[1][:, : self.n]), what
+
+
+def random_candidates(seed, n_narrow, n_wide):
+    e = V.Election(np.random.default_rng(seed), n_narrow, n_wide)
+    return Candidates(e, e.select(), e.pre())
+
+
+class Voters:
+    """Voters set up like a vote_request_frames.Scenario (s.setup, the caller's table s.table; s.frames the random
+    scenario's requests): the vote-request pass."""
+
+    PER_FRAME = (0, 1)
+
+    def __init__(self, s):
+        self.s, self.n = s, s.n
+
+    def frames(self, rng):
+        return self.s.frames(rng)
+
+    def fresh(self):
+        return arena_of(self.s), Q.state_of(self.s)
+
+    def run(self, a, state, buf, n_bytes, off, device, what):
+        c, vt = state
+        want = VR.batch(c, None, vt, buf, off, self.s.table, n_bytes=n_bytes)
+        got = PF.device(a, "vote_request_wire", buf, off, self.s.table, n_bytes=n_bytes) if device else \
+            a.vote_request_wire(PF.host_batch(buf, off, n_bytes), self.s.table)
+        PF.equal(want, got, ("status", "out", "response bytes", "response offsets", "totals"), what)
+        return got
+
+    def check(self, a, state, what):
+        check_columns(a, *state, self.n)
+
+
+PASSES = ("append", "heartbeat", "follower", "vote", "voter")
+
+
+def scenario(name, n=20_000):
+    """Each pass's random scenario at about n groups (a few of them wide pairs where the pass takes them)."""
+    if name in ("append", "heartbeat"):
+        return random_leaders(name, 0x57A6 + len(name), n)
+    if name == "follower":
+        return random_followers(0x57A7, n)
+    if name == "vote":
+        return random_candidates(0x57A8, n - 400, 200)
+    return Voters(Q.Scenario(np.random.default_rng(0x57A9), n - 400, 200))
+
+
+def stage_batch(sc, seed):
+    """The scenario's frames with the ballast of across_the_stage -> (frames, ballast mask)."""
+    rng = np.random.default_rng(seed)
+    return across_the_stage(sc.frames(rng), rng)
+
+
+def hostile_batches(sc, seed, device):
+    """hostile over the scenario's frames for every case of hostile_cases -> [(buf, n_bytes, offsets)]: a device
+    buffer holds 4 KiB or more of valid frames past n_bytes, and only offsets that end on those frames' boundaries go past
+    n_bytes; a host batch's offsets go at most 4 (n + 1) bytes past n_bytes, into the offsets the same call copies in."""
+    rng = np.random.default_rng(seed)
+    frames = sc.frames(rng)
+    tail, bounds = slack(frames[::-1])
+    out = []
+    for n, r in hostile_cases():
+        past = bounds if device else np.arange(4 * (n + 1) + 1)
+        blob, off = hostile(frames[int(rng.integers(0, len(frames) - n - 1)):], rng, n, r, past)
+        buf = np.concatenate([blob, np.frombuffer(tail, np.uint8)]) if device else blob
+        out.append((buf, len(blob), off))
+    return out
+
+
+GOLDEN_TYPE = {"append": 4, "heartbeat": 9, "follower": 8, "vote": 6, "voter": 5}
+
+
+CAP = 1 << 62                                            # log positions stay below this (SET_CONF takes last + 1)
+
+
+def golden_scenario(name, variant):
+    """One group per messages.json vector (retarget to the pass's type; a rejected vector as it is), its state
+    derived from the vector's decoded fields so that most frames reach the pass's decision:
+      append, heartbeat: a leader of voters {0, 1, 2} at m.term, a read pending under an 8-byte context;
+      follower: a selected follower at m.term whose log reaches m.commit, self id g + 1;
+      vote: a candidate at m.term whose committed is m.commit (variant 0) or one below it (variant 1: a rejection with
+        commit_term is COMMIT_VOTE);
+      voter: a selected follower at m.term with last_index = m.index and last_term = m.log_term (up to date), whose
+        priority is m.priority (variant 0: granted) or one more (variant 1: rejected, committed one below m.commit).
+    -> (scenario, frames, the vectors' kinds, their python-protobuf verdicts)."""
+    vs = golden()
+    n = len(vs)
+    typ = GOLDEN_TYPE[name]
+    raws, fields = zip(*[retarget(v, typ) for v in vs])
+    f = [x or {} for x in fields]
+    get = lambda k: np.array([int(x.get(k, 0)) for x in f], dtype=np.uint64)
+    term, commit, index = get("term"), get("commit"), get("index")
+    frames = [F.frame(g, 1, raws[g]) for g in range(n)]
+    kinds = np.array([v["kind"] for v in vs])
+    ok = np.array([v["ok"] for v in vs])
+    if name in ("append", "heartbeat"):
+        setup = cmds(*[r for g in range(n) for r in ((B.CTL_SET_CONF, g, 0, 0, (0b111, 0, 0, 11)),
+                                                     (B.CTL_RESET, g, 0, 0, (11, 10, 5, 10)), (B.CTL_BECOME_LEADER, g))])
+        ctx = [(g, int.from_bytes(m["context"], "little")) for g, m in enumerate(H.decode_message(r) for r in raws)
+               if m is not None and len(m["context"]) == 8]
+        return Leaders(name, n, setup, term, R.reqs(*ctx)), frames, kinds, ok
+    capped = np.minimum(commit, np.uint64(CAP))
+    if name == "follower":
+        cols = {B.COL_TERM: term, B.COL_LAST_INDEX: np.maximum(capped, np.uint64(10)),
+                B.COL_COMMITTED: np.full(n, 5, np.uint64), B.COL_TERM_START: np.full(n, B.NO_TERM_START, np.uint64)}
+        return Followers(n, cols, FL.bitmap(np.ones(n, bool)), np.arange(1, n + 1, dtype=np.uint64)), frames, kinds, ok
+    below = ((commit > 0) & (commit <= CAP)).astype(np.uint64)
+    if name == "vote":
+        com = capped - below * np.uint64(variant)
+        last = com + np.uint64(10)
+    else:
+        last = np.minimum(index, np.uint64(CAP))
+        com = np.minimum(capped - below, last)
+    rows, camp = [], []
+    for g in range(n):
+        rows += [(B.CTL_SET_CONF, g, 0, 0, (0b111, 0, 0, int(last[g]) + 1)),
+                 (B.CTL_RESET, g, 0, 0, (B.NO_TERM_START, int(last[g]), int(com[g]), int(last[g])))]
+        if term[g]:
+            rows.append((B.CTL_SET_TERM, g, 0, 0, (int(term[g]),)))
+        camp += [(B.CTL_RESET_VOTES, g), (B.CTL_RECORD_VOTE, g, 0, 1), (B.CTL_VOTE_RESULT, g)]
+    e = types.SimpleNamespace(n=n, n_narrow=n, n_wide=0, setup=cmds(*rows), campaign=cmds(*camp))
+    if name == "vote":
+        return Candidates(e, V.bitmap(np.ones(n, bool)), V.bitmap(np.zeros(n, bool))), frames, kinds, ok
+    e.campaign = None
+    e.table = Q.voters(n)
+    e.table["id"], e.table["last_term"], e.table["persisted"] = np.arange(1, n + 1), get("log_term"), last
+    e.table["commit_term"], e.table["flags"] = 3, B.VOTER_SELECT
+    pri = get("priority")
+    e.table["priority"] = pri if variant == 0 else np.where(pri < np.uint64(U64_MAX), pri + np.uint64(1), pri)
+    return Voters(e), frames, kinds, ok
