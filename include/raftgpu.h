@@ -653,7 +653,8 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
                                       On an arena with leader runs (raftgpu_arena_enable_leader_runs) only the rejections
                                       the stated runs cannot decide come back so.
                                       At raftgpu_follower_append: a MsgAppend with entries, or whose answer needs a term of
-                                      the follower's log outside the caller's run: RawNode::step on the host */
+                                      the follower's log outside the caller's run (and, on an arena with follower runs,
+                                      outside the row's two runs below it): RawNode::step on the host */
 #define RAFTGPU_WIRE_MALFORMED 4u  /* not a protobuf message, a bad frame, or a group that is not allocated */
 #define RAFTGPU_WIRE_DUP 5u        /* a later frame of a (group, peer) cell that already has one in this batch: cells are
                                       applied in arrival order, one message per step -- resubmit it with the next batch */
@@ -1374,7 +1375,9 @@ int32_t raftgpu_leader_term_wire(raftgpu_arena *arena, const void *bytes, uint64
  *                  RAFTGPU_CTL_COMMIT_TO; the response is {index = m.index, commit = committed after};
  *                - otherwise, with h = min(m.index, last_index) in the run and run_term <= m.log_term: the response is
  *                  {reject, index = m.index, reject_hint = h, log_term = run_term, commit = committed}
- *                  (RAFTGPU_FAPP_REJECT); every other rejection walks below the run and is NEEDS_LOG;
+ *                  (RAFTGPU_FAPP_REJECT); every other rejection walks below the run and is NEEDS_LOG -- on an arena
+ *                  with follower runs the match and the walk also read the row's runs below the table's run
+ *                  (raftgpu_arena_enable_follower_runs; this pass never writes the rows);
  *   DUP          every later frame of a group whose first frame reached the decision in this batch: resubmit DUP
  *                frames, in order, with the next batch.
  * A frame that is not OK changes nothing.  d_from (nullable, u64[n]) = m.from of every applied frame (0 for the
@@ -1438,7 +1441,10 @@ int32_t raftgpu_follower_append(raftgpu_arena *arena, const void *bytes, uint64_
  * The run.  For an appended frame, let t be the last entry's term and k the first index of the trailing block of
  * appended entries with term t.  When every appended entry has term t, t == run_term and conflict - 1 >= run_start,
  * the run stays; otherwise it becomes [k, last_index] with term t.  The device form writes d_log's row (the table is
- * read-write); the host form writes the caller's `log` rows of the appended frames from their records.
+ * read-write); the host form writes the caller's `log` rows of the appended frames from their records.  On an arena
+ * with follower runs (raftgpu_arena_enable_follower_runs) find_conflict also reads the row's runs, the log may be
+ * truncated into them, and an append that does not keep the run rewrites the run (which may then merge with the
+ * segment below, starting before k) and the row.
  * Appended.  d_appended (u64-aligned, n records) = raftgpu_follower_appended of every RAFTGPU_FAPP_APPENDED frame, all
  * zero for every other frame.  The span points into the caller's batch: the host hands those bytes to its log engine
  * (or decodes only them for RaftLog::unstable), lowers persisted to first_index - 1 (raft_log.rs:269-272) and sends the
@@ -1461,6 +1467,68 @@ int32_t raftgpu_follower_append_entries(raftgpu_arena *arena, const void *bytes,
                                         uint64_t n, raftgpu_follower_log *log, uint8_t *status, uint64_t *from,
                                         raftgpu_follower_appended *appended, uint8_t *resp_bytes,
                                         uint64_t resp_bytes_capacity, uint32_t *resp_offsets, uint64_t *totals);
+
+/* ---- the follower's earlier term runs: MsgAppend decided below the table's run ---- */
+
+/* The two passes above know term(i) on the table's run and above last_index.  After an election or a healed partition
+ * a follower's answer usually reads an older term: a rejection whose find_conflict_by_term walk (raft.rs:2429-2444,
+ * raft_log.rs:209-235) leaves the run, and the leader's next probe, whose m.index lies below it.  A row per group
+ * states up to two earlier term runs of the follower's log below the table's run; with it raftgpu_follower_append[_device]
+ * and raftgpu_follower_append_entries[_device] read term(i) there too:
+ *   - a match at m.index in run 1 or run 2: commit_to(min(m.commit, m.index)), or maybe_append with find_conflict
+ *     through every stated run (the log may be truncated into run 1 or run 2);
+ *   - a rejection: the walk goes down the table's run, run 1 and run 2 from h = min(m.index, last_index); the first
+ *     whose term is <= m.log_term answers {reject_hint = min(h, its end), log_term = its term}.  A walk that leaves the
+ *     lowest stated run stays RAFTGPU_WIRE_NEEDS_LOG (index 0 included: the pass cannot tell a compacted log).
+ * Everything else -- the statuses, the gap and entry-shape rules, the responses -- is as above.
+ *
+ * A row is used only while the arena has follower runs, the table's run is non-empty (run_start <= last_index, the
+ * pair's larger) and (run_start, run_term) equal the row's anchor with a non-zero term.  By the Log Matching Property
+ * the log below that entry is then the one the row was stated for, so a row survives term changes and
+ * become_follower.  A host-side change that moves the table's run off the anchor (a truncation or append that rewrites
+ * it, a snapshot) leaves the row inert until it is stated again.  Group alloc and free clear the row; a wide pair's row
+ * is on its low half.
+ *
+ * raftgpu_follower_append reads rows and never writes them.  raftgpu_follower_append_entries rewrites the row of every
+ * group it appends to so that, with the table's run, it describes the new log from the top: the appended blocks, the
+ * segment that held conflict - 1 cut there and the runs below it, equal neighbours merged, terms strictly decreasing
+ * downward.  Appended entries with more than two terms leave run 2, or both runs, unstated.  The table's new run (also
+ * raftgpu_follower_appended.run_start / run_term) may then start lower than the trailing block: it is still the log's
+ * last term run.  An append without an anchored row writes an anchored one from what the pass knows.
+ *
+ * Opt-in: call before groups are allocated.  Memory: 48 bytes per group slot.  An arena that does not call it behaves
+ * exactly as without the feature. */
+int32_t raftgpu_arena_enable_follower_runs(raftgpu_arena *arena);
+
+/* One group's row: 56 bytes.  Run 1 is [run_start[0], anchor_start - 1] at run_term[0], run 2 is [run_start[1],
+ * run_start[0] - 1] at run_term[1]; a run_start of 0 states no run.  Every stated run must still be readable by the
+ * follower's RaftLog::term (at or above first_index - 1): on compaction, restate the row or drop runs.  Fewer runs are
+ * never wrong; they leave more frames to the host. */
+typedef struct raftgpu_follower_runs {
+    uint32_t group;        /* the group (the low half of a wide pair) */
+    uint32_t reserved;     /* ignored; 0 from raftgpu_follower_runs_get */
+    uint64_t anchor_start; /* the table's run this row belongs to: raftgpu_follower_log.run_start ... */
+    uint64_t anchor_term;  /* ... and run_term */
+    uint64_t run_start[2];
+    uint64_t run_term[2];
+} raftgpu_follower_runs;
+
+/* State rows for many groups.  status[i] per row, and a refused row is not stored:
+ *   RAFTGPU_ERR_RANGE    the group is not allocated, or is the high half of a wide pair;
+ *   RAFTGPU_ERR_INVALID  anchor_term is 0, anchor_start is 0 or RAFTGPU_NO_TERM_START, run 2 without run 1, starts that
+ *                        do not satisfy 0 < run_start[1] < run_start[0] < anchor_start where stated, or run terms that
+ *                        do not satisfy 0 < run_term[1] < run_term[0] < anchor_term where stated.
+ * Returns RAFTGPU_OK when the list ran (n == 0 included), RAFTGPU_ERR_INVALID for an arena without follower runs or a
+ * NULL rows / status with n > 0.  The rows take effect at the call, in submission order on the compute stream;
+ * synchronous.  A later row of the same group wins. */
+int32_t raftgpu_follower_runs_set(raftgpu_arena *arena, const raftgpu_follower_runs *rows, uint64_t n, int32_t *status);
+
+/* The device's rows of groups [first, first + n) (group filled in), after the work already submitted on the compute
+ * stream: the entries pass rewrites rows on its own, and this is how a caller sees them.  The copy is not ordered after
+ * work on other streams: after raftgpu_follower_append_entries_device on a stream of the caller's, synchronise that
+ * stream first.  RAFTGPU_ERR_INVALID for an arena without follower runs or NULL rows with n > 0, RAFTGPU_ERR_RANGE past
+ * the arena's capacity. */
+int32_t raftgpu_follower_runs_get(raftgpu_arena *arena, uint32_t first, uint32_t n, raftgpu_follower_runs *rows);
 
 /* ---- votes (SURVEY 8(f) rank 1) ----------------------------------------- */
 

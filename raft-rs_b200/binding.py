@@ -69,6 +69,10 @@ assert FOLLOWER_LOG_DTYPE.itemsize == 32
 LEADER_RUNS_DTYPE = np.dtype([("group", "<u4"), ("reserved", "<u4"), ("term", "<u8"), ("term_start", "<u8"),
                               ("run_start", "<u8", (2,)), ("run_term", "<u8", (2,))])
 assert LEADER_RUNS_DTYPE.itemsize == 56
+# raftgpu_follower_runs_set / _get: one group's follower runs (raftgpu_follower_runs)
+FOLLOWER_RUNS_DTYPE = np.dtype([("group", "<u4"), ("reserved", "<u4"), ("anchor_start", "<u8"), ("anchor_term", "<u8"),
+                                ("run_start", "<u8", (2,)), ("run_term", "<u8", (2,))])
+assert FOLLOWER_RUNS_DTYPE.itemsize == 56
 # raftgpu_follower_append_entries: an applied frame's extra bit and its record (raftgpu_follower_appended)
 FAPP_APPENDED = 0x8
 FOLLOWER_APPENDED_DTYPE = np.dtype([("first_index", "<u8"), ("last_index", "<u8"), ("run_start", "<u8"),
@@ -322,6 +326,9 @@ def lib() -> C.CDLL:
             "raftgpu_arena_enable_inflights": ([vp, u32], i32),
             "raftgpu_arena_enable_leader_runs": ([vp], i32),
             "raftgpu_leader_runs_set": ([vp, vp, u64, vp], i32),
+            "raftgpu_arena_enable_follower_runs": ([vp], i32),
+            "raftgpu_follower_runs_set": ([vp, vp, u64, vp], i32),
+            "raftgpu_follower_runs_get": ([vp, u32, u32, vp], i32),
             "raftgpu_arena_set_wire_waves": ([vp, u32], i32),
             "raftgpu_inflights_get": ([vp, u32, u32, C.POINTER(u32), C.POINTER(u32), vp, u32], i32),
             "raftgpu_heartbeat_resp_device": ([vp, vp, vp, u64, vp, vp], i32),
@@ -891,6 +898,25 @@ class Arena:
         st = np.zeros(len(rows), dtype=np.int32)
         self._ck(self._L.raftgpu_leader_runs_set(self._h, rows.ctypes.data, len(rows), st.ctypes.data), "leader_runs_set")
         return st
+
+    # -- the follower's earlier term runs (include/raftgpu.h)
+    def enable_follower_runs(self):
+        self._ck(self._L.raftgpu_arena_enable_follower_runs(self._h), "arena_enable_follower_runs")
+
+    def follower_runs_set(self, rows: np.ndarray) -> np.ndarray:
+        """raftgpu_follower_runs_set: FOLLOWER_RUNS_DTYPE rows -> the i32 status of each row (a refused row is not
+        stored; only the call's own failure raises)."""
+        rows = np.ascontiguousarray(rows, dtype=FOLLOWER_RUNS_DTYPE)
+        st = np.zeros(len(rows), dtype=np.int32)
+        self._ck(self._L.raftgpu_follower_runs_set(self._h, rows.ctypes.data, len(rows), st.ctypes.data),
+                 "follower_runs_set")
+        return st
+
+    def follower_runs_get(self, first: int, n: int) -> np.ndarray:
+        """raftgpu_follower_runs_get: the device's rows of groups [first, first + n) as FOLLOWER_RUNS_DTYPE."""
+        rows = np.zeros(n, dtype=FOLLOWER_RUNS_DTYPE)
+        self._ck(self._L.raftgpu_follower_runs_get(self._h, first, n, rows.ctypes.data), "follower_runs_get")
+        return rows
 
     # -- ReadIndex, ReadOnlyOption::Safe (include/raftgpu.h)
     def enable_read_index(self, max_pending: int = 8):

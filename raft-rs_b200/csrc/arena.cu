@@ -279,6 +279,9 @@ struct raftgpu_arena {
     raftgpu_leader_runs *lr_stage = nullptr;
     uint64_t lr_stage_n = 0;
     std::vector<uint32_t> lr_pos;
+    // follower runs (raftgpu_arena_enable_follower_runs): the rows [cap], nullptr = off; their setter shares lr_stage and
+    // lr_pos
+    LeaderRuns *fr_rows = nullptr;
     // raftgpu_arena_set_wire_waves: frames of a cell (the wire step) or group (the follower's append passes) decided per
     // call, read by each call as it is queued
     uint32_t wire_waves = 1;
@@ -661,6 +664,7 @@ void destroy(raftgpu_arena *a) {
     cudaFree(a->rq_flag);
     cudaFree(a->lr_rows);
     cudaFree(a->lr_stage);
+    cudaFree(a->fr_rows);
     for (PassScratch &p : a->pass) {
         cudaFree(p.first);
         cudaFree(p.buf);
@@ -836,12 +840,13 @@ int32_t read_mark(raftgpu_arena *a, uint32_t first, uint32_t n, uint32_t value) 
     return sync_op(a, [&](cudaStream_t st) { read_mark_kernel<<<blocks, 256, 0, st>>>(a->cols.rq_hc, first, n, value); });
 }
 
-// Leader runs (arenas with raftgpu_arena_enable_leader_runs only): the rows of groups [first, first + n) are cleared, so
-// that a slot that is allocated or freed matches no anchor.
+// Leader and follower runs (arenas with raftgpu_arena_enable_leader_runs / _follower_runs only): the rows of groups
+// [first, first + n) are cleared, so that a slot that is allocated or freed matches no anchor.
 int32_t runs_clear(raftgpu_arena *a, uint32_t first, uint32_t n) {
-    if (!a->lr_rows || n == 0) return RAFTGPU_OK;
+    if ((!a->lr_rows && !a->fr_rows) || n == 0) return RAFTGPU_OK;
     CK(a, cudaSetDevice(a->device));
-    CK(a, cudaMemsetAsync(a->lr_rows + first, 0, sizeof(LeaderRuns) * n, a->s_compute));
+    if (a->lr_rows) CK(a, cudaMemsetAsync(a->lr_rows + first, 0, sizeof(LeaderRuns) * n, a->s_compute));
+    if (a->fr_rows) CK(a, cudaMemsetAsync(a->fr_rows + first, 0, sizeof(LeaderRuns) * n, a->s_compute));
     CK(a, cudaStreamSynchronize(a->s_compute));
     return RAFTGPU_OK;
 }
@@ -1190,22 +1195,34 @@ int32_t launch_wire_waves(raftgpu_arena *a, cudaStream_t st, const WireSrc &w, u
     return RAFTGPU_OK;
 }
 
-// The follower's append passes (abi_app_follow.inc), after afw_scan_kernel<kAppend>: afw_wave_apply_kernel over the
-// batch, then wire_wave_claim_kernel<true> and afw_wave_apply_kernel over each later wave's list.  Called from
+// The follower's append passes' decision (abi_app_follow.inc): afw_scan_kernel, then afw_apply_kernel at one wave; at
+// more, afw_wave_apply_kernel over the batch, then wire_wave_claim_kernel<true> and afw_wave_apply_kernel over each later
+// wave's list.  blk: reply_run's block sums, followed by the pass's extra words: the wave lists, then (kRuns and kAppend)
+// the new row of every frame (AfwRuns, 4 words each).  kRuns: an arena with follower runs (DESIGN 3.22).  Called from
 // reply_run's passes, which reports the launch errors.
-template <bool kAppend>
-void launch_afw_waves(raftgpu_arena *a, cudaStream_t st, const WireSrc &w, const raftgpu_follower_log *d_log, uint8_t *d_status,
-                      AfwRec *recs, uint32_t *first, uint64_t *d_from, uint32_t *blk, raftgpu_follower_appended *d_appended,
-                      uint32_t *lists, uint32_t waves) {
-    // (only the <true> kernel writes the table: raftgpu_follower_append_entries_device's, which is not const)
+template <bool kAppend, bool kRuns>
+void launch_afw(raftgpu_arena *a, cudaStream_t st, const WireSrc &w, const raftgpu_follower_log *d_log, uint8_t *d_status,
+                AfwRec *recs, uint32_t *first, uint64_t *d_from, uint32_t nb, uint32_t *blk,
+                raftgpu_follower_appended *d_appended, uint32_t waves) {
+    // (a later wave's claimant reads the table; only the kAppend kernels write it: raftgpu_follower_append_entries_device's,
+    // which is not const)
     raftgpu_follower_log *logs = const_cast<raftgpu_follower_log *>(d_log);
-    const uint32_t blocks = div_up(w.n, kWireThreads), grid = std::min<uint32_t>(blocks, a->grid_apply);
+    uint32_t *lists = blk + 2 * nb;
+    AfwRunsIo rio{kRuns ? a->fr_rows : nullptr, nullptr};
+    if (kRuns && kAppend) rio.next = reinterpret_cast<AfwRuns *>(reinterpret_cast<uint64_t *>(lists) + wave_list_words(w.n, waves));
+    afw_scan_kernel<kAppend, kRuns><<<nb, kWireThreads, 0, st>>>(a->cols, w, d_log, d_status, recs, first, d_appended, rio);
+    if (waves == 1) {
+        afw_apply_kernel<kAppend, kRuns && kAppend><<<nb, kWireThreads, 0, st>>>(a->cols, w.n, d_status, recs, first, d_from,
+                                                                               blk, logs, d_appended, rio);
+        return;
+    }
+    const uint32_t grid = std::min<uint32_t>(nb, a->grid_apply);
     cudaMemsetAsync(lists + 2ull * w.n, 0, 4ull * waves, st);
     for (uint32_t j = 0; j < waves; j++) {
         const WaveIo io = wave_io(lists, w.n, j);
         if (j) wire_wave_claim_kernel<true><<<grid, kWireThreads, 0, st>>>(w, a->cap, first, io.in, io.in_n);
-        afw_wave_apply_kernel<kAppend><<<j ? grid : blocks, kWireThreads, 0, st>>>(a->cols, w, d_status, recs, first, d_from,
-                                                                                  blk, logs, d_appended, io);
+        afw_wave_apply_kernel<kAppend, kRuns><<<j ? grid : nb, kWireThreads, 0, st>>>(a->cols, w, d_status, recs, first, d_from,
+                                                                                     blk, logs, d_appended, io, rio);
     }
 }
 

@@ -146,13 +146,26 @@ struct WireEntries {
 };
 constexpr uint32_t kEntsOk = 0, kEntsMalformed = 1, kEntsNeedsLog = 2;
 
-// kEntsMalformed: an Entry is not a well-formed protobuf message.  kEntsNeedsLog: a field 7 that is not length-
-// delimited, an index other than idx + 1, idx + 2, ..., a term 0, or appended entries with another field between them.
-__device__ __noinline__ uint32_t wire_entries(const uint8_t *p, uint32_t len, uint64_t idx, uint64_t last,
-                                                 uint64_t run_term, WireEntries &e) {
+// The walk of raftgpu_follower_append_entries on an arena with follower runs (k_app_follow.cuh, DESIGN 3.22): term(j)
+// for idx < j <= last is run_term on the table's run [run_start, last], t1 on the row's run 1 (down to s1) and t2 below
+// it (term(idx) is known, so every such j lies in one of them); pre / pre_term = the block of appended entries before
+// the trailing one (as tail / tail_term; 0 when the appended entries hold one term).
+struct WireEntriesRuns : WireEntries {
+    uint32_t pre;
+    uint64_t pre_term;
+};
+
+template <bool kRuns, class E>
+__device__ __forceinline__ uint32_t wire_entries_walk(const uint8_t *p, uint32_t len, uint64_t idx, uint64_t last,
+                                                      uint64_t run_start, uint64_t run_term, uint64_t s1, uint64_t t1,
+                                                      uint64_t t2, E &e) {
     e.count = e.conflict = e.tail = e.span_off = e.span_end = 0;
     e.tail_term = 0;
     e.uniform = true;
+    if constexpr (kRuns) {
+        e.pre = 0;
+        e.pre_term = 0;
+    }
     bool needs_log = false;
     uint32_t pos = 0;
     while (pos < len) {
@@ -196,7 +209,9 @@ __device__ __noinline__ uint32_t wire_entries(const uint8_t *p, uint32_t len, ui
         if (index != idx + k || term == 0) {
             needs_log = true;
         } else if (!e.conflict) {
-            if (idx + k > last || term != run_term) {  // the first entry the log takes
+            uint64_t have = run_term;  // term(idx + k), for idx + k <= last
+            if constexpr (kRuns) have = idx + k >= run_start ? run_term : idx + k >= s1 ? t1 : t2;
+            if (idx + k > last || term != have) {  // the first entry the log takes
                 e.conflict = e.tail = k;
                 e.tail_term = term;
                 e.span_off = at;
@@ -206,6 +221,10 @@ __device__ __noinline__ uint32_t wire_entries(const uint8_t *p, uint32_t len, ui
             if (at != e.span_end) needs_log = true;
             e.span_end = end;
             if (term != e.tail_term) {
+                if constexpr (kRuns) {
+                    e.pre = e.tail;
+                    e.pre_term = e.tail_term;
+                }
                 e.tail = k;
                 e.tail_term = term;
                 e.uniform = false;
@@ -213,6 +232,20 @@ __device__ __noinline__ uint32_t wire_entries(const uint8_t *p, uint32_t len, ui
         }
     }
     return needs_log ? kEntsNeedsLog : kEntsOk;
+}
+
+// kEntsMalformed: an Entry is not a well-formed protobuf message.  kEntsNeedsLog: a field 7 that is not length-
+// delimited, an index other than idx + 1, idx + 2, ..., a term 0, or appended entries with another field between them.
+__device__ __noinline__ uint32_t wire_entries(const uint8_t *p, uint32_t len, uint64_t idx, uint64_t last,
+                                                 uint64_t run_term, WireEntries &e) {
+    return wire_entries_walk<false>(p, len, idx, last, 0, run_term, 0, 0, 0, e);
+}
+
+// The same walk with the follower's runs (WireEntriesRuns).
+__device__ __noinline__ uint32_t wire_entries_runs(const uint8_t *p, uint32_t len, uint64_t idx, uint64_t last,
+                                                      uint64_t run_start, uint64_t run_term, uint64_t s1, uint64_t t1,
+                                                      uint64_t t2, WireEntriesRuns &e) {
+    return wire_entries_walk<true>(p, len, idx, last, run_start, run_term, s1, t1, t2, e);
 }
 
 // The context convention of the heartbeat paths (DESIGN 3.10): a read id travels as the 8 bytes of the context,
