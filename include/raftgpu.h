@@ -664,17 +664,20 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
                                       raftgpu_vote_request_wire, raftgpu_follower_term_wire) the group is not selected for the role the pass serves,
                                       or is a leader; at raftgpu_vote_wire also a response type that is not the
                                       candidate's own (step_candidate ignores it); at raftgpu_leader_term_wire the group
-                                      is not a leader: Raft::step on the host */
+                                      is not a leader; at raftgpu_follower_response_wire it is unselected or a leader:
+                                      Raft::step on the host */
 #define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat, raftgpu_follower_append) the commit_to the frame asks
                                         for -- m.commit, or min(m.commit, m.index) of a matching MsgAppend -- beyond
                                         max(committed, last_index): commit_to would be fatal! (raft_log.rs:291-298) */
 #define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire, raftgpu_vote_request_wire) m.commit != 0, m.commit_term != 0
                                         and m.commit beyond committed -- at raftgpu_vote_request_wire for a rejected
                                         request: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
-#define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire, raftgpu_leader_term_wire) the reference drops the frame:
-                                        a vote request in lease (raft.rs:1288-1316) or a MsgRequestVote at a lower term
-                                        (:1399-1409); at a leader a frame step_leader or step_follower has no arm for */
-#define RAFTGPU_WIRE_STALE 11u       /* (raftgpu_follower_term_wire, raftgpu_leader_term_wire) m.term below the group's (new)
+#define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire, raftgpu_leader_term_wire, raftgpu_follower_response_wire)
+                                        the reference drops the frame: a vote request in lease (raft.rs:1288-1316) or a
+                                        MsgRequestVote at a lower term (:1399-1409); a frame step_leader, step_candidate
+                                        or step_follower has no arm for */
+#define RAFTGPU_WIRE_STALE 11u       /* (raftgpu_follower_term_wire, raftgpu_leader_term_wire,
+                                        raftgpu_follower_response_wire) m.term below the group's (new)
                                         term: settled by the pass, which answered it when the low nibble is
                                         RAFTGPU_RES_OK; drop the frame */
 typedef struct raftgpu_wire_batch {
@@ -1181,6 +1184,10 @@ int32_t raftgpu_vote_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_by
 #define RAFTGPU_VOTER_LEASE 0x4u  /* check_quorum && leader_id != INVALID_ID && election_elapsed < election_timeout */
 #define RAFTGPU_VOTER_STALE_REPLY 0x8u /* check_quorum || pre_vote (raft.rs:1350): raftgpu_follower_term_wire answers a
                                           lower-term frame; raftgpu_vote_request_wire does not read it */
+#define RAFTGPU_VOTER_CANDIDATE 0x10u  /* a PreCandidate or a Candidate: raftgpu_follower_response_wire's role, and
+                                          raftgpu_follower_term_wire's step-down at the group's own term; the other
+                                          passes do not read it */
+#define RAFTGPU_VOTER_PRE_CANDIDATE 0x20u /* a PreCandidate (with RAFTGPU_VOTER_CANDIDATE): raftgpu_follower_response_wire */
 #define RAFTGPU_VREQ_GRANTED 0x1u /* the response has reject = false */
 #define RAFTGPU_VREQ_VOTED 0x2u   /* a granted MsgRequestVote: the caller sets vote = m.from, election_elapsed = 0 */
 #define RAFTGPU_VREQ_BUMPED 0x4u  /* the term was raised: the caller runs become_follower(m.term, INVALID_ID)'s host side */
@@ -1217,7 +1224,8 @@ int32_t raftgpu_vote_request_wire(raftgpu_arena *arena, const void *bytes, uint6
  * not read and is copied into the response's header.  d_bytes 16-byte aligned, n and n_bytes below 4 GiB.  d_voters
  * (16-byte aligned, read only) is raftgpu_vote_request_wire's table: the pass reads id, persisted and the flags
  * (RAFTGPU_VOTER_SELECT: a Follower, PreCandidate or Candidate, the roles whose term rule is the same;
- * RAFTGPU_VOTER_STALE_REPLY: check_quorum || pre_vote).
+ * RAFTGPU_VOTER_STALE_REPLY: check_quorum || pre_vote; RAFTGPU_VOTER_CANDIDATE: a PreCandidate or Candidate, which a
+ * frame at its own term steps down -- opt-in: a row without it is decided as if the group were a Follower).
  * Status.  status[i] = RAFTGPU_WIRE_* << 4 | a low nibble; the first failing check decides:
  *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot, or a wide pair's high half;
  *   SKIP_TYPE    any type but 3 and 8 (MsgSnapshot and MsgTimeoutNow stay with the host);
@@ -1230,7 +1238,11 @@ int32_t raftgpu_vote_request_wire(raftgpu_arena *arena, const void *bytes, uint6
  *                the group's term the lowest such frame is the group's claimant, with the low nibble
  *                RAFTGPU_FTERM_BUMPED: it runs become_follower(T, m.from)'s arena part (term = T, and RAFTGPU_CTL_RESET's
  *                reset on both halves of a pair with term_start RAFTGPU_NO_TERM_START, last_index, committed -- the
- *                larger of the halves' -- and the table's persisted), exactly RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET;
+ *                larger of the halves' -- and the table's persisted), exactly RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET.
+ *                When T equals the term of a group whose row has RAFTGPU_VOTER_CANDIDATE, the lowest frame at T is the
+ *                claimant too, with the low nibble RAFTGPU_FTERM_STEPPED: step_candidate's become_follower(term, m.from)
+ *                (raft.rs:2215-2224), whose arena part is RAFTGPU_CTL_RESET's reset alone (term unchanged, votes
+ *                cleared);
  *   STALE        m.term < T: settled here; drop the frame.  With RAFTGPU_VOTER_STALE_REPLY the pass answers it with one
  *                MsgAppendResponse {to = m.from, from = the table's id, term = T}, every other field zero
  *                (raft.rs:1375-1376), and the low nibble is RAFTGPU_RES_OK; without it the reference ignores the frame.
@@ -1252,15 +1264,19 @@ int32_t raftgpu_vote_request_wire(raftgpu_arena *arena, const void *bytes, uint6
  * Host side.  For every RAFTGPU_FTERM_BUMPED frame the caller runs become_follower's host side -- role Follower,
  * leader_id = m.from, vote = 0, election_elapsed = 0 -- and updates its select bitmap, log table and voter row before
  * the next call that reads them: a voter row left stale could grant a vote the reference, now following m.from,
- * refuses.
+ * refuses.  For every RAFTGPU_FTERM_STEPPED frame: role Follower, leader_id = m.from, election_elapsed = 0, the vote
+ * kept (the term is the same); clear RAFTGPU_VOTER_CANDIDATE and RAFTGPU_VOTER_PRE_CANDIDATE and set the group's
+ * follower select bits, so that the follower passes on the same buffer decide the frame.
  * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  When
- * one received buffer goes through several passes: raftgpu_vote_request_wire first, then this pass, then the follower
- * passes (their types are disjoint).  A candidate this pass bumps is a Follower only once the caller says so: the
- * follower passes of the same sequence return ROLE for it until then, and the host steps those frames.  The host form
- * copies (voters covers the groups below the highest allocated one), runs and waits; status, out, resp_bytes /
- * resp_offsets as above, totals u64[2]. */
+ * one received buffer goes through several passes: raftgpu_vote_request_wire first, then raftgpu_follower_response_wire
+ * and its host side, then this pass, then the follower passes (their types are disjoint).  A candidate this pass bumps
+ * or steps down is a Follower only once the caller says so: the follower passes of the same sequence return ROLE for it
+ * until then, and the host steps those frames.  The host form copies (voters covers the groups below the highest
+ * allocated one), runs and waits; status, out, resp_bytes / resp_offsets as above, totals u64[2]. */
 #define RAFTGPU_FTERM_BUMPED 0x4u /* the claimant: the term was raised, the caller runs become_follower(T, m.from)'s
                                      host side */
+#define RAFTGPU_FTERM_STEPPED 0x8u /* (raftgpu_follower_term_wire) the claimant at a (Pre)Candidate's own term: the
+                                      caller runs become_follower(term, m.from)'s host side */
 /* 39 bytes per frame: enough for the responses to any n frames. */
 uint64_t raftgpu_follower_term_wire_bound(uint64_t n);
 int32_t raftgpu_follower_term_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
@@ -1321,8 +1337,9 @@ int32_t raftgpu_follower_term_wire(raftgpu_arena *arena, const void *bytes, uint
  * leadership transferee, no pending conf index, the read-index map emptied; and updates its voter row and select
  * bitmaps before the next call that reads them.
  * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  When
- * one received buffer goes through several passes: raftgpu_vote_request_wire, raftgpu_follower_term_wire,
- * raftgpu_vote_wire, the leader passes (the wire step and raftgpu_heartbeat_wire), then this pass, then the host side
+ * one received buffer goes through several passes: raftgpu_vote_request_wire, raftgpu_follower_response_wire,
+ * raftgpu_follower_term_wire, raftgpu_vote_wire, the leader passes (the wire step and raftgpu_heartbeat_wire), then
+ * this pass, then the host side
  * of every BUMPED of raftgpu_follower_term_wire and of this pass, then the follower passes.  This pass must come after
  * the leader passes, which would apply the frames at T after a bump; after a step's begin is enough.  The follower
  * term pass must come before it, or a group bumped here could be answered twice.  Merging statuses: this pass's
@@ -1338,6 +1355,60 @@ int32_t raftgpu_leader_term_wire(raftgpu_arena *arena, const void *bytes, uint64
                                  uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
                                  uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
                                  uint64_t *totals);
+
+/* ---- the responses that reach a follower or a candidate ------------------------ */
+
+/* RawNode::step -> Raft::step's term rules (raft.rs:1280-1348) and the drop arms of step_follower and step_candidate
+ * (:2205-2255) for the MsgAppendResponse (4), MsgRequestVoteResponse (6), MsgHeartbeatResponse (9) and
+ * MsgRequestPreVoteResponse (18) frames of a wire batch at a Follower, PreCandidate or Candidate: the late responses
+ * of a deposed leader, the late votes of a lost or abandoned election, and a higher-term rejection at a candidate.
+ * become_follower(T, INVALID_ID)'s arena part for a higher term, and a verdict for every frame the reference drops.
+ * None of these frames is ever answered.
+ * Input.  The frames carry the receiver's cell (group << 4 | slot), as the wire step, raftgpu_vote_wire and
+ * raftgpu_leader_term_wire take them: a wide pair's high half stands for its pair's low half.  d_bytes 16-byte aligned,
+ * n and n_bytes below 4 GiB.  d_voters (16-byte aligned, read only) is raftgpu_vote_request_wire's table, one row per
+ * group slot below the highest allocated one (a pair's row is its low half's): the pass reads persisted and the flags
+ * (RAFTGPU_VOTER_SELECT; RAFTGPU_VOTER_CANDIDATE: a PreCandidate or Candidate; RAFTGPU_VOTER_PRE_CANDIDATE: a
+ * PreCandidate).  Leadership is the arena's own: term_start != RAFTGPU_NO_TERM_START.
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4 | a low nibble; the first failing check decides:
+ *   MALFORMED    a bad frame or protobuf, or a group at or past the highest allocated slot;
+ *   SKIP_TYPE    any type but 4, 6, 9 and 18;
+ *   ROLE         RAFTGPU_VOTER_SELECT is clear, or the group (a pair: its low half) is a leader;
+ *   TERM         the group's term (raftgpu_group_set_term) is 0, or m.term is 0 (a local message);
+ * then every passing frame is decided per group.  A MsgRequestPreVoteResponse with reject = false never raises the term
+ * (raft.rs:1319-1320).  Let T be the larger of the group's term and the largest m.term among its other passing frames:
+ *   OK | RAFTGPU_FTERM_BUMPED  T is above the term and this is the lowest frame at T: it runs
+ *                become_follower(T, INVALID_ID)'s arena part, exactly RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET (as
+ *                raftgpu_follower_term_wire's claimant);
+ *   OK           T is the group's term and the frame belongs to the group's own candidacy: a MsgRequestVoteResponse
+ *                at a Candidate at the term, or a MsgRequestPreVoteResponse at a PreCandidate at the term -- or, when
+ *                it grants, above it (raft.rs:1319-1330).  Nothing is written: raftgpu_vote_wire takes the frame;
+ *   IGNORED      any other frame at T, a granting pre-vote response at or above T included: step_follower and
+ *                step_candidate drop it;
+ *   STALE        m.term below T: settled here; drop the frame (no reply: raft.rs:1349-1411).
+ * There is no DUP: every frame gets its verdict in one call.  d_out (nullable, u64[n]) = T for each claimant, zero for
+ * every other frame.
+ * What the result equals.  The reference reaches the same state when a group's frames are delivered in this order: the
+ * claimant, the other frames at T, then the stale frames.  When there is no claimant, the frames left OK go through
+ * raftgpu_vote_wire.
+ * Refusals.  RAFTGPU_ERR_INVALID before any launch for a missing d_voters, d_status, d_bytes or d_offsets with n > 0,
+ * misaligned buffers, and the batch limits of the other wire passes.
+ * Host side.  For every RAFTGPU_FTERM_BUMPED frame the caller runs become_follower(T, INVALID_ID) (raft.rs:1082-1093)
+ * and the host part of reset (:942-971): role Follower, no leader, vote = 0, election_elapsed = 0; it clears
+ * RAFTGPU_VOTER_CANDIDATE and RAFTGPU_VOTER_PRE_CANDIDATE, sets the group's follower select bits and updates its
+ * voter row before the next call that reads them.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  When
+ * one received buffer goes through several passes: raftgpu_vote_request_wire, this pass and its host side,
+ * raftgpu_follower_term_wire and its host side, raftgpu_vote_wire, the leader passes, raftgpu_leader_term_wire and its
+ * host side, then the follower passes.  Merging statuses: this pass's STALE, IGNORED and BUMPED are settled; its OK
+ * defers to raftgpu_vote_wire's status, but for a group raftgpu_follower_term_wire then bumps or steps down: its
+ * step-down comes first, and step_follower drops the frame (settled as IGNORED; do not hand it to raftgpu_vote_wire).  The host form copies (voters covers the groups below the highest allocated
+ * one), runs and waits; status and out as above. */
+int32_t raftgpu_follower_response_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes, uint64_t n_bytes,
+                                              const uint32_t *d_offsets, uint64_t n, const raftgpu_voter *d_voters,
+                                              uint8_t *d_status, uint64_t *d_out);
+int32_t raftgpu_follower_response_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes, const uint32_t *offsets,
+                                       uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out);
 
 /* ---- MsgAppend at the follower ------------------------------------------------ */
 

@@ -46,8 +46,8 @@ BULK_SORTED = 0x1
 WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WIRE_CONTEXT = range(7)
 WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat (ROLE also raftgpu_vote_wire)
 WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire, raftgpu_vote_request_wire
-WIRE_IGNORED = 10  # raftgpu_vote_request_wire, raftgpu_leader_term_wire
-WIRE_STALE = 11  # raftgpu_follower_term_wire, raftgpu_leader_term_wire
+WIRE_IGNORED = 10  # raftgpu_vote_request_wire, raftgpu_leader_term_wire, raftgpu_follower_response_wire
+WIRE_STALE = 11  # raftgpu_follower_term_wire, raftgpu_leader_term_wire, raftgpu_follower_response_wire
 WIRE_WAVES_MAX = 64  # raftgpu_arena_set_wire_waves
 # raftgpu_vote_request_wire: the caller's table (raftgpu_voter), its flags, and the low nibble of an applied frame
 VOTER_SELECT, VOTER_LEADER, VOTER_LEASE = 0x1, 0x2, 0x4
@@ -55,6 +55,9 @@ VREQ_GRANTED, VREQ_VOTED, VREQ_BUMPED = 0x1, 0x2, 0x4
 # raftgpu_follower_term_wire: the voter table's extra flag and the claimant's low nibble
 VOTER_STALE_REPLY = 0x8
 FTERM_BUMPED = 0x4
+# raftgpu_follower_response_wire (and raftgpu_follower_term_wire's step-down): the candidate flags, the step-down's nibble
+VOTER_CANDIDATE, VOTER_PRE_CANDIDATE = 0x10, 0x20
+FTERM_STEPPED = 0x8
 VOTER_DTYPE = np.dtype([("id", "<u8"), ("vote", "<u8"), ("last_term", "<u8"), ("commit_term", "<u8"),
                         ("persisted", "<u8"), ("priority", "<u8"), ("flags", "<u4"), ("reserved", "<u4"),
                         ("reserved2", "<u8")])
@@ -363,6 +366,8 @@ def lib() -> C.CDLL:
             "raftgpu_follower_term_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_leader_term_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_leader_term_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_follower_response_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp], i32),
+            "raftgpu_follower_response_wire": ([vp, vp, u64, vp, u64, vp, vp, vp], i32),
             "raftgpu_follower_append_bound": ([u64], u64),
             "raftgpu_follower_append_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_append": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
@@ -1162,6 +1167,24 @@ class Arena:
         self._ck(self._L.raftgpu_leader_term_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters,
                                                          d_status, d_out, d_resp_bytes, resp_bytes_capacity,
                                                          d_resp_offsets, d_totals), "leader_term_wire_device")
+
+    def follower_response_wire(self, frames, voters):
+        """raftgpu_follower_response_wire: Raft::step's term rules and the drop arms of step_follower and step_candidate
+        for the MsgAppendResponse, MsgRequestVoteResponse, MsgHeartbeatResponse and MsgRequestPreVoteResponse frames of a
+        wire batch at this arena's followers and candidates (.bytes, .n_bytes, .offsets, .n).  voters: VOTER_DTYPE rows
+        covering the groups below the highest allocated one -> (status u8[n], out u64[n] = T of the claimants)."""
+        vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
+        assert len(vt) >= self.get_info().hi
+        n = frames.n
+        status, out = np.zeros(n, np.uint8), np.zeros(n, np.uint64)
+        self._ck(self._L.raftgpu_follower_response_wire(self._h, frames.bytes.ctypes.data, frames.n_bytes,
+                                                        frames.offsets.ctypes.data, n, vt.ctypes.data, status.ctypes.data,
+                                                        out.ctypes.data), "follower_response_wire")
+        return status, out
+
+    def follower_response_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_voters, d_status, d_out, stream=None):
+        self._ck(self._L.raftgpu_follower_response_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters,
+                                                               d_status, d_out), "follower_response_wire_device")
 
     def follower_append(self, frames, log):
         """raftgpu_follower_append: handle_append_entries at this arena's followers for the entry-less MsgAppend frames

@@ -234,6 +234,7 @@ enum Pass {
     kPassAppFollow,
     kPassFollowTerm,
     kPassLeaderTerm,
+    kPassFollowResp,
     kPassCount
 };
 
@@ -1463,5 +1464,6 @@ extern "C" {
 #include "abi_leader_runs.inc"
 #include "abi_follow_term.inc"
 #include "abi_leader_term.inc"
+#include "abi_follow_resp.inc"
 
 }  // extern "C"

@@ -8,7 +8,9 @@
 // Role, vote and leader stay with the caller: its raftgpu_voter table (one row per group slot) is read only.  The
 // frame's header is the follower's own (group << 4 | x); x is not read and goes back unchanged in the response's header.
 // Every frame gets its verdict in one call: T = max(the group's term, the largest m.term among its passing frames) does
-// not depend on the order in which they are applied, and the first one applied at T does the bump.
+// not depend on the order in which they are applied, and the first one applied at T does the bump.  A row with
+// RAFTGPU_VOTER_CANDIDATE opts in to step_candidate's step-down (raft.rs:2215-2224): when T is the group's term, the
+// first frame at T makes the (Pre)Candidate a Follower, become_follower(term, m.from), whose arena part is the reset.
 //
 // Five kernels and no waiting between blocks: ftm_scan_kernel stages and decodes every frame once, classifies it,
 // writes a 24-byte record per passing frame and atomicMax-es T into a per-group u64 table; ftm_claim_kernel lets the
@@ -17,10 +19,11 @@
 // into block starts; reply_write_kernel<FtmReply> (k_wire.cuh) encodes the replies (wire_put_app_resp_frame) and
 // stores them through shared memory.  Every kernel takes kWireThreads frames per block: one block sum per scan block.
 
-// A passing frame's record: w0 = its header | kFtmReply when the table's RAFTGPU_VOTER_STALE_REPLY is set; to = m.from;
-// term = m.term (the apply pass overwrites it with T for a stale reply); from = the table's id (written by the apply
-// pass for a stale reply only).
-constexpr uint64_t kFtmReply = 1ull << 32;
+// A passing frame's record: w0 = its header | kFtmReply when the table's RAFTGPU_VOTER_STALE_REPLY is set | kFtmCand
+// when its RAFTGPU_VOTER_CANDIDATE is; to = m.from; term = m.term (the apply pass overwrites it with T for a stale
+// reply); from = the table's id (written by the apply pass for a stale reply only).  No other pass sets kFtmCand, so
+// ftm_claim_kernel claims their groups at a raised term only.
+constexpr uint64_t kFtmReply = 1ull << 32, kFtmCand = 1ull << 36;
 struct __align__(16) FtmRec {
     uint64_t w0, to, term, from;
 };
@@ -45,7 +48,7 @@ __device__ __forceinline__ uint32_t ftm_frame(const Columns &c, const WireSrc &w
     if (!(flags & RAFTGPU_VOTER_SELECT) || c.term_start[g] != RAFTGPU_NO_TERM_START) return RAFTGPU_WIRE_ROLE;
     const uint64_t term = c.term[g];
     if (term == 0 || m.term == 0) return RAFTGPU_WIRE_TERM;  // m.term 0 is a local message
-    r.w0 = hdr | ((flags & RAFTGPU_VOTER_STALE_REPLY) ? kFtmReply : 0ull);
+    r.w0 = hdr | ((flags & RAFTGPU_VOTER_STALE_REPLY) ? kFtmReply : 0ull) | ((flags & RAFTGPU_VOTER_CANDIDATE) ? kFtmCand : 0ull);
     r.to = m.from;  // become_follower's leader_id, the stale reply's to (raft.rs:1347, 1375)
     r.term = m.term;
     top = umax64(m.term, term);
@@ -74,9 +77,9 @@ __global__ void __launch_bounds__(kWireThreads) ftm_scan_kernel(Columns c, WireS
     if (top[g] < t) atomicMax(&top[g], static_cast<unsigned long long>(t));
 }
 
-// Pass 2: a passing frame with m.term == T > term claims its group: first_frame[group] = the lowest such frame.
-// Algorithmic bytes per frame: 1 read; per passing frame 16 (w0, term) + 8 (T) read; per frame at a raised T 8 (term)
-// read and 4 (first_frame) written.
+// Pass 2: a passing frame with m.term == T > term, or with m.term == T and kFtmCand, claims its group: first_frame[group]
+// = the lowest such frame.  Algorithmic bytes per frame: 1 read; per passing frame 16 (w0, term) + 8 (T) read; per
+// frame at T 8 (term) read and 4 (first_frame) written.
 __global__ void __launch_bounds__(kWireThreads) ftm_claim_kernel(Columns c, uint32_t n, const uint8_t *__restrict__ status,
                                                                  const FtmRec *__restrict__ recs,
                                                                  const unsigned long long *__restrict__ top,
@@ -85,12 +88,13 @@ __global__ void __launch_bounds__(kWireThreads) ftm_claim_kernel(Columns c, uint
     if (i >= n || status[i] != (RAFTGPU_WIRE_OK << 4)) return;
     const uint32_t g = static_cast<uint32_t>(recs[i].w0) >> 4;
     const uint64_t t = recs[i].term;
-    if (t == top[g] && t > c.term[g]) atomicMin(&first_frame[g], i);
+    if (t == top[g] && (t > c.term[g] || (recs[i].w0 & kFtmCand))) atomicMin(&first_frame[g], i);
 }
 
 // Pass 3: the verdict of every passing frame, from T = top[group] and its own m.term -- never from the group's term,
-// which the claimant writes in this kernel.  The claimant runs become_follower(T, m.from)'s arena part
-// (become_follower_arena) and keeps RAFTGPU_WIRE_OK | RAFTGPU_FTERM_BUMPED; any other frame at T stays RAFTGPU_WIRE_OK
+// which the claimant writes in this kernel (only the claimant reads it, before).  The claimant runs
+// become_follower(T, m.from)'s arena part (become_follower_arena) and keeps RAFTGPU_WIRE_OK | RAFTGPU_FTERM_BUMPED, or
+// RAFTGPU_FTERM_STEPPED when T is the term (the reset alone); any other frame at T stays RAFTGPU_WIRE_OK
 // with nothing written; a frame below T is RAFTGPU_WIRE_STALE, | RAFTGPU_RES_OK with its reply's record completed
 // (from = the table's id, term = T) when kFtmReply is set.  out[2 i..] (nullable) = {m.from, T} of the claimant, 0
 // otherwise.  blk[2 * block + {0, 1}] = the block's replies and their bytes.  Algorithmic bytes per frame: 1 read + 1
@@ -110,8 +114,9 @@ __global__ void __launch_bounds__(kWireThreads) ftm_apply_kernel(Columns c, uint
             const uint32_t g = static_cast<uint32_t>(r.w0) >> 4;
             const uint64_t t = top[g];
             if (first_frame[g] == i) {
+                const uint32_t how = t > c.term[g] ? RAFTGPU_FTERM_BUMPED : RAFTGPU_FTERM_STEPPED;
                 become_follower_arena(c, g, t, voters);
-                status[i] = static_cast<uint8_t>((RAFTGPU_WIRE_OK << 4) | RAFTGPU_FTERM_BUMPED);
+                status[i] = static_cast<uint8_t>((RAFTGPU_WIRE_OK << 4) | how);
                 from = r.to;
                 term = t;
             } else if (r.term < t) {

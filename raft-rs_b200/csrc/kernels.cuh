@@ -33,5 +33,6 @@ namespace raftgpu {
 #include "k_app_follow.cuh"
 #include "k_follow_term.cuh"
 #include "k_leader_term.cuh"
+#include "k_follow_resp.cuh"
 
 }  // namespace raftgpu
