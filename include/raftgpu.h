@@ -664,15 +664,18 @@ int32_t raftgpu_heartbeat_commits_device(raftgpu_arena *arena, void *stream, uin
                                       raftgpu_vote_request_wire, raftgpu_follower_term_wire) the group is not selected for the role the pass serves,
                                       or is a leader; at raftgpu_vote_wire also a response type that is not the
                                       candidate's own (step_candidate ignores it); at raftgpu_leader_term_wire the group
-                                      is not a leader; at raftgpu_follower_response_wire it is unselected or a leader:
-                                      Raft::step on the host */
+                                      is not a leader; at raftgpu_follower_response_wire it is unselected or a leader;
+                                      at raftgpu_leader_vote_request_wire the group is not a leader: Raft::step on the
+                                      host */
 #define RAFTGPU_WIRE_COMMIT_RANGE 8u /* (raftgpu_follower_heartbeat, raftgpu_follower_append) the commit_to the frame asks
                                         for -- m.commit, or min(m.commit, m.index) of a matching MsgAppend -- beyond
                                         max(committed, last_index): commit_to would be fatal! (raft_log.rs:291-298) */
-#define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire, raftgpu_vote_request_wire) m.commit != 0, m.commit_term != 0
-                                        and m.commit beyond committed -- at raftgpu_vote_request_wire for a rejected
-                                        request: maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
-#define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire, raftgpu_leader_term_wire, raftgpu_follower_response_wire)
+#define RAFTGPU_WIRE_COMMIT_VOTE 9u  /* (raftgpu_vote_wire, raftgpu_vote_request_wire, raftgpu_leader_vote_request_wire)
+                                        m.commit != 0, m.commit_term != 0 and m.commit beyond committed -- at the vote
+                                        request passes for a rejected request (at a leader: one that deposes it):
+                                        maybe_commit_by_vote (raft.rs:2126-2164) needs the caller's log */
+#define RAFTGPU_WIRE_IGNORED 10u     /* (raftgpu_vote_request_wire, raftgpu_leader_vote_request_wire,
+                                        raftgpu_leader_term_wire, raftgpu_follower_response_wire)
                                         the reference drops the frame: a vote request in lease (raft.rs:1288-1316) or a
                                         MsgRequestVote at a lower term (:1399-1409); a frame step_leader, step_candidate
                                         or step_follower has no arm for */
@@ -1151,7 +1154,7 @@ int32_t raftgpu_vote_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_by
  *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot, or a wide pair's high half;
  *   SKIP_TYPE    any type but 5 and 17;
  *   ROLE         RAFTGPU_VOTER_SELECT is clear, or the group is a leader (term_start != RAFTGPU_NO_TERM_START): a leader
- *                that steps down has host-side consequences;
+ *                that steps down has host-side consequences (raftgpu_leader_vote_request_wire decides its frames);
  *   TERM         the group's term (raftgpu_group_set_term) is 0, or m.term is 0 (a local message);
  * then the first frame of each group in frame order that got this far is decided by the term rules:
  *   IGNORED      m.term > term in lease (RAFTGPU_VOTER_LEASE, and the context is not "CampaignTransfer"), or a
@@ -1355,6 +1358,67 @@ int32_t raftgpu_leader_term_wire(raftgpu_arena *arena, const void *bytes, uint64
                                  uint64_t n, const raftgpu_voter *voters, uint8_t *status, uint64_t *out,
                                  uint8_t *resp_bytes, uint64_t resp_bytes_capacity, uint32_t *resp_offsets,
                                  uint64_t *totals);
+
+/* ---- vote requests at a leader ------------------------------------------------- */
+
+/* RawNode::step -> Raft::step's term rules (raft.rs:1280-1411), then the MsgRequestVote | MsgRequestPreVote arm
+ * (:1418-1462) and one response through send, for the MsgRequestVote (5) and MsgRequestPreVote (17) frames of a wire
+ * batch at a leader: a winner's answer to the losing candidates, the lease against a healed partition, and the
+ * step-down at a higher-term vote.  raftgpu_vote_request_wire returns ROLE for these frames; this pass takes them.
+ * Input.  raftgpu_vote_request_wire's frames (the header names the group's own slot, x is copied back), its table and
+ * its buffers.  The pass reads id, vote, last_term, commit_term, persisted, priority and the flags RAFTGPU_VOTER_LEADER
+ * (the leader's own leader_id: set) and RAFTGPU_VOTER_LEASE; RAFTGPU_VOTER_SELECT is not read.  Leadership is the
+ * arena's own: term_start != RAFTGPU_NO_TERM_START, a pair's by its low half.
+ * Status.  status[i] = RAFTGPU_WIRE_* << 4 | RAFTGPU_VREQ_* for an answered frame; the first failing check decides:
+ *   MALFORMED    a bad frame or protobuf, a group at or past the highest allocated slot, or a wide pair's high half;
+ *   SKIP_TYPE    any type but 5 and 17;
+ *   ROLE         the group is not a leader;
+ *   TERM         the group's term (raftgpu_group_set_term) is 0, or m.term is 0 (a local message);
+ * then each group's frames in frame order.  The group's claimant b(g) is its first frame that changes state: a
+ * MsgRequestVote with m.term > term that the lease does not drop, or a granted MsgRequestVote at the term (only a frame
+ * whose m.from is the leader's own vote gets one).  The frames before b(g) are decided against the unchanged leader:
+ *   IGNORED      m.term > term in lease (RAFTGPU_VOTER_LEASE, and the context is not "CampaignTransfer"), or a
+ *                MsgRequestVote with m.term < term: the reference drops it;
+ *   OK           a MsgRequestPreVote at a lower term is rejected at the group's term (raft.rs:1395-1398); a
+ *                MsgRequestPreVote above the term (the term stays) and any frame at the term meet can_vote,
+ *                is_up_to_date and the priority rule: a grant answers at m.term, a rejection at the term with
+ *                commit_info() (maybe_commit_by_vote returns at once for a Leader, :2131);
+ * b(g) is decided as raftgpu_vote_request_wire decides a bumped frame:
+ *   COMMIT_VOTE  a MsgRequestVote above the term that is rejected with m.commit != 0, m.commit_term != 0 and m.commit
+ *                beyond committed (maybe_commit_by_vote at the Follower it becomes needs the log): nothing is applied;
+ *   OK           applied: above the term, become_follower(m.term, INVALID_ID)'s arena part (term = m.term, and
+ *                RAFTGPU_CTL_RESET's reset on both halves with term_start RAFTGPU_NO_TERM_START, last_index, committed and
+ *                the table's persisted), then the grant with vote 0 and no leader (RAFTGPU_VREQ_BUMPED, and
+ *                RAFTGPU_VREQ_VOTED on a grant) or the rejection at m.term; at the term, the grant (RAFTGPU_VREQ_VOTED);
+ *   DUP          every frame after b(g): its decision depends on b(g)'s host side.  Resubmit DUP frames, in order,
+ *                after it: through raftgpu_vote_request_wire once the group is a Follower, through this pass otherwise.
+ * A frame that is not OK changes nothing: run RawNode::step on it (IGNORED ones may be dropped).  d_out (nullable,
+ * u64[2 n]) = {m.from, the group's term after the frame} per OK frame, zero for the others.
+ * Output, bound and refusals.  raftgpu_vote_request_wire's: one response per OK frame in frame order, resp_bytes_capacity
+ * at least raftgpu_vote_request_wire_bound(n), RAFTGPU_ERR_INVALID before any launch otherwise, as for a missing
+ * d_voters, d_status, d_bytes or d_offsets with n > 0, misaligned buffers and a batch past 4 GiB.  The caller sends the
+ * responses only after it has made the changed HardState (term, vote) durable.
+ * Host side.  For a RAFTGPU_VREQ_BUMPED frame the caller runs become_follower (raft.rs:1082-1093) and the host part of
+ * reset (:942-971): role Follower, no leader, vote = 0 -- then m.from for RAFTGPU_VREQ_VOTED --, election_elapsed = 0,
+ * no leadership transferee, no pending conf index, the read-index map emptied; it clears RAFTGPU_VOTER_LEADER and
+ * RAFTGPU_VOTER_LEASE, sets the group's follower select bits and updates its voter row before the next call that reads
+ * them.  For RAFTGPU_VREQ_VOTED at the term: vote = m.from, election_elapsed = 0.
+ * Ordering.  Runs between steps on `stream`, with its own scratch in the arena (run it on one stream at a time).  When
+ * one received buffer goes through several passes, this pass is the last of the leader side: after
+ * raftgpu_leader_term_wire and its host side.  A group raftgpu_leader_term_wire deposed is ROLE here: once the caller
+ * has made it a Follower, it resubmits those frames through raftgpu_vote_request_wire, after the follower passes.  The
+ * reference reaches the same state when a leader's frames are delivered in that order: its other frames, then its vote
+ * requests in frame order.  The host form copies (voters covers the groups below the highest allocated one), runs and
+ * waits; status, out, resp_bytes / resp_offsets as above, totals u64[2]. */
+int32_t raftgpu_leader_vote_request_wire_device(raftgpu_arena *arena, void *stream, const void *d_bytes,
+                                                uint64_t n_bytes, const uint32_t *d_offsets, uint64_t n,
+                                                const raftgpu_voter *d_voters, uint8_t *d_status, uint64_t *d_out,
+                                                uint8_t *d_resp_bytes, uint64_t resp_bytes_capacity,
+                                                uint32_t *d_resp_offsets, uint64_t *d_totals);
+int32_t raftgpu_leader_vote_request_wire(raftgpu_arena *arena, const void *bytes, uint64_t n_bytes,
+                                         const uint32_t *offsets, uint64_t n, const raftgpu_voter *voters,
+                                         uint8_t *status, uint64_t *out, uint8_t *resp_bytes,
+                                         uint64_t resp_bytes_capacity, uint32_t *resp_offsets, uint64_t *totals);
 
 /* ---- the responses that reach a follower or a candidate ------------------------ */
 

@@ -45,8 +45,9 @@ BULK_SORTED = 0x1
  COL_LAST_INDEX, COL_TERM, COL_INS_META) = range(14)
 WIRE_OK, WIRE_SKIP_TYPE, WIRE_TERM, WIRE_NEEDS_LOG, WIRE_MALFORMED, WIRE_DUP, WIRE_CONTEXT = range(7)
 WIRE_ROLE, WIRE_COMMIT_RANGE = 7, 8  # raftgpu_follower_heartbeat (ROLE also raftgpu_vote_wire)
-WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire, raftgpu_vote_request_wire
-WIRE_IGNORED = 10  # raftgpu_vote_request_wire, raftgpu_leader_term_wire, raftgpu_follower_response_wire
+WIRE_COMMIT_VOTE = 9  # raftgpu_vote_wire, raftgpu_vote_request_wire, raftgpu_leader_vote_request_wire
+WIRE_IGNORED = 10  # raftgpu_vote_request_wire, raftgpu_leader_vote_request_wire, raftgpu_leader_term_wire,
+#                    raftgpu_follower_response_wire
 WIRE_STALE = 11  # raftgpu_follower_term_wire, raftgpu_leader_term_wire, raftgpu_follower_response_wire
 WIRE_WAVES_MAX = 64  # raftgpu_arena_set_wire_waves
 # raftgpu_vote_request_wire: the caller's table (raftgpu_voter), its flags, and the low nibble of an applied frame
@@ -366,6 +367,8 @@ def lib() -> C.CDLL:
             "raftgpu_follower_term_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_leader_term_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_leader_term_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_leader_vote_request_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
+            "raftgpu_leader_vote_request_wire": ([vp, vp, u64, vp, u64, vp, vp, vp, vp, u64, vp, vp], i32),
             "raftgpu_follower_response_wire_device": ([vp, vp, vp, u64, vp, u64, vp, vp, vp], i32),
             "raftgpu_follower_response_wire": ([vp, vp, u64, vp, u64, vp, vp, vp], i32),
             "raftgpu_follower_append_bound": ([u64], u64),
@@ -1167,6 +1170,22 @@ class Arena:
         self._ck(self._L.raftgpu_leader_term_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters,
                                                          d_status, d_out, d_resp_bytes, resp_bytes_capacity,
                                                          d_resp_offsets, d_totals), "leader_term_wire_device")
+
+    def leader_vote_request_wire(self, frames, voters):
+        """raftgpu_leader_vote_request_wire: Raft::step's term rules and the vote arm for the MsgRequestVote /
+        MsgRequestPreVote frames of a wire batch at this arena's leaders (.bytes, .n_bytes, .offsets, .n; headers name
+        the leader's group slot), each group's frames after its claimant DUP.  voters: VOTER_DTYPE rows covering the
+        groups below the highest allocated one -> (status u8[n], out u64[n][2] = {m.from, term after} of the OK frames,
+        response blob, response offsets u32[responses + 1], totals u64[2])."""
+        vt = np.ascontiguousarray(voters, dtype=VOTER_DTYPE)
+        assert len(vt) >= self.get_info().hi
+        return self._reply("leader_vote_request_wire", frames, (vt,), (2,), vote_request_wire_bound)
+
+    def leader_vote_request_wire_device(self, d_bytes, n_bytes, d_offsets, n, d_voters, d_status, d_out, d_resp_bytes,
+                                        resp_bytes_capacity, d_resp_offsets, d_totals, stream=None):
+        self._ck(self._L.raftgpu_leader_vote_request_wire_device(self._h, stream, d_bytes, n_bytes, d_offsets, n, d_voters,
+                                                                 d_status, d_out, d_resp_bytes, resp_bytes_capacity,
+                                                                 d_resp_offsets, d_totals), "leader_vote_request_wire_device")
 
     def follower_response_wire(self, frames, voters):
         """raftgpu_follower_response_wire: Raft::step's term rules and the drop arms of step_follower and step_candidate

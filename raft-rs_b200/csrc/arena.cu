@@ -235,6 +235,7 @@ enum Pass {
     kPassFollowTerm,
     kPassLeaderTerm,
     kPassFollowResp,
+    kPassLeaderVoteRequest,
     kPassCount
 };
 

@@ -13,6 +13,12 @@
 // block_starts_kernel<2> (k_wire.cuh) turns the sums into block starts; reply_write_kernel<VrqReply> (k_wire.cuh) encodes
 // the responses (wire_put_vote_frame) and stores them through shared memory.  Every kernel takes kWireThreads frames per
 // block: one block sum per scan block.
+//
+// kLeader (DESIGN 3.24): the same frames at a leader (term_start != RAFTGPU_NO_TERM_START; SELECT is not read).  Only
+// a group's claimant b(g) changes state -- its first MsgRequestVote above the term that the lease does not drop, or a
+// granted MsgRequestVote at the term -- so the frames before it are decided against the unchanged leader, b(g) is
+// applied, and only the frames after it are DUP.  COMMIT_VOTE is tested on the bumped path alone: maybe_commit_by_vote
+// returns at once for a Leader (raft.rs:2131).
 
 // A decided frame's record: w0 = its header | the kVrq* bits; the response's to (= m.from), from (the table's id),
 // term, commit and commit_term.  A bumped frame's new term is its response's term (m.term: a bump is only decided at
@@ -33,7 +39,9 @@ __device__ __forceinline__ bool vrq_transfer(const WireMsg &m, const uint8_t *ms
 }
 
 // Frame i: its status before the duplicate rule (checks in the order of raftgpu.h) and, for the frames that reach the
-// term rules (OK, IGNORED, COMMIT_VOTE), its record (w0 alone for the last two).
+// term rules (OK, IGNORED, COMMIT_VOTE), its record (w0 alone for the last two).  kLeader: a claimant's w0 has
+// kVrqBumped or kVrqVoted.
+template <bool kLeader>
 __device__ __forceinline__ uint32_t vrq_frame(const Columns &c, const WireSrc &w, const raftgpu_voter *__restrict__ voters,
                                               const WireStage &s, const uint8_t *stage, uint32_t i, VrqRec &r) {
     uint32_t hdr;
@@ -45,7 +53,11 @@ __device__ __forceinline__ uint32_t vrq_frame(const Columns &c, const WireSrc &w
     if (m.msg_type != 5u && m.msg_type != 17u) return RAFTGPU_WIRE_SKIP_TYPE;  // eraftpb.proto:55, 67
     const raftgpu_voter &v = voters[g];
     const uint32_t flags = v.flags;
-    if (!(flags & RAFTGPU_VOTER_SELECT) || c.term_start[g] != RAFTGPU_NO_TERM_START) return RAFTGPU_WIRE_ROLE;
+    if constexpr (kLeader) {
+        if (c.term_start[g] == RAFTGPU_NO_TERM_START) return RAFTGPU_WIRE_ROLE;
+    } else {
+        if (!(flags & RAFTGPU_VOTER_SELECT) || c.term_start[g] != RAFTGPU_NO_TERM_START) return RAFTGPU_WIRE_ROLE;
+    }
     const uint64_t term = c.term[g];
     if (term == 0 || m.term == 0) return RAFTGPU_WIRE_TERM;
     const bool pre = m.msg_type == 17u;
@@ -84,8 +96,9 @@ __device__ __forceinline__ uint32_t vrq_frame(const Columns &c, const WireSrc &w
         if (!pre) r.w0 |= kVrqVoted;
         return RAFTGPU_WIRE_OK;
     }
-    // maybe_commit_by_vote (raft.rs:2126-2164) would read the caller's log
-    if (m.commit != 0 && m.commit_term != 0 && m.commit > committed) return RAFTGPU_WIRE_COMMIT_VOTE;
+    // maybe_commit_by_vote (raft.rs:2126-2164) would read the caller's log; a leader's returns at once (:2131)
+    if ((!kLeader || (r.w0 & kVrqBumped)) && m.commit != 0 && m.commit_term != 0 && m.commit > committed)
+        return RAFTGPU_WIRE_COMMIT_VOTE;
     r.w0 |= kVrqReject;
     r.term = (r.w0 & kVrqBumped) ? m.term : term;
     r.commit = committed;  // raft_log.commit_info() (raft.rs:1456-1458)
@@ -95,20 +108,31 @@ __device__ __forceinline__ uint32_t vrq_frame(const Columns &c, const WireSrc &w
 
 // Pass 1: classify every frame; status[i] = wire status << 4; the record of a frame that reached the term rules,
 // first_frame[group] = the lowest such frame of the group.  Launched with kWireThreads threads per block.
+// kLeader: first_frame[group] = the group's claimant b(g), and out[2 i..] (nullable) = {m.from, the group's term} of
+// every OK frame, 0 otherwise -- the term before b(g)'s bump, which the apply pass of the frames before b(g) could not
+// read while b(g) writes it.
+template <bool kLeader>
 __global__ void __launch_bounds__(kWireThreads) vrq_scan_kernel(Columns c, WireSrc w, const raftgpu_voter *__restrict__ voters,
                                                                 uint8_t *__restrict__ status, VrqRec *__restrict__ recs,
-                                                                uint32_t *__restrict__ first_frame) {
+                                                                uint32_t *__restrict__ first_frame, uint64_t *__restrict__ out) {
     __shared__ __align__(16) uint8_t stage[kWireStage + 16];
     WireStage s;
     const uint32_t i = wire_block_frame(w, stage, s);
     if (i == kNoFrame) return;
     VrqRec r;
-    const uint32_t st = vrq_frame(c, w, voters, s, stage, i, r);
+    const uint32_t st = vrq_frame<kLeader>(c, w, voters, s, stage, i, r);
     status[i] = static_cast<uint8_t>(st << 4);
+    if constexpr (kLeader) {
+        if (out) {
+            const bool ok = st == RAFTGPU_WIRE_OK;
+            out[2ull * i] = ok ? r.to : 0;
+            out[2ull * i + 1] = ok ? c.term[static_cast<uint32_t>(r.w0) >> 4] : 0;
+        }
+    }
     if (st == RAFTGPU_WIRE_OK) recs[i] = r;
     else if (st == RAFTGPU_WIRE_IGNORED || st == RAFTGPU_WIRE_COMMIT_VOTE) recs[i].w0 = r.w0;
     else return;
-    atomicMin(&first_frame[static_cast<uint32_t>(r.w0) >> 4], i);
+    if (!kLeader || (r.w0 & (kVrqBumped | kVrqVoted))) atomicMin(&first_frame[static_cast<uint32_t>(r.w0) >> 4], i);
 }
 
 // become_follower(term, ..)'s arena part (raft.rs:1087-1096) for group g, a wide pair by its low half: the term, then
@@ -136,8 +160,12 @@ __device__ __forceinline__ void become_follower_arena(const Columns &c, uint32_t
 // resets both halves of a pair (reset_group with RAFTGPU_CTL_RESET's arguments: no term_start, last_index, committed,
 // the table's persisted), exactly as RAFTGPU_CTL_SET_TERM + RAFTGPU_CTL_RESET.  out[2 i..] (nullable) = {m.from, the
 // term after} of an applied frame, 0 otherwise.  blk[2 * block + {0, 1}] = the block's responses and their bytes.
+// kLeader: the frames after b(g) are DUP, b(g) is applied as the first frame is, and the OK frames before it answer
+// with nothing applied (their out is the scan's).
 // Algorithmic bytes per frame: 1 read + 1 written (+ 16 out); per frame that reached the term rules 8 (w0) + 4
-// (first_frame) read; per applied one 40 (record) + 8 (term) read, and a bump's reset of its group.
+// (first_frame) read; per applied one 40 (record) + 8 (term) read, and a bump's reset of its group.  kLeader: per
+// frame 16 out written by the scan, here only for DUP frames and b(g); per OK frame before b(g) 40 (record) read.
+template <bool kLeader>
 __global__ void __launch_bounds__(kWireThreads) vrq_apply_kernel(Columns c, uint32_t n, const raftgpu_voter *__restrict__ voters,
                                                                  uint8_t *__restrict__ status, const VrqRec *__restrict__ recs,
                                                                  const uint32_t *__restrict__ first_frame,
@@ -146,15 +174,20 @@ __global__ void __launch_bounds__(kWireThreads) vrq_apply_kernel(Columns c, uint
     uint32_t resp = 0, bytes = 0;
     if (i < n) {
         uint64_t from = 0, term = 0;
+        bool put = !kLeader;  // kLeader: out is written for DUP frames and b(g) only
         const uint32_t st = status[i] >> 4;
         if (st == RAFTGPU_WIRE_OK || st == RAFTGPU_WIRE_IGNORED || st == RAFTGPU_WIRE_COMMIT_VOTE) {
             const uint64_t w0 = recs[i].w0;
-            const uint32_t g = static_cast<uint32_t>(w0) >> 4;
-            if (first_frame[g] != i) {
+            const uint32_t g = static_cast<uint32_t>(w0) >> 4, first = first_frame[g];
+            if (kLeader ? i > first : first != i) {
                 status[i] = static_cast<uint8_t>(RAFTGPU_WIRE_DUP << 4);
+                put = true;
             } else if (st == RAFTGPU_WIRE_OK) {
                 const VrqRec r = recs[i];
-                term = c.term[g];
+                if (!kLeader || i == first) {
+                    term = c.term[g];
+                    put = true;
+                }
                 if (w0 & kVrqBumped) {
                     term = r.term;
                     become_follower_arena(c, g, term, voters);
@@ -167,7 +200,7 @@ __global__ void __launch_bounds__(kWireThreads) vrq_apply_kernel(Columns c, uint
                 bytes = vrq_len(r);
             }
         }
-        if (out) {
+        if (out && put) {
             out[2ull * i] = from;
             out[2ull * i + 1] = term;
         }
